@@ -2,6 +2,7 @@
 
   python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path (one process per GPU)
   python bench.py --impl reference --steps K --warmup W    # CPU restatement of the reference path (oracle)
+  python bench.py ... --dump-outputs DIR                   # also write the last timed step's outputs as DIR/*.npy
 
 Headline workload (config.workload) = BASELINE.json configs[1]: ddpm-mel-32seq-512.cfg (TransformerDDPM L6/H8/K2/M2048,
 C=42 after slice-mel-512), batch 128 per GPU, one optimizer step = device threefry draws + q_sample + forward +
@@ -99,11 +100,9 @@ class ClockSampler(threading.Thread):
 
 
 def peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        p = json.load(open(path))
-        return p.get("bf16_tflops", 1590.0), p.get("bf16_tflops_sustained", 1400.0), p.get("hbm_gbs", 6650.0), "measured"
-    return 1590.0, 1400.0, 6650.0, "fallback"
+    """(bf16 dense TFLOP/s, the same used as the sustained figure, HBM GB/s, source): NVIDIA's H100 SXM data sheet
+    (700 W).  These are not measured; a card with a lower power limit runs below them."""
+    return 989.0, 989.0, 3350.0, "H100 SXM data sheet"
 
 
 # ----------------------------------------------------------------------------------------------- CPU arm (oracle)
@@ -238,7 +237,7 @@ def time_dominant_gemm(eng, M_tokens: int, cta_group: int, iters: int = 20):
         flush.zero_()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        L.check(lib.smd_gemm_bf16(A.data_ptr(), B.data_ptr(), M_tokens, 2048, 2048, 0, 0, 256, cta_group,
+        L.check(lib.smd_gemm_bf16(A.data_ptr(), B.data_ptr(), M_tokens, 2048, 2048, 0, 0, 0, cta_group,
                                   bias.data_ptr(), None, 0, out.data_ptr(), None, stats.data_ptr(), None, None, st))
         e1.record()
         torch.cuda.synchronize()
@@ -301,9 +300,11 @@ def make_train(ctx: Ctx, model: str, B: int):
         # rows [rank*B, (rank+1)*B) of the global batch's threefry streams (utils/losses.py:270-294)
         return eng.draws((i, 17), B, global_batch=B * world, first_row=rank * B)
 
+    last = {}
+
     def step_resident(i):
         u, e = draws(i)
-        eng.train_step(x_dev, u, e, lr=1e-3, world_size=world)
+        last["loss"], last["grad_norm"] = eng.train_step(x_dev, u, e, lr=1e-3, world_size=world)
 
     def step_e2e(i):
         xb = x_host.to(ctx.dev, non_blocking=True)                   # H2D of this step's batch (pinned)
@@ -320,8 +321,15 @@ def make_train(ctx: Ctx, model: str, B: int):
         ev.record()
         loss_done[j] = ev
 
+    def outputs():
+        # what a caller of train_step receives (loss, post-clip grad norm) and the parameters it updated: a fixed,
+        # seeded sample of 2^20 of them (the full vector is larger than the 64 MB dump budget)
+        idx = torch.from_numpy(np.sort(np.random.default_rng(7).choice(eng.params.numel(), min(1 << 20, eng.params.numel()),
+                                                                       replace=False))).to(eng.params.device)
+        return {"loss": last["loss"], "grad_norm": last["grad_norm"], "params_sample": eng.params.reshape(-1)[idx]}
+
     return dict(eng=eng, cfg=cfg, units=B, flops=3.0 * cfg.flops_fwd_per_sample() * B, resident=step_resident,
-                e2e=step_e2e, h2d=x_host.numel() * 4, d2h=4, tokens=B * 32, x_host=x_host)
+                e2e=step_e2e, h2d=x_host.numel() * 4, d2h=4, tokens=B * 32, x_host=x_host, outputs=outputs)
 
 
 def make_sample(ctx: Ctx, model: str, N: int):
@@ -347,7 +355,7 @@ def make_sample(ctx: Ctx, model: str, N: int):
         torch.cuda.current_stream().synchronize()
 
     return dict(eng=eng, cfg=cfg, units=N, flops=cfg.flops_fwd_per_sample() * N, resident=step_resident, e2e=step_e2e,
-                h2d=x_host.numel() * 4, d2h=x_host.numel() * 4, tokens=N * 32)
+                h2d=x_host.numel() * 4, d2h=x_host.numel() * 4, tokens=N * 32, outputs=lambda: {"x": x_dev})
 
 
 def extra_entry(ctx: Ctx, name: str, what: str, job, steps: int, warmup: int):
@@ -391,6 +399,15 @@ def dp_proof(ctx: Ctx, eng, B: int):
     return divergence, rel, dl
 
 
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Each array as out_dir/<name>.npy in float32 (float64 stays float64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy() if torch.is_tensor(t) else np.asarray(t)
+        a = a if a.dtype == np.float64 else a.astype(np.float32)
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a))
+
+
 def run_gpu(args):
     ctx = Ctx(args)
     if not torch.cuda.is_available():
@@ -413,7 +430,7 @@ def run_gpu(args):
     eng = job["eng"]
 
     # multi-rank runs: NCCL finishes setting up its channels / buffer registrations during the first few dozen
-    # collectives (measured at 2 and 8 GPUs: the first ~25 steps run 5-20 % slower, profiles/r02_dp_warmup_ab.txt), so
+    # collectives (the first few dozen steps can run slower), so
     # a fixed number of extra untimed steps runs before the W warm-up steps; K timed steps stay exactly K
     settle = 30 if world > 1 else 0
     for i in range(settle):
@@ -423,6 +440,8 @@ def run_gpu(args):
     ms_step, launches = ctx.timed(job["resident"], args.steps, args.warmup, eng)
     clocks.stop_flag.set()
     clocks.join(timeout=2)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, job["outputs"]())
     ms_e2e, _ = ctx.timed(job["e2e"], args.steps, max(3, args.warmup // 2), eng)
 
     units, flops_step = job["units"], job["flops"]
@@ -434,9 +453,9 @@ def run_gpu(args):
                        "cta_group": args.cta_group, "steps_per_s": 1e3 / ms_step,
                        "step_tflops": flops_step * world / (ms_step / 1e3) / 1e12,
                        "step_frac_of_sustained_peak": flops_step / (ms_step / 1e3) / 1e12 / ctx.tsust,
-                       "l2": ("per-step working set (params+grads+Adam ~400 MB, activations ~1 GB) >> 126 MB L2; no flush"
+                       "l2": ("per-step working set (params+grads+Adam ~400 MB, activations ~1 GB) >> 50 MB L2; no flush"
                               if args.workload == "train" else
-                              "per-step working set (bf16 weights 51 MB + activations ~1 GB at 32000 tokens) >> 126 MB L2; "
+                              "per-step working set (bf16 weights 51 MB + activations ~1 GB at 32000 tokens) >> 50 MB L2; "
                               "no flush"),
                        "precision": "bf16 tensor-core operands, fp32 accumulate / master weights / LN / softmax / Adam",
                        "rng": "device threefry draws (labels, alpha-bar, eps) are inside the timed step",
@@ -487,10 +506,10 @@ def run_gpu(args):
         ach = gflop / (g_ms / 1e3) / 1e12
         line["roofline"] = {"bound": "tensor", "achieved": ach, "peak": ctx.tpeak, "unit": "TFLOP/s",
                             "frac": ach / ctx.tpeak,
-                            "traffic": None,     # DRAM bytes need an ncu capture; see profiles/ (not measurable in-run)
+                            "traffic": None,     # DRAM bytes are not measurable in-run
                             "algorithmic_bytes": m_tokens * 2048 * 6 + 2048 * 2048 * 2 + m_tokens * 8 + 8192,
-                            "peak_source": f"MEASURED_PEAKS.json bf16_tflops ({ctx.peak_src}, burst: kernel timed alone)",
-                            "kernel": f"gemm_bf16_tcgen05_kernel<{args.cta_group}> [{m_tokens}x2048x2048] res-block GEMM "
+                            "peak_source": f"{ctx.peak_src} bf16 dense (kernel timed alone)",
+                            "kernel": f"gemm_bf16_wgmma_kernel [{m_tokens}x2048x2048] res-block GEMM "
                                       "+ bias + row-stat epilogue", "ms_per_launch": g_ms}
         if not args.no_cpu:
             threads = host_threads()
@@ -515,6 +534,8 @@ def main():
     ap.add_argument("--cta-group", dest="cta_group", type=int, default=2)
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-extra", action="store_true", help="skip the extra BASELINE configs")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write what the last timed step computed as DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

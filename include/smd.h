@@ -1,4 +1,4 @@
-/* libsmd -- C ABI of the B200-native DDPM noise-prediction hot path.
+/* libsmd -- C ABI of the native (sm_90a) DDPM noise-prediction hot path.
  *
  * The reference (magenta/symbolic-music-diffusion @ 469204d) has no FFI: its only host->device boundary is the
  * jax.jit boundary of three Python callables.  Each entry point below replaces one of them (or a piece of one)
@@ -55,7 +55,7 @@ typedef struct smd_config {
   int seq_len;         /* S: data_shape[0] (32) for TransformerDDPM, 1 for DenseDDPM */
   int channels;        /* C: data_shape[-1] after --slice_ckpt (42 / 146 / 512) */
   int max_batch;       /* largest number of examples one call may pass */
-  int cta_group;       /* 1 or 2: tcgen05 cta_group used by the GEMMs (2 = CTA pairs, M=256 tiles) */
+  int cta_group;       /* 1 or 2 (accepted for compatibility; sm_90a GEMMs use one CTA per tile) */
   int training;        /* 1: reserve the saved-activation / gradient buffers of smd_ddpm_grads */
   int sampler_T;       /* > 0: reserve a (K, sampler_T, 2*mlp_dims) FiLM table so the sampler evaluates the FiLM
                           generator once per schedule instead of once per step (all samples share t) */
@@ -74,7 +74,7 @@ int smd_version(void);
 int smd_plan_create(const smd_config* cfg, smd_plan** out);
 void smd_plan_destroy(smd_plan* plan);
 /* fp32 parameter arena: `smd_num_tensors` named tensors laid out back to back (each start 16-byte aligned)
- * inside `smd_arena_floats` floats.  Names mirror the flax module tree (DESIGN.md "Parameter arena"). */
+ * inside `smd_arena_floats` floats.  Names mirror the flax module tree. */
 int smd_num_tensors(const smd_plan* plan);
 long long smd_arena_floats(const smd_plan* plan);
 int smd_tensor_info(const smd_plan* plan, int index, char* name, int name_cap, long long* offset, int* shape4,
@@ -198,7 +198,7 @@ int smd_threefry_uniform(const uint32_t host_key[2], float* out, long long n, fl
 int smd_threefry_split(const uint32_t host_key[2], int num, uint32_t* host_out_keys);
 
 /* ---- test hooks (used by tests/ only) --------------------------------------------------------------------- */
-/* D[M,N] = A * B^T with the production tcgen05 kernel.  A: bf16, K-major [M][K] or MN-major [K][M];
+/* D[M,N] = A * B^T with the production wgmma kernel.  A: bf16, K-major [M][K] or MN-major [K][M];
  * B: bf16, K-major [N][K] or MN-major [K][N].  Optional fused epilogue pieces (NULL to skip). */
 int smd_gemm_bf16(const void* A, const void* B, int M, int N, int K, int a_mn, int b_mn, int BN, int cta_group,
                   const float* bias, const float* residual, int act, float* out_f32, void* out_bf16,
@@ -206,7 +206,7 @@ int smd_gemm_bf16(const void* A, const void* B, int M, int N, int K, int a_mn, i
 /* forward pass that keeps every intermediate in the training save buffers (plan must have training = 1) */
 int smd_debug_forward_save(smd_plan* plan, const float* params, const float* x, const float* t, int batch, float* y,
                            smd_stream_t stream);
-/* device pointer / size of a named workspace region (names: DESIGN.md "Workspace"), for stage-by-stage parity */
+/* device pointer / size of a named workspace region (names as allocated in smd_api.cu), for stage-by-stage parity */
 int smd_debug_buffer(smd_plan* plan, const char* name, void** dev_ptr, size_t* bytes);
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
 long long smd_launch_count(void);

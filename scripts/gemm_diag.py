@@ -1,4 +1,4 @@
-"""Diagnostic sweep of the tcgen05 GEMM on a GPU box: every case runs in its own process (a trap or fault cannot
+"""Diagnostic sweep of the wgmma GEMM on a GPU: every case runs in its own process (a trap or fault cannot
 poison the next) and prints error structure, not just pass/fail.  Usage: python scripts/gemm_diag.py"""
 import json
 import os

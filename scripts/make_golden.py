@@ -1,5 +1,5 @@
 """Generates tests/golden/*.npz from the float64 oracle (the reference has no golden vectors and cannot be run:
-JAX 0.2.8 / flax 0.3.0 are not installable here -- see DESIGN.md).  Re-run: python scripts/make_golden.py"""
+JAX 0.2.8 / flax 0.3.0 are not installable here).  Re-run: python scripts/make_golden.py"""
 import os
 import sys
 

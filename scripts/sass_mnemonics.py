@@ -1,6 +1,6 @@
-"""Per-kernel SASS mnemonic counts of libsmd.so (cuobjdump -sass): the evidence that the hot kernels use tcgen05
-(UTCHMMA / UTCBAR / LDTM / STTM), TMA (UTMALDG), mbarriers (SYNCS), packed fp32 (FADD2 / FMUL2 / FFMA2), mma.sync (HMMA)
-and programmatic dependent launch.  Usage: python scripts/sass_mnemonics.py > profiles/rNN_sass_mnemonics.txt"""
+"""Per-kernel SASS mnemonic counts of libsmd.so (cuobjdump -sass): the evidence that the hot kernels use wgmma (HGMMA),
+TMA (UTMALDG), mbarriers (SYNCS), mma.sync (HMMA) and programmatic dependent launch.
+Usage: python scripts/sass_mnemonics.py"""
 import collections
 import os
 import re
@@ -9,8 +9,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "symbolic-music-diffusion_b200", "libsmd.so")
-KEYS = ["UTCHMMA", "UTCBAR", "UTMALDG", "UTMASTG", "LDTM", "STTM", "UTCATOMSWS", "SYNCS", "HMMA", "MUFU.TANH", "FFMA2", "FMUL2",
-        "FADD2", "LDGSTS", "UBLKCP", "ACQBULK", "RED", "ATOM"]
+KEYS = ["HGMMA", "UTMALDG", "UTMASTG", "SYNCS", "HMMA", "MUFU.TANH", "LDGSTS", "UBLKCP", "ACQBULK", "RED", "ATOM"]
 
 
 def main():
@@ -40,8 +39,8 @@ def main():
         d = re.sub(r"^void ", "", d)
         d = re.sub(r"\(.*$", "", d).replace("smd::", "")
         names[mangled] = d
-    print("# SASS mnemonics per kernel (cuobjdump -sass libsmd.so, sm_100a): tcgen05 = UTCHMMA / UTCBAR / LDTM / STTM /")
-    print("# UTCATOMSWS (TMEM alloc); TMA = UTMALDG; mbarrier = SYNCS; mma.sync = HMMA; packed fp32 = FFMA2 / FMUL2 / FADD2;")
+    print("# SASS mnemonics per kernel (cuobjdump -sass libsmd.so, sm_90a): wgmma = HGMMA;")
+    print("# TMA = UTMALDG; mbarrier = SYNCS; mma.sync = HMMA;")
     print("# cp.async = LDGSTS; programmatic dependent launch = ACQBULK")
     seen = set()
     for mangled in sorted(counts, key=lambda k: names[k]):

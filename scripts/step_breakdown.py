@@ -1,7 +1,7 @@
 """Phase breakdown of one train step from a CUPTI timeline written by scripts/timeline.py (eager or graph replay):
-prologue, trunk forward, tail forward, tail backward, trunk backward, optimizer -- the table in DESIGN.md section 7.
+prologue, trunk forward, tail forward, tail backward, trunk backward, optimizer.
 Phases are cut on the main (dX) stream at well-defined kernels; the other two streams overlap and are reported as
-busy time.  Usage: python scripts/step_breakdown.py profiles/r02_timeline_train_eager.json"""
+busy time.  Usage: python scripts/step_breakdown.py <timeline.json written by scripts/timeline.py>"""
 import json
 import sys
 from collections import defaultdict

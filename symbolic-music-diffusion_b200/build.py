@@ -1,4 +1,4 @@
-"""Builds libsmd.so (hand-written sm_100a CUDA + C ABI) in-tree with nvcc.  No torch extension machinery:
+"""Builds libsmd.so (hand-written sm_90a CUDA + C ABI) in-tree with nvcc.  No torch extension machinery:
 the product boundary is a plain C-ABI shared library loaded with ctypes (include/smd.h)."""
 from __future__ import annotations
 
@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libsmd.so")
 SOURCES = ["smd_api.cu", "kernels.cu", "train.cu", "backward.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xptxas", "-v",
 ]
 
@@ -61,7 +61,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=4) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [nvcc, "-shared", "-o", OUT, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    cmd = [nvcc, "-shared", "-o", OUT, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

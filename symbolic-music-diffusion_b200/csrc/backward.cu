@@ -1,6 +1,6 @@
 // Hand-written backward pass of the DDPM objective: what jax.value_and_grad(loss_fn) produces at
 // train_ncsn.py:282-283 for diffusion_loss (utils/losses.py:250-308) over TransformerDDPM / DenseDDPM.
-// Every matmul runs on the tcgen05 GEMM (dX: K-major operands, dW: MN-major operands reducing over tokens,
+// Every matmul runs on the wgmma GEMM (dX: K-major operands, dW: MN-major operands reducing over tokens,
 // split-K + atomics for the skinny ones); everything else is SIMT (backward_kernels.cuh).
 #include "plan.cuh"
 #include "backward_kernels.cuh"

@@ -1,4 +1,4 @@
-// Host side of the tcgen05 GEMM: tensor-map construction (cuTensorMapEncodeTiled through the runtime's
+// Host side of the wgmma GEMM: tensor-map construction (cuTensorMapEncodeTiled through the runtime's
 // driver-entry-point lookup, so libsmd.so has no link-time dependency on libcuda) and the launcher.
 #pragma once
 #include <cstdlib>
@@ -7,9 +7,8 @@
 #include <cudaTypedefs.h>
 #include <atomic>
 #include <string>
-#include "gemm_tcgen05.cuh"
-#include "ffn_fused.cuh"
-#include "attn_block.cuh"
+#include "gemm_wgmma.cuh"
+#include "fused_wgmma.cuh"
 #include "pdl_launch.cuh"
 
 namespace smd {
@@ -54,15 +53,14 @@ struct GemmOp {
   int N = 0, K = 0, BN = 0, cg = 1, a_mn = 0, b_mn = 0, k_splits = 1;
 };
 
-inline int choose_bn(int N, int cg) {
-  if (N % 256 == 0) return 256;
-  if (N % 128 == 0) return 128;
-  const int q = 16 * cg;
-  if (N < 256) return ((N + q - 1) / q) * q;
-  return 256;
+inline int choose_bn(int N, int /*cg*/) {
+  if (N % kBNMax == 0 || N > kBNMax) return kBNMax;
+  return ((N + 15) / 16) * 16;
 }
 
 // A: K-major [a_rows][K] (a_mn=0) or MN-major [K][a_rows] (a_mn=1); same for B with N rows.
+// Every tile is computed by one CTA (sm_90 has no paired-CTA MMA): `cg` is accepted for interface compatibility and the
+// op is recorded as cg = 1.  A requested BN above kBNMax is lowered to kBNMax (the widest accumulator tile).
 inline bool make_gemm_op(GemmOp* op, const void* A, uint64_t a_rows, const void* B, uint64_t b_rows_total, int N,
                          int K, int BN, int cg, int a_mn, int b_mn, uint64_t k_rows_a = 0, uint64_t k_rows_b = 0,
                          size_t lo_bytes = 0) {
@@ -72,15 +70,17 @@ inline bool make_gemm_op(GemmOp* op, const void* A, uint64_t a_rows, const void*
                       b_rows_total, N, K, BN, cg, a_mn, b_mn, k_rows_a, k_rows_b, 0)) return false;
     op->tmA_lo = lo.tmA; op->tmB_lo = lo.tmB; op->has_lo = true;
   }
-  op->N = N; op->K = K; op->BN = BN; op->cg = cg; op->a_mn = a_mn; op->b_mn = b_mn; op->k_splits = 1;
+  if (cg != 1 && cg != 2) { set_error("cta_group must be 1 or 2"); return false; }
+  if (BN > kBNMax) BN = kBNMax;
+  op->N = N; op->K = K; op->BN = BN; op->cg = 1; op->a_mn = a_mn; op->b_mn = b_mn; op->k_splits = 1;
   if (K % 64 != 0) { set_error("GEMM K must be a multiple of 64"); return false; }
-  if (BN % (16 * cg) != 0 || BN > 256 || BN < 16 * cg) { set_error("bad BN " + std::to_string(BN)); return false; }
-  if (b_mn && (BN / cg) % 64 != 0) { set_error("MN-major B needs BN/cta_group % 64 == 0"); return false; }
+  if (BN % 16 != 0 || BN < 16) { set_error("bad BN " + std::to_string(BN)); return false; }
+  if (b_mn && BN % 64 != 0) { set_error("MN-major B needs BN % 64 == 0"); return false; }
   bool ok;
   if (!a_mn) ok = make_tmap_bf16(&op->tmA, A, a_rows, static_cast<uint64_t>(K), 128);
   else ok = make_tmap_bf16(&op->tmA, A, k_rows_a ? k_rows_a : static_cast<uint64_t>(K), a_rows, 64);
   if (!ok) return false;
-  if (!b_mn) ok = make_tmap_bf16(&op->tmB, B, b_rows_total, static_cast<uint64_t>(K), static_cast<uint32_t>(BN / cg));
+  if (!b_mn) ok = make_tmap_bf16(&op->tmB, B, b_rows_total, static_cast<uint64_t>(K), static_cast<uint32_t>(BN));
   else ok = make_tmap_bf16(&op->tmB, B, k_rows_b ? k_rows_b : static_cast<uint64_t>(K), b_rows_total, 64);
   return ok;
 }
@@ -91,7 +91,7 @@ inline int device_sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   return sms;
 }
@@ -136,12 +136,12 @@ inline int stats_slots_for(const GemmOp& op, const GemmEpilogue& ep) {
   return ((op.N + op.BN - 1) / op.BN) * (epi_warps_for(op, ep) / 4);
 }
 
-template <int kCG, uint32_t kF, int kEW = 8>
+template <uint32_t kF, int kEW = 8>
 inline cudaError_t launch_gemm_inst(const GemmOp& op, int M, const GemmEpilogue& ep, cudaStream_t st) {
-  using SM = GemmSmem<kCG, kEW, lnf_kind(kF), scr_floats(kF)>;
+  using SM = GemmSmem<kEW, lnf_kind(kF), scr_floats(kF)>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tcgen05_kernel<kCG, kF, kEW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<kF, kEW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          SM::kTotal);
     if (e != cudaSuccess) return e;
     attr_set = true;
@@ -155,9 +155,9 @@ inline cudaError_t launch_gemm_inst(const GemmOp& op, int M, const GemmEpilogue&
   const int per = (num_kb + splits - 1) / splits;
   splits = (num_kb + per - 1) / per;
   sh.k_splits = splits;
-  const int rows_per_tile = kBM * kCG;
+  const int rows_per_tile = kBM;
   const int tiles = ((M + rows_per_tile - 1) / rows_per_tile) * ((op.N + op.BN - 1) / op.BN) * splits;
-  int groups = device_sm_count() / kCG;
+  int groups = device_sm_count();
   if (tiles < groups) groups = tiles;
   if constexpr ((kF & F_LNF) != 0 && (kF & F_RAGGED) == 0) {
     // the n-tiles of one row block exchange LayerNorm partials: keep them in the same scheduling round
@@ -166,64 +166,52 @@ inline cudaError_t launch_gemm_inst(const GemmOp& op, int M, const GemmEpilogue&
   }
   if (groups < 1) groups = 1;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>(groups * kCG));
+  cfg.gridDim = dim3(static_cast<unsigned>(groups));
   cfg.blockDim = dim3(SM::kThreads);
   cfg.dynamicSmemBytes = SM::kTotal;
   cfg.stream = st;
-  cudaLaunchAttribute attrs[2];
-  attrs[0].id = cudaLaunchAttributeClusterDimension;
-  attrs[0].val.clusterDim.x = kCG;
-  attrs[0].val.clusterDim.y = 1;
-  attrs[0].val.clusterDim.z = 1;
-  attrs[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attrs[1].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attrs[1];
+  attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attrs[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attrs;
-  cfg.numAttrs = pdl_enabled() ? 2 : 1;
+  cfg.numAttrs = pdl_enabled() ? 1 : 0;
   g_launches.fetch_add(1, std::memory_order_relaxed);
-  return cudaLaunchKernelEx(&cfg, gemm_bf16_tcgen05_kernel<kCG, kF, kEW>, op.tmA, op.tmB, sh, ep);
-}
-
-template <int kCG>
-inline cudaError_t launch_gemm_cg(const GemmOp& op, int M, const GemmEpilogue& ep, cudaStream_t st) {
-  if (ep.lnf_part != nullptr) {
-    // LN-fused two-pass epilogue (the caller arms it only for full, aligned tiles; see smd_api.cu::arm_lnf)
-    if (!epi_clean(op, ep) || op.N % op.BN != 0 || op.BN % 64 != 0 || op.k_splits > 1) return cudaErrorInvalidValue;
-    if constexpr (kCG == 2) {   // (the 64 KB parking buffer only fits next to the 32 KB pipeline slots of CTA pairs)
-      // epilogue warps per kind: SMD_LNF_WARPS_A / _B = 8 (default) | 12 (three warps per TMEM quadrant, <= 128 registers;
-      // measured slower: 280 / 371 us against 217 / 298 us per launch at 32000 tokens)
-      static const int wa = [] { const char* v = getenv("SMD_LNF_WARPS_A"); return (v && atoi(v) == 12) ? 12 : 8; }();
-      static const int wb = [] { const char* v = getenv("SMD_LNF_WARPS_B"); return (v && atoi(v) == 12) ? 12 : 8; }();
-      if (ep.residual != nullptr || ep.out_f32 != nullptr)
-        return wb == 12 ? launch_gemm_inst<kCG, kEpiLnfB, 12>(op, M, ep, st) : launch_gemm_inst<kCG, kEpiLnfB, 8>(op, M, ep, st);
-      return wa == 12 ? launch_gemm_inst<kCG, kEpiLnfA, 12>(op, M, ep, st) : launch_gemm_inst<kCG, kEpiLnfA, 8>(op, M, ep, st);
-    } else {
-      return cudaErrorInvalidValue;
-    }
-  }
-  if (ep.lo_delta != 0) return launch_gemm_inst<kCG, kEpiStrict>(op, M, ep, st);   // strict-precision mode (bf16x3)
-  const uint32_t need = epi_needs(ep);
-  if (epi_clean(op, ep)) {
-    auto fits = [&](uint32_t kind) { return (need & ~kind) == 0; };
-    // short-K GEMMs are epilogue-bound: give them a third epilogue warp per TMEM quadrant
-    const bool short_k = op.K <= 256;
-    if (fits(kEpiF32)) return short_k ? launch_gemm_inst<kCG, kEpiF32, 12>(op, M, ep, st) : launch_gemm_inst<kCG, kEpiF32>(op, M, ep, st);
-    if (fits(kEpiAtomic)) return launch_gemm_inst<kCG, kEpiAtomic>(op, M, ep, st);
-    if (fits(kEpiF32Res)) return launch_gemm_inst<kCG, kEpiF32Res>(op, M, ep, st);
-    if (fits(kEpiAct)) return short_k ? launch_gemm_inst<kCG, kEpiAct, 12>(op, M, ep, st) : launch_gemm_inst<kCG, kEpiAct>(op, M, ep, st);
-    if (fits(kEpiGG)) return launch_gemm_inst<kCG, kEpiGG>(op, M, ep, st);
-    if ((need & F_LN) && fits(kEpiLn) && op.N == op.BN && op.BN <= 128 && op.BN % 64 == 0 && op.k_splits <= 1)
-      return launch_gemm_inst<kCG, kEpiLn>(op, M, ep, st);
-  }
-  return launch_gemm_inst<kCG, kEpiGeneric>(op, M, ep, st);
+  return cudaLaunchKernelEx(&cfg, gemm_bf16_wgmma_kernel<kF, kEW>, op.tmA, op.tmB, sh, ep);
 }
 
 inline cudaError_t launch_gemm(const GemmOp& op, int M, const GemmEpilogue& ep, cudaStream_t st) {
-  return op.cg == 2 ? launch_gemm_cg<2>(op, M, ep, st) : launch_gemm_cg<1>(op, M, ep, st);
+  if (ep.lnf_part != nullptr) {
+    // LN-fused two-pass epilogue (the caller arms it only for full, aligned tiles; see smd_api.cu::arm_lnf)
+    if (!epi_clean(op, ep) || op.N % op.BN != 0 || op.BN % 64 != 0 || op.k_splits > 1) return cudaErrorInvalidValue;
+    // epilogue warps per kind: SMD_LNF_WARPS_A / _B = 8 (default) | 12 (three warps per row quadrant)
+    static const int wa = [] { const char* v = getenv("SMD_LNF_WARPS_A"); return (v && atoi(v) == 12) ? 12 : 8; }();
+    static const int wb = [] { const char* v = getenv("SMD_LNF_WARPS_B"); return (v && atoi(v) == 12) ? 12 : 8; }();
+    if (ep.residual != nullptr || ep.out_f32 != nullptr)
+      return wb == 12 ? launch_gemm_inst<kEpiLnfB, 12>(op, M, ep, st) : launch_gemm_inst<kEpiLnfB, 8>(op, M, ep, st);
+    return wa == 12 ? launch_gemm_inst<kEpiLnfA, 12>(op, M, ep, st) : launch_gemm_inst<kEpiLnfA, 8>(op, M, ep, st);
+  }
+  // full-row LayerNorm needs the whole row in one tile (N <= BN; BN is at most kBNMax)
+  if (ep.ln_gamma != nullptr && op.N > op.BN) return cudaErrorInvalidValue;
+  if (ep.lo_delta != 0) return launch_gemm_inst<kEpiStrict>(op, M, ep, st);   // strict-precision mode (bf16x3)
+  const uint32_t need = epi_needs(ep);
+  if (epi_clean(op, ep)) {
+    auto fits = [&](uint32_t kind) { return (need & ~kind) == 0; };
+    // short-K GEMMs are epilogue-bound: give them a third epilogue warp per row quadrant
+    const bool short_k = op.K <= 256;
+    if (fits(kEpiF32)) return short_k ? launch_gemm_inst<kEpiF32, 12>(op, M, ep, st) : launch_gemm_inst<kEpiF32>(op, M, ep, st);
+    if (fits(kEpiAtomic)) return launch_gemm_inst<kEpiAtomic>(op, M, ep, st);
+    if (fits(kEpiF32Res)) return launch_gemm_inst<kEpiF32Res>(op, M, ep, st);
+    if (fits(kEpiAct)) return short_k ? launch_gemm_inst<kEpiAct, 12>(op, M, ep, st) : launch_gemm_inst<kEpiAct>(op, M, ep, st);
+    if (fits(kEpiGG)) return launch_gemm_inst<kEpiGG>(op, M, ep, st);
+    if ((need & F_LN) && fits(kEpiLn) && op.N == op.BN && op.BN <= 128 && op.BN % 64 == 0 && op.k_splits <= 1)
+      return launch_gemm_inst<kEpiLn>(op, M, ep, st);
+  }
+  return launch_gemm_inst<kEpiGeneric>(op, M, ep, st);
 }
 
 
 // ---------------------------------------------------------------------------------------------------
-// fused FFN (ffn_fused.cuh)
+// fused FFN (fused_wgmma.cuh)
 // ---------------------------------------------------------------------------------------------------
 struct FfnOp {
   CUtensorMap tmA, tmW1, tmW2;
@@ -244,7 +232,28 @@ inline bool ffn_fused_forced() {
   static const bool on = [] { const char* v = getenv("SMD_FFN_FUSED"); return v && v[0] == '2'; }();
   return on;
 }
+// persistent grid of min(#SMs, tiles) CTAs, programmatic dependent launch when enabled
+template <typename Kern, typename Args>
+inline cudaError_t launch_fused(Kern kern, int tiles, int threads, int smem, const CUtensorMap& t0, const CUtensorMap& t1,
+                                const CUtensorMap& t2, const Args& a, cudaStream_t st) {
+  int grid = device_sm_count();
+  if (tiles < grid) grid = tiles;
+  if (grid < 1) grid = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(static_cast<unsigned>(grid));
+  cfg.blockDim = dim3(static_cast<unsigned>(threads));
+  cfg.dynamicSmemBytes = static_cast<size_t>(smem);
+  cfg.stream = st;
+  cudaLaunchAttribute attrs[1];
+  attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attrs[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attrs;
+  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return cudaLaunchKernelEx(&cfg, kern, t0, t1, t2, a);
+}
 inline cudaError_t launch_ffn_fused(const FfnOp& op, const FfnFusedArgs& a, cudaStream_t st) {
+  if (a.Md % 128 != 0) return cudaErrorInvalidValue;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(ffn_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FfnSmem::kTotal);
@@ -253,36 +262,24 @@ inline cudaError_t launch_ffn_fused(const FfnOp& op, const FfnFusedArgs& a, cuda
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  const int tiles = (a.M + 255) / 256;
-  int pairs = device_sm_count() / 2;
-  if (tiles < pairs) pairs = tiles;
-  if (pairs < 1) pairs = 1;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>(2 * pairs));
-  cfg.blockDim = dim3(FfnSmem::kThreads);
-  cfg.dynamicSmemBytes = FfnSmem::kTotal;
-  cfg.stream = st;
-  cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attrs[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attrs;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  if (a.hidden_pre != nullptr || a.hidden != nullptr) return cudaLaunchKernelEx(&cfg, ffn_fused_kernel<true>, op.tmA, op.tmW1, op.tmW2, a);
-  return cudaLaunchKernelEx(&cfg, ffn_fused_kernel<false>, op.tmA, op.tmW1, op.tmW2, a);
+  const int tiles = (a.M + 127) / 128;
+  if (a.hidden_pre != nullptr || a.hidden != nullptr)
+    return launch_fused(ffn_fused_kernel<true>, tiles, FfnSmem::kThreads, FfnSmem::kTotal, op.tmA, op.tmW1, op.tmW2, a, st);
+  return launch_fused(ffn_fused_kernel<false>, tiles, FfnSmem::kThreads, FfnSmem::kTotal, op.tmA, op.tmW1, op.tmW2, a, st);
 }
 
 
 // ---------------------------------------------------------------------------------------------------
-// fused attention block (attn_block.cuh)
+// fused attention block (fused_wgmma.cuh)
 // ---------------------------------------------------------------------------------------------------
 struct AttnOp {
   CUtensorMap tmA, tmWqkv, tmWo;
   bool ok = false;
 };
-// A: bf16 [rows][128] K-major; Wqkv: bf16 (128, 384) row-major; Wo: bf16 (128, 128) row-major (MN-major B operands)
+// A: bf16 [rows][128] K-major (64-row tiles); Wqkv: bf16 (128, 384) row-major; Wo: bf16 (128, 128) row-major
+inline bool make_attn_a(CUtensorMap* tm, const void* A, uint64_t rows) { return make_tmap_bf16(tm, A, rows, 128, 64); }
 inline bool make_attn_op(AttnOp* op, const void* A, uint64_t rows, const void* Wqkv, const void* Wo) {
-  op->ok = make_tmap_bf16(&op->tmA, A, rows, 128, 128) && make_tmap_bf16(&op->tmWqkv, Wqkv, 128, 384, 64) &&
+  op->ok = make_attn_a(&op->tmA, A, rows) && make_tmap_bf16(&op->tmWqkv, Wqkv, 128, 384, 64) &&
            make_tmap_bf16(&op->tmWo, Wo, 128, 128, 64);
   return op->ok;
 }
@@ -291,16 +288,15 @@ inline bool attn_block_enabled() {
   static const bool on = [] { const char* v = getenv("SMD_ATTN_BLOCK"); return !(v && v[0] == '0'); }();
   return on;
 }
-// SMD_ATTN_BLOCK_TRAIN=1: the training forward uses the block kernel too (kTrain: q | k | v, probabilities and the
-// attention output are written out for the backward pass).  Off by default: at batch 128 only 16 CTA pairs are busy and
-// the scattered saves make the launch 34 us against 25 us for the three-launch path (profiles/r02_bench_train_attn*.json).
+// SMD_ATTN_BLOCK_TRAIN=1: the training forward uses the block kernel too (q | k | v, probabilities and the attention
+// output are written out for the backward pass).  Off by default (not measured against the three-launch path on H100).
 inline bool attn_block_train_enabled() {
   static const bool on = [] { const char* v = getenv("SMD_ATTN_BLOCK_TRAIN"); return v && v[0] == '1'; }();
   return on;
 }
 inline cudaError_t launch_attn_block(const AttnOp& op, const AttnBlockArgs& a, cudaStream_t st) {
   const int dh = 128 / a.H;
-  if (dh != 8 && dh != 16) return cudaErrorInvalidValue;
+  if ((dh != 8 && dh != 16) || a.M % 32 != 0) return cudaErrorInvalidValue;
   const bool train = a.qkv_out != nullptr;
   if (train && (a.probs_out == nullptr || a.o_out == nullptr)) return cudaErrorInvalidValue;
   static bool attr_set = false;
@@ -315,27 +311,14 @@ inline cudaError_t launch_attn_block(const AttnOp& op, const AttnBlockArgs& a, c
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  const int tiles = (a.M + 255) / 256;
-  int pairs = device_sm_count() / 2;
-  if (tiles < pairs) pairs = tiles;
-  if (pairs < 1) pairs = 1;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>(2 * pairs));
-  cfg.blockDim = dim3(AttnSmem::kThreads);
-  cfg.dynamicSmemBytes = AttnSmem::kTotal;
-  cfg.stream = st;
-  cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attrs[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attrs;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  g_launches.fetch_add(1, std::memory_order_relaxed);
+  const int tiles = (a.M + 63) / 64;
+  const int T = AttnSmem::kThreads, B = AttnSmem::kTotal;
   if (train) {
-    if (dh == 16) return cudaLaunchKernelEx(&cfg, attn_block_kernel<16, true>, op.tmA, op.tmWqkv, op.tmWo, a);
-    return cudaLaunchKernelEx(&cfg, attn_block_kernel<8, true>, op.tmA, op.tmWqkv, op.tmWo, a);
+    if (dh == 16) return launch_fused(attn_block_kernel<16, true>, tiles, T, B, op.tmA, op.tmWqkv, op.tmWo, a, st);
+    return launch_fused(attn_block_kernel<8, true>, tiles, T, B, op.tmA, op.tmWqkv, op.tmWo, a, st);
   }
-  if (dh == 16) return cudaLaunchKernelEx(&cfg, attn_block_kernel<16, false>, op.tmA, op.tmWqkv, op.tmWo, a);
-  return cudaLaunchKernelEx(&cfg, attn_block_kernel<8, false>, op.tmA, op.tmWqkv, op.tmWo, a);
+  if (dh == 16) return launch_fused(attn_block_kernel<16, false>, tiles, T, B, op.tmA, op.tmWqkv, op.tmWo, a, st);
+  return launch_fused(attn_block_kernel<8, false>, tiles, T, B, op.tmA, op.tmWqkv, op.tmWo, a, st);
 }
 
 }  // namespace smd

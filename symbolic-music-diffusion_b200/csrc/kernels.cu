@@ -255,7 +255,7 @@ __global__ void attention_kernel(const float* __restrict__ qkv, __nv_bfloat16* _
 }
 // ---------------------------------------------------------------------------------------------------
 // Tensor-core variant (DH % 8 == 0): same CTA / warp mapping, but Q K^T and P V run on mma.sync m16n8k8 tf32
-// (a 32x32x16 problem per head is far below a tcgen05 tile; ~350 instructions per warp instead of ~2000).
+// (a 32x32x16 problem per head is far below a wgmma tile; ~350 instructions per warp instead of ~2000).
 // q, k, v are rounded to tf32 once while the CTA stages them in shared memory (row pitch = W + 4 words, so every
 // fragment read is bank-conflict free); scores, softmax and the P V accumulation stay fp32.  The softmax output is
 // fed to the second MMA straight from the accumulator registers: within each block of 8 keys, k-slot t holds key 2t

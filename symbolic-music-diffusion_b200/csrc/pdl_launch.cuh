@@ -10,8 +10,8 @@
 namespace smd {
 
 // SMD_PDL: 0 = programmatic dependent launch off, 1 (default) = tensor-core GEMM launches only, 2 = SIMT kernels
-// too.  Measured on B200 (train step, batch 128): 2.17 ms / 1.98 ms / 2.21 ms -- early-resident SIMT CTAs hold
-// shared memory that the 214 KB GEMM CTAs of the weight-gradient stream need, so level 2 stays opt-in.
+// too.  Early-resident SIMT CTAs can hold shared memory that the
+// ~220 KB GEMM CTAs of the weight-gradient stream need, so level 2 stays opt-in (not re-measured on H100).
 inline int pdl_level() {
   static const int lvl = [] { const char* v = getenv("SMD_PDL"); return (v && v[0] >= '0' && v[0] <= '2') ? v[0] - '0' : 1; }();
   return lvl;
@@ -19,8 +19,7 @@ inline int pdl_level() {
 inline bool pdl_enabled() { return pdl_level() >= 1; }
 // SMD_PDL_SIMT: bit mask of SIMT kernel groups that also launch programmatically at level 1
 // (1: ln128_bwd, 2: attention fwd / bwd, 4: LayerNorm-FiLM forward, 8: LayerNorm-FiLM backward, 16: the rest).
-// Measured per group on the train step (1.761 ms with mask 0): 1 -> 1.836, 2 -> 1.828, 4 -> 1.809, 8 -> 1.764,
-// 16 -> 1.758 ms; sampling 1.912 -> 1.906 .. 1.953 ms.  None pays, so the default mask is 0.
+// Default mask 0 (no group measured to pay off; not re-measured on H100).
 inline int pdl_simt_mask() {
   static const int m = [] { const char* v = getenv("SMD_PDL_SIMT"); return v ? atoi(v) : SMD_PDL_SIMT_DEFAULT; }();
   return m;

@@ -75,8 +75,8 @@ struct smd_plan {
   int pack_tiles = 0;
   // ---- GEMM ops ----
   std::vector<GemmOp> op_qkv, op_o, op_ffn1, op_ffn2, op_a, op_b, op_b2;
-  std::vector<FfnOp> op_ffn;   // fused FFN (cta_group 2, mlp_dims % 128 == 0)
-  std::vector<AttnOp> op_attn; // fused attention block (cta_group 2, head dim 8 / 16, inference)
+  std::vector<FfnOp> op_ffn;   // fused FFN (mlp_dims % 128 == 0)
+  std::vector<AttnOp> op_attn; // fused attention block (head dim 8 / 16)
   GemmOp op_post, op_out, op_in;
   // sampler
   int T = 0;
@@ -125,10 +125,9 @@ struct smd_plan {
 
 namespace smd {
 // Split-K of the two K = mlp_dims, N = 128 trunk GEMMs (FFN-down forward, FFN-up dX backward) when the token count
-// leaves most CTA pairs idle: 16 tiles at batch 128 -> 64 tile-splits, fp32 slabs added in a fixed order by the
-// consumer.  Opt-in (SMD_FFN_SPLITK=1): the GEMMs themselves drop from 17 to 7-12 us, but the extra reduce launch and
-// the 64 CTA pairs now competing with the weight-gradient stream make the whole step 2 % slower
-// (profiles/r02_bench_train_splitk{0,1}.json).
+// leaves most CTAs idle, fp32 slabs added in a fixed order by the consumer.  Opt-in (SMD_FFN_SPLITK=1): the extra
+// reduce launch and the split GEMMs competing with the weight-gradient stream can cost more than the split saves
+// (not measured on H100).
 static constexpr int kFfnSplitMax = 4;
 static constexpr int kFfnSplitRows = 9728;   // largest token count that still splits (38 tiles x 2 <= 76)
 inline int ffn_splits(int M, int cta_group) {

@@ -123,7 +123,8 @@ static void build_workspace(smd_plan* p) {
   // per-row LayerNorm (sum, sumsq) of the 2K+1 wide LayerNorms, followed by the arrival counters of the LN-fused GEMM
   // epilogues (one u32 per 32 rows and fused launch); the whole region is zeroed once per forward
   ws_add(p, "stats", (2 * K + 1) * Mp * 2 * 4 + (2 * K + 2) * (Mp / 32) * 4);
-  ws_add(p, "lnf_part", Mp * (Md / 256 * 3) * 2 * 4);   // per-tile partial sums [row][n_tile * (2 or 3) + column group][2]
+  // per-tile partial sums [row][n_tile * (2 or 3) + column group][2]
+  ws_add(p, "lnf_part", Mp * ((Md + kBNMax - 1) / kBNMax * 3) * 2 * 4);
   // FiLM generator
   ws_add(p, "tvec", B * 4);
   ws_add(p, "enc", B * kFilmEmb * 4);
@@ -188,9 +189,9 @@ static int build_ops(smd_plan* p) {
       if (!fwd(&p->op_o[l], "o", pre + "attn.out.kernel", kE, kE, 128)) return SMD_ERR_CUDA;
       if (!fwd(&p->op_ffn1[l], "a", pre + "ffn1.kernel", kE, Md, 256)) return SMD_ERR_CUDA;
       if (!fwd(&p->op_ffn2[l], "hidden", pre + "ffn2.kernel", Md, kE, 128)) return SMD_ERR_CUDA;
-      if (cg == 2 && Md % 128 == 0 &&
+      if (Md % 128 == 0 &&
           !make_ffn_op(&p->op_ffn[l], A("a"), Mp, Wsh(pre + "ffn1.kernel"), Wsh(pre + "ffn2.kernel"), Md)) return SMD_ERR_CUDA;
-      if (cg == 2 && (c.num_heads == 8 || c.num_heads == 16) &&
+      if ((c.num_heads == 8 || c.num_heads == 16) &&
           !make_attn_op(&p->op_attn[l], A("a"), Mp, Wsh(pre + "attn.qkv.kernel"), Wsh(pre + "attn.out.kernel"))) return SMD_ERR_CUDA;
     }
     if (!fwd(&p->op_post, "a", "post.kernel", kE, Md, 256)) return SMD_ERR_CUDA;
@@ -293,10 +294,9 @@ int ensure_side_stream(smd_plan* p) {
   return SMD_OK;
 }
 
-// LN-fused GEMM epilogues (gemm_tcgen05.cuh, F_LNF): opt-in with SMD_LNF=1.  Measured on B200 (same box, A/B): the
-// fused tail is 4 launches shorter and moves ~40% fewer HBM bytes, but the two-pass epilogue costs 15-21 us per 256x256
-// tile on 8 warps against an 11.6 us mainloop, so the sampling step is 1.95 ms fused vs 1.89 ms with the stand-alone
-// ln_film_act kernels (which run at 98% of the HBM peak), the train step 1.66 vs 1.63 ms.  Default: off.
+// LN-fused GEMM epilogues (gemm_wgmma.cuh, F_LNF): opt-in with SMD_LNF=1.  The fused tail is 4
+// launches shorter and moves fewer HBM bytes, but its two-pass epilogue is long next to the mainloop and it runs with a
+// two-stage operand ring; whether it beats the stand-alone ln_film_act kernels on H100 is not measured.  Default: off.
 static bool lnf_enabled() {
   static const bool on = [] { const char* v = getenv("SMD_LNF"); return v && v[0] == '1'; }();
   return on;
@@ -304,8 +304,7 @@ static bool lnf_enabled() {
 // one FiLM (scale | shift) row per sample of 32 rows, or one row for everybody (sampler): the fused epilogue cannot
 // serve DenseDDPM's one-row-per-example case (a 32-row warp tile would span 32 FiLM rows)
 bool lnf_usable(const smd_plan* p, int S, int t_broadcast) {
-  // (cta_group 1 stages 48 KB per pipeline slot: no room for the 64 KB parking buffer next to >= 3 slots)
-  return lnf_enabled() && p->lo_bytes == 0 && p->cfg.cta_group == 2 && (S == 32 || t_broadcast || p->film_tab_on) &&
+  return lnf_enabled() && p->lo_bytes == 0 && (S == 32 || t_broadcast || p->film_tab_on) &&
          p->cfg.mlp_dims % 256 == 0;
 }
 // FiLM table / row selection of block k (shared by the fused epilogue and the stand-alone kernel)
@@ -389,8 +388,8 @@ static int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadc
                     smd::TrainState* save, bool fuse_tail, bool act0_ready) {
   if (fuse_tail) {
     if (!act0_ready) {
-      // first block's operand from the stand-alone kernel (the K = 128 post GEMM is epilogue-bound: fusing there costs
-      // more than the launch it saves -- measured 187 us against 27 + 61 us at 32000 tokens)
+      // first block's operand from the stand-alone kernel (the K = 128 post GEMM is epilogue-bound: the two-pass fused
+      // epilogue there is opt-in, SMD_LNF_POST=1)
       const float* scale; int bcast; const int* row_dev;
       film_source(p, 0, t_broadcast, &scale, &bcast, &row_dev);
       const LnStats ls = ln_stats(p, 0);
@@ -531,7 +530,7 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
         // QKV GEMM -> attention -> out-projection + residual + LayerNorm in ONE launch; q / k / v stay on chip
         // (training: they are also written out, with the probabilities and the attention output, for the backward pass)
         AttnOp ao = p->op_attn[l];
-        if (save && !make_tmap_bf16(&ao.tmA, a1, p->Mp, 128, 128)) return SMD_ERR_CUDA;
+        if (save && !make_attn_a(&ao.tmA, a1, p->Mp)) return SMD_ERR_CUDA;
         AttnBlockArgs aa;
         aa.qkv_out = save ? qkv : nullptr; aa.probs_out = save ? probs : nullptr; aa.o_out = save ? o : nullptr;
         aa.b_qkv = p->P(params, pre + "attn.qkv.bias"); aa.b_o = p->P(params, pre + "attn.out.bias");
@@ -554,8 +553,8 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
       SMD_CUDA(gemm(p, oo, M, e, st));
       }
       const std::string nl = (l + 1 < c.num_layers) ? ("l" + std::to_string(l + 1) + ".ln1.") : std::string("post_ln.");
-      // worth it once the token count fills the machine (one CTA pair per 256 tokens); training keeps the two-GEMM
-      // path: it has to write the hidden activations anyway and at batch 128 only 16 pairs would be busy
+      // worth it once the token count fills the machine; training keeps the two-GEMM path by default: it has to write
+      // the hidden activations anyway
       if (p->op_ffn[l].ok && p->lo_bytes == 0 && ffn_fused_enabled() && (ffn_fused_forced() || (!save && M >= 32 * 256))) {
         // FFN up + GELU + FFN down + residual + next LayerNorm in one launch; the hidden activation stays on chip
         FfnOp fo = p->op_ffn[l];
@@ -577,7 +576,7 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
       SMD_CUDA(gemm(p, o1, M, e, st));
       const int fsp = p->lo_bytes == 0 ? ffn_splits(M, c.cta_group) : 1;
       if (fsp > 1) {
-        // few tokens: a 256 x 128 output tile per CTA pair leaves most of the machine idle while each pair streams all
+        // few tokens: a 128 x 128 output tile per CTA leaves most of the machine idle while each CTA streams all
         // of K = mlp_dims.  Cut K into `fsp` slabs (fp32 partials, no atomics), then one small kernel adds them in a
         // fixed order with bias + residual and emits the next LayerNorm.
         float* slabs = p->buf<float>("ffn.slabs");

@@ -1,7 +1,7 @@
 """Training entry point with the reference's flag surface (train_ncsn.py:48-128), so configs/ddpm-*.cfg run
 unchanged:  python -m smd_b200.train_ncsn --flagfile=configs/ddpm-mel-32seq-512.cfg [--synthetic]
 
-Only the DDPM family is on the B200 hot path: --loss=ddpm, --sampling=ddpm, --architecture in
+Only the DDPM family is on the GPU hot path: --loss=ddpm, --sampling=ddpm, --architecture in
 {TransformerDDPM, TransformerDDPM4, DenseDDPM}.  Other values raise ValueError exactly where the reference would
 dispatch on them.  Data-parallel: launch with torchrun (one process per GPU); the batch is sharded across ranks
 and gradients are summed with one NCCL all-reduce over the flat arena (SURVEY section 8(e)).

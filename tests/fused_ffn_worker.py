@@ -1,7 +1,7 @@
 """Worker for tests/test_gpu_forward.py::test_fused_ffn_kernel.  Run with SMD_FFN_FUSED=2 so that the fused FFN kernel
-(csrc/ffn_fused.cuh) is used at every size and in training mode; checks it against the CPU oracle:
-  * small and ragged batches (partial 256-token tiles), inference;
-  * 600 samples = 75 tiles on 74 CTA pairs (a pair that runs two tiles exercises every barrier phase wrap);
+(csrc/fused_wgmma.cuh) is used at every size and in training mode; checks it against the CPU oracle:
+  * small and ragged batches (partial 128-token tiles), inference;
+  * 600 samples = 150 tiles on at most 132 CTAs (CTAs that run two tiles exercise every barrier phase wrap);
   * training mode: saved hidden activations feed the backward pass -> gradient parity with torch autograd."""
 import os
 import sys

@@ -1,6 +1,6 @@
 """Worker for tests/test_gpu_forward.py::test_ln_fused_epilogue.  Run with SMD_LNF=1 (and once more with
-SMD_LNF_POST=1) so the res-block GEMMs finish the next LayerNorm -> FiLM -> swish in their epilogue (csrc/gemm_tcgen05.cuh,
-F_LNF).  Checks against the CPU oracle: forward at small / ragged / multi-round sizes (75 row blocks on 72 CTA pairs:
+SMD_LNF_POST=1) so the res-block GEMMs finish the next LayerNorm -> FiLM -> swish in their epilogue (csrc/gemm_wgmma.cuh,
+F_LNF).  Checks against the CPU oracle: forward at small / ragged / multi-round sizes (150 row blocks on at most 132 CTAs:
 the inter-CTA statistics exchange crosses scheduling rounds), one reverse step through the graph + FiLM-table path,
 gradient parity in training mode (the fused kernels also write the pre-LayerNorm copy and the statistics totals), and
 that two runs are bit-identical."""

@@ -1,6 +1,6 @@
 """Worker for tests/test_gpu_train.py::test_opt_in_trunk_paths.  The switches are read once per process, so each variant
 runs in its own process:
-  SMD_ATTN_BLOCK_TRAIN=1  training forward through the attention block kernel (csrc/attn_block.cuh, kTrain: q | k | v,
+  SMD_ATTN_BLOCK_TRAIN=1  training forward through the attention block kernel (csrc/fused_wgmma.cuh: q | k | v,
                           probabilities and attention output written out for the backward pass);
   SMD_FFN_SPLITK=1        deterministic split-K (fp32 slabs) of the K = mlp_dims trunk GEMMs + ln128_reduce_fwd /
                           slab-summing ln128_bwd.

@@ -3,7 +3,7 @@
 Tolerances (stated): vs the bf16-operand-emulating oracle rel-L2 <= 1e-2 (kernel logic; only accumulation order,
 fast-exp and flipped bf16 roundings differ -- measured 2e-3 at 2 layers, 4e-3 at 6); vs the true fp32/fp64 oracle rel-L2
 <= 1.2e-2 and max-abs <= 6e-2 on eps_hat, |d loss| <= 5e-3 loss per example (bf16 tensor-core operands, fp32 accumulate --
-2x the values measured at the benchmarked sizes, profiles/r02_parity_measured.json; SURVEY section 7)."""
+about 2x the errors tests/test_gpu_bench_shapes.py records at the benchmarked sizes; SURVEY section 7)."""
 import os
 
 import numpy as np
@@ -103,7 +103,7 @@ def test_ddpm_loss_parity(lib):
 
 
 def test_fused_ffn_kernel(lib):
-    """The fused FFN kernel (csrc/ffn_fused.cuh) only engages on its own at >= 8192 tokens; SMD_FFN_FUSED=2 forces
+    """The fused FFN kernel (csrc/fused_wgmma.cuh) only engages on its own at >= 8192 tokens; SMD_FFN_FUSED=2 forces
     it everywhere (training included) in a worker process -- the switch is read once per process."""
     import subprocess
     import sys
@@ -116,7 +116,7 @@ def test_fused_ffn_kernel(lib):
 
 @pytest.mark.parametrize("post", ["0", "1"])
 def test_ln_fused_epilogue(lib, post):
-    """The LN-fused GEMM epilogue (csrc/gemm_tcgen05.cuh, F_LNF) is opt-in (SMD_LNF=1, read once per process): parity,
+    """The LN-fused GEMM epilogue (csrc/gemm_wgmma.cuh, F_LNF) is opt-in (SMD_LNF=1, read once per process): parity,
     bit-reproducibility and gradient checks run in a worker process; SMD_LNF_POST=1 also fuses the K = 128 post GEMM."""
     import subprocess
     import sys

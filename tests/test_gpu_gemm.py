@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (through the C ABI test hook) against a plain PyTorch fp32 reference of the same op on the same
+"""wgmma GEMM (through the C ABI test hook) against a plain PyTorch fp32 reference of the same op on the same
 bf16-rounded operands.  Tolerance: fp32 accumulation-order noise only (rel-L2 <= 2e-5, max-abs <= 2e-3*sqrt(K/64))."""
 import ctypes as C
 import math

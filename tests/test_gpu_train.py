@@ -2,8 +2,7 @@
 
 Tolerances (stated): per-tensor rel-L2 <= 3e-2 for tensors carrying >= 1e-4 of the gradient energy, global cosine
 >= 0.9995 and |norm ratio - 1| <= 1e-2 (bf16 tensor-core operands in both forward and backward GEMMs; at the benchmarked
-sizes the measured values are 9e-3 / 1 - 1e-4 / 1e-3, profiles/r02_parity_measured.json -- the small batches here are
-noisier per tensor)."""
+sizes tests/test_gpu_bench_shapes.py asserts tighter bounds -- the small batches here are noisier per tensor)."""
 import numpy as np
 import pytest
 import torch
@@ -220,9 +219,9 @@ def test_graph_replayed_step_equals_eager_launches(lib):
 @pytest.mark.gpu
 @pytest.mark.parametrize("switch", ["SMD_ATTN_BLOCK_TRAIN", "SMD_FFN_SPLITK"])
 def test_opt_in_trunk_paths(switch):
-    """Two opt-in trunk paths that measured slower than the default at batch 128 and therefore stay behind a switch
-    (read once per process -> worker): the attention-block kernel in the training forward, and the deterministic
-    split-K of the K = mlp_dims trunk GEMMs.  Forward and gradient parity against the oracle."""
+    """Two opt-in trunk paths behind a switch (read once per process -> worker): the attention-block kernel in the
+    training forward, and the deterministic split-K of the K = mlp_dims trunk GEMMs.  Forward and gradient parity
+    against the oracle."""
     import os
     import subprocess
     import sys

@@ -1,6 +1,6 @@
 """Independent cross-checks of the oracle's building blocks (CPU only).
 
-Upstream ships no golden vectors and cannot run here, so the oracle is "unpinned by the reference" (DESIGN.md section 2).
+Upstream ships no golden vectors and cannot run here, so the oracle is "unpinned by the reference".
 What CAN be done is to check every primitive it restates against an independent implementation of the same published
 algorithm: PyTorch's own LayerNorm / tanh-GELU / SiLU / MultiheadAttention / pre-LN TransformerEncoderLayer / Adam /
 clip_grad_norm_, and the closed-form DDPM posterior of Ho et al. 2020 (eqs. 6-7) in float64.  These are different code

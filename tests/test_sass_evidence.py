@@ -1,7 +1,6 @@
-"""The built library really contains the Blackwell instructions the design claims (CPU only: cuobjdump on libsmd.so):
-tcgen05.mma / commit / ld (UTCHMMA, UTCBAR, LDTM), TMA tensor loads (UTMALDG), mbarriers (SYNCS), packed fp32 pairs in
-the fused FFN epilogue (FFMA2 / FMUL2 / FADD2), mma.sync tf32 in the attention kernels (HMMA) and programmatic dependent
-launch (ACQBULK)."""
+"""The built library really contains the Hopper instructions the design claims (CPU only: cuobjdump on libsmd.so):
+wgmma (HGMMA) and TMA tensor loads (UTMALDG) with mbarriers (SYNCS) in the GEMM and in the fused FFN / attention-block
+kernels, mma.sync tf32 in the attention kernels (HMMA) and programmatic dependent launch (ACQBULK)."""
 import os
 import shutil
 import subprocess
@@ -43,22 +42,24 @@ def _get(table, prefix):
     return hits
 
 
-def test_gemm_family_uses_tcgen05_tma_and_mbarriers(table):
-    for c in _get(table, "gemm_bf16_tcgen05_kernel<"):
-        assert c.get("UTCHMMA", 0) > 0 and c.get("UTMALDG", 0) > 0 and c.get("LDTM", 0) > 0
-        assert c.get("UTCBAR", 0) > 0 and c.get("SYNCS", 0) > 0 and c.get("ACQBULK", 0) > 0
+def test_gemm_family_uses_wgmma_tma_and_mbarriers(table):
+    for c in _get(table, "gemm_bf16_wgmma_kernel<"):
+        assert c.get("HGMMA", 0) > 0 and c.get("UTMALDG", 0) > 0
+        assert c.get("SYNCS", 0) > 0 and c.get("ACQBULK", 0) > 0
         assert c.get("HMMA", 0) == 0                      # no legacy mma.sync in the GEMM path
 
 
-def test_fused_ffn_uses_packed_fp32_and_tcgen05(table):
+def test_fused_ffn_uses_wgmma_and_tma(table):
     for c in _get(table, "ffn_fused_kernel<"):
-        assert c.get("UTCHMMA", 0) > 0 and c.get("UTMALDG", 0) > 0 and c.get("LDTM", 0) > 0
-        assert c.get("FFMA2", 0) > 0 and c.get("FMUL2", 0) > 0 and c.get("FADD2", 0) > 0
+        assert c.get("HGMMA", 0) > 0 and c.get("UTMALDG", 0) > 0 and c.get("SYNCS", 0) > 0
         assert c.get("MUFU.TANH", 0) >= 64                # 64 columns of tanh-GELU per thread and chunk
 
 
-def test_attention_block_combines_tcgen05_gemms_with_an_mma_sync_core(table):
+def test_attention_block_uses_wgmma_gemms(table):
     for c in _get(table, "attn_block_kernel<"):
-        assert c.get("UTCHMMA", 0) > 0 and c.get("UTMALDG", 0) > 0 and c.get("LDTM", 0) > 0 and c.get("HMMA", 0) > 0
+        assert c.get("HGMMA", 0) > 0 and c.get("UTMALDG", 0) > 0 and c.get("SYNCS", 0) > 0
+
+
+def test_attention_kernels_use_an_mma_sync_core(table):
     for c in _get(table, "attention_mma_kernel<") + _get(table, "attention_bwd_mma_kernel<"):
         assert c.get("HMMA", 0) > 0
