@@ -90,7 +90,9 @@ struct GemmShape {
 static constexpr int kBM = 128;
 static constexpr int kBK = 64;
 static constexpr int kBNMax = 128;                 // widest n-tile: one m64n128 wgmma per consumer warpgroup
-static constexpr int kAccPitch = kBNMax + 4;       // floats per staged accumulator row (conflict-free 16-byte row reads)
+// floats per staged accumulator row: unpadded, the 16-byte chunks of each row are XOR-swizzled instead (acc_chunk), which
+// leaves room in shared memory for a fourth operand stage in the 8-epilogue-warp kinds
+static constexpr int kAccPitch = kBNMax;
 
 // kEW = number of epilogue warps (8: two per 32-row quadrant; 12: three, for epilogue-bound small-K GEMMs).  The first
 // eight of them are the two wgmma warpgroups.  The pipeline depth is whatever fits next to the accumulator staging tile
@@ -103,7 +105,7 @@ struct GemmSmem {
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kBarBytes = 256;
   static constexpr int kEpiWarps = kEW;
-  static constexpr int kAccBytes = kBM * kAccPitch * 4;                    // 66 KB fp32 accumulator tile
+  static constexpr int kAccBytes = kBM * kAccPitch * 4;                    // 64 KB fp32 accumulator tile
   static constexpr int kScrPerWarp = kScrFloats;                           // floats of scratch per epilogue warp
   static constexpr int kScratchBytes = kEpiWarps * kScrFloats * 4;         // per-epilogue-warp transpose scratch
   static constexpr int kParkBytes = kPark ? kBM * kBNMax * 2 : 0;          // 32 KB
@@ -112,6 +114,8 @@ struct GemmSmem {
   static constexpr int kTotal = kStages * kStageBytes + kBarBytes + kAccBytes + kScratchBytes + kParkBytes + 1024;
   static constexpr int kThreads = 128 + 32 * kEpiWarps;
 };
+// the 8-epilogue-warp kinds (every res-block GEMM of the train step) keep four 32 KB stages in flight
+static_assert(GemmSmem<8>::kStages == 4, "the 8-warp GEMM ring should hold four stages");
 static constexpr bool lnf_kind(uint32_t kF) { return (kF & F_LNF) != 0 && (kF & F_RAGGED) == 0; }
 // LN-fused kinds without residual / fp32 output need no 32x33 transpose tile, only the staged coefficients
 static constexpr int scr_floats(uint32_t kF) {
@@ -202,28 +206,33 @@ __device__ __forceinline__ uint64_t gelu_tanh_x2(uint64_t v) {
   return f32x2_fma(h, f32x2_pack(tanh_fast(u0), tanh_fast(u1)), h);
 }
 
-// the staged accumulator row of this thread: 32 / 16 consecutive columns (16-byte shared accesses)
-__device__ __forceinline__ void acc_ld32(const float* p, uint32_t (&r)[32]) {
+// Staged accumulator tile [128][kAccPitch]: 16-byte chunk q of row r sits at chunk q ^ (r & 7) of the row, so that
+// 16-byte row reads with one row per lane, and the wgmma fragment stores, are free of bank conflicts without padding.
+__device__ __forceinline__ int acc_chunk(int q, int sw) { return q ^ sw; }
+// the staged accumulator row `p` (row & 7 == sw) of this thread: 32 / 16 consecutive columns from column c0 (a multiple
+// of 16), 16-byte shared accesses
+__device__ __forceinline__ void acc_ld32(const float* p, int c0, int sw, uint32_t (&r)[32]) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    const float4 t = reinterpret_cast<const float4*>(p)[i];
+    const float4 t = reinterpret_cast<const float4*>(p)[acc_chunk((c0 >> 2) + i, sw)];
     r[4 * i] = __float_as_uint(t.x); r[4 * i + 1] = __float_as_uint(t.y);
     r[4 * i + 2] = __float_as_uint(t.z); r[4 * i + 3] = __float_as_uint(t.w);
   }
 }
-__device__ __forceinline__ void acc_ld16(const float* p, uint32_t (&r)[16]) {
+__device__ __forceinline__ void acc_ld16(const float* p, int c0, int sw, uint32_t (&r)[16]) {
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    const float4 t = reinterpret_cast<const float4*>(p)[i];
+    const float4 t = reinterpret_cast<const float4*>(p)[acc_chunk((c0 >> 2) + i, sw)];
     r[4 * i] = __float_as_uint(t.x); r[4 * i + 1] = __float_as_uint(t.y);
     r[4 * i + 2] = __float_as_uint(t.z); r[4 * i + 3] = __float_as_uint(t.w);
   }
 }
-__device__ __forceinline__ void acc_st32(float* p, const uint32_t (&r)[32]) {
+__device__ __forceinline__ void acc_st32(float* p, int c0, int sw, const uint32_t (&r)[32]) {
 #pragma unroll
   for (int i = 0; i < 8; ++i)
-    reinterpret_cast<float4*>(p)[i] = make_float4(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]),
-                                                  __uint_as_float(r[4 * i + 2]), __uint_as_float(r[4 * i + 3]));
+    reinterpret_cast<float4*>(p)[acc_chunk((c0 >> 2) + i, sw)] =
+        make_float4(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]), __uint_as_float(r[4 * i + 2]),
+                    __uint_as_float(r[4 * i + 3]));
 }
 
 // the K loop of one warpgroup: rows [64 wg, 64 wg + 64) of the tile, all kBNMax columns
@@ -360,7 +369,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 #pragma unroll
         for (int i = 0; i < 64; i += 2) {
           const int rr = r0 + 8 * ((i >> 1) & 1), cc = 8 * (i >> 2) + c;
-          *reinterpret_cast<float2*>(acc_tile + rr * kAccPitch + cc) = make_float2(d[i], d[i + 1]);
+          *reinterpret_cast<float2*>(acc_tile + rr * kAccPitch + acc_chunk(cc >> 2, rr & 7) * 4 + (cc & 3)) =
+              make_float2(d[i], d[i + 1]);
         }
       }
       epi_bar();
@@ -373,6 +383,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     constexpr bool H_STRICT = (kF & F_STRICT) != 0;
     const long long lo_delta = H_STRICT ? ep.lo_delta : 0;
     const uint32_t q = warp & 3u;                      // 32-row quadrant of the tile this warp owns
+    const int asw = static_cast<int>(lane & 7u);       // swizzle of this thread's staged row (q * 32 + lane)
     const int eg = static_cast<int>(warp - 4u) >> 2;   // column group 0/1: the two warps of a quadrant split the chunks
     float* scr = reinterpret_cast<float*>(epi_smem) + (warp - 4u) * SM::kScrPerWarp;
     uint32_t* scrw = reinterpret_cast<uint32_t*>(scr);
@@ -452,7 +463,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         for (int c0 = eg * 32; c0 < BN; c0 += 32 * G) {
           __syncwarp();
           uint32_t r[32];
-          acc_ld32(arow + c0, r);
+          acc_ld32(arow, c0, asw, r);
           const int col0 = n0 + c0;
           float4 bq[8];
           if (has_bias) {
@@ -513,7 +524,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                 f32x2_unpack(v2[i], a, b);
                 r[2 * i] = __float_as_uint(a); r[2 * i + 1] = __float_as_uint(b);
               }
-              acc_st32(arow + c0, r);
+              acc_st32(arow, c0, asw, r);
             }
           }
         }
@@ -536,7 +547,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
             for (int c0 = eg * 32; c0 < BN; c0 += 32 * G) {
               __syncwarp();
               uint32_t r[32];
-              acc_ld32(arow + c0, r);
+              acc_ld32(arow, c0, asw, r);
 #pragma unroll
               for (int i = 0; i < 8; ++i)
                 *tsw(static_cast<int>(lane), i) = make_float4(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]),
@@ -701,7 +712,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
             const int c0 = eg * 32 + 64 * j;
             __syncwarp();
             uint32_t r[32];
-            acc_ld32(arow + c0, r);
+            acc_ld32(arow, c0, asw, r);
 #pragma unroll
             for (int i = 0; i < 32; ++i) vv[j][i] = __uint_as_float(r[i]);
             if (has_bias) {
@@ -849,10 +860,10 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           bool half = false;
           if constexpr (H_RAGGED) half = (BN - c0) < 32;  // 16-column tail
           if (!half) {
-            acc_ld32(arow + c0, r);
+            acc_ld32(arow, c0, asw, r);
           } else {
             uint32_t r16[16];
-            acc_ld16(arow + c0, r16);
+            acc_ld16(arow, c0, asw, r16);
 #pragma unroll
             for (int i = 0; i < 16; ++i) { r[i] = r16[i]; r[16 + i] = 0u; }
           }
