@@ -1,5 +1,6 @@
 """Per-kernel SASS mnemonic counts of libsmd.so (cuobjdump -sass): the evidence that the hot kernels use wgmma (HGMMA),
-TMA (UTMALDG), mbarriers (SYNCS), mma.sync (HMMA) and programmatic dependent launch.
+TMA (UTMALDG), mbarriers (SYNCS), mma.sync (HMMA), programmatic dependent launch and per-warpgroup register budgets
+(USETMAXREG), and which of them touch local memory (STL / LDL: register spills).
 Usage: python scripts/sass_mnemonics.py"""
 import collections
 import os
@@ -9,7 +10,8 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "symbolic-music-diffusion_b200", "libsmd.so")
-KEYS = ["HGMMA", "UTMALDG", "UTMASTG", "SYNCS", "HMMA", "MUFU.TANH", "LDGSTS", "UBLKCP", "ACQBULK", "RED", "ATOM"]
+KEYS = ["HGMMA", "UTMALDG", "UTMASTG", "SYNCS", "HMMA", "MUFU.TANH", "LDGSTS", "UBLKCP", "ACQBULK", "RED", "ATOM",
+        "USETMAXREG", "STL", "LDL"]
 
 
 def main():
@@ -41,7 +43,7 @@ def main():
         names[mangled] = d
     print("# SASS mnemonics per kernel (cuobjdump -sass libsmd.so, sm_90a): wgmma = HGMMA;")
     print("# TMA = UTMALDG; mbarrier = SYNCS; mma.sync = HMMA;")
-    print("# cp.async = LDGSTS; programmatic dependent launch = ACQBULK")
+    print("# cp.async = LDGSTS; programmatic dependent launch = ACQBULK; setmaxnreg = USETMAXREG; spills = STL / LDL")
     seen = set()
     for mangled in sorted(counts, key=lambda k: names[k]):
         n = names[mangled]

@@ -121,19 +121,32 @@ inline bool epi_clean(const GemmOp& op, const GemmEpilogue& e) {
          (!e.bias || a16(e.bias)) && (!e.ln_gamma || (a16(e.ln_gamma) && a16(e.ln_beta)));
 }
 
-// Number of epilogue warps of the instantiation launch_gemm will pick (mirrors launch_gemm_cg): the per-tile statistics
-// partials (GemmEpilogue::stats_part) have (epi warps / 4) slots per n-tile.
-inline int epi_warps_for(const GemmOp& op, const GemmEpilogue& ep) {
-  if (ep.lnf_part != nullptr || ep.lo_delta != 0 || !epi_clean(op, ep)) return 8;
+// Column groups per tile (GemmSmem::kEpiGroups) of the instantiation launch_gemm will pick: the per-tile statistics
+// partials (GemmEpilogue::stats_part) have that many slots per n-tile.  3 for the short-K 12-warp kinds, 2 for every
+// other kind, in the 8-warp and the dedicated-epilogue layouts alike.
+inline int epi_groups_for(const GemmOp& op, const GemmEpilogue& ep) {
+  if (ep.lnf_part != nullptr || ep.lo_delta != 0 || !epi_clean(op, ep)) return 2;
   const uint32_t need = epi_needs(ep);
   const bool short_k = op.K <= 256;
-  if ((need & ~kEpiF32) == 0) return short_k ? 12 : 8;
-  if ((need & ~kEpiAtomic) == 0 || (need & ~kEpiF32Res) == 0) return 8;
-  if ((need & ~kEpiAct) == 0) return short_k ? 12 : 8;
-  return 8;
+  if ((need & ~kEpiF32) == 0) return short_k ? 3 : 2;
+  if ((need & ~kEpiAtomic) == 0 || (need & ~kEpiF32Res) == 0) return 2;
+  if ((need & ~kEpiAct) == 0) return short_k ? 3 : 2;
+  return 2;
 }
 inline int stats_slots_for(const GemmOp& op, const GemmEpilogue& ep) {
-  return ((op.N + op.BN - 1) / op.BN) * (epi_warps_for(op, ep) / 4);
+  return ((op.N + op.BN - 1) / op.BN) * epi_groups_for(op, ep);
+}
+
+// the K-split count every split of which owns at least one 64-wide k block
+inline int gemm_k_splits(const GemmOp& op) {
+  const int num_kb = op.K / kBK;
+  int splits = op.k_splits < 1 ? 1 : op.k_splits;
+  if (splits > num_kb) splits = num_kb;
+  const int per = (num_kb + splits - 1) / splits;
+  return (num_kb + per - 1) / per;
+}
+inline int gemm_tiles(const GemmOp& op, int M) {
+  return ((M + kBM - 1) / kBM) * ((op.N + op.BN - 1) / op.BN) * gemm_k_splits(op);
 }
 
 template <uint32_t kF, int kEW = 8>
@@ -148,15 +161,8 @@ inline cudaError_t launch_gemm_inst(const GemmOp& op, int M, const GemmEpilogue&
   }
   GemmShape sh;
   sh.M = M; sh.N = op.N; sh.K = op.K; sh.BN = op.BN; sh.a_mn = op.a_mn; sh.b_mn = op.b_mn;
-  // normalise the split count so that every split owns at least one 64-wide k block
-  const int num_kb = op.K / kBK;
-  int splits = op.k_splits < 1 ? 1 : op.k_splits;
-  if (splits > num_kb) splits = num_kb;
-  const int per = (num_kb + splits - 1) / splits;
-  splits = (num_kb + per - 1) / per;
-  sh.k_splits = splits;
-  const int rows_per_tile = kBM;
-  const int tiles = ((M + rows_per_tile - 1) / rows_per_tile) * ((op.N + op.BN - 1) / op.BN) * splits;
+  sh.k_splits = gemm_k_splits(op);
+  const int tiles = gemm_tiles(op, M);
   int groups = device_sm_count();
   if (tiles < groups) groups = tiles;
   if constexpr ((kF & F_LNF) != 0 && (kF & F_RAGGED) == 0) {
@@ -198,10 +204,19 @@ inline cudaError_t launch_gemm(const GemmOp& op, int M, const GemmEpilogue& ep, 
     auto fits = [&](uint32_t kind) { return (need & ~kind) == 0; };
     // short-K GEMMs are epilogue-bound: give them a third epilogue warp per row quadrant
     const bool short_k = op.K <= 256;
-    if (fits(kEpiF32)) return short_k ? launch_gemm_inst<kEpiF32, 12>(op, M, ep, st) : launch_gemm_inst<kEpiF32>(op, M, ep, st);
+    // long-K launches of several rounds: a dedicated epilogue warpgroup hides each tile's epilogue behind the next
+    // tile's K loop.  A single round has no next tile to overlap with; its exposed epilogue keeps the 8-warp layout,
+    // which runs it on twice as many warps.
+    const bool overlap = !short_k && gemm_tiles(op, M) > device_sm_count();
+    if (fits(kEpiF32))
+      return short_k ? launch_gemm_inst<kEpiF32, 12>(op, M, ep, st)
+                     : overlap ? launch_gemm_inst<kEpiF32, 4>(op, M, ep, st) : launch_gemm_inst<kEpiF32>(op, M, ep, st);
     if (fits(kEpiAtomic)) return launch_gemm_inst<kEpiAtomic>(op, M, ep, st);
-    if (fits(kEpiF32Res)) return launch_gemm_inst<kEpiF32Res>(op, M, ep, st);
-    if (fits(kEpiAct)) return short_k ? launch_gemm_inst<kEpiAct, 12>(op, M, ep, st) : launch_gemm_inst<kEpiAct>(op, M, ep, st);
+    if (fits(kEpiF32Res))
+      return overlap ? launch_gemm_inst<kEpiF32Res, 4>(op, M, ep, st) : launch_gemm_inst<kEpiF32Res>(op, M, ep, st);
+    if (fits(kEpiAct))
+      return short_k ? launch_gemm_inst<kEpiAct, 12>(op, M, ep, st)
+                     : overlap ? launch_gemm_inst<kEpiAct, 4>(op, M, ep, st) : launch_gemm_inst<kEpiAct>(op, M, ep, st);
     if (fits(kEpiGG)) return launch_gemm_inst<kEpiGG>(op, M, ep, st);
     if ((need & F_LN) && fits(kEpiLn) && op.N == op.BN && op.BN <= 128 && op.BN % 64 == 0 && op.k_splits <= 1)
       return launch_gemm_inst<kEpiLn>(op, M, ep, st);

@@ -5,8 +5,17 @@
 //
 //   D[M,N] = A[M,K] * B[N,K]^T     (both operands may independently be K-major or MN-major in global memory)
 //
-// One CTA per 128 x BN tile (BN <= 128).  The epilogue warps are also the MMA warps: while they run the epilogue of
-// tile i, the TMA warp already streams the operands of tile i + 1 into the ring.
+// One CTA per 128 x BN tile (BN <= 128).  Two thread layouts (kEW below):
+//   * dedicated epilogue (kEW = 4, 512 threads): warpgroup 0 is the TMA producer, warpgroups 1 and 2 only run the K
+//     loops and store their accumulators to `acc_tile`, warpgroup 3 runs the epilogue.  The accumulator hand-off goes
+//     through two mbarriers (acc_full / acc_empty), so the MMA warps start tile i + 1 while the epilogue warps still
+//     work on tile i: the tensor cores do not wait for the epilogue's HBM traffic.  setmaxnreg moves registers from
+//     the producer and MMA warpgroups to the epilogue warpgroup.  Used for the long-K fp32 / bf16 kinds of launches
+//     with more tiles than CTAs;
+//   * shared (kEW = 8 or 12): the two wgmma warpgroups are also epilogue warps (plus a third, epilogue-only warpgroup
+//     for kEW = 12).  While they run the epilogue of tile i, the TMA warp already streams the operands of tile i + 1
+//     into the ring, but no MMA runs.  Single-round launches gain nothing from the overlap and keep the wider
+//     epilogue; so do the short-K, LayerNorm-fused, generic and strict kinds.
 //
 // This is the kernel behind every Dense layer on the hot path (reference: flax.nn.Dense call sites
 // models/ncsn.py:155-178, models/shared.py:65,69).
@@ -53,9 +62,10 @@ struct GemmEpilogue {
   int ld_bf16;
   int act;                      // activation applied on the bf16 output path
   float* row_stats;             // [M][2] += (sum v, sum v^2) over this tile's columns (atomics), or null
-  float* stats_part;            // if set (with row_stats): instead of atomics every (n-tile, column-group) warp stores its
-                                // partial to stats_part[(row * nslots + n_tile * (epi_warps / 4) + group) * 2]; the
-                                // consumer (ln_film_act) adds the slots in a fixed order: bit-reproducible statistics
+  float* stats_part;            // if set (with row_stats): instead of atomics every (n-tile, column-group) pair stores its
+                                // partial to stats_part[(row * nslots + n_tile * groups + group) * 2], groups =
+                                // GemmSmem::kEpiGroups; the consumer (ln_film_act) adds the slots in a fixed order:
+                                // bit-reproducible statistics
   const float* ln_gamma;        // full-row LayerNorm (requires N <= BN, a single n-tile): bf16 out = LN(v)*g+b
   const float* ln_beta;
   __nv_bfloat16* out_bf16_pre;  // bf16 [M][ld_bf16] <- v before the activation (training saves), or null
@@ -94,9 +104,14 @@ static constexpr int kBNMax = 128;                 // widest n-tile: one m64n128
 // leaves room in shared memory for a fourth operand stage in the 8-epilogue-warp kinds
 static constexpr int kAccPitch = kBNMax;
 
-// kEW = number of epilogue warps (8: two per 32-row quadrant; 12: three, for epilogue-bound small-K GEMMs).  The first
-// eight of them are the two wgmma warpgroups.  The pipeline depth is whatever fits next to the accumulator staging tile
-// and the epilogue scratch in the 227 KB of shared memory.
+// kEW = number of epilogue warps.  8: two per 32-row quadrant; 12: three, for epilogue-bound small-K GEMMs.  The first
+// eight of them are the two wgmma warpgroups.  4: the dedicated-epilogue layout, one warp per quadrant in a warpgroup
+// of its own, after the two wgmma warpgroups.
+// Each tile's columns are split into kEpiGroups column groups (group g owns the 32-column chunks g, g + kEpiGroups,
+// ...): one per warp of a quadrant in the shared layouts; a dedicated epilogue warp runs both groups of its quadrant
+// one after the other, so its arithmetic and its statistics slots are those of the 8-warp layout.
+// The pipeline depth is whatever fits next to the accumulator staging tile and the epilogue scratch in the 227 KB of
+// shared memory.
 // kPark: the LN-fused epilogue (F_LNF) parks the tile as bf16 [128][128] in shared memory between its two passes.
 template <int kEW = 8, bool kPark = false, int kScrFloats = 32 * 33>
 struct GemmSmem {
@@ -105,6 +120,8 @@ struct GemmSmem {
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kBarBytes = 256;
   static constexpr int kEpiWarps = kEW;
+  static constexpr bool kDedicated = kEW == 4;
+  static constexpr int kEpiGroups = kDedicated ? 2 : kEW / 4;
   static constexpr int kAccBytes = kBM * kAccPitch * 4;                    // 64 KB fp32 accumulator tile
   static constexpr int kScrPerWarp = kScrFloats;                           // floats of scratch per epilogue warp
   static constexpr int kScratchBytes = kEpiWarps * kScrFloats * 4;         // per-epilogue-warp transpose scratch
@@ -112,10 +129,16 @@ struct GemmSmem {
   static constexpr int kMaxSmem = 232448;                                  // 227 KB
   static constexpr int kStages = (kMaxSmem - 1024 - kBarBytes - kAccBytes - kScratchBytes - kParkBytes) / kStageBytes;
   static constexpr int kTotal = kStages * kStageBytes + kBarBytes + kAccBytes + kScratchBytes + kParkBytes + 1024;
-  static constexpr int kThreads = 128 + 32 * kEpiWarps;
+  static constexpr int kThreads = kDedicated ? 512 : 128 + 32 * kEpiWarps;
+  // dedicated layout: per-thread register budgets of the producer, MMA and epilogue warpgroups (setmaxnreg).  The CTA
+  // starts with 128 per thread (512 threads, one CTA per SM), so the four warpgroups' budgets may add up to 4 x 128.
+  static constexpr int kProdRegs = 40, kMmaRegs = 120, kEpiRegs = 232;
+  static_assert(!kDedicated || kProdRegs + 2 * kMmaRegs + kEpiRegs <= 512, "register budgets exceed the CTA's file");
 };
-// the 8-epilogue-warp kinds (every res-block GEMM of the train step) keep four 32 KB stages in flight
+// the 8-epilogue-warp and dedicated-epilogue kinds (every res-block GEMM of the train step) keep four 32 KB stages in
+// flight
 static_assert(GemmSmem<8>::kStages == 4, "the 8-warp GEMM ring should hold four stages");
+static_assert(GemmSmem<4>::kStages == 4, "the dedicated-epilogue GEMM ring should hold four stages");
 static constexpr bool lnf_kind(uint32_t kF) { return (kF & F_LNF) != 0 && (kF & F_RAGGED) == 0; }
 // LN-fused kinds without residual / fp32 output need no 32x33 transpose tile, only the staged coefficients
 static constexpr int scr_floats(uint32_t kF) {
@@ -264,13 +287,18 @@ __device__ __forceinline__ void gemm_mainloop(float (&d)[64], uint8_t* smem, int
 }
 
 template <uint32_t kF, int kEW = 8>
-__global__ void __launch_bounds__(128 + 32 * kEW, 1)
+__global__ void __launch_bounds__(GemmSmem<kEW>::kThreads, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                        const GemmShape sh, const GemmEpilogue ep) {
   using SM = GemmSmem<kEW, lnf_kind(kF), scr_floats(kF)>;
+  constexpr bool kDedicated = SM::kDedicated;
+  constexpr int kGroups = SM::kEpiGroups;
   // (the LN-fused kinds also hold a 32 KB parking buffer: two stages, each TMA load still overlaps one k block of MMAs)
   static_assert(SM::kStages >= (lnf_kind(kF) ? 2 : 3), "pipeline too shallow");
   static_assert(!((kF & F_LN) && !(kF & F_RAGGED)) || kEW == 8, "the paired LayerNorm epilogue needs 8 epilogue warps");
+  static_assert(!kDedicated || (kF & (F_LN | F_LNF | F_RAGGED | F_STRICT)) == 0,
+                "the dedicated-epilogue layout runs the non-LayerNorm fast-path epilogue only");
+  static_assert(2 * SM::kStages + 2 <= SM::kBarBytes / 8, "mbarriers do not fit their region");
   extern __shared__ uint8_t smem_raw[];
   // 1 KiB alignment by OFFSET from the __shared__ symbol (not by integer-casting the pointer): the compiler keeps the
   // shared address space, so the epilogue's staging accesses are LDS/STS instead of generic LD/ST.
@@ -278,6 +306,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM::kStages * SM::kStageBytes);
   uint64_t* full_bar = bars;                         // [kStages]
   uint64_t* empty_bar = bars + SM::kStages;          // [kStages]
+  uint64_t* acc_full = bars + 2 * SM::kStages;       // dedicated layout: acc_tile holds a finished tile
+  uint64_t* acc_empty = acc_full + 1;                // dedicated layout: the epilogue is done reading acc_tile
   float* acc_tile = reinterpret_cast<float*>(smem + SM::kStages * SM::kStageBytes + SM::kBarBytes);   // [128][kAccPitch]
   uint8_t* epi_smem = smem + SM::kStages * SM::kStageBytes + SM::kBarBytes + SM::kAccBytes;         // scratch | park
 
@@ -306,6 +336,10 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);   // one arrival per MMA warp
     }
+    if (kDedicated) {
+      mbar_init(acc_full, 256);      // every MMA thread, after its fragment stores
+      mbar_init(acc_empty, 128);     // every epilogue thread, after its last read of the tile
+    }
     fence_barrier_init();
   }
   __syncthreads();
@@ -313,9 +347,35 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   // it overlaps the tail of the previous kernel.  From here on operands are read.
   pdl_wait();
 
-  if (warp == 0) {
-    // ===================== TMA producer (one lane) =====================
-    if (elect_one()) {
+  const uint32_t wg = (warp - 4u) >> 2;          // consumer warpgroup (0, 1: MMA; 2: epilogue only)
+  int mma_stage = 0; uint32_t mma_phase = 0;
+  // the K loop of one tile: this warpgroup's 64 rows, all kBNMax columns, into d
+  auto mainloop = [&](int tile, float (&d)[64]) {
+    const int split = tile % splits;
+    const int kb0 = split * kb_per, kb1 = min(num_kb_total, kb0 + kb_per);
+    const int nkb = kb1 - kb0;
+    const bool rel = lane == 0;
+    if (!sh.a_mn && !sh.b_mn) gemm_mainloop<0, 0>(d, smem, SM::kStageBytes, SM::kABytes, SM::kStages, full_bar, empty_bar, mma_stage, mma_phase, nkb, wg, rel);
+    else if (!sh.a_mn) gemm_mainloop<0, 1>(d, smem, SM::kStageBytes, SM::kABytes, SM::kStages, full_bar, empty_bar, mma_stage, mma_phase, nkb, wg, rel);
+    else if (!sh.b_mn) gemm_mainloop<1, 0>(d, smem, SM::kStageBytes, SM::kABytes, SM::kStages, full_bar, empty_bar, mma_stage, mma_phase, nkb, wg, rel);
+    else gemm_mainloop<1, 1>(d, smem, SM::kStageBytes, SM::kABytes, SM::kStages, full_bar, empty_bar, mma_stage, mma_phase, nkb, wg, rel);
+  };
+  // the warpgroup's accumulator fragments -> acc_tile
+  auto stage_acc = [&](const float (&d)[64]) {
+    const int r0 = static_cast<int>(wg * 64u + ((warp - 4u) & 3u) * 16u + (lane >> 2));
+    const int c = 2 * static_cast<int>(lane & 3u);
+#pragma unroll
+    for (int i = 0; i < 64; i += 2) {
+      const int rr = r0 + 8 * ((i >> 1) & 1), cc = 8 * (i >> 2) + c;
+      *reinterpret_cast<float2*>(acc_tile + rr * kAccPitch + acc_chunk(cc >> 2, rr & 7) * 4 + (cc & 3)) =
+          make_float2(d[i], d[i + 1]);
+    }
+  };
+
+  if (warp < 4) {
+    // ===================== TMA producer (one lane of warp 0) =====================
+    if constexpr (kDedicated) setmaxnreg_dec<SM::kProdRegs>();
+    if (warp == 0 && elect_one()) {
       int stage = 0; uint32_t phase = 0;
       const uint32_t stage_tx = static_cast<uint32_t>((kBM + b_rows) * kBK * 2);
       for (int tile = group; tile < num_tiles; tile += num_groups) {
@@ -339,40 +399,35 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         }
       }
     }
-  } else if (warp >= 4) {
-    // ===================== MMA + epilogue warps =====================
-    // Per tile: the two wgmma warpgroups (epilogue warps 0-7) run the K loop, every epilogue warp waits until the
-    // previous tile's staged accumulators have been consumed, the warpgroups store theirs to `acc_tile`, and then each
-    // warp reads its 32 rows back one row per thread, exactly like the epilogue expects: every global tile access goes
-    // through a per-warp 32x33 shared-memory scratch and is issued as whole 128-byte (fp32) / 64-byte (bf16) row
-    // segments.
-    const uint32_t wg = (warp - 4u) >> 2;          // consumer warpgroup (0, 1: MMA; 2: epilogue only)
-    int mma_stage = 0; uint32_t mma_phase = 0;
+  } else if (kDedicated && wg < 2) {
+    // ===================== dedicated layout: MMA warps =====================
+    // Tile i's accumulators go to acc_tile as soon as the epilogue has released tile i - 1, then tile i + 1's K loop
+    // starts while the epilogue warpgroup works on tile i.
+    setmaxnreg_dec<SM::kMmaRegs>();
+    uint32_t acc_phase = 0;
+    for (int tile = group; tile < num_tiles; tile += num_groups) {
+      float d[64];
+      mainloop(tile, d);
+      mbar_wait(acc_empty, acc_phase ^ 1u);
+      stage_acc(d);
+      mbar_arrive(acc_full);
+      acc_phase ^= 1u;
+    }
+  } else {
+    // ===================== epilogue warps (and, in the shared layouts, MMA warps) =====================
+    // Per tile in the shared layouts: the two wgmma warpgroups (epilogue warps 0-7) run the K loop, every epilogue
+    // warp waits until the previous tile's staged accumulators have been consumed, the warpgroups store theirs to
+    // `acc_tile`.  In the dedicated layout the epilogue warps wait on acc_full instead.  Then each warp reads its 32
+    // rows back one row per thread, exactly like the epilogue expects: every global tile access goes through a
+    // per-warp 32x33 shared-memory scratch and is issued as whole 128-byte (fp32) / 64-byte (bf16) row segments.
+    if constexpr (kDedicated) setmaxnreg_inc<SM::kEpiRegs>();
     auto epi_bar = [] { asm volatile("bar.sync 5, %0;" ::"n"(32 * kEW) : "memory"); };
     auto mma_tile = [&](int tile) {
       float d[64];
       const bool mma_warp = wg < 2;
-      if (mma_warp) {
-        const int split = tile % splits;
-        const int kb0 = split * kb_per, kb1 = min(num_kb_total, kb0 + kb_per);
-        const int nkb = kb1 - kb0;
-        const bool rel = lane == 0;
-        if (!sh.a_mn && !sh.b_mn) gemm_mainloop<0, 0>(d, smem, SM::kStageBytes, SM::kABytes, SM::kStages, full_bar, empty_bar, mma_stage, mma_phase, nkb, wg, rel);
-        else if (!sh.a_mn) gemm_mainloop<0, 1>(d, smem, SM::kStageBytes, SM::kABytes, SM::kStages, full_bar, empty_bar, mma_stage, mma_phase, nkb, wg, rel);
-        else if (!sh.b_mn) gemm_mainloop<1, 0>(d, smem, SM::kStageBytes, SM::kABytes, SM::kStages, full_bar, empty_bar, mma_stage, mma_phase, nkb, wg, rel);
-        else gemm_mainloop<1, 1>(d, smem, SM::kStageBytes, SM::kABytes, SM::kStages, full_bar, empty_bar, mma_stage, mma_phase, nkb, wg, rel);
-      }
+      if (mma_warp) mainloop(tile, d);
       epi_bar();                                 // the previous tile's accumulators have been read by every warp
-      if (mma_warp) {
-        const int r0 = static_cast<int>(wg * 64u + ((warp - 4u) & 3u) * 16u + (lane >> 2));
-        const int c = 2 * static_cast<int>(lane & 3u);
-#pragma unroll
-        for (int i = 0; i < 64; i += 2) {
-          const int rr = r0 + 8 * ((i >> 1) & 1), cc = 8 * (i >> 2) + c;
-          *reinterpret_cast<float2*>(acc_tile + rr * kAccPitch + acc_chunk(cc >> 2, rr & 7) * 4 + (cc & 3)) =
-              make_float2(d[i], d[i + 1]);
-        }
-      }
+      if (mma_warp) stage_acc(d);
       epi_bar();
     };
     constexpr bool H_BIAS = (kF & F_BIAS) != 0, H_RES = (kF & F_RES) != 0, H_F32 = (kF & F_F32) != 0;
@@ -384,8 +439,10 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     const long long lo_delta = H_STRICT ? ep.lo_delta : 0;
     const uint32_t q = warp & 3u;                      // 32-row quadrant of the tile this warp owns
     const int asw = static_cast<int>(lane & 7u);       // swizzle of this thread's staged row (q * 32 + lane)
-    const int eg = static_cast<int>(warp - 4u) >> 2;   // column group 0/1: the two warps of a quadrant split the chunks
-    float* scr = reinterpret_cast<float*>(epi_smem) + (warp - 4u) * SM::kScrPerWarp;
+    const uint32_t ew = warp - (kDedicated ? 12u : 4u);   // epilogue warp index
+    // column group of this warp in the shared layouts: the warps of a quadrant split the chunks
+    const int eg = static_cast<int>(ew) >> 2;
+    float* scr = reinterpret_cast<float*>(epi_smem) + ew * SM::kScrPerWarp;
     uint32_t* scrw = reinterpret_cast<uint32_t*>(scr);
     // fp32 transpose tile addressing for the coalesced residual loads / fp32 stores: 16-byte chunk j of row r at chunk
     // slot r * 8 + (j ^ (r & 7)) -- 128-bit shared accesses, conflict-free for "lane = row" and "8 lanes = one row"
@@ -803,8 +860,20 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           }
         }
       }
-    } else
-    for (int tile = group; tile < num_tiles; tile += num_groups) {
+    } else {
+    // Work items are (tile, column group) pairs: a shared-layout warp runs its own group `eg` of each of its tiles, a
+    // dedicated epilogue warp both groups of each tile, one after the other.
+    constexpr int kPer = kDedicated ? kGroups : 1;
+    const int warp_eg = eg;
+    uint32_t acc_phase = 0;
+    for (int item = 0;; ++item) {
+      const int tile = group + (item / kPer) * num_groups;
+      if (tile >= num_tiles) break;
+      const int eg = kDedicated ? item % kPer : warp_eg;
+      if (item % kPer == 0) {
+        if constexpr (kDedicated) mbar_wait(acc_full, acc_phase);
+        else mma_tile(tile);
+      }
       const int mn = tile / splits;
       const bool first_split = (tile % splits) == 0;
       float* const out_f32_s = ep.out_f32 ? ep.out_f32 + static_cast<long long>(tile % splits) * ep.split_stride : nullptr;
@@ -812,14 +881,13 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       const int row = row_base + static_cast<int>(lane);
       const int n0 = (mn % num_n) * BN;
       const bool row_ok = row < sh.M;
-      mma_tile(tile);
       float* const arow = acc_tile + (q * 32u + lane) * kAccPitch;
       float s1 = 0.f, s2 = 0.f;
       float mean = 0.f, rstd = 0.f;
       const int npass = do_ln ? 2 : 1;
       // full-row LayerNorm needs one warp to see the whole row: group 1 sits those tiles out
       const int c_begin = do_ln ? (eg == 0 ? 0 : BN) : eg * 32;
-      const int c_step = do_ln ? 32 : 32 * (kEW / 4);
+      const int c_step = do_ln ? 32 : 32 * kGroups;
       // software prefetch of the residual / gelu-grad tiles of the NEXT chunk (their global latency would
       // otherwise be fully exposed: only two warps per SM sub-partition work on the epilogue)
       float4 rpre[H_RES ? 8 : 1];
@@ -1142,9 +1210,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       if constexpr (H_STATS) {
         if (has_stats && row_ok) {
           if (ep.stats_part != nullptr && !do_ln) {
-            const int per_tile = kEW / 4;
             float2* slot = reinterpret_cast<float2*>(ep.stats_part) +
-                           static_cast<size_t>(row) * (num_n * per_tile) + ((mn % num_n) * per_tile + eg);
+                           static_cast<size_t>(row) * (num_n * kGroups) + ((mn % num_n) * kGroups + eg);
             *slot = make_float2(s1, s2);
           } else {
             atomicAdd(ep.row_stats + 2 * static_cast<size_t>(row), s1);
@@ -1152,6 +1219,11 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           }
         }
       }
+      if (kDedicated && item % kPer == kPer - 1) {
+        mbar_arrive(acc_empty);     // the staged tile may be overwritten
+        acc_phase ^= 1u;
+      }
+    }
     }
   }
 

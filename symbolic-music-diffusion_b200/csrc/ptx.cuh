@@ -126,6 +126,13 @@ __device__ __forceinline__ void wgmma_m64n128k16_bf16_rs(float (&d)[64], const u
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate), "n"(kTB));
 }
 
+// ---------------------------------------------------------------- per-warpgroup register budget
+// Hands registers back to / takes them from the CTA's pool; executed by all 128 threads of a warpgroup.
+template <int kRegs>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <int kRegs>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+
 // ---------------------------------------------------------------- global-memory flags (inter-CTA hand-off)
 __device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
   uint32_t v;
