@@ -121,22 +121,6 @@ inline bool epi_clean(const GemmOp& op, const GemmEpilogue& e) {
          (!e.bias || a16(e.bias)) && (!e.ln_gamma || (a16(e.ln_gamma) && a16(e.ln_beta)));
 }
 
-// Column groups per tile (GemmSmem::kEpiGroups) of the instantiation launch_gemm will pick: the per-tile statistics
-// partials (GemmEpilogue::stats_part) have that many slots per n-tile.  3 for the short-K 12-warp kinds, 2 for every
-// other kind, in the 8-warp and the dedicated-epilogue layouts alike.
-inline int epi_groups_for(const GemmOp& op, const GemmEpilogue& ep) {
-  if (ep.lnf_part != nullptr || ep.lo_delta != 0 || !epi_clean(op, ep)) return 2;
-  const uint32_t need = epi_needs(ep);
-  const bool short_k = op.K <= 256;
-  if ((need & ~kEpiF32) == 0) return short_k ? 3 : 2;
-  if ((need & ~kEpiAtomic) == 0 || (need & ~kEpiF32Res) == 0) return 2;
-  if ((need & ~kEpiAct) == 0) return short_k ? 3 : 2;
-  return 2;
-}
-inline int stats_slots_for(const GemmOp& op, const GemmEpilogue& ep) {
-  return ((op.N + op.BN - 1) / op.BN) * epi_groups_for(op, ep);
-}
-
 // the K-split count every split of which owns at least one 64-wide k block
 inline int gemm_k_splits(const GemmOp& op) {
   const int num_kb = op.K / kBK;
@@ -149,9 +133,61 @@ inline int gemm_tiles(const GemmOp& op, int M) {
   return ((M + kBM - 1) / kBM) * ((op.N + op.BN - 1) / op.BN) * gemm_k_splits(op);
 }
 
+// persistent grid of min(#SMs, tiles) CTAs, programmatic dependent launch when enabled
+template <typename Kern, typename... Args>
+inline cudaError_t launch_persistent(Kern kern, int tiles, int threads, int smem, cudaStream_t st, const Args&... args) {
+  int grid = device_sm_count();
+  if (tiles < grid) grid = tiles;
+  if (grid < 1) grid = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(static_cast<unsigned>(grid));
+  cfg.blockDim = dim3(static_cast<unsigned>(threads));
+  cfg.dynamicSmemBytes = static_cast<size_t>(smem);
+  cfg.stream = st;
+  cudaLaunchAttribute attrs[1];
+  attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attrs[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attrs;
+  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return cudaLaunchKernelEx(&cfg, kern, args...);
+}
+
+// The GEMM instantiation a launch runs: epilogue feature set and thread layout (GemmSmem's kEW).
+struct GemmKind {
+  uint32_t flags;
+  int ew;
+};
+inline GemmKind gemm_kind(const GemmOp& op, int M, const GemmEpilogue& ep) {
+  if (ep.lo_delta != 0) return {kEpiStrict, 8};   // strict-precision mode (bf16x3)
+  const uint32_t need = epi_needs(ep);
+  if (epi_clean(op, ep)) {
+    auto fits = [&](uint32_t kind) { return (need & ~kind) == 0; };
+    // short-K GEMMs are epilogue-bound: give them a third epilogue warp per row quadrant
+    const bool short_k = op.K <= 256;
+    // long-K launches of several rounds: a dedicated epilogue warpgroup hides each tile's epilogue behind the next
+    // tile's K loop.  A single round has no next tile to overlap with; its exposed epilogue keeps the 8-warp layout,
+    // which runs it on twice as many warps.
+    const bool overlap = !short_k && gemm_tiles(op, M) > device_sm_count();
+    if (fits(kEpiF32)) return {kEpiF32, short_k ? 12 : overlap ? 4 : 8};
+    if (fits(kEpiAtomic)) return {kEpiAtomic, 8};
+    if (fits(kEpiF32Res)) return {kEpiF32Res, overlap ? 4 : 8};
+    if (fits(kEpiAct)) return {kEpiAct, short_k ? 12 : overlap ? 4 : 8};
+    if (fits(kEpiGG)) return {kEpiGG, 8};
+    if ((need & F_LN) && fits(kEpiLn) && op.N == op.BN && op.BN <= 128 && op.BN % 64 == 0 && op.k_splits <= 1)
+      return {kEpiLn, 8};
+  }
+  return {kEpiGeneric, 8};
+}
+// Slots per row of the per-tile statistics partials (GemmEpilogue::stats_part) the launch writes: one per n-tile and
+// column group of its instantiation.
+inline int stats_slots_for(const GemmOp& op, int M, const GemmEpilogue& ep) {
+  return ((op.N + op.BN - 1) / op.BN) * epi_groups(gemm_kind(op, M, ep).ew);
+}
+
 template <uint32_t kF, int kEW = 8>
 inline cudaError_t launch_gemm_inst(const GemmOp& op, int M, const GemmEpilogue& ep, cudaStream_t st) {
-  using SM = GemmSmem<kEW, lnf_kind(kF), scr_floats(kF)>;
+  using SM = GemmSmem<kEW>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<kF, kEW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -162,68 +198,32 @@ inline cudaError_t launch_gemm_inst(const GemmOp& op, int M, const GemmEpilogue&
   GemmShape sh;
   sh.M = M; sh.N = op.N; sh.K = op.K; sh.BN = op.BN; sh.a_mn = op.a_mn; sh.b_mn = op.b_mn;
   sh.k_splits = gemm_k_splits(op);
-  const int tiles = gemm_tiles(op, M);
-  int groups = device_sm_count();
-  if (tiles < groups) groups = tiles;
-  if constexpr ((kF & F_LNF) != 0 && (kF & F_RAGGED) == 0) {
-    // the n-tiles of one row block exchange LayerNorm partials: keep them in the same scheduling round
-    const int num_n = (op.N + op.BN - 1) / op.BN;
-    if (groups > num_n) groups -= groups % num_n;
-  }
-  if (groups < 1) groups = 1;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>(groups));
-  cfg.blockDim = dim3(SM::kThreads);
-  cfg.dynamicSmemBytes = SM::kTotal;
-  cfg.stream = st;
-  cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attrs[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attrs;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  return cudaLaunchKernelEx(&cfg, gemm_bf16_wgmma_kernel<kF, kEW>, op.tmA, op.tmB, sh, ep);
+  return launch_persistent(gemm_bf16_wgmma_kernel<kF, kEW>, gemm_tiles(op, M), SM::kThreads, SM::kTotal, st, op.tmA,
+                           op.tmB, sh, ep);
+}
+// the kEpiF32 / kEpiAct kinds exist in all three layouts
+template <uint32_t kF>
+inline cudaError_t launch_gemm_ew(int ew, const GemmOp& op, int M, const GemmEpilogue& ep, cudaStream_t st) {
+  return ew == 12 ? launch_gemm_inst<kF, 12>(op, M, ep, st)
+                  : ew == 4 ? launch_gemm_inst<kF, 4>(op, M, ep, st) : launch_gemm_inst<kF, 8>(op, M, ep, st);
 }
 
 inline cudaError_t launch_gemm(const GemmOp& op, int M, const GemmEpilogue& ep, cudaStream_t st) {
-  if (ep.lnf_part != nullptr) {
-    // LN-fused two-pass epilogue (the caller arms it only for full, aligned tiles; see smd_api.cu::arm_lnf)
-    if (!epi_clean(op, ep) || op.N % op.BN != 0 || op.BN % 64 != 0 || op.k_splits > 1) return cudaErrorInvalidValue;
-    // epilogue warps per kind: SMD_LNF_WARPS_A / _B = 8 (default) | 12 (three warps per row quadrant)
-    static const int wa = [] { const char* v = getenv("SMD_LNF_WARPS_A"); return (v && atoi(v) == 12) ? 12 : 8; }();
-    static const int wb = [] { const char* v = getenv("SMD_LNF_WARPS_B"); return (v && atoi(v) == 12) ? 12 : 8; }();
-    if (ep.residual != nullptr || ep.out_f32 != nullptr)
-      return wb == 12 ? launch_gemm_inst<kEpiLnfB, 12>(op, M, ep, st) : launch_gemm_inst<kEpiLnfB, 8>(op, M, ep, st);
-    return wa == 12 ? launch_gemm_inst<kEpiLnfA, 12>(op, M, ep, st) : launch_gemm_inst<kEpiLnfA, 8>(op, M, ep, st);
-  }
   // full-row LayerNorm needs the whole row in one tile (N <= BN; BN is at most kBNMax)
   if (ep.ln_gamma != nullptr && op.N > op.BN) return cudaErrorInvalidValue;
-  if (ep.lo_delta != 0) return launch_gemm_inst<kEpiStrict>(op, M, ep, st);   // strict-precision mode (bf16x3)
-  const uint32_t need = epi_needs(ep);
-  if (epi_clean(op, ep)) {
-    auto fits = [&](uint32_t kind) { return (need & ~kind) == 0; };
-    // short-K GEMMs are epilogue-bound: give them a third epilogue warp per row quadrant
-    const bool short_k = op.K <= 256;
-    // long-K launches of several rounds: a dedicated epilogue warpgroup hides each tile's epilogue behind the next
-    // tile's K loop.  A single round has no next tile to overlap with; its exposed epilogue keeps the 8-warp layout,
-    // which runs it on twice as many warps.
-    const bool overlap = !short_k && gemm_tiles(op, M) > device_sm_count();
-    if (fits(kEpiF32))
-      return short_k ? launch_gemm_inst<kEpiF32, 12>(op, M, ep, st)
-                     : overlap ? launch_gemm_inst<kEpiF32, 4>(op, M, ep, st) : launch_gemm_inst<kEpiF32>(op, M, ep, st);
-    if (fits(kEpiAtomic)) return launch_gemm_inst<kEpiAtomic>(op, M, ep, st);
-    if (fits(kEpiF32Res))
-      return overlap ? launch_gemm_inst<kEpiF32Res, 4>(op, M, ep, st) : launch_gemm_inst<kEpiF32Res>(op, M, ep, st);
-    if (fits(kEpiAct))
-      return short_k ? launch_gemm_inst<kEpiAct, 12>(op, M, ep, st)
-                     : overlap ? launch_gemm_inst<kEpiAct, 4>(op, M, ep, st) : launch_gemm_inst<kEpiAct>(op, M, ep, st);
-    if (fits(kEpiGG)) return launch_gemm_inst<kEpiGG>(op, M, ep, st);
-    if ((need & F_LN) && fits(kEpiLn) && op.N == op.BN && op.BN <= 128 && op.BN % 64 == 0 && op.k_splits <= 1)
-      return launch_gemm_inst<kEpiLn>(op, M, ep, st);
+  const GemmKind k = gemm_kind(op, M, ep);
+  switch (k.flags) {
+    case kEpiStrict: return launch_gemm_inst<kEpiStrict>(op, M, ep, st);
+    case kEpiF32: return launch_gemm_ew<kEpiF32>(k.ew, op, M, ep, st);
+    case kEpiAtomic: return launch_gemm_inst<kEpiAtomic>(op, M, ep, st);
+    case kEpiF32Res:
+      return k.ew == 4 ? launch_gemm_inst<kEpiF32Res, 4>(op, M, ep, st) : launch_gemm_inst<kEpiF32Res>(op, M, ep, st);
+    case kEpiAct: return launch_gemm_ew<kEpiAct>(k.ew, op, M, ep, st);
+    case kEpiGG: return launch_gemm_inst<kEpiGG>(op, M, ep, st);
+    case kEpiLn: return launch_gemm_inst<kEpiLn>(op, M, ep, st);
+    default: return launch_gemm_inst<kEpiGeneric>(op, M, ep, st);
   }
-  return launch_gemm_inst<kEpiGeneric>(op, M, ep, st);
 }
-
 
 // ---------------------------------------------------------------------------------------------------
 // fused FFN (fused_wgmma.cuh)
@@ -247,26 +247,6 @@ inline bool ffn_fused_forced() {
   static const bool on = [] { const char* v = getenv("SMD_FFN_FUSED"); return v && v[0] == '2'; }();
   return on;
 }
-// persistent grid of min(#SMs, tiles) CTAs, programmatic dependent launch when enabled
-template <typename Kern, typename Args>
-inline cudaError_t launch_fused(Kern kern, int tiles, int threads, int smem, const CUtensorMap& t0, const CUtensorMap& t1,
-                                const CUtensorMap& t2, const Args& a, cudaStream_t st) {
-  int grid = device_sm_count();
-  if (tiles < grid) grid = tiles;
-  if (grid < 1) grid = 1;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>(grid));
-  cfg.blockDim = dim3(static_cast<unsigned>(threads));
-  cfg.dynamicSmemBytes = static_cast<size_t>(smem);
-  cfg.stream = st;
-  cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attrs[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attrs;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  return cudaLaunchKernelEx(&cfg, kern, t0, t1, t2, a);
-}
 inline cudaError_t launch_ffn_fused(const FfnOp& op, const FfnFusedArgs& a, cudaStream_t st) {
   if (a.Md % 128 != 0) return cudaErrorInvalidValue;
   static bool attr_set = false;
@@ -279,8 +259,8 @@ inline cudaError_t launch_ffn_fused(const FfnOp& op, const FfnFusedArgs& a, cuda
   }
   const int tiles = (a.M + 127) / 128;
   if (a.hidden_pre != nullptr || a.hidden != nullptr)
-    return launch_fused(ffn_fused_kernel<true>, tiles, FfnSmem::kThreads, FfnSmem::kTotal, op.tmA, op.tmW1, op.tmW2, a, st);
-  return launch_fused(ffn_fused_kernel<false>, tiles, FfnSmem::kThreads, FfnSmem::kTotal, op.tmA, op.tmW1, op.tmW2, a, st);
+    return launch_persistent(ffn_fused_kernel<true>, tiles, FfnSmem::kThreads, FfnSmem::kTotal, st, op.tmA, op.tmW1, op.tmW2, a);
+  return launch_persistent(ffn_fused_kernel<false>, tiles, FfnSmem::kThreads, FfnSmem::kTotal, st, op.tmA, op.tmW1, op.tmW2, a);
 }
 
 
@@ -329,11 +309,11 @@ inline cudaError_t launch_attn_block(const AttnOp& op, const AttnBlockArgs& a, c
   const int tiles = (a.M + 63) / 64;
   const int T = AttnSmem::kThreads, B = AttnSmem::kTotal;
   if (train) {
-    if (dh == 16) return launch_fused(attn_block_kernel<16, true>, tiles, T, B, op.tmA, op.tmWqkv, op.tmWo, a, st);
-    return launch_fused(attn_block_kernel<8, true>, tiles, T, B, op.tmA, op.tmWqkv, op.tmWo, a, st);
+    if (dh == 16) return launch_persistent(attn_block_kernel<16, true>, tiles, T, B, st, op.tmA, op.tmWqkv, op.tmWo, a);
+    return launch_persistent(attn_block_kernel<8, true>, tiles, T, B, st, op.tmA, op.tmWqkv, op.tmWo, a);
   }
-  if (dh == 16) return launch_fused(attn_block_kernel<16, false>, tiles, T, B, op.tmA, op.tmWqkv, op.tmWo, a, st);
-  return launch_fused(attn_block_kernel<8, false>, tiles, T, B, op.tmA, op.tmWqkv, op.tmWo, a, st);
+  if (dh == 16) return launch_persistent(attn_block_kernel<16, false>, tiles, T, B, st, op.tmA, op.tmWqkv, op.tmWo, a);
+  return launch_persistent(attn_block_kernel<8, false>, tiles, T, B, st, op.tmA, op.tmWqkv, op.tmWo, a);
 }
 
 }  // namespace smd

@@ -74,7 +74,7 @@ struct smd_plan {
   std::vector<int> stat_slots;   // per wide LayerNorm: partial slots per row its producing GEMM wrote (0: atomics / totals)
   int pack_tiles = 0;
   // ---- GEMM ops ----
-  std::vector<GemmOp> op_qkv, op_o, op_ffn1, op_ffn2, op_a, op_b, op_b2;
+  std::vector<GemmOp> op_qkv, op_o, op_ffn1, op_ffn2, op_a, op_b;
   std::vector<FfnOp> op_ffn;   // fused FFN (mlp_dims % 128 == 0)
   std::vector<AttnOp> op_attn; // fused attention block (head dim 8 / 16)
   GemmOp op_post, op_out, op_in;

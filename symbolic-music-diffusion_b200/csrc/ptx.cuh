@@ -133,16 +133,6 @@ __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.
 template <int kRegs>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
 
-// ---------------------------------------------------------------- global-memory flags (inter-CTA hand-off)
-__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
-  uint32_t v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_release_gpu_add(uint32_t* p, uint32_t v) {
-  asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-
 // ---------------------------------------------------------------- wgmma descriptors
 // Shared-memory matrix descriptor (sm_90), canonical SWIZZLE_128B layouts produced by TMA with a 128-byte inner box:
 //   K-major  operand tile [rows][64 bf16]: rows at 128 B pitch, 8-row swizzle atoms -> SBO = 1024 B, LBO unused.

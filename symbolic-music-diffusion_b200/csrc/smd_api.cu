@@ -120,11 +120,10 @@ static void build_workspace(smd_plan* p) {
   ws_add(p, "u", Mp * Md * 4);
   ws_add(p, "r1", Mp * Md * 4);
   ws_add(p, "act", Mp * Md * 2);
-  // per-row LayerNorm (sum, sumsq) of the 2K+1 wide LayerNorms, followed by the arrival counters of the LN-fused GEMM
-  // epilogues (one u32 per 32 rows and fused launch); the whole region is zeroed once per forward
-  ws_add(p, "stats", (2 * K + 1) * Mp * 2 * 4 + (2 * K + 2) * (Mp / 32) * 4);
-  // per-tile partial sums [row][n_tile * (2 or 3) + column group][2]
-  ws_add(p, "lnf_part", Mp * ((Md + kBNMax - 1) / kBNMax * 3) * 2 * 4);
+  // per-row LayerNorm (sum, sumsq) of the 2K+1 wide LayerNorms; zeroed once per forward
+  ws_add(p, "stats", (2 * K + 1) * Mp * 2 * 4);
+  // per-tile partial sums of the GEMM feeding the next wide LayerNorm: [row][n_tile * (2 or 3) + column group][2]
+  ws_add(p, "stats_part", Mp * ((Md + kBNMax - 1) / kBNMax * 3) * 2 * 4);
   // FiLM generator
   ws_add(p, "tvec", B * 4);
   ws_add(p, "enc", B * kFilmEmb * 4);
@@ -198,14 +197,11 @@ static int build_ops(smd_plan* p) {
   } else {
     if (!fwd(&p->op_in, "xb", "in.kernel", C, Md, 256)) return SMD_ERR_CUDA;
   }
-  p->op_a.resize(p->K); p->op_b.resize(p->K); p->op_b2.resize(p->K);
+  p->op_a.resize(p->K); p->op_b.resize(p->K);
   for (int k = 0; k < p->K; ++k) {
     const std::string pre = "k" + std::to_string(k) + ".res.";
     if (!fwd(&p->op_a[k], "act", pre + "a.kernel", Md, Md, 256)) return SMD_ERR_CUDA;
     if (!fwd(&p->op_b[k], "act", pre + "b.kernel", Md, Md, 256)) return SMD_ERR_CUDA;
-    // LN-fused tail: GEMM a writes the next operand while other CTAs still read `act`, so the two GEMMs ping-pong
-    // between `act` and the (then unused) r1 region
-    if (!fwd(&p->op_b2[k], "r1", pre + "b.kernel", Md, Md, 256)) return SMD_ERR_CUDA;
   }
   // output projection from the padded copy [Md][Cp]: N = C columns are valid, the tile is Cp (<= 256) wide
   {
@@ -226,8 +222,8 @@ static int build_ops(smd_plan* p) {
 static cudaError_t gemm(smd_plan* p, const GemmOp& op, int M, GemmEpilogue e, cudaStream_t st, int ln_slot = -1) {
   auto arm_stats = [&](GemmEpilogue& ef) {
     if (ln_slot < 0 || ef.row_stats == nullptr) return;
-    ef.stats_part = p->buf<float>("lnf_part");
-    p->stat_slots[ln_slot] = stats_slots_for(op, ef);
+    ef.stats_part = p->buf<float>("stats_part");
+    p->stat_slots[ln_slot] = stats_slots_for(op, M, ef);
   };
   if (p->lo_bytes == 0) { arm_stats(e); return launch_gemm(op, M, e, st); }
   if (!op.has_lo) return cudaErrorInvalidValue;
@@ -254,7 +250,7 @@ struct LnStats { const float* part; int nslots; float* totals; };
 static LnStats ln_stats(smd_plan* p, int ln_slot) {
   float* totals = p->buf<float>("stats") + static_cast<size_t>(ln_slot) * p->Mp * 2;
   const int n = p->stat_slots[ln_slot];
-  return n > 0 ? LnStats{p->buf<float>("lnf_part"), n, totals} : LnStats{nullptr, 0, totals};
+  return n > 0 ? LnStats{p->buf<float>("stats_part"), n, totals} : LnStats{nullptr, 0, totals};
 }
 
 // FiLM generator for all K blocks: t (R values) -> ss[k][R][2*Md]   (models/ncsn.py:47-61)
@@ -294,112 +290,10 @@ int ensure_side_stream(smd_plan* p) {
   return SMD_OK;
 }
 
-// LN-fused GEMM epilogues (gemm_wgmma.cuh, F_LNF): opt-in with SMD_LNF=1.  The fused tail is 4
-// launches shorter and moves fewer HBM bytes, but its two-pass epilogue is long next to the mainloop and it runs with a
-// two-stage operand ring; whether it beats the stand-alone ln_film_act kernels on H100 is not measured.  Default: off.
-static bool lnf_enabled() {
-  static const bool on = [] { const char* v = getenv("SMD_LNF"); return v && v[0] == '1'; }();
-  return on;
-}
-// one FiLM (scale | shift) row per sample of 32 rows, or one row for everybody (sampler): the fused epilogue cannot
-// serve DenseDDPM's one-row-per-example case (a 32-row warp tile would span 32 FiLM rows)
-bool lnf_usable(const smd_plan* p, int S, int t_broadcast) {
-  return lnf_enabled() && p->lo_bytes == 0 && (S == 32 || t_broadcast || p->film_tab_on) &&
-         p->cfg.mlp_dims % 256 == 0;
-}
-// FiLM table / row selection of block k (shared by the fused epilogue and the stand-alone kernel)
-static void film_source(const smd_plan* p, int k, int t_broadcast, const float** scale, int* bcast, const int** row_dev) {
-  const int Md = p->cfg.mlp_dims;
-  *scale = p->buf<float>("ss") + static_cast<size_t>(k) * p->cfg.max_batch * 2 * Md;
-  *row_dev = nullptr;
-  *bcast = t_broadcast;
-  if (p->film_tab_on) {
-    *scale = p->buf<float>("ftab") + static_cast<size_t>(k) * p->T * 2 * Md;
-    *bcast = 1;
-    if (p->film_row_dev) *row_dev = p->film_row_dev; else *scale += static_cast<size_t>(p->film_row) * 2 * Md;
-  }
-}
-// Arms `e` so that the GEMM's epilogue also produces act = act2(film_k(LN(v; ln.scale, ln.bias))) for LayerNorm slot
-// `ln_slot` (0 .. 2K): k < 0 means no FiLM / no activation (the final LayerNorm).
-void arm_lnf(const smd_plan* p, const float* params, GemmEpilogue* e, const std::string& ln, int k, int ln_slot,
-             int t_broadcast, __nv_bfloat16* out, bool want_totals) {
-  const int Md = p->cfg.mlp_dims;
-  float* stats = p->buf<float>("stats");
-  const size_t sstride = static_cast<size_t>(p->Mp) * 2;
-  uint32_t* cnt0 = reinterpret_cast<uint32_t*>(stats + static_cast<size_t>(2 * p->K + 1) * sstride);
-  e->ln_gamma = p->P(params, ln + "scale"); e->ln_beta = p->P(params, ln + "bias");
-  e->out_bf16 = out; e->ld_bf16 = Md;
-  e->lnf_part = p->buf<float>("lnf_part");
-  e->lnf_cnt = cnt0 + static_cast<size_t>(ln_slot) * (p->Mp / 32);
-  e->row_stats = want_totals ? stats + static_cast<size_t>(ln_slot) * sstride : nullptr;
-  e->film = nullptr; e->film_ld = 2 * Md; e->film_bcast = 0; e->film_row_dev = nullptr; e->act2 = ACT_NONE;
-  static const int nowait = [] { const char* v = getenv("SMD_LNF_NOWAIT"); return (v && v[0] == '1') ? 1 : 0; }();
-  e->lnf_nowait = nowait;
-  if (k >= 0) {
-    film_source(p, k, t_broadcast, &e->film, &e->film_bcast, &e->film_row_dev);
-    e->act2 = ACT_SWISH;
-  }
-}
-
-// LN-fused tail: every 2048-wide LayerNorm -> FiLM -> swish runs inside the epilogue of the GEMM that produces its
-// input, so the tail is 2K + 1 launches and the activations cross HBM once (as bf16 operands) instead of three times.
-// On entry `act` (or save->act_a(0)) already holds the first block's operand (written by the post / in GEMM).
-static int run_tail_fused(smd_plan* p, const float* params, int M, int S, int t_broadcast, float* y, cudaStream_t st,
-                          smd::TrainState* save) {
-  const int Md = p->cfg.mlp_dims, C = p->cfg.channels;
-  float* u = p->buf<float>("u");
-  __nv_bfloat16* act = p->buf<__nv_bfloat16>("act");
-  __nv_bfloat16* act2 = p->buf<__nv_bfloat16>("r1");
-  for (int k = 0; k < p->K; ++k) {
-    const std::string pre = "k" + std::to_string(k) + ".res.";
-    float* u_in = save ? save->u(p->ws, k) : u;
-    float* u_out = save ? save->u(p->ws, k + 1) : u;
-    __nv_bfloat16* act_a = save ? save->act_a(p->ws, k) : act;
-    __nv_bfloat16* act_b = save ? save->act_b(p->ws, k) : act2;
-    __nv_bfloat16* act_n = save ? ((k + 1 < p->K) ? save->act_a(p->ws, k + 1) : save->act_out(p->ws)) : act;
-    GemmOp opa = p->op_a[k], opb = p->op_b2[k];
-    if (save) { if (!retarget_a(&opa, act_a, p->Mp) || !retarget_a(&opb, act_b, p->Mp)) return SMD_ERR_CUDA; }
-    GemmEpilogue e = epi();
-    e.bias = p->P(params, pre + "a.bias");
-    if (save) e.out_bf16_pre = reinterpret_cast<__nv_bfloat16*>(save->r1(p->ws, k));   // pre-LN value for the backward
-    arm_lnf(p, params, &e, pre + "ln_b.", k, 2 * k + 1, t_broadcast, act_b, save != nullptr);
-    SMD_CUDA(launch_gemm(opa, M, e, st));
-    e = epi();
-    e.bias = p->P(params, pre + "b.bias");
-    e.residual = u_in; e.ld_res = Md;
-    e.out_f32 = u_out; e.ld_f32 = Md;
-    if (k + 1 < p->K) arm_lnf(p, params, &e, "k" + std::to_string(k + 1) + ".res.ln_a.", k + 1, 2 * k + 2, t_broadcast, act_n, save != nullptr);
-    else arm_lnf(p, params, &e, "out_ln.", -1, 2 * k + 2, t_broadcast, act_n, save != nullptr);
-    SMD_CUDA(launch_gemm(opb, M, e, st));
-  }
-  GemmEpilogue e = epi();
-  e.bias = p->P(params, "out.bias");
-  e.out_f32 = y; e.ld_f32 = C;
-  GemmOp opo = p->op_out;
-  if (save) { if (!retarget_a(&opo, save->act_out(p->ws), p->Mp)) return SMD_ERR_CUDA; }
-  SMD_CUDA(launch_gemm(opo, M, e, st));
-  SMD_LAUNCH_CHECK("tail (fused)");
-  return SMD_OK;
-}
-
 // The FiLM'd residual tail shared by both architectures (models/ncsn.py:173-178, models/shared.py:61-75).
 // On entry u (fp32 [M][Md]) and stats[0] hold the block input and its row statistics.
 static int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, float* y, cudaStream_t st,
-                    smd::TrainState* save, bool fuse_tail, bool act0_ready) {
-  if (fuse_tail) {
-    if (!act0_ready) {
-      // first block's operand from the stand-alone kernel (the K = 128 post GEMM is epilogue-bound: the two-pass fused
-      // epilogue there is opt-in, SMD_LNF_POST=1)
-      const float* scale; int bcast; const int* row_dev;
-      film_source(p, 0, t_broadcast, &scale, &bcast, &row_dev);
-      const LnStats ls = ln_stats(p, 0);
-      launch_ln_film_act(save ? save->u(p->ws, 0) : p->buf<float>("u"), ls.totals, p->P(params, "k0.res.ln_a.scale"),
-                         p->P(params, "k0.res.ln_a.bias"), scale, scale + p->cfg.mlp_dims, 2 * p->cfg.mlp_dims, bcast, 2,
-                         save ? save->act_a(p->ws, 0) : p->buf<__nv_bfloat16>("act"), M, p->cfg.mlp_dims, S, st, row_dev,
-                         nullptr, 0, ls.part, ls.nslots, ls.totals); CNT();
-    }
-    return run_tail_fused(p, params, M, S, t_broadcast, y, st, save);
-  }
+                    smd::TrainState* save) {
   const int Md = p->cfg.mlp_dims, C = p->cfg.channels;
   float* u = p->buf<float>("u");
   float* r1 = p->buf<float>("r1");
@@ -476,8 +370,7 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
   const int M = batch * S;
   float* stats = p->buf<float>("stats");
   p->stat_slots.assign(static_cast<size_t>(2 * p->K + 1), 0);
-  SMD_CUDA(cudaMemsetAsync(stats, 0, static_cast<size_t>(2 * p->K + 1) * p->Mp * 2 * 4 +
-                                         static_cast<size_t>(2 * p->K + 2) * (p->Mp / 32) * 4, st));
+  SMD_CUDA(cudaMemsetAsync(stats, 0, static_cast<size_t>(2 * p->K + 1) * p->Mp * 2 * 4, st));
   int rc = SMD_OK;
   bool film_on_side = false;
   if (!p->film_tab_on) {
@@ -497,9 +390,6 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
   }
   if (rc) return rc;
   float* u0 = save ? save->u(p->ws, 0) : p->buf<float>("u");
-  const bool fuse_tail = c.arch == SMD_ARCH_TRANSFORMER_DDPM && lnf_usable(p, S, t_broadcast);
-  static const bool lnf_post = [] { const char* v = getenv("SMD_LNF_POST"); return v && v[0] == '1'; }();
-  const bool fuse_post = fuse_tail && lnf_post;
   if (c.arch == SMD_ARCH_TRANSFORMER_DDPM) {
     float* h = p->buf<float>("h");
     __nv_bfloat16* a = p->buf<__nv_bfloat16>("a");
@@ -601,15 +491,9 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
     e.bias = p->P(params, "post.bias");
     e.out_f32 = u0; e.ld_f32 = Md;
     e.row_stats = stats;
-    if (fuse_post) {
-      // the first res-block's LayerNorm -> FiLM -> swish happens in this GEMM's epilogue: needs the FiLM rows now
-      if (film_on_side) { SMD_CUDA(cudaStreamWaitEvent(st, p->ev_film, 0)); film_on_side = false; }
-      arm_lnf(p, params, &e, "k0.res.ln_a.", 0, 0, t_broadcast, save ? save->act_a(p->ws, 0) : p->buf<__nv_bfloat16>("act"),
-              save != nullptr);
-    }
     GemmOp op = p->op_post;
     if (save) { if (!retarget_a(&op, save->a_post(p->ws), p->Mp)) return SMD_ERR_CUDA; }
-    SMD_CUDA(gemm(p, op, M, e, st, fuse_post ? -1 : 0));
+    SMD_CUDA(gemm(p, op, M, e, st, 0));
   } else {
     __nv_bfloat16* xb = p->buf<__nv_bfloat16>("xb");
     const int Cp = (C + 63) / 64 * 64;
@@ -623,7 +507,7 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
   }
   SMD_LAUNCH_CHECK("trunk");
   if (film_on_side) SMD_CUDA(cudaStreamWaitEvent(st, p->ev_film, 0));
-  rc = run_tail(p, params, M, S, t_broadcast, y, st, save, fuse_tail, fuse_post);
+  rc = run_tail(p, params, M, S, t_broadcast, y, st, save);
   if (rc) return rc;
   if (c.arch == SMD_ARCH_DENSE_NCSN && !raw_out) {   // models/ncsn.py:97: output = x / sigmas
     launch_scale_rows(y, t, t_broadcast, batch, S * C, st); CNT();

@@ -44,15 +44,19 @@ def test_transformer_forward_parity(lib, case, cg):
 
 def test_forward_batch_ragged_and_broadcast_t(lib):
     kw, _ = TRANSFORMER_CASES["tiny"]
-    eng, flat = _engine(kw, 13, 2)
+    eng, flat = _engine(kw, 600, 2)
     p = params_torch(eng, flat)
     okw = oracle_kwargs(eng.cfg)
-    for batch in (1, 5, 13):   # 32, 160, 416 token rows: partial 128/256-row tiles
+    # 32, 160, 416 token rows: partial 128/256-row tiles; 19200 rows: more tiles than SMs, several scheduling rounds
+    for batch in (1, 5, 13, 600):
         x, _ = make_inputs(batch, batch, (32, 42))
         t = np.full((batch,), 0.37, np.float32)
         y = eng.forward(torch.from_numpy(x).cuda(), torch.tensor([0.37], device="cuda"))  # broadcast t
         ref = O.transformer_ddpm(p, torch.from_numpy(x), torch.from_numpy(t), emulate_bf16=True, **okw)
         assert rel_l2(y, ref) < 1e-2
+    # the LayerNorm statistics are added in a fixed order: the same forward twice is bit-identical
+    y2 = eng.forward(torch.from_numpy(x).cuda(), torch.tensor([0.37], device="cuda"))
+    assert torch.equal(y, y2)
 
 
 def test_dense_ddpm_forward_parity(lib):
@@ -113,15 +117,3 @@ def test_fused_ffn_kernel(lib):
                        capture_output=True, text=True, timeout=600)
     assert r.returncode == 0 and "fused-ok" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]
 
-
-@pytest.mark.parametrize("post", ["0", "1"])
-def test_ln_fused_epilogue(lib, post):
-    """The LN-fused GEMM epilogue (csrc/gemm_wgmma.cuh, F_LNF) is opt-in (SMD_LNF=1, read once per process): parity,
-    bit-reproducibility and gradient checks run in a worker process; SMD_LNF_POST=1 also fuses the K = 128 post GEMM."""
-    import subprocess
-    import sys
-    env = dict(os.environ, SMD_LNF="1", SMD_LNF_POST=post)
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, os.path.join(root, "tests", "lnf_worker.py")], env=env, cwd=root,
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "lnf-ok" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]

@@ -75,8 +75,8 @@ def test_sharded_sampling_equals_the_single_process_chain(lib):
         assert torch.equal(x, x_all[4 * r:4 * r + 4])
         m = torch.zeros((4, 1000), device="cuda")
         eng.sample(x, steps=steps, metrics=m, use_graph=(r == 0))      # graph replay and plain launches alike
-        # identical inputs and noise: with the LN-fused epilogues (fixed-order LayerNorm statistics) the forward pass
-        # is bit-reproducible and independent of where a row sits in the batch, so the shards match exactly
+        # identical inputs and noise: the LayerNorm statistics partials (stats_part slots) are added in a fixed order, so
+        # the forward pass is bit-reproducible and independent of where a row sits in the batch: the shards match exactly
         assert torch.equal(x, ref[4 * r:4 * r + 4]), float((x - ref[4 * r:4 * r + 4]).abs().max())
         m_sum += m * 0.5
     torch.testing.assert_close(m_sum[[0, 1, 3], :steps], m_all[[0, 1, 3], :steps], rtol=1e-5, atol=1e-7)
