@@ -8,32 +8,30 @@
 namespace smd {
 
 // Split count for a dW GEMM that runs beside the dX chain: ~48 CTAs, leaving two thirds of the SMs to `st`.
-static int pick_splits_side(int m_rows, int n_cols, int BN, int cg, int num_kb) {
-  const int tiles = ((m_rows + 128 * cg - 1) / (128 * cg)) * ((n_cols + BN - 1) / BN);
-  int s = 48 / (tiles * cg);
+static int pick_splits_side(int m_rows, int n_cols, int BN, int num_kb) {
+  const int tiles = ((m_rows + 127) / 128) * ((n_cols + BN - 1) / BN);
+  int s = 48 / tiles;
   if (s < 1) s = 1;
   if (s > num_kb) s = num_kb;
   return s;
 }
 
 // dW GEMM: A = X (MN-major [tokens][in]), B = G (MN-major [tokens][out]) -> out_f32 [in][out]
-static bool make_dw(GemmOp* op, const void* X, int in_f, const void* G, int g_cols, int out_f, uint64_t rows, int cg) {
-  int BN = (out_f >= 256) ? 256 : ((out_f + 63) / 64 * 64);
-  if (BN / cg < 64) cg = 1;
-  if (in_f <= 128) cg = 1;
+static bool make_dw(GemmOp* op, const void* X, int in_f, const void* G, int g_cols, int out_f, uint64_t rows) {
+  const int BN = (out_f >= 256) ? 256 : ((out_f + 63) / 64 * 64);
   return make_gemm_op(op, X, static_cast<uint64_t>(in_f), G, static_cast<uint64_t>(g_cols), out_f,
-                      static_cast<int>(rows), BN, cg, 1, 1);
+                      static_cast<int>(rows), BN, 1, 1);
 }
 // dX GEMM: A = G (K-major [tokens][out]), B = W plain (in,out) = [N=in][K=out] -> [tokens][in]
-static bool make_dx(GemmOp* op, const void* G, int out_f, const void* W, int in_f, uint64_t rows, int cg) {
-  return make_gemm_op(op, G, rows, W, static_cast<uint64_t>(in_f), in_f, out_f, choose_bn(in_f, cg), cg, 0, 0);
+static bool make_dx(GemmOp* op, const void* G, int out_f, const void* W, int in_f, uint64_t rows) {
+  return make_gemm_op(op, G, rows, W, static_cast<uint64_t>(in_f), in_f, out_f, choose_bn(in_f), 0, 0);
 }
 
 int train_bind(smd_plan* p) {
   TrainState& ts = p->train;
   uint8_t* ws = p->ws;
   const smd_config& c = p->cfg;
-  const int Md = c.mlp_dims, C = c.channels, cg = c.cta_group;
+  const int Md = c.mlp_dims, C = c.channels;
   const int Cp = (C + 63) / 64 * 64;
   const uint64_t Mp = p->Mp;
   auto B16 = [&](size_t off) { return ts.at<__nv_bfloat16>(ws, off); };
@@ -45,37 +43,37 @@ int train_bind(smd_plan* p) {
   ts.dWss.resize(ts.K); ts.dXss.resize(ts.K);
   const uint64_t Bp = (static_cast<uint64_t>(c.max_batch) + 127) / 128 * 128;
   for (int k = 0; k < ts.K; ++k) {
-    if (!make_dw(&ts.dWb[k], ts.act_b(ws, k), Md, B16(ts.off_du16[k + 1]), Md, Md, Mp, cg)) return SMD_ERR_CUDA;
-    if (!make_dx(&ts.dXb[k], B16(ts.off_du16[k + 1]), Md, Wsh(KN(k) + "res.b.kernel"), Md, Mp, cg)) return SMD_ERR_CUDA;
-    if (!make_dw(&ts.dWa[k], ts.act_a(ws, k), Md, B16(ts.off_dr16t[k]), Md, Md, Mp, cg)) return SMD_ERR_CUDA;
-    if (!make_dx(&ts.dXa[k], B16(ts.off_dr16t[k]), Md, Wsh(KN(k) + "res.a.kernel"), Md, Mp, cg)) return SMD_ERR_CUDA;
-    if (!make_dw(&ts.dWss[k], B16(ts.off_e2_16), 512, B16(ts.off_dss16), 2 * Md, 2 * Md, Bp, 1)) return SMD_ERR_CUDA;
-    if (!make_dx(&ts.dXss[k], B16(ts.off_dss16), 2 * Md, Wsh(KN(k) + "film.ss.kernel"), 512, Bp, 1)) return SMD_ERR_CUDA;
+    if (!make_dw(&ts.dWb[k], ts.act_b(ws, k), Md, B16(ts.off_du16[k + 1]), Md, Md, Mp)) return SMD_ERR_CUDA;
+    if (!make_dx(&ts.dXb[k], B16(ts.off_du16[k + 1]), Md, Wsh(KN(k) + "res.b.kernel"), Md, Mp)) return SMD_ERR_CUDA;
+    if (!make_dw(&ts.dWa[k], ts.act_a(ws, k), Md, B16(ts.off_dr16t[k]), Md, Md, Mp)) return SMD_ERR_CUDA;
+    if (!make_dx(&ts.dXa[k], B16(ts.off_dr16t[k]), Md, Wsh(KN(k) + "res.a.kernel"), Md, Mp)) return SMD_ERR_CUDA;
+    if (!make_dw(&ts.dWss[k], B16(ts.off_e2_16), 512, B16(ts.off_dss16), 2 * Md, 2 * Md, Bp)) return SMD_ERR_CUDA;
+    if (!make_dx(&ts.dXss[k], B16(ts.off_dss16), 2 * Md, Wsh(KN(k) + "film.ss.kernel"), 512, Bp)) return SMD_ERR_CUDA;
   }
   // output projection: dpred16 is zero-padded to Cp columns; the plain weight copy is [Md][Cp]
   if (!make_gemm_op(&ts.dWout, ts.act_out(ws), static_cast<uint64_t>(Md), B16(ts.off_dpred16), static_cast<uint64_t>(Cp),
-                    C, static_cast<int>(Mp), (Cp >= 256) ? 256 : Cp, (Cp / cg >= 64 && Cp % (64 * cg) == 0) ? cg : 1, 1, 1))
+                    C, static_cast<int>(Mp), (Cp >= 256) ? 256 : Cp, 1, 1))
     return SMD_ERR_CUDA;
   if (!make_gemm_op(&ts.dXout, B16(ts.off_dpred16), Mp, p->buf<__nv_bfloat16>("w.out_pad"), static_cast<uint64_t>(Md), Md, Cp,
-                    choose_bn(Md, cg), cg, 0, 0)) return SMD_ERR_CUDA;
+                    choose_bn(Md), 0, 0)) return SMD_ERR_CUDA;
   if (ts.L > 0) {
-    if (!make_dw(&ts.dWpost, ts.a_post(ws), 128, B16(ts.off_du16[0]), Md, Md, Mp, 1)) return SMD_ERR_CUDA;
-    if (!make_dx(&ts.dXpost, B16(ts.off_du16[0]), Md, Wsh("post.kernel"), 128, Mp, cg)) return SMD_ERR_CUDA;
+    if (!make_dw(&ts.dWpost, ts.a_post(ws), 128, B16(ts.off_du16[0]), Md, Md, Mp)) return SMD_ERR_CUDA;
+    if (!make_dx(&ts.dXpost, B16(ts.off_du16[0]), Md, Wsh("post.kernel"), 128, Mp)) return SMD_ERR_CUDA;
     ts.dW2.resize(ts.L); ts.dX2.resize(ts.L); ts.dW1.resize(ts.L); ts.dX1.resize(ts.L);
     ts.dWo.resize(ts.L); ts.dXo.resize(ts.L); ts.dWqkv.resize(ts.L); ts.dXqkv.resize(ts.L);
     for (int l = 0; l < ts.L; ++l) {
-      if (!make_dw(&ts.dW2[l], ts.hidden(ws, l), Md, B16(ts.off_dh16a[l]), 128, 128, Mp, cg)) return SMD_ERR_CUDA;
-      if (!make_dx(&ts.dX2[l], B16(ts.off_dh16a[l]), 128, Wsh(LN(l) + "ffn2.kernel"), Md, Mp, cg)) return SMD_ERR_CUDA;
-      if (!make_dw(&ts.dW1[l], ts.a2(ws, l), 128, B16(ts.off_dr16[l]), Md, Md, Mp, 1)) return SMD_ERR_CUDA;
-      if (!make_dx(&ts.dX1[l], B16(ts.off_dr16[l]), Md, Wsh(LN(l) + "ffn1.kernel"), 128, Mp, cg)) return SMD_ERR_CUDA;
-      if (!make_dw(&ts.dWo[l], ts.o(ws, l), 128, B16(ts.off_dh16b[l]), 128, 128, Mp, 1)) return SMD_ERR_CUDA;
-      if (!make_dx(&ts.dXo[l], B16(ts.off_dh16b[l]), 128, Wsh(LN(l) + "attn.out.kernel"), 128, Mp, cg)) return SMD_ERR_CUDA;
-      if (!make_dw(&ts.dWqkv[l], ts.a1(ws, l), 128, B16(ts.off_dqkv16[l]), 384, 384, Mp, 1)) return SMD_ERR_CUDA;
+      if (!make_dw(&ts.dW2[l], ts.hidden(ws, l), Md, B16(ts.off_dh16a[l]), 128, 128, Mp)) return SMD_ERR_CUDA;
+      if (!make_dx(&ts.dX2[l], B16(ts.off_dh16a[l]), 128, Wsh(LN(l) + "ffn2.kernel"), Md, Mp)) return SMD_ERR_CUDA;
+      if (!make_dw(&ts.dW1[l], ts.a2(ws, l), 128, B16(ts.off_dr16[l]), Md, Md, Mp)) return SMD_ERR_CUDA;
+      if (!make_dx(&ts.dX1[l], B16(ts.off_dr16[l]), Md, Wsh(LN(l) + "ffn1.kernel"), 128, Mp)) return SMD_ERR_CUDA;
+      if (!make_dw(&ts.dWo[l], ts.o(ws, l), 128, B16(ts.off_dh16b[l]), 128, 128, Mp)) return SMD_ERR_CUDA;
+      if (!make_dx(&ts.dXo[l], B16(ts.off_dh16b[l]), 128, Wsh(LN(l) + "attn.out.kernel"), 128, Mp)) return SMD_ERR_CUDA;
+      if (!make_dw(&ts.dWqkv[l], ts.a1(ws, l), 128, B16(ts.off_dqkv16[l]), 384, 384, Mp)) return SMD_ERR_CUDA;
       ts.dWqkv[l].BN = 128;
-      if (!make_dx(&ts.dXqkv[l], B16(ts.off_dqkv16[l]), 384, Wsh(LN(l) + "attn.qkv.kernel"), 128, Mp, cg)) return SMD_ERR_CUDA;
+      if (!make_dx(&ts.dXqkv[l], B16(ts.off_dqkv16[l]), 384, Wsh(LN(l) + "attn.qkv.kernel"), 128, Mp)) return SMD_ERR_CUDA;
     }
   } else {
-    if (!make_dw(&ts.dWin, p->buf<__nv_bfloat16>("xb"), C, B16(ts.off_du16[0]), Md, Md, Mp, cg)) return SMD_ERR_CUDA;
+    if (!make_dw(&ts.dWin, p->buf<__nv_bfloat16>("xb"), C, B16(ts.off_du16[0]), Md, Md, Mp)) return SMD_ERR_CUDA;
   }
   return SMD_OK;
 }
@@ -182,7 +180,7 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
   {
     GemmEpilogue e = epi();
     e.out_f32 = G("out.kernel"); e.ld_f32 = C;
-    const int sp = pick_splits_side(Md, C, ts.dWout.BN, ts.dWout.cg, nkb);
+    const int sp = pick_splits_side(Md, C, ts.dWout.BN, nkb);
     e.atomic_out = sp > 1;
     SMD_CUDA(gemm_k(ts.dWout, Md, Mk, sp, e, dws));
     e = epi();
@@ -294,7 +292,7 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
   {
     GemmEpilogue e = epi();
     e.out_f32 = G("post.kernel"); e.ld_f32 = Md;
-    const int sp = pick_splits_side(128, Md, ts.dWpost.BN, ts.dWpost.cg, nkb);
+    const int sp = pick_splits_side(128, Md, ts.dWpost.BN, nkb);
     e.atomic_out = sp > 1;
     SMD_CUDA(fork_dw());
     SMD_CUDA(gemm_k(ts.dWpost, 128, Mk, sp, e, dws));
@@ -323,28 +321,21 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     SMD_CUDA(fork_dw());
     e = epi();
     e.out_f32 = G(pre + "ffn2.kernel"); e.ld_f32 = 128;
-    int sp = pick_splits_side(Md, 128, ts.dW2[l].BN, ts.dW2[l].cg, nkb);
+    int sp = pick_splits_side(Md, 128, ts.dW2[l].BN, nkb);
     e.atomic_out = sp > 1;
     SMD_CUDA(gemm_k(ts.dW2[l], Md, Mk, sp, e, dws));
     launch_colsum<__nv_bfloat16>(dr16l, Md, G(pre + "ffn1.bias"), M, Md, dws); CNT();
     e = epi();
     e.out_f32 = G(pre + "ffn1.kernel"); e.ld_f32 = Md;
-    sp = pick_splits_side(128, Md, ts.dW1[l].BN, ts.dW1[l].cg, nkb);
+    sp = pick_splits_side(128, Md, ts.dW1[l].BN, nkb);
     e.atomic_out = sp > 1;
     SMD_CUDA(gemm_k(ts.dW1[l], 128, Mk, sp, e, dws));
     e = epi();
     e.out_f32 = da32; e.ld_f32 = 128;
-    const int fsp = ffn_splits(M, ts.dX1[l].cg);
-    const long long fstride = static_cast<long long>(p->Mp < kFfnSplitRows ? p->Mp : kFfnSplitRows) * 128;
-    GemmOp dx1 = ts.dX1[l];
-    if (fsp > 1) {   // K = mlp_dims, 16 output tiles at batch 128: deterministic split-K, ln128_bwd adds the slabs
-      e.out_f32 = p->buf<float>("ffn.slabs"); e.split_stride = fstride;
-      dx1.k_splits = fsp;
-    }
-    SMD_CUDA(launch_gemm(dx1, M, e, st));
+    SMD_CUDA(launch_gemm(ts.dX1[l], M, e, st));
     Ln128BwdArgs a;
     memset(&a, 0, sizeof(a));
-    a.g = e.out_f32; a.g_splits = fsp; a.g_stride = fstride;
+    a.g = da32;
     a.h = ts.h(ws, 2 * l + 1); a.gamma = p->P(params, pre + "ln2.scale");
     a.dres = dh32; a.dx32 = dh32; a.dx16 = B16(ts.off_dh16b[l]);
     a.dgamma = G(pre + "ln2.scale"); a.dbeta = G(pre + "ln2.bias");
@@ -355,7 +346,7 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     SMD_CUDA(fork_dw());
     e = epi();
     e.out_f32 = G(pre + "attn.out.kernel"); e.ld_f32 = 128;
-    sp = pick_splits_side(128, 128, ts.dWo[l].BN, ts.dWo[l].cg, nkb);
+    sp = pick_splits_side(128, 128, ts.dWo[l].BN, nkb);
     e.atomic_out = sp > 1;
     SMD_CUDA(gemm_k(ts.dWo[l], 128, Mk, sp, e, dws));
     e = epi();
@@ -367,7 +358,7 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     SMD_CUDA(fork_dw());
     e = epi();
     e.out_f32 = G(pre + "attn.qkv.kernel"); e.ld_f32 = 384;
-    sp = pick_splits_side(128, 384, ts.dWqkv[l].BN, ts.dWqkv[l].cg, nkb);
+    sp = pick_splits_side(128, 384, ts.dWqkv[l].BN, nkb);
     e.atomic_out = sp > 1;
     SMD_CUDA(gemm_k(ts.dWqkv[l], 128, Mk, sp, e, dws));
     e = epi();

@@ -425,7 +425,7 @@ inline void launch_ln_film_act_bwd(const LnFilmBwdArgs& a, cudaStream_t st) {
 #define SMD_LNB_FAST(U, R, F)                                                                               \
   {                                                                                                          \
     cudaFuncSetAttribute(ln_film_bwd_fast_kernel<U, R, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); \
-    launch_pdl_g(kPdlLnFilmBwd, ln_film_bwd_fast_kernel<U, R, F>, dim3(fb), dim3(threads), smem, st, a);                                          \
+    ln_film_bwd_fast_kernel<U, R, F><<<fb, threads, smem, st>>>(a);                                          \
   }
     switch (key) {
       case 0: SMD_LNB_FAST(false, false, false) break;
@@ -464,10 +464,8 @@ inline void launch_ln_film_act_bwd(const LnFilmBwdArgs& a, cudaStream_t st) {
 // narrow (128-wide) LayerNorm backward, one warp per row; statistics recomputed from the saved input
 // ---------------------------------------------------------------------------------------------------
 struct Ln128BwdArgs {
-  const float* g;       // [M][128] gradient wrt the LayerNorm output; with g_splits > 1 the sum of that many slabs
-  int g_splits;         //   g + s * g_stride (deterministic split-K partials of the producing GEMM), 0 / 1: a single array
-  long long g_stride;
-  const float* h;       // [M][128] LayerNorm input
+  const float* g;       // [M][128] gradient wrt the LayerNorm output
+  const float* h;      // [M][128] LayerNorm input
   const float* gamma;   // [128]
   const float* dres;    // [M][128] or null (may alias dx32)
   float* dx32;          // [M][128]
@@ -489,11 +487,7 @@ __global__ void __launch_bounds__(256) ln128_bwd_kernel(const Ln128BwdArgs a) {
   float adg[4] = {0, 0, 0, 0}, adb[4] = {0, 0, 0, 0}, abias[4] = {0, 0, 0, 0};
   for (int row = gw; row < a.M; row += nw) {
     const float4 h4 = *reinterpret_cast<const float4*>(a.h + static_cast<size_t>(row) * 128 + c);
-    float4 g4 = *reinterpret_cast<const float4*>(a.g + static_cast<size_t>(row) * 128 + c);
-    for (int sp = 1; sp < a.g_splits; ++sp) {     // fixed order: bit-reproducible
-      const float4 t = *reinterpret_cast<const float4*>(a.g + sp * a.g_stride + static_cast<size_t>(row) * 128 + c);
-      g4.x += t.x; g4.y += t.y; g4.z += t.z; g4.w += t.w;
-    }
+    const float4 g4 = *reinterpret_cast<const float4*>(a.g + static_cast<size_t>(row) * 128 + c);
     const float hh[4] = {h4.x, h4.y, h4.z, h4.w};
     const float gg[4] = {g4.x, g4.y, g4.z, g4.w};
     float s1 = hh[0] + hh[1] + hh[2] + hh[3];
@@ -546,7 +540,7 @@ __global__ void __launch_bounds__(256) ln128_bwd_kernel(const Ln128BwdArgs a) {
 inline void launch_ln128_bwd(const Ln128BwdArgs& a, cudaStream_t st) {
   int blocks = (a.M + 7) / 8;
   if (blocks > 148 * 2) blocks = 148 * 2;
-  launch_pdl_g(kPdlLn128, ln128_bwd_kernel, dim3(blocks), dim3(256), 0, st, a);
+  ln128_bwd_kernel<<<blocks, 256, 0, st>>>(a);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -931,15 +925,15 @@ inline cudaError_t launch_attention_bwd(const float* qkv, const float* probs, co
   while (hpb > 4 && hpb % 2 == 0) hpb /= 2;
   const size_t smem = (4 * 32 * static_cast<size_t>(hpb) * dh + static_cast<size_t>(hpb) * 32 * 33) * sizeof(float);
   const dim3 grid(B, H / hpb);
-  static const bool simt = [] { const char* v = getenv("SMD_ATTENTION_SIMT"); return v && v[0] == '1'; }();
-  if (!simt && dh % 8 == 0 && dh <= 32) {
+  if (dh % 8 == 0 && dh <= 32) {
     const size_t sm2 = (4 * 32 * static_cast<size_t>(hpb * dh + 4) + static_cast<size_t>(hpb) * 32 * 36) * sizeof(uint32_t);
 #define SMD_ATT_BWD_MMA(DHV)                                                                                        \
   {                                                                                                                 \
     cudaError_t e = cudaFuncSetAttribute(attention_bwd_mma_kernel<DHV>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
                                          static_cast<int>(sm2));                                                    \
     if (e != cudaSuccess) return e;                                                                                 \
-    return launch_pdl_g(kPdlAttention, attention_bwd_mma_kernel<DHV>, grid, dim3(hpb * 32), sm2, st, qkv, probs, dO, dqkv16, dbias, H); \
+    attention_bwd_mma_kernel<DHV><<<grid, hpb * 32, sm2, st>>>(qkv, probs, dO, dqkv16, dbias, H);                   \
+    return cudaPeekAtLastError();                                                                                   \
   }
     if (dh == 16) SMD_ATT_BWD_MMA(16)
     else if (dh == 8) SMD_ATT_BWD_MMA(8)
@@ -951,7 +945,7 @@ inline cudaError_t launch_attention_bwd(const float* qkv, const float* probs, co
     cudaError_t e = cudaFuncSetAttribute(attention_bwd_kernel<DHV>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                                          static_cast<int>(smem));                                              \
     if (e != cudaSuccess) return e;                                                                            \
-    launch_pdl_g(kPdlAttention, attention_bwd_kernel<DHV>, dim3(grid), dim3(hpb * 32), smem, st, qkv, probs, dO, dqkv16, dbias, H);                       \
+    attention_bwd_kernel<DHV><<<grid, hpb * 32, smem, st>>>(qkv, probs, dO, dqkv16, dbias, H);                 \
   }
   if (dh == 16) SMD_ATT_BWD(16)
   else if (dh == 8) SMD_ATT_BWD(8)
@@ -1011,7 +1005,7 @@ embed_bwd_kernel(const float* __restrict__ x, const float* __restrict__ dh, floa
   }
 }
 inline void launch_embed_bwd(const float* x, const float* dh, float* dW, int M, int C, cudaStream_t st) {
-  launch_pdl_g(kPdlMisc, embed_bwd_kernel, dim3((M + 127) / 128), dim3(256), 0, st, x, dh, dW, M, C);
+  embed_bwd_kernel<<<(M + 127) / 128, 256, 0, st>>>(x, dh, dW, M, C);
 }
 
 // small fp32 linear layers of the FiLM generator: weight gradient and input gradient (tiled SGEMM, kernels.cu)
@@ -1074,24 +1068,6 @@ ddpm_loss_bwd_kernel(const float* __restrict__ eps, const float* __restrict__ pr
     acc = warp_sum(acc);
     if (threadIdx.x == 0) { loss_sum[0] = acc; loss_sum[1] = acc * inv_global_batch; }
   }
-}
-
-// bf16 dst[r][0..cols) = src[r][0..cols), dst row pitch ld (padding columns untouched)
-__global__ void cast_pad_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, int rows, int cols,
-                                     int ld) {
-  const size_t total = static_cast<size_t>(rows) * cols;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const size_t r = i / cols, c = i % cols;
-    dst[r * ld + c] = __float2bfloat16_rn(src[i]);
-  }
-}
-inline void launch_cast_pad_bf16(const float* src, __nv_bfloat16* dst, int rows, int cols, int ld, cudaStream_t st) {
-  const size_t total = static_cast<size_t>(rows) * cols;
-  int blocks = static_cast<int>((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
-  if (blocks < 1) blocks = 1;
-  cast_pad_bf16_kernel<<<blocks, 256, 0, st>>>(src, dst, rows, cols, ld);
 }
 
 }  // namespace smd

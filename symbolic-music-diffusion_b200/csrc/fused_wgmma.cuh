@@ -5,7 +5,7 @@
 //       GEMM1_j : acc1 = A[64 x 128] . W1[:, chunk j]        (wgmma, both operands from shared memory, K = 128)
 //       epi1_j  : + b1 -> gelu -> bf16, in registers.  The m64 x n128 accumulator fragment rounded to bf16 is exactly the
 //                 register A-operand fragment of an m64 x k16 wgmma, so the hidden activation never leaves the
-//                 registers (training additionally streams it out, pre- and post-GELU, for the backward pass)
+//                 registers
 //       GEMM2_j : acc2 += H_j[64 x 128] . W2[chunk j, :]    (wgmma, A from registers, K = 128)
 //
 //   attn_block_kernel : h_mid = SelfAttention(a) + h_in ;  a2 = LayerNorm(h_mid)
@@ -14,7 +14,7 @@
 //       attention: one warp per head, lane = query, fp32 scores / max-subtracted softmax / P V (the same arithmetic as
 //                  attention_kernel in kernels.cu) -> o as bf16, written in the K-major SWIZZLE_128B operand layout
 //       GEMM out : O[64 x 128] . Wo (wgmma from shared memory)
-//     q, k and v never leave the SM (training additionally stores q | k | v, the probabilities and o).
+//     q, k and v never leave the SM.
 //
 // Both: warp 0 is the TMA producer (activation tile once per tile, 32 KB weight blocks through a small mbarrier ring,
 // re-read from L2 for every tile), the consumer warpgroups run the wgmma chains and the epilogues, and the final
@@ -98,8 +98,6 @@ struct FfnFusedArgs {
   const float* ln_gamma;         // [128] LayerNorm applied to the new residual stream -> out_bf16
   const float* ln_beta;
   __nv_bfloat16* out_bf16;       // bf16 [M][128]
-  __nv_bfloat16* hidden_pre;     // bf16 [M][Md] pre-GELU (training) or null
-  __nv_bfloat16* hidden;         // bf16 [M][Md] post-GELU (training) or null
   int M, Md;
 };
 
@@ -115,7 +113,9 @@ struct FfnSmem {
   static constexpr int kThreads = 128 + 256;   // producer warpgroup (warp 0 works) + two consumer warpgroups
 };
 
-template <bool kTrain>
+// kAct: the activation between the two GEMMs (ACT_GELU_TANH in the model).  A template parameter, like those of every
+// kernel defined in a header that several translation units include.
+template <int kAct>
 __global__ void __launch_bounds__(FfnSmem::kThreads, 1)
 ffn_fused_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW1,
                  const __grid_constant__ CUtensorMap tmW2, const FfnFusedArgs p) {
@@ -187,17 +187,10 @@ ffn_fused_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (++ws == S::kStages) { ws = 0; wph ^= 1u; }
 #pragma unroll
           for (int i = 0; i < 64; i += 2) {
-            const int col = 128 * j + 8 * (i >> 2) + c, r = row + 8 * ((i >> 1) & 1);
+            const int col = 128 * j + 8 * (i >> 2) + c;
             const float2 b = __ldg(reinterpret_cast<const float2*>(p.b1 + col));
             const float v0 = acc1[i] + b.x, v1 = acc1[i + 1] + b.y;
-            hr[i >> 1] = pack_bf16x2(act_apply(v0, ACT_GELU_TANH), act_apply(v1, ACT_GELU_TANH));
-            if constexpr (kTrain) {
-              if (r < p.M) {
-                const size_t off = static_cast<size_t>(r) * p.Md + col;
-                if (p.hidden_pre) *reinterpret_cast<uint32_t*>(p.hidden_pre + off) = pack_bf16x2(v0, v1);
-                if (p.hidden) *reinterpret_cast<uint32_t*>(p.hidden + off) = hr[i >> 1];
-              }
-            }
+            hr[i >> 1] = pack_bf16x2(act_apply(v0, kAct), act_apply(v1, kAct));
           }
         }
         mbar_wait(&w_full[ws], wph);
@@ -231,10 +224,6 @@ struct AttnBlockArgs {
   const float* ln_gamma;         // [128] LayerNorm of the new residual stream -> out_bf16
   const float* ln_beta;
   __nv_bfloat16* out_bf16;       // bf16 [M][128]
-  // training (kTrain): what the backward pass needs (csrc/backward.cu), in the layouts of the three-launch path
-  float* qkv_out;                // fp32 [M][384] = (q | k | v) + bias, q unscaled
-  float* probs_out;              // fp32 [M / 32][H][32][32] softmax probabilities
-  __nv_bfloat16* o_out;          // bf16 [M][128] attention output (operand of the out-projection's weight gradient)
   int M, H;                      // tokens (a multiple of 32); heads (dh = 128 / H in {8, 16})
 };
 
@@ -256,7 +245,7 @@ struct AttnSmem {
   static_assert(offO % 1024 == 0, "O operand must be 1024-byte aligned");
 };
 
-template <int DH, bool kTrain>
+template <int DH>
 __global__ void __launch_bounds__(AttnSmem::kThreads, 1)
 attn_block_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmWqkv,
                   const __grid_constant__ CUtensorMap tmWo, const AttnBlockArgs p) {
@@ -327,11 +316,7 @@ attn_block_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         for (int i = 0; i < 64; i += 2) {
           const int col = 128 * w + 8 * (i >> 2) + c, lr = lrow + 8 * ((i >> 1) & 1);
           const float2 b = __ldg(reinterpret_cast<const float2*>(p.b_qkv + col));
-          const float2 v = make_float2(acc[i] + b.x, acc[i + 1] + b.y);
-          *reinterpret_cast<float2*>(qkv_s + lr * S::kQkvPitch + col) = v;
-          if constexpr (kTrain) {
-            if (m0 + lr < p.M) *reinterpret_cast<float2*>(p.qkv_out + static_cast<size_t>(m0 + lr) * 384 + col) = v;
-          }
+          *reinterpret_cast<float2*>(qkv_s + lr * S::kQkvPitch + col) = make_float2(acc[i] + b.x, acc[i + 1] + b.y);
         }
       }
       asm volatile("bar.sync 1, 128;" ::: "memory");
@@ -370,7 +355,6 @@ attn_block_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
           for (int j = 0; j < 32; ++j) {
             const float pj = sc[j] * inv;
-            sc[j] = pj;
             const float4* vr = reinterpret_cast<const float4*>(base + j * S::kQkvPitch + 256 + h * DH);
 #pragma unroll
             for (int d4 = 0; d4 < DH / 4; ++d4) {
@@ -383,16 +367,9 @@ attn_block_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
           for (int d = 0; d < DH; d += 2) {
             const int col = h * DH + d;
-            const uint32_t ob = pack_bf16x2(o[d], o[d + 1]);
             // K-major SWIZZLE_128B: 16-byte chunk (col % 64) / 8 of row orow sits at chunk ^ (orow & 7)
             *reinterpret_cast<uint32_t*>(o_s + (col >> 6) * 8192 + orow * 128 + ((((col & 63) >> 3) ^ (orow & 7)) << 4) +
-                                         (col & 7) * 2) = ob;
-            if constexpr (kTrain) *reinterpret_cast<uint32_t*>(p.o_out + static_cast<size_t>(m0 + orow) * 128 + col) = ob;
-          }
-          if constexpr (kTrain) {
-            float* pr = p.probs_out + ((static_cast<size_t>(smp) * p.H + h) * 32 + lane) * 32;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(pr + j) = make_float4(sc[j], sc[j + 1], sc[j + 2], sc[j + 3]);
+                                         (col & 7) * 2) = pack_bf16x2(o[d], o[d + 1]);
           }
         }
       }

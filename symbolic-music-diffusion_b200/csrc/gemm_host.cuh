@@ -9,7 +9,6 @@
 #include <string>
 #include "gemm_wgmma.cuh"
 #include "fused_wgmma.cuh"
-#include "pdl_launch.cuh"
 
 namespace smd {
 
@@ -50,29 +49,27 @@ struct GemmOp {
   CUtensorMap tmA, tmB;
   CUtensorMap tmA_lo, tmB_lo;   // strict-precision mode: the lo halves of both operands (has_lo)
   bool has_lo = false;
-  int N = 0, K = 0, BN = 0, cg = 1, a_mn = 0, b_mn = 0, k_splits = 1;
+  int N = 0, K = 0, BN = 0, a_mn = 0, b_mn = 0, k_splits = 1;
 };
 
-inline int choose_bn(int N, int /*cg*/) {
+inline int choose_bn(int N) {
   if (N % kBNMax == 0 || N > kBNMax) return kBNMax;
   return ((N + 15) / 16) * 16;
 }
 
 // A: K-major [a_rows][K] (a_mn=0) or MN-major [K][a_rows] (a_mn=1); same for B with N rows.
-// Every tile is computed by one CTA (sm_90 has no paired-CTA MMA): `cg` is accepted for interface compatibility and the
-// op is recorded as cg = 1.  A requested BN above kBNMax is lowered to kBNMax (the widest accumulator tile).
+// A requested BN above kBNMax is lowered to kBNMax (the widest accumulator tile).
 inline bool make_gemm_op(GemmOp* op, const void* A, uint64_t a_rows, const void* B, uint64_t b_rows_total, int N,
-                         int K, int BN, int cg, int a_mn, int b_mn, uint64_t k_rows_a = 0, uint64_t k_rows_b = 0,
+                         int K, int BN, int a_mn, int b_mn, uint64_t k_rows_a = 0, uint64_t k_rows_b = 0,
                          size_t lo_bytes = 0) {
   if (lo_bytes) {
     GemmOp lo;
     if (!make_gemm_op(&lo, static_cast<const uint8_t*>(A) + lo_bytes, a_rows, static_cast<const uint8_t*>(B) + lo_bytes,
-                      b_rows_total, N, K, BN, cg, a_mn, b_mn, k_rows_a, k_rows_b, 0)) return false;
+                      b_rows_total, N, K, BN, a_mn, b_mn, k_rows_a, k_rows_b, 0)) return false;
     op->tmA_lo = lo.tmA; op->tmB_lo = lo.tmB; op->has_lo = true;
   }
-  if (cg != 1 && cg != 2) { set_error("cta_group must be 1 or 2"); return false; }
   if (BN > kBNMax) BN = kBNMax;
-  op->N = N; op->K = K; op->BN = BN; op->cg = 1; op->a_mn = a_mn; op->b_mn = b_mn; op->k_splits = 1;
+  op->N = N; op->K = K; op->BN = BN; op->a_mn = a_mn; op->b_mn = b_mn; op->k_splits = 1;
   if (K % 64 != 0) { set_error("GEMM K must be a multiple of 64"); return false; }
   if (BN % 16 != 0 || BN < 16) { set_error("bad BN " + std::to_string(BN)); return false; }
   if (b_mn && BN % 64 != 0) { set_error("MN-major B needs BN % 64 == 0"); return false; }
@@ -133,7 +130,14 @@ inline int gemm_tiles(const GemmOp& op, int M) {
   return ((M + kBM - 1) / kBM) * ((op.N + op.BN - 1) / op.BN) * gemm_k_splits(op);
 }
 
-// persistent grid of min(#SMs, tiles) CTAs, programmatic dependent launch when enabled
+// SMD_PDL=0 launches the persistent kernels without programmatic dependent launch.  That is faster for the sampler's
+// forward passes and slower for the train step, so it stays selectable until the code makes that choice itself.
+inline bool pdl_enabled() {
+  static const bool on = [] { const char* v = getenv("SMD_PDL"); return !(v && v[0] == '0'); }();
+  return on;
+}
+
+// persistent grid of min(#SMs, tiles) CTAs, programmatic dependent launch unless SMD_PDL=0
 template <typename Kern, typename... Args>
 inline cudaError_t launch_persistent(Kern kern, int tiles, int threads, int smem, cudaStream_t st, const Args&... args) {
   int grid = device_sm_count();
@@ -211,6 +215,8 @@ inline cudaError_t launch_gemm_ew(int ew, const GemmOp& op, int M, const GemmEpi
 inline cudaError_t launch_gemm(const GemmOp& op, int M, const GemmEpilogue& ep, cudaStream_t st) {
   // full-row LayerNorm needs the whole row in one tile (N <= BN; BN is at most kBNMax)
   if (ep.ln_gamma != nullptr && op.N > op.BN) return cudaErrorInvalidValue;
+  // the K splits of a tile add into the same output elements
+  if (gemm_k_splits(op) > 1 && !ep.atomic_out) return cudaErrorInvalidValue;
   const GemmKind k = gemm_kind(op, M, ep);
   switch (k.flags) {
     case kEpiStrict: return launch_gemm_inst<kEpiStrict>(op, M, ep, st);
@@ -238,29 +244,16 @@ inline bool make_ffn_op(FfnOp* op, const void* A, uint64_t rows, const void* W1,
            make_tmap_bf16(&op->tmW2, W2, static_cast<uint64_t>(Md), 128, 64);
   return op->ok;
 }
-inline bool ffn_fused_enabled() {
-  static const bool on = [] { const char* v = getenv("SMD_FFN_FUSED"); return !(v && v[0] == '0'); }();
-  return on;
-}
-// SMD_FFN_FUSED=2: use the fused kernel at every size and in training too (tests)
-inline bool ffn_fused_forced() {
-  static const bool on = [] { const char* v = getenv("SMD_FFN_FUSED"); return v && v[0] == '2'; }();
-  return on;
-}
 inline cudaError_t launch_ffn_fused(const FfnOp& op, const FfnFusedArgs& a, cudaStream_t st) {
   if (a.Md % 128 != 0) return cudaErrorInvalidValue;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(ffn_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FfnSmem::kTotal);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(ffn_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FfnSmem::kTotal);
+    cudaError_t e = cudaFuncSetAttribute(ffn_fused_kernel<ACT_GELU_TANH>, cudaFuncAttributeMaxDynamicSharedMemorySize, FfnSmem::kTotal);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
   const int tiles = (a.M + 127) / 128;
-  if (a.hidden_pre != nullptr || a.hidden != nullptr)
-    return launch_persistent(ffn_fused_kernel<true>, tiles, FfnSmem::kThreads, FfnSmem::kTotal, st, op.tmA, op.tmW1, op.tmW2, a);
-  return launch_persistent(ffn_fused_kernel<false>, tiles, FfnSmem::kThreads, FfnSmem::kTotal, st, op.tmA, op.tmW1, op.tmW2, a);
+  return launch_persistent(ffn_fused_kernel<ACT_GELU_TANH>, tiles, FfnSmem::kThreads, FfnSmem::kTotal, st, op.tmA, op.tmW1, op.tmW2, a);
 }
 
 
@@ -272,48 +265,26 @@ struct AttnOp {
   bool ok = false;
 };
 // A: bf16 [rows][128] K-major (64-row tiles); Wqkv: bf16 (128, 384) row-major; Wo: bf16 (128, 128) row-major
-inline bool make_attn_a(CUtensorMap* tm, const void* A, uint64_t rows) { return make_tmap_bf16(tm, A, rows, 128, 64); }
 inline bool make_attn_op(AttnOp* op, const void* A, uint64_t rows, const void* Wqkv, const void* Wo) {
-  op->ok = make_attn_a(&op->tmA, A, rows) && make_tmap_bf16(&op->tmWqkv, Wqkv, 128, 384, 64) &&
+  op->ok = make_tmap_bf16(&op->tmA, A, rows, 128, 64) && make_tmap_bf16(&op->tmWqkv, Wqkv, 128, 384, 64) &&
            make_tmap_bf16(&op->tmWo, Wo, 128, 128, 64);
   return op->ok;
-}
-// SMD_ATTN_BLOCK=0 keeps the three-launch path (QKV GEMM, attention kernel, out-projection GEMM)
-inline bool attn_block_enabled() {
-  static const bool on = [] { const char* v = getenv("SMD_ATTN_BLOCK"); return !(v && v[0] == '0'); }();
-  return on;
-}
-// SMD_ATTN_BLOCK_TRAIN=1: the training forward uses the block kernel too (q | k | v, probabilities and the attention
-// output are written out for the backward pass).  Off by default (not measured against the three-launch path on H100).
-inline bool attn_block_train_enabled() {
-  static const bool on = [] { const char* v = getenv("SMD_ATTN_BLOCK_TRAIN"); return v && v[0] == '1'; }();
-  return on;
 }
 inline cudaError_t launch_attn_block(const AttnOp& op, const AttnBlockArgs& a, cudaStream_t st) {
   const int dh = 128 / a.H;
   if ((dh != 8 && dh != 16) || a.M % 32 != 0) return cudaErrorInvalidValue;
-  const bool train = a.qkv_out != nullptr;
-  if (train && (a.probs_out == nullptr || a.o_out == nullptr)) return cudaErrorInvalidValue;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_block_kernel<16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem::kTotal);
+    cudaError_t e = cudaFuncSetAttribute(attn_block_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem::kTotal);
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(attn_block_kernel<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem::kTotal);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(attn_block_kernel<16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem::kTotal);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(attn_block_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem::kTotal);
+    e = cudaFuncSetAttribute(attn_block_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem::kTotal);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
   const int tiles = (a.M + 63) / 64;
   const int T = AttnSmem::kThreads, B = AttnSmem::kTotal;
-  if (train) {
-    if (dh == 16) return launch_persistent(attn_block_kernel<16, true>, tiles, T, B, st, op.tmA, op.tmWqkv, op.tmWo, a);
-    return launch_persistent(attn_block_kernel<8, true>, tiles, T, B, st, op.tmA, op.tmWqkv, op.tmWo, a);
-  }
-  if (dh == 16) return launch_persistent(attn_block_kernel<16, false>, tiles, T, B, st, op.tmA, op.tmWqkv, op.tmWo, a);
-  return launch_persistent(attn_block_kernel<8, false>, tiles, T, B, st, op.tmA, op.tmWqkv, op.tmWo, a);
+  if (dh == 16) return launch_persistent(attn_block_kernel<16>, tiles, T, B, st, op.tmA, op.tmWqkv, op.tmWo, a);
+  return launch_persistent(attn_block_kernel<8>, tiles, T, B, st, op.tmA, op.tmWqkv, op.tmWo, a);
 }
 
 }  // namespace smd

@@ -53,8 +53,6 @@ struct GemmEpilogue {
   int ld_res;
   float* out_f32;               // fp32 [M][ld_f32] <- v, or null
   int ld_f32;
-  long long split_stride;       // k_splits > 1 without atomics: split s stores its partial at out_f32 + s * split_stride
-                                // (floats); the consumer adds the slabs in a fixed order (deterministic split-K)
   __nv_bfloat16* out_bf16;      // bf16 [M][ld_bf16] <- act(v)   (or LayerNorm(v) when ln_gamma != null), or null
   int ld_bf16;
   int act;                      // activation applied on the bf16 output path
@@ -79,7 +77,7 @@ struct GemmShape {
   int M, N, K;     // logical problem; K % 64 == 0
   int BN;          // n-tile width: multiple of 16, <= kBNMax
   int a_mn, b_mn;  // 0: operand is K-major ([rows][K], K contiguous); 1: MN-major ([K][rows], rows contiguous)
-  int k_splits;    // >= 1: the K loop is cut into this many independent tiles (needs atomic_out or split_stride when > 1)
+  int k_splits;    // >= 1: the K loop is cut into this many independent tiles (needs atomic_out when > 1)
 };
 
 static constexpr int kBM = 128;
@@ -380,10 +378,12 @@ __device__ __forceinline__ void gemm_mainloop(float (&d)[64], uint8_t* smem, int
   if (prev >= 0 && releaser) mbar_arrive(&empty_bar[prev]);
 }
 
+// (ep is __grid_constant__ like the tensor maps: its fields are read in place from parameter space; without it ptxas
+// allocates the 8- and 12-warp epilogue kinds with more spills)
 template <uint32_t kF, int kEW = 8>
 __global__ void __launch_bounds__(GemmSmem<kEW>::kThreads, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                       const GemmShape sh, const GemmEpilogue ep) {
+                       const GemmShape sh, const __grid_constant__ GemmEpilogue ep) {
   using SM = GemmSmem<kEW>;
   constexpr bool kDedicated = SM::kDedicated;
   constexpr int kGroups = SM::kEpiGroups;
@@ -567,7 +567,6 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       }
       const int mn = tile / splits;
       const bool first_split = (tile % splits) == 0;
-      float* const out_f32_s = ep.out_f32 ? ep.out_f32 + static_cast<long long>(tile % splits) * ep.split_stride : nullptr;
       const int row_base = (mn / num_n) * rows_per_tile + static_cast<int>(q * 32u);
       const int row = row_base + static_cast<int>(lane);
       const int n0 = (mn % num_n) * BN;
@@ -703,7 +702,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                 for (int it = 0; it < 8; ++it) {
                   const int rr = it * 4 + f_r, grow = row_base + rr;
                   float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
-                  if (grow < sh.M) t = *reinterpret_cast<const float4*>(out_f32_s + static_cast<size_t>(grow) * ep.ld_f32 + col0 + f_c);
+                  if (grow < sh.M) t = *reinterpret_cast<const float4*>(ep.out_f32 + static_cast<size_t>(grow) * ep.ld_f32 + col0 + f_c);
                   float* d = scr + rr * 33 + f_c;
                   d[0] = t.x; d[1] = t.y; d[2] = t.z; d[3] = t.w;
                 }
@@ -754,7 +753,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                   if (has_stats || do_ln) chunk_stats(v, s1, s2);
                 }
                 if constexpr (H_F32) {
-                  if (has_f32) store_f32_chunk(scr, v, lane, row_base, sh.M, out_f32_s, ep.ld_f32, col0, H_ATOMIC && atomic_out);
+                  if (has_f32) store_f32_chunk(scr, v, lane, row_base, sh.M, ep.out_f32, ep.ld_f32, col0, H_ATOMIC && atomic_out);
                 }
                 if constexpr (H_PRE) {
                   if (has_pre) {
@@ -789,7 +788,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
               // ------------------------------ slow path: ragged / unaligned chunk (row per thread) -------------
               if (!row_ok) continue;
               if (reload) {
-                const float* op = out_f32_s + static_cast<size_t>(row) * ep.ld_f32 + col0;
+                const float* op = ep.out_f32 + static_cast<size_t>(row) * ep.ld_f32 + col0;
 #pragma unroll
                 for (int i = 0; i < 32; ++i)
                   if (i < ncols && col0 + i < sh.N) v[i] = op[i];
@@ -819,7 +818,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                     if (i < ncols && col0 + i < sh.N) { s1 += v[i]; s2 += v[i] * v[i]; }
                 }
                 if (has_f32) {
-                  float* op = out_f32_s + static_cast<size_t>(row) * ep.ld_f32 + col0;
+                  float* op = ep.out_f32 + static_cast<size_t>(row) * ep.ld_f32 + col0;
 #pragma unroll
                   for (int i = 0; i < 32; ++i) {
                     if (i < ncols && col0 + i < sh.N) {

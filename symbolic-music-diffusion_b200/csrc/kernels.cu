@@ -42,7 +42,7 @@ void launch_q_sample(const float* x0, const float* eps, const float* used_alpha,
   const size_t total = static_cast<size_t>(B) * per_sample;
   int blocks = static_cast<int>((total + 255) / 256);
   if (blocks > 148 * 8) blocks = 148 * 8;
-  launch_pdl_g(kPdlMisc, q_sample_kernel, dim3(blocks), dim3(256), 0, st, x0, eps, used_alpha, xt, cond, B, per_sample, ind, mode);
+  q_sample_kernel<<<blocks, 256, 0, st>>>(x0, eps, used_alpha, xt, cond, B, per_sample, ind, mode);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -167,13 +167,12 @@ void launch_embed(const float* x, const float* W_in, const float* b_in, const fl
   if (C <= 64 && (reinterpret_cast<uintptr_t>(W_in) & 15u) == 0) {
     int blocks = (M + 31) / 32;
     if (blocks > 148 * 4) blocks = 148 * 4;
-    launch_pdl_g(kPdlMisc, embed_smem_kernel<4>, dim3(blocks), dim3(256), static_cast<size_t>(C) * 128 * sizeof(float), st, x, W_in,
-                 b_in, posenc, ln_g, ln_b, h, a, M, C, S, lo_delta);
+    embed_smem_kernel<4><<<blocks, 256, static_cast<size_t>(C) * 128 * sizeof(float), st>>>(x, W_in, b_in, posenc, ln_g,
+                                                                                          ln_b, h, a, M, C, S, lo_delta);
     return;
   }
   const int blocks = (M + 7) / 8;
-  launch_pdl_g(kPdlMisc, embed_kernel, dim3(blocks), dim3(256), 0, st, x, W_in, b_in, posenc, ln_g, ln_b, h, a, M, C, S,
-               lo_delta);
+  embed_kernel<<<blocks, 256, 0, st>>>(x, W_in, b_in, posenc, ln_g, ln_b, h, a, M, C, S, lo_delta);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -392,8 +391,7 @@ void launch_attention(const float* qkv, __nv_bfloat16* o, float* probs_or_null, 
   while (hpb > 4 && hpb % 2 == 0) hpb /= 2;
   const dim3 grid(B, H / hpb);
   const int threads = hpb * 32;
-  static const bool simt = [] { const char* v = getenv("SMD_ATTENTION_SIMT"); return v && v[0] == '1'; }();
-  if (!simt && lo_delta == 0 && dh % 8 == 0 && dh <= 32) {   // (strict mode: fp32 SIMT attention, no tf32 rounding)
+  if (lo_delta == 0 && dh % 8 == 0 && dh <= 32) {   // (strict mode: fp32 SIMT attention, no tf32 rounding)
     const size_t smem = 3 * 32 * static_cast<size_t>(hpb * dh + 4) * sizeof(uint32_t);
 #define SMD_ATT_MMA(DHV)                                                                                          \
   {                                                                                                               \
@@ -402,7 +400,7 @@ void launch_attention(const float* qkv, __nv_bfloat16* o, float* probs_or_null, 
       cudaFuncSetAttribute(attention_mma_kernel<DHV>, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * 32 * 132 * 4); \
       attr = true;                                                                                                \
     }                                                                                                             \
-    launch_pdl_g(kPdlAttention, attention_mma_kernel<DHV>, grid, dim3(threads), smem, st, qkv, o, probs_or_null, B, H);            \
+    attention_mma_kernel<DHV><<<grid, threads, smem, st>>>(qkv, o, probs_or_null, B, H);                          \
   }
     if (dh == 16) SMD_ATT_MMA(16)
     else if (dh == 8) SMD_ATT_MMA(8)
@@ -410,10 +408,10 @@ void launch_attention(const float* qkv, __nv_bfloat16* o, float* probs_or_null, 
 #undef SMD_ATT_MMA
     return;
   }
-  if (dh == 16) launch_pdl_g(kPdlAttention, attention_kernel<16>, dim3(grid), dim3(threads), 0, st, qkv, o, probs_or_null, B, H, lo_delta);
-  else if (dh == 8) launch_pdl_g(kPdlAttention, attention_kernel<8>, dim3(grid), dim3(threads), 0, st, qkv, o, probs_or_null, B, H, lo_delta);
-  else if (dh == 32) launch_pdl_g(kPdlAttention, attention_kernel<32>, dim3(grid), dim3(threads), 0, st, qkv, o, probs_or_null, B, H, lo_delta);
-  else if (dh == 4) launch_pdl_g(kPdlAttention, attention_kernel<4>, dim3(grid), dim3(threads), 0, st, qkv, o, probs_or_null, B, H, lo_delta);
+  if (dh == 16) attention_kernel<16><<<grid, threads, 0, st>>>(qkv, o, probs_or_null, B, H, lo_delta);
+  else if (dh == 8) attention_kernel<8><<<grid, threads, 0, st>>>(qkv, o, probs_or_null, B, H, lo_delta);
+  else if (dh == 32) attention_kernel<32><<<grid, threads, 0, st>>>(qkv, o, probs_or_null, B, H, lo_delta);
+  else if (dh == 4) attention_kernel<4><<<grid, threads, 0, st>>>(qkv, o, probs_or_null, B, H, lo_delta);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -580,7 +578,7 @@ void launch_ln_film_act(const float* u, const float* stats, const float* g, cons
       cudaFuncSetAttribute(ln_film_act_kernel<MAXT, BF>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 4 * 4096 * 4 + 64); \
       attr = true;                                                                                               \
     }                                                                                                            \
-    launch_pdl_g(kPdlLnFilmFwd, ln_film_act_kernel<MAXT, BF>, dim3(blocks), dim3(threads), smem, st, in, stats, g, b, scale, shift, film_ld, film_bcast, act, \
+    ln_film_act_kernel<MAXT, BF><<<blocks, threads, smem, st>>>(in, stats, g, b, scale, shift, film_ld, film_bcast, act, \
                                                                 out, M, N, S, film_row_dev, lo_delta, part, nslots, stats_out); \
   }
   if (threads <= 512) {
@@ -708,69 +706,6 @@ void launch_small_linear(const float* x, const float* W, const float* b, float* 
 // ---------------------------------------------------------------------------------------------------
 // weight packing
 // ---------------------------------------------------------------------------------------------------
-__global__ void pack_transpose_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, int K, int N) {
-  __shared__ float tile[32][33];
-  const int k0 = blockIdx.y * 32, n0 = blockIdx.x * 32;
-  for (int i = threadIdx.y; i < 32; i += 8) {
-    const int k = k0 + i, n = n0 + threadIdx.x;
-    tile[i][threadIdx.x] = (k < K && n < N) ? src[static_cast<size_t>(k) * N + n] : 0.f;
-  }
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += 8) {
-    const int n = n0 + i, k = k0 + threadIdx.x;
-    if (n < N && k < K) dst[static_cast<size_t>(n) * K + k] = __float2bfloat16_rn(tile[threadIdx.x][i]);
-  }
-}
-void launch_pack_transpose_bf16(const float* src, __nv_bfloat16* dst, int K, int N, cudaStream_t st) {
-  dim3 grid((N + 31) / 32, (K + 31) / 32), block(32, 8);
-  pack_transpose_bf16_kernel<<<grid, block, 0, st>>>(src, dst, K, N);
-}
-// ---------------------------------------------------------------------------------------------------
-// split-K tail of the FFN-down projection at small token counts: the GEMM leaves `splits` fp32 partial slabs
-// [M][128]; this kernel adds them in a fixed order with bias and residual and emits the next LayerNorm.
-// ---------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-ln128_reduce_fwd_kernel(const float* __restrict__ slabs, int splits, long long stride, const float* __restrict__ bias,
-                        const float* residual, const float* __restrict__ gamma, const float* __restrict__ beta,
-                        float* h_out, __nv_bfloat16* __restrict__ a_out, int M) {
-  pdl_trigger();
-  pdl_wait();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int c = lane * 4;
-  const float4 b4 = *reinterpret_cast<const float4*>(bias + c);
-  const float4 g4 = *reinterpret_cast<const float4*>(gamma + c);
-  const float4 e4 = *reinterpret_cast<const float4*>(beta + c);
-  for (int row = blockIdx.x * 8 + warp; row < M; row += gridDim.x * 8) {
-    const size_t off = static_cast<size_t>(row) * 128 + c;
-    float4 v = *reinterpret_cast<const float4*>(slabs + off);
-    for (int s = 1; s < splits; ++s) {
-      const float4 t = *reinterpret_cast<const float4*>(slabs + s * stride + off);
-      v.x += t.x; v.y += t.y; v.z += t.z; v.w += t.w;
-    }
-    const float4 r = *reinterpret_cast<const float4*>(residual + off);
-    v.x += b4.x + r.x; v.y += b4.y + r.y; v.z += b4.z + r.z; v.w += b4.w + r.w;
-    *reinterpret_cast<float4*>(h_out + off) = v;
-    float s1 = v.x + v.y + v.z + v.w;
-    float s2 = v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
-    s1 = warp_sum(s1); s2 = warp_sum(s2);
-    const float mean = s1 * (1.0f / 128.0f);
-    const float rstd = rsqrtf(s2 * (1.0f / 128.0f) - mean * mean + 1e-6f);   // flax LayerNorm: E[x^2] - E[x]^2, eps 1e-6
-    __nv_bfloat162 p0 = __floats2bfloat162_rn((v.x - mean) * (rstd * g4.x) + e4.x, (v.y - mean) * (rstd * g4.y) + e4.y);
-    __nv_bfloat162 p1 = __floats2bfloat162_rn((v.z - mean) * (rstd * g4.z) + e4.z, (v.w - mean) * (rstd * g4.w) + e4.w);
-    uint2 pk;
-    pk.x = *reinterpret_cast<uint32_t*>(&p0); pk.y = *reinterpret_cast<uint32_t*>(&p1);
-    *reinterpret_cast<uint2*>(a_out + off) = pk;
-  }
-}
-void launch_ln128_reduce_fwd(const float* slabs, int splits, long long stride, const float* bias, const float* residual,
-                             const float* gamma, const float* beta, float* h_out, __nv_bfloat16* a_out, int M,
-                             cudaStream_t st) {
-  int blocks = (M + 7) / 8;
-  if (blocks > 148 * 4) blocks = 148 * 4;
-  launch_pdl_g(kPdlLn128, ln128_reduce_fwd_kernel, dim3(blocks), dim3(256), 0, st, slabs, splits, stride, bias, residual,
-               gamma, beta, h_out, a_out, M);
-}
-
 // All weight repacks of one optimizer step in ONE launch: blockmap[b] = (job, tile) for every 64x64 tile.
 __global__ void __launch_bounds__(256) pack_multi_kernel(const float* __restrict__ params, const PackJob* __restrict__ jobs,
                                                          const int2* __restrict__ blockmap, long long lo_delta) {
@@ -903,7 +838,7 @@ reverse_step_kernel(const ReverseStepArgs a) {
 }
 void launch_reverse_step(const ReverseStepArgs& a, cudaStream_t st) {
   const int NC = a.N * a.C;
-  launch_pdl_g(kPdlMisc, reverse_step_kernel, dim3((4 * NC + 255) / 256), dim3(256), 0, st, a);
+  reverse_step_kernel<<<(4 * NC + 255) / 256, 256, 0, st>>>(a);
 }
 __global__ void step_advance_kernel(int* t_ptr) { *t_ptr -= 1; }
 void launch_step_advance(int* t_ptr, cudaStream_t st) { step_advance_kernel<<<1, 1, 0, st>>>(t_ptr); }
@@ -914,7 +849,7 @@ __global__ void fill_cond_kernel(const float* coef, const int* t_ptr, float* con
   if (i < n) cond[i] = coef[8 * (*t_ptr) + 5];
 }
 void launch_fill_cond(const float* coef, const int* t_ptr, float* cond, int n, cudaStream_t st) {
-  launch_pdl_g(kPdlMisc, fill_cond_kernel, dim3((n + 255) / 256), dim3(256), 0, st, coef, t_ptr, cond, n);
+  fill_cond_kernel<<<(n + 255) / 256, 256, 0, st>>>(coef, t_ptr, cond, n);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -954,8 +889,7 @@ ddpm_loss_kernel(const float* __restrict__ eps, const float* __restrict__ pred, 
 }
 void launch_ddpm_loss(const float* eps, const float* pred, float* loss_per_example, float* dpred_or_null,
                       float gscale, int B, int per_sample, cudaStream_t st, const float* sigma) {
-  launch_pdl_g(kPdlMisc, ddpm_loss_kernel, dim3(B), dim3(256), 0, st, eps, pred, loss_per_example, dpred_or_null, gscale,
-               per_sample, sigma);
+  ddpm_loss_kernel<<<B, 256, 0, st>>>(eps, pred, loss_per_example, dpred_or_null, gscale, per_sample, sigma);
 }
 
 // y[b, :] /= sigma[b]   (DenseNCSN: `output = x / sigmas`, models/ncsn.py:97)

@@ -6,7 +6,6 @@
 #include <stdint.h>
 #include <cstdlib>
 #include "ptx.cuh"
-#include "pdl_launch.cuh"
 
 namespace smd {
 
@@ -153,11 +152,6 @@ void launch_embed(const float* x, const float* W_in, const float* b_in, const fl
 
 // unmasked multi-head self-attention over S = 32 positions (flax.nn.SelfAttention core, models/ncsn.py:161)
 // qkv fp32 [M][3E] -> o bf16 [M][E];  optionally saves the probabilities P [B][H][32][32] fp32 for backward
-// h_out = residual + bias + sum of `splits` split-K slabs of the FFN-down GEMM (fixed order); a_out = LayerNorm(h_out)
-// as bf16 (models/ncsn.py:164-166 followed by the next sub-block's LayerNorm).  One warp per 128-wide row.
-void launch_ln128_reduce_fwd(const float* slabs, int splits, long long stride, const float* bias, const float* residual,
-                             const float* gamma, const float* beta, float* h_out, __nv_bfloat16* a_out, int M,
-                             cudaStream_t st);
 void launch_attention(const float* qkv, __nv_bfloat16* o, float* probs_or_null, int B, int H, cudaStream_t st,
                       long long lo_delta = 0);
 
@@ -183,8 +177,6 @@ void launch_small_linear(const float* x, const float* W, const float* b, float* 
 void launch_sgemm_small(int mode, const float* A, const float* B, const float* bias, float* C, float* pre_out,
                         const float* mul_pre, int M, int N, int K, int act, cudaStream_t st);
 
-// bf16 dst[n][k] = src[k][n]  (fp32 (in,out) Dense kernel -> K-major tensor-core operand)
-void launch_pack_transpose_bf16(const float* src, __nv_bfloat16* dst, int K, int N, cudaStream_t st);
 // one launch for a list of repack jobs (mode 0: transpose to [N][K] with pitch ld; mode 1: plain cast, pitch ld)
 struct PackJob { long long src_off; void* dst; int K, N, mode, ld, tile0, tiles_n; };
 void launch_pack_multi(const float* params, const PackJob* jobs_dev, const void* blockmap_dev, int total_tiles,

@@ -124,22 +124,6 @@ struct smd_plan {
 
 
 namespace smd {
-// Split-K of the two K = mlp_dims, N = 128 trunk GEMMs (FFN-down forward, FFN-up dX backward) when the token count
-// leaves most CTAs idle, fp32 slabs added in a fixed order by the consumer.  Opt-in (SMD_FFN_SPLITK=1): the extra
-// reduce launch and the split GEMMs competing with the weight-gradient stream can cost more than the split saves
-// (not measured on H100).
-static constexpr int kFfnSplitMax = 4;
-static constexpr int kFfnSplitRows = 9728;   // largest token count that still splits (38 tiles x 2 <= 76)
-inline int ffn_splits(int M, int cta_group) {
-  static const bool on = [] { const char* v = getenv("SMD_FFN_SPLITK"); return v && v[0] == '1'; }();
-  if (!on || M > kFfnSplitRows) return 1;
-  const int tiles = (M + 128 * cta_group - 1) / (128 * cta_group);
-  const int groups = 148 / cta_group;
-  if (tiles * 4 <= groups) return 4;
-  if (tiles * 2 <= groups) return 2;
-  return 1;
-}
-
 inline GemmEpilogue epi() {
   GemmEpilogue e;
   memset(&e, 0, sizeof(e));

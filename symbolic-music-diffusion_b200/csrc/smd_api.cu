@@ -112,8 +112,6 @@ static void build_workspace(smd_plan* p) {
     ws_add(p, "qkv", Mp * 3 * kE * 4);
     ws_add(p, "o", Mp * kE * 2);
     ws_add(p, "hidden", Mp * Md * 2);
-    // fp32 partial slabs of the split-K FFN-down (forward) / FFN-up dX (backward) GEMMs at small token counts
-    ws_add(p, "ffn.slabs", static_cast<size_t>(kFfnSplitMax) * (Mp < kFfnSplitRows ? Mp : kFfnSplitRows) * kE * 4);
   } else {
     ws_add(p, "xb", Mp * ((C + 63) / 64 * 64) * 2);
   }
@@ -168,14 +166,14 @@ static void host_freqs(float* f) {
 
 static int build_ops(smd_plan* p) {
   const smd_config& c = p->cfg;
-  const int Md = c.mlp_dims, C = c.channels, cg = c.cta_group;
+  const int Md = c.mlp_dims, C = c.channels;
   const int Cp = (C + 63) / 64 * 64;
   const uint64_t Mp = p->Mp;
   auto A = [&](const std::string& n) { return p->buf<void>(n); };
   auto Wsh = [&](const std::string& n) { return static_cast<const void*>(p->buf<__nv_bfloat16>("wshadow") + p->off.at(n)); };
   // forward GEMM: A K-major activations [Mp][K], B = (in,out) weight read MN-major ([K][N]) from the shadow arena
   auto fwd = [&](GemmOp* op, const std::string& a, const std::string& w, int K, int N, int BN) {
-    return make_gemm_op(op, A(a), Mp, Wsh(w), static_cast<uint64_t>(N), N, K, BN, cg, 0, 1, 0, 0, p->lo_bytes);
+    return make_gemm_op(op, A(a), Mp, Wsh(w), static_cast<uint64_t>(N), N, K, BN, 0, 1, 0, 0, p->lo_bytes);
   };
   if (c.arch == SMD_ARCH_TRANSFORMER_DDPM) {
     p->op_qkv.resize(c.num_layers); p->op_o.resize(c.num_layers);
@@ -206,8 +204,7 @@ static int build_ops(smd_plan* p) {
   // output projection from the padded copy [Md][Cp]: N = C columns are valid, the tile is Cp (<= 256) wide
   {
     const int BN = Cp >= 256 ? 256 : Cp;
-    const int ocg = (BN % (64 * cg) == 0) ? cg : 1;
-    if (!make_gemm_op(&p->op_out, A("act"), Mp, A("w.out_pad"), static_cast<uint64_t>(Cp), C, Md, BN, ocg, 0, 1, 0, 0,
+    if (!make_gemm_op(&p->op_out, A("act"), Mp, A("w.out_pad"), static_cast<uint64_t>(Cp), C, Md, BN, 0, 1, 0, 0,
                       p->lo_bytes))
       return SMD_ERR_CUDA;
   }
@@ -416,19 +413,15 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
             !retarget_a(&o2, hidden, p->Mp)) return SMD_ERR_CUDA;
       }
       GemmEpilogue e = epi();
-      if (p->lo_bytes == 0 && p->op_attn[l].ok && attn_block_enabled() && (!save || attn_block_train_enabled())) {
+      if (!save && p->op_attn[l].ok && p->lo_bytes == 0) {
         // QKV GEMM -> attention -> out-projection + residual + LayerNorm in ONE launch; q / k / v stay on chip
-        // (training: they are also written out, with the probabilities and the attention output, for the backward pass)
-        AttnOp ao = p->op_attn[l];
-        if (save && !make_attn_a(&ao.tmA, a1, p->Mp)) return SMD_ERR_CUDA;
         AttnBlockArgs aa;
-        aa.qkv_out = save ? qkv : nullptr; aa.probs_out = save ? probs : nullptr; aa.o_out = save ? o : nullptr;
         aa.b_qkv = p->P(params, pre + "attn.qkv.bias"); aa.b_o = p->P(params, pre + "attn.out.bias");
         aa.residual = h_in; aa.out_f32 = h_mid;
         aa.ln_gamma = p->P(params, pre + "ln2.scale"); aa.ln_beta = p->P(params, pre + "ln2.bias");
         aa.out_bf16 = a2;
         aa.M = M; aa.H = c.num_heads;
-        SMD_CUDA(launch_attn_block(ao, aa, st));
+        SMD_CUDA(launch_attn_block(p->op_attn[l], aa, st));
       } else {
       e.bias = p->P(params, pre + "attn.qkv.bias");
       e.out_f32 = qkv; e.ld_f32 = 3 * kE;
@@ -443,20 +436,17 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
       SMD_CUDA(gemm(p, oo, M, e, st));
       }
       const std::string nl = (l + 1 < c.num_layers) ? ("l" + std::to_string(l + 1) + ".ln1.") : std::string("post_ln.");
-      // worth it once the token count fills the machine; training keeps the two-GEMM path by default: it has to write
-      // the hidden activations anyway
-      if (p->op_ffn[l].ok && p->lo_bytes == 0 && ffn_fused_enabled() && (ffn_fused_forced() || (!save && M >= 32 * 256))) {
+      // worth it once the token count fills the machine; training keeps the two-GEMM path: it has to write the hidden
+      // activations anyway
+      if (!save && M >= 32 * 256 && p->op_ffn[l].ok && p->lo_bytes == 0) {
         // FFN up + GELU + FFN down + residual + next LayerNorm in one launch; the hidden activation stays on chip
-        FfnOp fo = p->op_ffn[l];
-        if (save && !make_tmap_bf16(&fo.tmA, a2, p->Mp, 128, 128)) return SMD_ERR_CUDA;
         FfnFusedArgs fa;
         fa.b1 = p->P(params, pre + "ffn1.bias"); fa.b2 = p->P(params, pre + "ffn2.bias");
         fa.residual = h_mid; fa.out_f32 = h_out;
         fa.ln_gamma = p->P(params, nl + "scale"); fa.ln_beta = p->P(params, nl + "bias");
         fa.out_bf16 = a_next;
-        fa.hidden_pre = hid_pre; fa.hidden = save ? hidden : nullptr;
         fa.M = M; fa.Md = Md;
-        SMD_CUDA(launch_ffn_fused(fo, fa, st));
+        SMD_CUDA(launch_ffn_fused(p->op_ffn[l], fa, st));
         continue;
       }
       e = epi();
@@ -464,21 +454,6 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
       e.out_bf16 = hidden; e.ld_bf16 = Md; e.act = ACT_GELU_TANH;
       e.out_bf16_pre = hid_pre;
       SMD_CUDA(gemm(p, o1, M, e, st));
-      const int fsp = p->lo_bytes == 0 ? ffn_splits(M, c.cta_group) : 1;
-      if (fsp > 1) {
-        // few tokens: a 128 x 128 output tile per CTA leaves most of the machine idle while each CTA streams all
-        // of K = mlp_dims.  Cut K into `fsp` slabs (fp32 partials, no atomics), then one small kernel adds them in a
-        // fixed order with bias + residual and emits the next LayerNorm.
-        float* slabs = p->buf<float>("ffn.slabs");
-        const long long stride = static_cast<long long>(p->Mp < kFfnSplitRows ? p->Mp : kFfnSplitRows) * kE;
-        e = epi();
-        e.out_f32 = slabs; e.ld_f32 = kE; e.split_stride = stride;
-        o2.k_splits = fsp;
-        SMD_CUDA(gemm(p, o2, M, e, st));
-        launch_ln128_reduce_fwd(slabs, fsp, stride, p->P(params, pre + "ffn2.bias"), h_mid, p->P(params, nl + "scale"),
-                                p->P(params, nl + "bias"), h_out, a_next, M, st); CNT();
-        continue;
-      }
       e = epi();
       e.bias = p->P(params, pre + "ffn2.bias");
       e.residual = h_mid; e.ld_res = kE;
@@ -1190,9 +1165,10 @@ int smd_debug_buffer(smd_plan* plan, const char* name, void** dev_ptr, size_t* b
 int smd_gemm_bf16(const void* A, const void* B, int M, int N, int K, int a_mn, int b_mn, int BN, int cta_group,
                   const float* bias, const float* residual, int act, float* out_f32, void* out_bf16,
                   float* row_stats, const float* ln_gamma, const float* ln_beta, smd_stream_t stream) {
+  if (cta_group != 1 && cta_group != 2) { set_error("cta_group must be 1 or 2"); return SMD_ERR_INVALID; }
   GemmOp op;
-  if (BN <= 0) BN = choose_bn(N, cta_group);
-  if (!make_gemm_op(&op, A, static_cast<uint64_t>(M), B, static_cast<uint64_t>(N), N, K, BN, cta_group, a_mn, b_mn))
+  if (BN <= 0) BN = choose_bn(N);
+  if (!make_gemm_op(&op, A, static_cast<uint64_t>(M), B, static_cast<uint64_t>(N), N, K, BN, a_mn, b_mn))
     return SMD_ERR_CUDA;
   GemmEpilogue e = epi();
   e.bias = bias; e.residual = residual; e.ld_res = N; e.act = act;

@@ -215,19 +215,3 @@ def test_graph_replayed_step_equals_eager_launches(lib):
         assert torch.equal(snap, graph.grads[first:first + count]), step   # the tail slice was final at the event
         assert abs(float(graph.loss_sum) - float(eager.loss_sum)) <= 1e-6 * abs(float(eager.loss_sum))
 
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("switch", ["SMD_ATTN_BLOCK_TRAIN", "SMD_FFN_SPLITK"])
-def test_opt_in_trunk_paths(switch):
-    """Two opt-in trunk paths behind a switch (read once per process -> worker): the attention-block kernel in the
-    training forward, and the deterministic split-K of the K = mlp_dims trunk GEMMs.  Forward and gradient parity
-    against the oracle."""
-    import os
-    import subprocess
-    import sys
-    env = dict(os.environ)
-    env[switch] = "1"
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, os.path.join(root, "tests", "optin_paths_worker.py")], env=env, cwd=root,
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "optin-ok" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]
