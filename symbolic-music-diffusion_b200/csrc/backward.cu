@@ -18,7 +18,7 @@ static int pick_splits_side(int m_rows, int n_cols, int BN, int num_kb) {
 
 // dW GEMM: A = X (MN-major [tokens][in]), B = G (MN-major [tokens][out]) -> out_f32 [in][out]
 static bool make_dw(GemmOp* op, const void* X, int in_f, const void* G, int g_cols, int out_f, uint64_t rows) {
-  const int BN = (out_f >= 256) ? 256 : ((out_f + 63) / 64 * 64);
+  const int BN = std::min((out_f + 63) / 64 * 64, kBNMax);
   return make_gemm_op(op, X, static_cast<uint64_t>(in_f), G, static_cast<uint64_t>(g_cols), out_f,
                       static_cast<int>(rows), BN, 1, 1);
 }
@@ -29,51 +29,49 @@ static bool make_dx(GemmOp* op, const void* G, int out_f, const void* W, int in_
 
 int train_bind(smd_plan* p) {
   TrainState& ts = p->train;
-  uint8_t* ws = p->ws;
+  const WorkspaceLayout& w = p->reg;
+  const ParamLayout& par = p->par;
   const smd_config& c = p->cfg;
-  const int Md = c.mlp_dims, C = c.channels;
+  const int Md = c.mlp_dims, C = c.channels, K = p->K, L = p->L;
   const int Cp = (C + 63) / 64 * 64;
   const uint64_t Mp = p->Mp;
-  auto B16 = [&](size_t off) { return ts.at<__nv_bfloat16>(ws, off); };
-  // (in,out) weights straight from the bf16 shadow arena: [N = in][K = out], K-major
-  auto Wsh = [&](const std::string& n) { return p->buf<__nv_bfloat16>("wshadow") + p->off.at(n); };
-  auto KN = [&](int k) { return "k" + std::to_string(k) + "."; };
-  auto LN = [&](int l) { return "l" + std::to_string(l) + "."; };
-  ts.dWb.resize(ts.K); ts.dXb.resize(ts.K); ts.dWa.resize(ts.K); ts.dXa.resize(ts.K);
-  ts.dWss.resize(ts.K); ts.dXss.resize(ts.K);
+  auto B16 = [&](size_t off) { return p->at<__nv_bfloat16>(off); };
+  ts.dWb.resize(K); ts.dXb.resize(K); ts.dWa.resize(K); ts.dXa.resize(K);
+  ts.dWss.resize(K); ts.dXss.resize(K);
   const uint64_t Bp = (static_cast<uint64_t>(c.max_batch) + 127) / 128 * 128;
-  for (int k = 0; k < ts.K; ++k) {
-    if (!make_dw(&ts.dWb[k], ts.act_b(ws, k), Md, B16(ts.off_du16[k + 1]), Md, Md, Mp)) return SMD_ERR_CUDA;
-    if (!make_dx(&ts.dXb[k], B16(ts.off_du16[k + 1]), Md, Wsh(KN(k) + "res.b.kernel"), Md, Mp)) return SMD_ERR_CUDA;
-    if (!make_dw(&ts.dWa[k], ts.act_a(ws, k), Md, B16(ts.off_dr16t[k]), Md, Md, Mp)) return SMD_ERR_CUDA;
-    if (!make_dx(&ts.dXa[k], B16(ts.off_dr16t[k]), Md, Wsh(KN(k) + "res.a.kernel"), Md, Mp)) return SMD_ERR_CUDA;
-    if (!make_dw(&ts.dWss[k], B16(ts.off_e2_16), 512, B16(ts.off_dss16), 2 * Md, 2 * Md, Bp)) return SMD_ERR_CUDA;
-    if (!make_dx(&ts.dXss[k], B16(ts.off_dss16), 2 * Md, Wsh(KN(k) + "film.ss.kernel"), 512, Bp)) return SMD_ERR_CUDA;
+  for (int k = 0; k < K; ++k) {
+    const BlockParams& bp = par.block[k];
+    if (!make_dw(&ts.dWb[k], B16(w.act[2 * k + 1]), Md, B16(ts.du16[k + 1]), Md, Md, Mp)) return SMD_ERR_CUDA;
+    if (!make_dx(&ts.dXb[k], B16(ts.du16[k + 1]), Md, p->wsh(bp.b.kernel), Md, Mp)) return SMD_ERR_CUDA;
+    if (!make_dw(&ts.dWa[k], B16(w.act[2 * k]), Md, B16(ts.dr16t[k]), Md, Md, Mp)) return SMD_ERR_CUDA;
+    if (!make_dx(&ts.dXa[k], B16(ts.dr16t[k]), Md, p->wsh(bp.a.kernel), Md, Mp)) return SMD_ERR_CUDA;
+    if (!make_dw(&ts.dWss[k], B16(ts.e2_16), 512, B16(ts.dss16), 2 * Md, 2 * Md, Bp)) return SMD_ERR_CUDA;
+    if (!make_dx(&ts.dXss[k], B16(ts.dss16), 2 * Md, p->wsh(bp.film.ss.kernel), 512, Bp)) return SMD_ERR_CUDA;
   }
   // output projection: dpred16 is zero-padded to Cp columns; the plain weight copy is [Md][Cp]
-  if (!make_gemm_op(&ts.dWout, ts.act_out(ws), static_cast<uint64_t>(Md), B16(ts.off_dpred16), static_cast<uint64_t>(Cp),
-                    C, static_cast<int>(Mp), (Cp >= 256) ? 256 : Cp, 1, 1))
+  if (!make_gemm_op(&ts.dWout, B16(w.act[2 * K]), static_cast<uint64_t>(Md), B16(ts.dpred16), static_cast<uint64_t>(Cp),
+                    C, static_cast<int>(Mp), std::min(Cp, kBNMax), 1, 1))
     return SMD_ERR_CUDA;
-  if (!make_gemm_op(&ts.dXout, B16(ts.off_dpred16), Mp, p->buf<__nv_bfloat16>("w.out_pad"), static_cast<uint64_t>(Md), Md, Cp,
+  if (!make_gemm_op(&ts.dXout, B16(ts.dpred16), Mp, B16(w.out_pad), static_cast<uint64_t>(Md), Md, Cp,
                     choose_bn(Md), 0, 0)) return SMD_ERR_CUDA;
-  if (ts.L > 0) {
-    if (!make_dw(&ts.dWpost, ts.a_post(ws), 128, B16(ts.off_du16[0]), Md, Md, Mp)) return SMD_ERR_CUDA;
-    if (!make_dx(&ts.dXpost, B16(ts.off_du16[0]), Md, Wsh("post.kernel"), 128, Mp)) return SMD_ERR_CUDA;
-    ts.dW2.resize(ts.L); ts.dX2.resize(ts.L); ts.dW1.resize(ts.L); ts.dX1.resize(ts.L);
-    ts.dWo.resize(ts.L); ts.dXo.resize(ts.L); ts.dWqkv.resize(ts.L); ts.dXqkv.resize(ts.L);
-    for (int l = 0; l < ts.L; ++l) {
-      if (!make_dw(&ts.dW2[l], ts.hidden(ws, l), Md, B16(ts.off_dh16a[l]), 128, 128, Mp)) return SMD_ERR_CUDA;
-      if (!make_dx(&ts.dX2[l], B16(ts.off_dh16a[l]), 128, Wsh(LN(l) + "ffn2.kernel"), Md, Mp)) return SMD_ERR_CUDA;
-      if (!make_dw(&ts.dW1[l], ts.a2(ws, l), 128, B16(ts.off_dr16[l]), Md, Md, Mp)) return SMD_ERR_CUDA;
-      if (!make_dx(&ts.dX1[l], B16(ts.off_dr16[l]), Md, Wsh(LN(l) + "ffn1.kernel"), 128, Mp)) return SMD_ERR_CUDA;
-      if (!make_dw(&ts.dWo[l], ts.o(ws, l), 128, B16(ts.off_dh16b[l]), 128, 128, Mp)) return SMD_ERR_CUDA;
-      if (!make_dx(&ts.dXo[l], B16(ts.off_dh16b[l]), 128, Wsh(LN(l) + "attn.out.kernel"), 128, Mp)) return SMD_ERR_CUDA;
-      if (!make_dw(&ts.dWqkv[l], ts.a1(ws, l), 128, B16(ts.off_dqkv16[l]), 384, 384, Mp)) return SMD_ERR_CUDA;
-      ts.dWqkv[l].BN = 128;
-      if (!make_dx(&ts.dXqkv[l], B16(ts.off_dqkv16[l]), 384, Wsh(LN(l) + "attn.qkv.kernel"), 128, Mp)) return SMD_ERR_CUDA;
+  if (L > 0) {
+    if (!make_dw(&ts.dWpost, B16(w.a[2 * L]), 128, B16(ts.du16[0]), Md, Md, Mp)) return SMD_ERR_CUDA;
+    if (!make_dx(&ts.dXpost, B16(ts.du16[0]), Md, p->wsh(par.post.kernel), 128, Mp)) return SMD_ERR_CUDA;
+    ts.dW2.resize(L); ts.dX2.resize(L); ts.dW1.resize(L); ts.dX1.resize(L);
+    ts.dWo.resize(L); ts.dXo.resize(L); ts.dWqkv.resize(L); ts.dXqkv.resize(L);
+    for (int l = 0; l < L; ++l) {
+      const LayerParams& lp = par.layer[l];
+      if (!make_dw(&ts.dW2[l], B16(w.hidden[l]), Md, B16(ts.dh16a[l]), 128, 128, Mp)) return SMD_ERR_CUDA;
+      if (!make_dx(&ts.dX2[l], B16(ts.dh16a[l]), 128, p->wsh(lp.ffn2.kernel), Md, Mp)) return SMD_ERR_CUDA;
+      if (!make_dw(&ts.dW1[l], B16(w.a[2 * l + 1]), 128, B16(ts.dr16[l]), Md, Md, Mp)) return SMD_ERR_CUDA;
+      if (!make_dx(&ts.dX1[l], B16(ts.dr16[l]), Md, p->wsh(lp.ffn1.kernel), 128, Mp)) return SMD_ERR_CUDA;
+      if (!make_dw(&ts.dWo[l], B16(w.o[l]), 128, B16(ts.dh16b[l]), 128, 128, Mp)) return SMD_ERR_CUDA;
+      if (!make_dx(&ts.dXo[l], B16(ts.dh16b[l]), 128, p->wsh(lp.out.kernel), 128, Mp)) return SMD_ERR_CUDA;
+      if (!make_dw(&ts.dWqkv[l], B16(w.a[2 * l]), 128, B16(ts.dqkv16[l]), 384, 384, Mp)) return SMD_ERR_CUDA;
+      if (!make_dx(&ts.dXqkv[l], B16(ts.dqkv16[l]), 384, p->wsh(lp.qkv.kernel), 128, Mp)) return SMD_ERR_CUDA;
     }
   } else {
-    if (!make_dw(&ts.dWin, p->buf<__nv_bfloat16>("xb"), C, B16(ts.off_du16[0]), Md, Md, Mp)) return SMD_ERR_CUDA;
+    if (!make_dw(&ts.dWin, B16(w.xb), C, B16(ts.du16[0]), Md, Md, Mp)) return SMD_ERR_CUDA;
   }
   return SMD_OK;
 }
@@ -98,7 +96,6 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
                       cudaStream_t st, bool capturing, int objective) {
   const unsigned ext = capturing ? cudaEventRecordExternal : cudaEventRecordDefault;
   TrainState& ts = p->train;
-  uint8_t* ws = p->ws;
   const smd_config& c = p->cfg;
   const int S = c.seq_len, C = c.channels, Md = c.mlp_dims;
   const int Cp = (C + 63) / 64 * 64;
@@ -106,9 +103,11 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
   const int Mk = (M + 63) / 64 * 64;           // reduction length of the dW GEMMs
   const int Bk = (batch + 63) / 64 * 64;
   const int per = S * C;
-  auto G = [&](const std::string& n) { return grads + p->off.at(n); };
-  auto B16 = [&](size_t off) { return ts.at<__nv_bfloat16>(ws, off); };
-  auto F32 = [&](size_t off) { return ts.at<float>(ws, off); };
+  const WorkspaceLayout& w = p->reg;
+  const ParamLayout& par = p->par;
+  const int K = p->K, L = p->L;
+  auto B16 = [&](size_t off) { return p->at<__nv_bfloat16>(off); };
+  auto F32 = [&](size_t off) { return p->at<float>(off); };
 
   { int rcs = ensure_side_stream(p); if (rcs) return rcs; }
   cudaStream_t side = p->side_stream;
@@ -121,12 +120,12 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     return cudaStreamWaitEvent(dws, p->ev_dw, 0);
   };
   // dX GEMM outputs (gradient wrt a bf16 activation), stored as bf16: half the epilogue / LayerNorm-backward bytes
-  __nv_bfloat16* g16 = B16(ts.off_g32a);
-  float* du32 = F32(ts.off_g32b);   // gradient of the fp32 residual stream u
-  float* stats = p->buf<float>("stats");
+  __nv_bfloat16* g16 = B16(ts.g16);
+  float* du32 = F32(ts.du32);   // gradient of the fp32 residual stream u
+  float* stats = F32(w.stats);
   const size_t sstride = static_cast<size_t>(p->Mp) * 2;
   const int nkb = Mk / 64;
-  float* xt = p->buf<float>("xt");
+  float* xt = F32(w.xt);
 
   // Zeroing the 100 MB gradient arena (~20 us) goes to the weight-gradient stream: the forward pass does not touch it
   // and every writer either runs on that stream or is ordered after ev_gz below.
@@ -134,32 +133,32 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
   SMD_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * p->arena, dws));
   SMD_CUDA(cudaEventRecord(p->ev_gz, dws));
   // FiLM (scale|shift) gradients are accumulated with atomics by the two CTAs of a sample and by both uses of a pair
-  SMD_CUDA(cudaMemsetAsync(ts.at<float>(ws, ts.off_dss), 0,
-                           sizeof(float) * static_cast<size_t>(ts.K > 0 ? ts.K : 1) * c.max_batch * 2 * Md, st));
+  SMD_CUDA(cudaMemsetAsync(F32(ts.dss), 0,
+                           sizeof(float) * static_cast<size_t>(K) * c.max_batch * 2 * Md, st));
   if (Mk != M) {  // zero the reduction-tail rows of every MN-major gradient operand
     const size_t tail = static_cast<size_t>(Mk - M);
-    for (size_t off : ts.off_du16) SMD_CUDA(cudaMemsetAsync(B16(off) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
-    for (size_t off : ts.off_dr16t) SMD_CUDA(cudaMemsetAsync(B16(off) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
-    for (int l = 0; l < ts.L; ++l) {
-      SMD_CUDA(cudaMemsetAsync(B16(ts.off_dh16a[l]) + static_cast<size_t>(M) * 128, 0, tail * 128 * 2, st));
-      SMD_CUDA(cudaMemsetAsync(B16(ts.off_dh16b[l]) + static_cast<size_t>(M) * 128, 0, tail * 128 * 2, st));
-      SMD_CUDA(cudaMemsetAsync(B16(ts.off_dr16[l]) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
-      SMD_CUDA(cudaMemsetAsync(B16(ts.off_dqkv16[l]) + static_cast<size_t>(M) * 384, 0, tail * 384 * 2, st));
+    for (size_t off : ts.du16) SMD_CUDA(cudaMemsetAsync(B16(off) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
+    for (size_t off : ts.dr16t) SMD_CUDA(cudaMemsetAsync(B16(off) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
+    for (int l = 0; l < L; ++l) {
+      SMD_CUDA(cudaMemsetAsync(B16(ts.dh16a[l]) + static_cast<size_t>(M) * 128, 0, tail * 128 * 2, st));
+      SMD_CUDA(cudaMemsetAsync(B16(ts.dh16b[l]) + static_cast<size_t>(M) * 128, 0, tail * 128 * 2, st));
+      SMD_CUDA(cudaMemsetAsync(B16(ts.dr16[l]) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
+      SMD_CUDA(cudaMemsetAsync(B16(ts.dqkv16[l]) + static_cast<size_t>(M) * 384, 0, tail * 384 * 2, st));
     }
-    SMD_CUDA(cudaMemsetAsync(B16(ts.off_dpred16) + static_cast<size_t>(M) * Cp, 0, tail * Cp * 2, st));
+    SMD_CUDA(cudaMemsetAsync(B16(ts.dpred16) + static_cast<size_t>(M) * Cp, 0, tail * Cp * 2, st));
   }
   if (Bk != batch) {
-    SMD_CUDA(cudaMemsetAsync(B16(ts.off_dss16) + static_cast<size_t>(batch) * 2 * Md, 0,
+    SMD_CUDA(cudaMemsetAsync(B16(ts.dss16) + static_cast<size_t>(batch) * 2 * Md, 0,
                              static_cast<size_t>(Bk - batch) * 2 * Md * 2, st));
-    SMD_CUDA(cudaMemsetAsync(B16(ts.off_e2_16) + static_cast<size_t>(batch) * 512, 0,
+    SMD_CUDA(cudaMemsetAsync(B16(ts.e2_16) + static_cast<size_t>(batch) * 512, 0,
                              static_cast<size_t>(Bk - batch) * 512 * 2, st));
   }
 
   // ---------------- forward (keeps every activation) ----------------
-  float* cond = p->buf<float>("tvec");
-  float* pred = p->buf<float>("eps_hat");
+  float* cond = F32(w.tvec);
+  float* pred = F32(w.eps_hat);
   launch_q_sample(x0, eps, used_alpha, xt, cond, batch, per, st, ind, objective); CNT();
-  int rc = run_forward(p, params, xt, cond, 0, batch, pred, st, &ts, /*raw_out=*/true);
+  int rc = run_forward(p, params, xt, cond, 0, batch, pred, st, /*save=*/true, /*raw_out=*/true);
   if (rc) return rc;
   SMD_CUDA(cudaStreamWaitEvent(st, p->ev_gz, 0));   // gradient arena zeroed (long done by now)
 
@@ -167,19 +166,19 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
   // ddpm: mean over (S, C) and the global batch; dsm: sum over (S, C) (x 0.5), mean over the global batch
   const float gscale = objective == 1 ? 1.0f / static_cast<float>(global_batch)
                                       : 1.0f / (static_cast<float>(global_batch) * static_cast<float>(per));
-  float* dpred32 = F32(ts.off_dpred32);
-  __nv_bfloat16* dpred16 = B16(ts.off_dpred16);
-  ddpm_loss_bwd_kernel<<<batch, 256, 0, st>>>(eps, pred, F32(ts.off_loss), loss_sum, ts.at<unsigned int>(ws, ts.off_loss_ctr),
+  float* dpred32 = F32(ts.dpred32);
+  __nv_bfloat16* dpred16 = B16(ts.dpred16);
+  ddpm_loss_bwd_kernel<<<batch, 256, 0, st>>>(eps, pred, F32(ts.loss), loss_sum, p->at<unsigned int>(ts.loss_ctr),
                                               1.0f / static_cast<float>(global_batch), dpred32, dpred16, gscale, S, C, Cp,
                                               ind, objective);
   CNT();
   SMD_CUDA(fork_dw());
-  launch_colsum<float>(dpred32, C, G("out.bias"), M, C, dws); CNT();
+  launch_colsum<float>(dpred32, C, grads + par.out.bias, M, C, dws); CNT();
 
   // ---------------- output projection + final LayerNorm ----------------
   {
     GemmEpilogue e = epi();
-    e.out_f32 = G("out.kernel"); e.ld_f32 = C;
+    e.out_f32 = grads + par.out.kernel; e.ld_f32 = C;
     const int sp = pick_splits_side(Md, C, ts.dWout.BN, nkb);
     e.atomic_out = sp > 1;
     SMD_CUDA(gemm_k(ts.dWout, Md, Mk, sp, e, dws));
@@ -188,54 +187,54 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     SMD_CUDA(launch_gemm(ts.dXout, M, e, st));
     LnFilmBwdArgs a;
     memset(&a, 0, sizeof(a));
-    a.g16 = g16; a.u = ts.u(ws, ts.K); a.stats = stats + (2 * ts.K) * sstride;
-    a.gamma = p->P(params, "out_ln.scale"); a.beta = p->P(params, "out_ln.bias");
-    a.dx32 = du32; a.dx16 = B16(ts.off_du16[ts.K]);
-    a.dgamma = G("out_ln.scale"); a.dbeta = G("out_ln.bias");
-    a.dbias = G("k" + std::to_string(ts.K - 1) + ".res.b.bias");
+    a.g16 = g16; a.u = F32(w.u[K]); a.stats = stats + (2 * K) * sstride;
+    a.gamma = params + par.out_ln.scale; a.beta = params + par.out_ln.bias;
+    a.dx32 = du32; a.dx16 = B16(ts.du16[K]);
+    a.dgamma = grads + par.out_ln.scale; a.dbeta = grads + par.out_ln.bias;
+    a.dbias = grads + par.block[K - 1].b.bias;
     a.M = M; a.N = Md; a.S = S;
     launch_ln_film_act_bwd(a, st); CNT();
   }
 
   // ---------------- FiLM'd residual blocks ----------------
-  float* ssbuf = p->buf<float>("ss");
-  float* dss_all = F32(ts.off_dss);
-  for (int k = ts.K - 1; k >= 0; --k) {
-    const std::string pre = "k" + std::to_string(k) + ".";
+  float* ssbuf = F32(w.ss);
+  float* dss_all = F32(ts.dss);
+  for (int k = K - 1; k >= 0; --k) {
+    const BlockParams& bp = par.block[k];
     const float* ss_k = ssbuf + static_cast<size_t>(k) * c.max_batch * 2 * Md;
     float* dss = dss_all + static_cast<size_t>(k) * c.max_batch * 2 * Md;
     SMD_CUDA(fork_dw());
     GemmEpilogue e = epi();
-    e.out_f32 = G(pre + "res.b.kernel"); e.ld_f32 = Md;
+    e.out_f32 = grads + bp.b.kernel; e.ld_f32 = Md;
     SMD_CUDA(gemm_k(ts.dWb[k], Md, Mk, 1, e, dws));
     e = epi();
     e.out_bf16 = g16; e.ld_bf16 = Md;
     SMD_CUDA(launch_gemm(ts.dXb[k], M, e, st));
     LnFilmBwdArgs a;
     memset(&a, 0, sizeof(a));
-    a.g16 = g16; a.u16 = reinterpret_cast<const __nv_bfloat16*>(ts.r1(ws, k)); a.stats = stats + (2 * k + 1) * sstride;
-    a.gamma = p->P(params, pre + "res.ln_b.scale"); a.beta = p->P(params, pre + "res.ln_b.bias");
+    a.g16 = g16; a.u16 = B16(w.r1[k]); a.stats = stats + (2 * k + 1) * sstride;
+    a.gamma = params + bp.ln_b.scale; a.beta = params + bp.ln_b.bias;
     a.ss = ss_k; a.act = 2;
-    a.dx32 = nullptr; a.dx16 = B16(ts.off_dr16t[k]);   // dr1 is only consumed as a bf16 GEMM operand
-    a.dgamma = G(pre + "res.ln_b.scale"); a.dbeta = G(pre + "res.ln_b.bias");
-    a.dbias = G(pre + "res.a.bias");
+    a.dx32 = nullptr; a.dx16 = B16(ts.dr16t[k]);   // dr1 is only consumed as a bf16 GEMM operand
+    a.dgamma = grads + bp.ln_b.scale; a.dbeta = grads + bp.ln_b.bias;
+    a.dbias = grads + bp.a.bias;
     a.dss = dss; a.dss_accum = 0;
     a.M = M; a.N = Md; a.S = S;
     launch_ln_film_act_bwd(a, st); CNT();
     SMD_CUDA(fork_dw());
     e = epi();
-    e.out_f32 = G(pre + "res.a.kernel"); e.ld_f32 = Md;
+    e.out_f32 = grads + bp.a.kernel; e.ld_f32 = Md;
     SMD_CUDA(gemm_k(ts.dWa[k], Md, Mk, 1, e, dws));
     e = epi();
     e.out_bf16 = g16; e.ld_bf16 = Md;
     SMD_CUDA(launch_gemm(ts.dXa[k], M, e, st));
     memset(&a, 0, sizeof(a));
-    a.g16 = g16; a.u = ts.u(ws, k); a.stats = stats + (2 * k) * sstride;
-    a.gamma = p->P(params, pre + "res.ln_a.scale"); a.beta = p->P(params, pre + "res.ln_a.bias");
+    a.g16 = g16; a.u = F32(w.u[k]); a.stats = stats + (2 * k) * sstride;
+    a.gamma = params + bp.ln_a.scale; a.beta = params + bp.ln_a.bias;
     a.ss = ss_k; a.act = 2;
-    a.dres = du32; a.dx32 = du32; a.dx16 = B16(ts.off_du16[k]);
-    a.dgamma = G(pre + "res.ln_a.scale"); a.dbeta = G(pre + "res.ln_a.bias");
-    a.dbias = (k > 0) ? G("k" + std::to_string(k - 1) + ".res.b.bias") : G(ts.L ? "post.bias" : "in.bias");
+    a.dres = du32; a.dx32 = du32; a.dx16 = B16(ts.du16[k]);
+    a.dgamma = grads + bp.ln_a.scale; a.dbeta = grads + bp.ln_a.bias;
+    a.dbias = grads + (k > 0 ? par.block[k - 1].b.bias : L ? par.post.bias : par.in.bias);
     a.dss = dss; a.dss_accum = 1;
     a.M = M; a.N = Md; a.S = S;
     launch_ln_film_act_bwd(a, st); CNT();
@@ -244,26 +243,26 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     // independent of the rest of the backward pass: runs on the side stream once this block's dss is complete
     SMD_CUDA(cudaEventRecord(p->ev_dss, st));
     SMD_CUDA(cudaStreamWaitEvent(side, p->ev_dss, 0));
-    float* enc = p->buf<float>("enc");
-    float* e1pre = F32(ts.off_e1pre[k]);
-    float* e1 = F32(ts.off_e1[k]);
-    float* e2 = F32(ts.off_e2[k]);
-    float* de2 = F32(ts.off_de2);
-    float* de1 = F32(ts.off_de);
-    launch_colsum<float>(dss, 2 * Md, G(pre + "film.ss.bias"), batch, 2 * Md, side); CNT();
-    launch_cast_bf16(dss, B16(ts.off_dss16), static_cast<size_t>(batch) * 2 * Md, side); CNT();
-    launch_cast_bf16(e2, B16(ts.off_e2_16), static_cast<size_t>(batch) * 512, side); CNT();
+    float* enc = F32(w.enc);
+    float* e1pre = F32(w.e1pre[k]);
+    float* e1 = F32(w.e1[k]);
+    float* e2 = F32(w.e2[k]);
+    float* de2 = F32(ts.de2);
+    float* de1 = F32(ts.de);
+    launch_colsum<float>(dss, 2 * Md, grads + bp.film.ss.bias, batch, 2 * Md, side); CNT();
+    launch_cast_bf16(dss, B16(ts.dss16), static_cast<size_t>(batch) * 2 * Md, side); CNT();
+    launch_cast_bf16(e2, B16(ts.e2_16), static_cast<size_t>(batch) * 512, side); CNT();
     e = epi();
-    e.out_f32 = G(pre + "film.ss.kernel"); e.ld_f32 = 2 * Md;
+    e.out_f32 = grads + bp.film.ss.kernel; e.ld_f32 = 2 * Md;
     SMD_CUDA(gemm_k(ts.dWss[k], 512, Bk, 1, e, side));
     e = epi();
     e.out_f32 = de2; e.ld_f32 = 512;
     SMD_CUDA(launch_gemm(ts.dXss[k], batch, e, side));
-    launch_colsum<float>(de2, 512, G(pre + "film.d2.bias"), batch, 512, side); CNT();
-    launch_small_linear_bwd_w(e1, de2, G(pre + "film.d2.kernel"), batch, 512, 512, side); CNT();
-    launch_small_linear_bwd_x(de2, p->P(params, pre + "film.d2.kernel"), e1pre, de1, batch, 512, 512, side); CNT();
-    launch_colsum<float>(de1, 512, G(pre + "film.d1.bias"), batch, 512, side); CNT();
-    launch_small_linear_bwd_w(enc, de1, G(pre + "film.d1.kernel"), batch, 128, 512, side); CNT();
+    launch_colsum<float>(de2, 512, grads + bp.film.d2.bias, batch, 512, side); CNT();
+    launch_small_linear_bwd_w(e1, de2, grads + bp.film.d2.kernel, batch, 512, 512, side); CNT();
+    launch_small_linear_bwd_x(de2, params + bp.film.d2.kernel, e1pre, de1, batch, 512, 512, side); CNT();
+    launch_colsum<float>(de1, 512, grads + bp.film.d1.bias, batch, 512, side); CNT();
+    launch_small_linear_bwd_w(enc, de1, grads + bp.film.d1.kernel, batch, 128, 512, side); CNT();
   }
   // every k*. / out_ln / out gradient is final once these three have fired (smd_wait_tail_grads)
   SMD_CUDA(cudaEventRecordWithFlags(p->evx_join, side, ext));
@@ -272,10 +271,10 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
   SMD_CUDA(cudaEventRecordWithFlags(p->ev_dwtail, dws, ext));
   SMD_LAUNCH_CHECK("backward tail");
 
-  if (ts.L == 0) {
+  if (L == 0) {
     // DenseDDPM: input projection weight gradient (models/ncsn.py:129)
     GemmEpilogue e = epi();
-    e.out_f32 = G("in.kernel"); e.ld_f32 = Md;
+    e.out_f32 = grads + par.in.kernel; e.ld_f32 = Md;
     SMD_CUDA(gemm_k(ts.dWin, C, Mk, 1, e, st));
     SMD_CUDA(cudaEventRecord(p->ev_dwjoin, dws));
     SMD_CUDA(cudaStreamWaitEvent(st, p->ev_dwjoin, 0));
@@ -285,13 +284,13 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
   }
 
   // ---------------- post dense + post LayerNorm ----------------
-  float* da32 = F32(ts.off_dh2);
-  float* dh32 = F32(ts.off_dh);
+  float* da32 = F32(ts.dh2);
+  float* dh32 = F32(ts.dh);
   // (the trunk's weight-gradient GEMMs and bias column sums go to dw_stream as well, with a reduced CTA count, while
   // the dX chain -- the critical path, mostly 32-CTA launches -- keeps `st`)
   {
     GemmEpilogue e = epi();
-    e.out_f32 = G("post.kernel"); e.ld_f32 = Md;
+    e.out_f32 = grads + par.post.kernel; e.ld_f32 = Md;
     const int sp = pick_splits_side(128, Md, ts.dWpost.BN, nkb);
     e.atomic_out = sp > 1;
     SMD_CUDA(fork_dw());
@@ -301,32 +300,32 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     SMD_CUDA(launch_gemm(ts.dXpost, M, e, st));
     Ln128BwdArgs a;
     memset(&a, 0, sizeof(a));
-    a.g = da32; a.h = ts.h(ws, 2 * ts.L); a.gamma = p->P(params, "post_ln.scale");
-    a.dx32 = dh32; a.dx16 = B16(ts.off_dh16a[ts.L - 1]);
-    a.dgamma = G("post_ln.scale"); a.dbeta = G("post_ln.bias");
-    a.dbias = G("l" + std::to_string(ts.L - 1) + ".ffn2.bias");
+    a.g = da32; a.h = F32(w.h[2 * L]); a.gamma = params + par.post_ln.scale;
+    a.dx32 = dh32; a.dx16 = B16(ts.dh16a[L - 1]);
+    a.dgamma = grads + par.post_ln.scale; a.dbeta = grads + par.post_ln.bias;
+    a.dbias = grads + par.layer[L - 1].ffn2.bias;
     a.M = M;
     launch_ln128_bwd(a, st); CNT();
   }
 
   // ---------------- transformer trunk ----------------
-  for (int l = ts.L - 1; l >= 0; --l) {
-    const std::string pre = "l" + std::to_string(l) + ".";
-    __nv_bfloat16* dr16l = B16(ts.off_dr16[l]);
+  for (int l = L - 1; l >= 0; --l) {
+    const LayerParams& lp = par.layer[l];
+    __nv_bfloat16* dr16l = B16(ts.dr16[l]);
     // FFN: h_out = gelu(a2 W1 + b1) W2 + b2 + h_mid
     GemmEpilogue e = epi();
     e.out_bf16 = dr16l; e.ld_bf16 = Md;
-    e.gelu_grad_of = ts.hidden_pre(ws, l); e.ld_gg = Md;
+    e.gelu_grad_of = B16(w.hidden_pre[l]); e.ld_gg = Md;
     SMD_CUDA(launch_gemm(ts.dX2[l], M, e, st));
     SMD_CUDA(fork_dw());
     e = epi();
-    e.out_f32 = G(pre + "ffn2.kernel"); e.ld_f32 = 128;
+    e.out_f32 = grads + lp.ffn2.kernel; e.ld_f32 = 128;
     int sp = pick_splits_side(Md, 128, ts.dW2[l].BN, nkb);
     e.atomic_out = sp > 1;
     SMD_CUDA(gemm_k(ts.dW2[l], Md, Mk, sp, e, dws));
-    launch_colsum<__nv_bfloat16>(dr16l, Md, G(pre + "ffn1.bias"), M, Md, dws); CNT();
+    launch_colsum<__nv_bfloat16>(dr16l, Md, grads + lp.ffn1.bias, M, Md, dws); CNT();
     e = epi();
-    e.out_f32 = G(pre + "ffn1.kernel"); e.ld_f32 = Md;
+    e.out_f32 = grads + lp.ffn1.kernel; e.ld_f32 = Md;
     sp = pick_splits_side(128, Md, ts.dW1[l].BN, nkb);
     e.atomic_out = sp > 1;
     SMD_CUDA(gemm_k(ts.dW1[l], 128, Mk, sp, e, dws));
@@ -336,28 +335,28 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     Ln128BwdArgs a;
     memset(&a, 0, sizeof(a));
     a.g = da32;
-    a.h = ts.h(ws, 2 * l + 1); a.gamma = p->P(params, pre + "ln2.scale");
-    a.dres = dh32; a.dx32 = dh32; a.dx16 = B16(ts.off_dh16b[l]);
-    a.dgamma = G(pre + "ln2.scale"); a.dbeta = G(pre + "ln2.bias");
-    a.dbias = G(pre + "attn.out.bias");
+    a.h = F32(w.h[2 * l + 1]); a.gamma = params + lp.ln2.scale;
+    a.dres = dh32; a.dx32 = dh32; a.dx16 = B16(ts.dh16b[l]);
+    a.dgamma = grads + lp.ln2.scale; a.dbeta = grads + lp.ln2.bias;
+    a.dbias = grads + lp.out.bias;
     a.M = M;
     launch_ln128_bwd(a, st); CNT();
     // attention: h_mid = attn(a1) Wo + bo + h_in
     SMD_CUDA(fork_dw());
     e = epi();
-    e.out_f32 = G(pre + "attn.out.kernel"); e.ld_f32 = 128;
+    e.out_f32 = grads + lp.out.kernel; e.ld_f32 = 128;
     sp = pick_splits_side(128, 128, ts.dWo[l].BN, nkb);
     e.atomic_out = sp > 1;
     SMD_CUDA(gemm_k(ts.dWo[l], 128, Mk, sp, e, dws));
     e = epi();
     e.out_f32 = da32; e.ld_f32 = 128;
     SMD_CUDA(launch_gemm(ts.dXo[l], M, e, st));
-    SMD_CUDA(launch_attention_bwd(ts.qkv(ws, l), ts.probs(ws, l), da32, B16(ts.off_dqkv16[l]), G(pre + "attn.qkv.bias"),
+    SMD_CUDA(launch_attention_bwd(F32(w.qkv[l]), F32(w.probs[l]), da32, B16(ts.dqkv16[l]), grads + lp.qkv.bias,
                                   batch, c.num_heads, st));
     CNT();
     SMD_CUDA(fork_dw());
     e = epi();
-    e.out_f32 = G(pre + "attn.qkv.kernel"); e.ld_f32 = 384;
+    e.out_f32 = grads + lp.qkv.kernel; e.ld_f32 = 384;
     sp = pick_splits_side(128, 384, ts.dWqkv[l].BN, nkb);
     e.atomic_out = sp > 1;
     SMD_CUDA(gemm_k(ts.dWqkv[l], 128, Mk, sp, e, dws));
@@ -365,16 +364,16 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     e.out_f32 = da32; e.ld_f32 = 128;
     SMD_CUDA(launch_gemm(ts.dXqkv[l], M, e, st));
     memset(&a, 0, sizeof(a));
-    a.g = da32; a.h = ts.h(ws, 2 * l); a.gamma = p->P(params, pre + "ln1.scale");
-    a.dres = dh32; a.dx32 = dh32; a.dx16 = (l > 0) ? B16(ts.off_dh16a[l - 1]) : nullptr;
-    a.dgamma = G(pre + "ln1.scale"); a.dbeta = G(pre + "ln1.bias");
-    a.dbias = (l > 0) ? G("l" + std::to_string(l - 1) + ".ffn2.bias") : G("in.bias");
+    a.g = da32; a.h = F32(w.h[2 * l]); a.gamma = params + lp.ln1.scale;
+    a.dres = dh32; a.dx32 = dh32; a.dx16 = (l > 0) ? B16(ts.dh16a[l - 1]) : nullptr;
+    a.dgamma = grads + lp.ln1.scale; a.dbeta = grads + lp.ln1.bias;
+    a.dbias = grads + (l > 0 ? par.layer[l - 1].ffn2.bias : par.in.bias);
     a.M = M;
     launch_ln128_bwd(a, st); CNT();
   }
   SMD_CUDA(cudaEventRecord(p->ev_dwjoin, dws));
   // ---------------- input projection ----------------
-  launch_embed_bwd(xt, dh32, G("in.kernel"), M, C, st); CNT();
+  launch_embed_bwd(xt, dh32, grads + par.in.kernel, M, C, st); CNT();
   SMD_CUDA(cudaStreamWaitEvent(st, p->ev_dwjoin, 0));
   SMD_CUDA(cudaStreamWaitEvent(st, p->ev_join, 0));
   SMD_LAUNCH_CHECK("backward trunk");
@@ -408,7 +407,7 @@ static int grads_entry(smd_plan* p, const float* params, const float* x0, const 
   // data-parallel caller waits on (smd_wait_tail_grads) are external event-record nodes of the graph.
   const bool same = p->tg_valid && p->tg_params == params && p->tg_grads == grads && p->tg_loss == loss_sum &&
                     p->tg_batch == batch && p->tg_global == global_batch && p->tg_objective == objective;
-  const float** ind = p->buf<const float*>("t.ind");
+  const float** ind = p->at<const float*>(p->train.ind);
   if (!same) {
     const bool warm = p->tg_warm && p->tg_params == params && p->tg_batch == batch && p->tg_objective == objective;
     drop_train_graph(p);

@@ -703,48 +703,18 @@ void launch_small_linear(const float* x, const float* W, const float* b, float* 
   launch_sgemm_small(0, x, W, b, y, pre, nullptr, R, N, K, act, st);
 }
 
-// ---------------------------------------------------------------------------------------------------
-// weight packing
-// ---------------------------------------------------------------------------------------------------
-// All weight repacks of one optimizer step in ONE launch: blockmap[b] = (job, tile) for every 64x64 tile.
-__global__ void __launch_bounds__(256) pack_multi_kernel(const float* __restrict__ params, const PackJob* __restrict__ jobs,
-                                                         const int2* __restrict__ blockmap, long long lo_delta) {
-  __shared__ float tile[64][65];
-  const int2 bm = blockmap[blockIdx.x];
-  const PackJob job = jobs[bm.x];
-  const int t = bm.y;
-  const int k0 = (t / job.tiles_n) * 64, n0 = (t % job.tiles_n) * 64;
-  const float* src = params + job.src_off;
-  __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(job.dst);
-  const int K = job.K, N = job.N;
-  const int tx = threadIdx.x & 63, ty = threadIdx.x >> 6;   // 64 x 4
-  if (job.mode == 0) {   // dst[n][k] = src[k][n]
-    for (int i = ty; i < 64; i += 4) {
-      const int k = k0 + i, n = n0 + tx;
-      tile[i][tx] = (k < K && n < N) ? src[static_cast<size_t>(k) * N + n] : 0.f;
-    }
-    __syncthreads();
-    for (int i = ty; i < 64; i += 4) {
-      const int n = n0 + i, k = k0 + tx;
-      if (n < N && k < K) {
-        dst[static_cast<size_t>(n) * job.ld + k] = __float2bfloat16_rn(tile[tx][i]);
-        if (lo_delta) dst[static_cast<size_t>(n) * job.ld + k + lo_delta] = bf16_lo_part(tile[tx][i]);
-      }
-    }
-  } else {               // dst[k][n] = src[k][n] with row pitch ld
-    for (int i = ty; i < 64; i += 4) {
-      const int k = k0 + i, n = n0 + tx;
-      if (k < K && n < N) {
-        const float w = src[static_cast<size_t>(k) * N + n];
-        dst[static_cast<size_t>(k) * job.ld + n] = __float2bfloat16_rn(w);
-        if (lo_delta) dst[static_cast<size_t>(k) * job.ld + n + lo_delta] = bf16_lo_part(w);
-      }
-    }
+__global__ void pad_cast_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, int rows, int cols,
+                                     int ld, long long lo_delta) {
+  const int n = rows * cols;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const size_t o = static_cast<size_t>(i / cols) * ld + i % cols;
+    dst[o] = __float2bfloat16_rn(src[i]);
+    if (lo_delta) dst[o + lo_delta] = bf16_lo_part(src[i]);
   }
 }
-void launch_pack_multi(const float* params, const PackJob* jobs_dev, const void* blockmap_dev, int total_tiles,
-                       cudaStream_t st, long long lo_delta) {
-  pack_multi_kernel<<<total_tiles, 256, 0, st>>>(params, jobs_dev, static_cast<const int2*>(blockmap_dev), lo_delta);
+void launch_pad_cast_bf16(const float* src, __nv_bfloat16* dst, int rows, int cols, int ld, cudaStream_t st,
+                          long long lo_delta) {
+  pad_cast_bf16_kernel<<<(rows * cols + 255) / 256, 256, 0, st>>>(src, dst, rows, cols, ld, lo_delta);
 }
 
 __global__ void cast_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, size_t n,

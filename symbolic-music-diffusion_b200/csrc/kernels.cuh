@@ -177,10 +177,9 @@ void launch_small_linear(const float* x, const float* W, const float* b, float* 
 void launch_sgemm_small(int mode, const float* A, const float* B, const float* bias, float* C, float* pre_out,
                         const float* mul_pre, int M, int N, int K, int act, cudaStream_t st);
 
-// one launch for a list of repack jobs (mode 0: transpose to [N][K] with pitch ld; mode 1: plain cast, pitch ld)
-struct PackJob { long long src_off; void* dst; int K, N, mode, ld, tile0, tiles_n; };
-void launch_pack_multi(const float* params, const PackJob* jobs_dev, const void* blockmap_dev, int total_tiles,
-                       cudaStream_t st, long long lo_delta = 0);
+// bf16 dst[r * ld + c] = src[r * cols + c] for c < cols (columns cols .. ld-1 are left as they are)
+void launch_pad_cast_bf16(const float* src, __nv_bfloat16* dst, int rows, int cols, int ld, cudaStream_t st,
+                          long long lo_delta = 0);
 // bf16 dst[i] = src[i]
 void launch_cast_bf16(const float* src, __nv_bfloat16* dst, size_t n, cudaStream_t st, long long lo_delta = 0);
 

@@ -1,14 +1,12 @@
-// Shared internals of libsmd: the plan object, error helpers and launch-count macros.
+// Shared internals of libsmd: the plan object, its parameter and workspace layouts, error helpers and launch-count macros.
 #pragma once
 #include <cstring>
-#include <map>
 #include <string>
 #include <vector>
 
 #include "../../include/smd.h"
 #include "gemm_host.cuh"
 #include "kernels.cuh"
-#include "train.cuh"
 
 #define SMD_CUDA(expr)                                                                              \
   do {                                                                                              \
@@ -50,6 +48,66 @@ static constexpr int kFilmEmb = 128; // DenseFiLM embedding_channels (models/ncs
 static constexpr int kFilmHid = 512; // embedding_channels * 4
 static constexpr int kMaxT = 8192;
 
+// Parameter arena offsets (in floats).  The same offset indexes the fp32 parameters, the gradients and the bf16 shadow.
+struct Dense { long long kernel = 0, bias = 0; };
+struct Norm { long long scale = 0, bias = 0; };
+struct LayerParams { Norm ln1; Dense qkv, out; Norm ln2; Dense ffn1, ffn2; };
+struct FilmParams { Dense d1, d2, ss; };
+struct BlockParams { FilmParams film; Norm ln_a; Dense a; Norm ln_b; Dense b; };
+struct ParamLayout {
+  Dense in;
+  std::vector<LayerParams> layer;   // TransformerDDPM only
+  Norm post_ln;                     // TransformerDDPM only
+  Dense post;                       // TransformerDDPM only
+  std::vector<BlockParams> block;   // FiLM'd residual blocks
+  Norm out_ln;
+  Dense out;
+};
+
+// Workspace byte offsets of everything the forward pass, the objectives and the sampler use.
+struct WorkspaceLayout {
+  size_t wshadow = 0, out_pad = 0, xb = 0, stats = 0, stats_part = 0, tvec = 0, enc = 0, ss = 0, posenc = 0, freqs = 0;
+  size_t xt = 0, eps_hat = 0, coef = 0, keys = 0, slots = 0, t_ptr = 0, abar = 0, sigmas = 0;
+  size_t ftab_t = 0, ftab_enc = 0, ftab_e1 = 0, ftab_e2 = 0, ftab = 0;   // sampler FiLM table (sampler_T > 0)
+  size_t x3_scratch = 0;                                                 // bf16x3 only
+  // Forward activations by position: h[0..2L] (residual stream); a[2l] / a[2l+1] (LN1 / LN2 output of layer l),
+  // a[2L] (post-LN output); qkv, o, hidden per layer; u[0..K] (tail residual stream); r1 per block; act[2k] / act[2k+1]
+  // (LN-a / LN-b output of block k), act[2K] (out-LN output); e1, e2 per block.  A training plan has one region per
+  // index (the backward pass reads them all); an inference plan gives every index of a family the same region.
+  std::vector<size_t> h, a, qkv, o, hidden, u, r1, act, e1, e2;
+  std::vector<size_t> hidden_pre, probs, e1pre;   // written by the training forward only; empty in an inference plan
+};
+
+// Named workspace region, for smd_debug_buffer.
+struct WsRegion { std::string name; size_t offset, bytes; };
+
+// Backward-only state of a training plan: its workspace regions (byte offsets) and GEMM descriptors.
+struct TrainState {
+  size_t g16 = 0;                      // bf16 [Mp][Md]: output of the tail's dX GEMMs
+  size_t du32 = 0;                     // fp32 [Mp][Md]: gradient wrt the tail's residual stream u
+  // bf16 gradient operands of the tail, one buffer per use (their dW GEMMs run on the weight-gradient stream):
+  std::vector<size_t> du16;            // bf16 [Mp][Md] x (K+1): gradient wrt the residual stream u_j entering block j
+  std::vector<size_t> dr16t;           // bf16 [Mp][Md] x K: gradient wrt r1 (after LayerNorm-b backward)
+  size_t dh = 0, dh2 = 0;              // fp32 [Mp][128]
+  // per-layer bf16 gradient operands: the dW GEMMs that read them run on their own stream, so no buffer is
+  // rewritten within one backward pass
+  std::vector<size_t> dh16a;           // bf16 [Mp][128] x L: gradient entering layer l (from LN1 of l+1 / post-LN)
+  std::vector<size_t> dh16b;           // bf16 [Mp][128] x L: gradient at the attention output (from LN2)
+  std::vector<size_t> dr16;            // bf16 [Mp][Md]  x L: gradient at the FFN pre-activation
+  std::vector<size_t> dqkv16;          // bf16 [Mp][384] x L
+  size_t dpred16 = 0;                  // bf16 [Mp][Cp64]
+  size_t dpred32 = 0;                  // fp32 [Mp][C]
+  size_t dss = 0;                      // fp32 [K][B][2Md]
+  size_t de = 0, de2 = 0;              // fp32 [B][512] x2
+  size_t loss = 0;                     // fp32 [B]
+  size_t loss_ctr = 0;                 // u32: block-completion counter of the loss kernel (zeroed at bind, self-resetting)
+  size_t ind = 0;                      // device table {x0, used_alpha, eps} of the graph-replayed step
+  size_t e2_16 = 0, dss16 = 0;         // bf16 [Bp][512], [Bp][2Md]
+  std::vector<GemmOp> dWb, dXb, dWa, dXa, dWss, dXss;
+  std::vector<GemmOp> dW2, dX2, dW1, dX1, dWo, dXo, dWqkv, dXqkv;
+  GemmOp dWout, dXout, dWpost, dXpost, dWin;
+};
+
 }  // namespace smd
 
 using namespace smd;
@@ -57,22 +115,22 @@ using namespace smd;
 struct smd_plan {
   smd_config cfg;
   std::vector<TensorInfo> tensors;
-  std::map<std::string, long long> off;
+  ParamLayout par;
   long long arena = 0;
   int Mp = 0;  // padded token rows
   // strict-precision mode: the workspace is allocated twice; the lo half of a bf16 operand at byte offset o lives at
   // o + lo_bytes (lo_elems in bf16 elements; both 0 when the mode is off)
   size_t lo_bytes = 0;
   long long lo_elems = 0;
+  int L = 0;   // transformer layers (0 for the dense networks)
   int K = 0;   // number of FiLM res-blocks (num_mlp_layers, or num_layers for DenseDDPM)
-  // ---- workspace carve (byte offsets) ----
-  std::map<std::string, size_t> ws_off;
+  // ---- workspace ----
+  WorkspaceLayout reg;
+  std::vector<WsRegion> regions;
   size_t ws_bytes = 0;
   uint8_t* ws = nullptr;
   bool packed = false;
-  std::vector<smd::PackJob> pack_jobs;
   std::vector<int> stat_slots;   // per wide LayerNorm: partial slots per row its producing GEMM wrote (0: atomics / totals)
-  int pack_tiles = 0;
   // ---- GEMM ops ----
   std::vector<GemmOp> op_qkv, op_o, op_ffn1, op_ffn2, op_a, op_b;
   std::vector<FfnOp> op_ffn;   // fused FFN (mlp_dims % 128 == 0)
@@ -118,8 +176,8 @@ struct smd_plan {
   int tg_batch = 0, tg_global = 0, tg_objective = 0;
 
   template <typename Tp>
-  Tp* buf(const std::string& n) const { return reinterpret_cast<Tp*>(ws + ws_off.at(n)); }
-  const float* P(const float* params, const std::string& n) const { return params + off.at(n); }
+  Tp* at(size_t off) const { return reinterpret_cast<Tp*>(ws + off); }
+  __nv_bfloat16* wsh(long long off) const { return at<__nv_bfloat16>(reg.wshadow) + off; }   // bf16 shadow of a tensor
 };
 
 
@@ -130,9 +188,9 @@ inline GemmEpilogue epi() {
   return e;
 }
 // raw_out: DenseNCSN only -- leave out the final division by sigma (the training path differentiates through it itself)
+// save: training forward -- keep the unfused kernels and write the save-only outputs the backward pass reads
 int run_forward(smd_plan* p, const float* params, const float* x, const float* t, int t_broadcast, int batch,
-                float* y, cudaStream_t st, TrainState* save, bool raw_out = false);
+                float* y, cudaStream_t st, bool save, bool raw_out = false);
 int train_bind(smd_plan* p);
 int ensure_side_stream(smd_plan* p);
-void add_pack_job_ptr(smd_plan* p, const std::string& src, void* dst, int K, int N, int mode, int ld);
 }  // namespace smd

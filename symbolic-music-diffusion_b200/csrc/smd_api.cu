@@ -6,7 +6,6 @@
 #include <cstdio>
 #include <algorithm>
 #include <cstring>
-#include <map>
 #include <string>
 #include <vector>
 
@@ -19,7 +18,7 @@ static thread_local std::string g_err;
 void set_error(const std::string& msg) { g_err = msg; }
 const char* get_error() { return g_err.c_str(); }
 
-static void add_tensor(smd_plan* p, const std::string& name, std::initializer_list<int> shape) {
+static long long add_tensor(smd_plan* p, const std::string& name, std::initializer_list<int> shape) {
   TensorInfo t;
   t.name = name;
   t.ndim = static_cast<int>(shape.size());
@@ -27,131 +26,171 @@ static void add_tensor(smd_plan* p, const std::string& name, std::initializer_li
   for (int s : shape) t.shape[i++] = s;
   for (; i < 4; ++i) t.shape[i] = 1;
   t.offset = p->arena;
-  p->off[name] = t.offset;
   p->arena += (t.size() + 7) / 8 * 8;  // 32-byte aligned in fp32 => 16-byte aligned in the bf16 shadow arena (TMA)
   p->tensors.push_back(t);
+  return t.offset;
 }
-
-static void add_film_resblock(smd_plan* p, const std::string& pre, int Mdim) {
-  add_tensor(p, pre + "film.d1.kernel", {kFilmEmb, kFilmHid});
-  add_tensor(p, pre + "film.d1.bias", {kFilmHid});
-  add_tensor(p, pre + "film.d2.kernel", {kFilmHid, kFilmHid});
-  add_tensor(p, pre + "film.d2.bias", {kFilmHid});
-  add_tensor(p, pre + "film.ss.kernel", {kFilmHid, 2 * Mdim});
-  add_tensor(p, pre + "film.ss.bias", {2 * Mdim});
-  add_tensor(p, pre + "res.ln_a.scale", {Mdim});
-  add_tensor(p, pre + "res.ln_a.bias", {Mdim});
-  add_tensor(p, pre + "res.a.kernel", {Mdim, Mdim});
-  add_tensor(p, pre + "res.a.bias", {Mdim});
-  add_tensor(p, pre + "res.ln_b.scale", {Mdim});
-  add_tensor(p, pre + "res.ln_b.bias", {Mdim});
-  add_tensor(p, pre + "res.b.kernel", {Mdim, Mdim});
-  add_tensor(p, pre + "res.b.bias", {Mdim});
+static Dense add_dense(smd_plan* p, const std::string& pre, int in, int out) {
+  Dense d;
+  d.kernel = add_tensor(p, pre + "kernel", {in, out});
+  d.bias = add_tensor(p, pre + "bias", {out});
+  return d;
+}
+static Norm add_norm(smd_plan* p, const std::string& pre, int n) {
+  Norm r;
+  r.scale = add_tensor(p, pre + "scale", {n});
+  r.bias = add_tensor(p, pre + "bias", {n});
+  return r;
 }
 
 static void build_layout(smd_plan* p) {
   const smd_config& c = p->cfg;
   const int C = c.channels, Md = c.mlp_dims;
+  ParamLayout& par = p->par;
   if (c.arch == SMD_ARCH_TRANSFORMER_DDPM) {
-    add_tensor(p, "in.kernel", {C, kE});
-    add_tensor(p, "in.bias", {kE});
-    for (int l = 0; l < c.num_layers; ++l) {
+    par.in = add_dense(p, "in.", C, kE);
+    p->L = c.num_layers;
+    par.layer.resize(p->L);
+    for (int l = 0; l < p->L; ++l) {
       const std::string pre = "l" + std::to_string(l) + ".";
-      add_tensor(p, pre + "ln1.scale", {kE});
-      add_tensor(p, pre + "ln1.bias", {kE});
-      add_tensor(p, pre + "attn.qkv.kernel", {kE, 3 * kE});
-      add_tensor(p, pre + "attn.qkv.bias", {3 * kE});
-      add_tensor(p, pre + "attn.out.kernel", {kE, kE});
-      add_tensor(p, pre + "attn.out.bias", {kE});
-      add_tensor(p, pre + "ln2.scale", {kE});
-      add_tensor(p, pre + "ln2.bias", {kE});
-      add_tensor(p, pre + "ffn1.kernel", {kE, Md});
-      add_tensor(p, pre + "ffn1.bias", {Md});
-      add_tensor(p, pre + "ffn2.kernel", {Md, kE});
-      add_tensor(p, pre + "ffn2.bias", {kE});
+      LayerParams& lp = par.layer[l];
+      lp.ln1 = add_norm(p, pre + "ln1.", kE);
+      lp.qkv = add_dense(p, pre + "attn.qkv.", kE, 3 * kE);
+      lp.out = add_dense(p, pre + "attn.out.", kE, kE);
+      lp.ln2 = add_norm(p, pre + "ln2.", kE);
+      lp.ffn1 = add_dense(p, pre + "ffn1.", kE, Md);
+      lp.ffn2 = add_dense(p, pre + "ffn2.", Md, kE);
     }
-    add_tensor(p, "post_ln.scale", {kE});
-    add_tensor(p, "post_ln.bias", {kE});
-    add_tensor(p, "post.kernel", {kE, Md});
-    add_tensor(p, "post.bias", {Md});
+    par.post_ln = add_norm(p, "post_ln.", kE);
+    par.post = add_dense(p, "post.", kE, Md);
     p->K = c.num_mlp_layers;
   } else {
-    add_tensor(p, "in.kernel", {C, Md});
-    add_tensor(p, "in.bias", {Md});
+    par.in = add_dense(p, "in.", C, Md);
     p->K = c.num_layers;
   }
-  for (int k = 0; k < p->K; ++k) add_film_resblock(p, "k" + std::to_string(k) + ".", Md);
-  add_tensor(p, "out_ln.scale", {Md});
-  add_tensor(p, "out_ln.bias", {Md});
-  add_tensor(p, "out.kernel", {Md, C});
-  add_tensor(p, "out.bias", {C});
+  par.block.resize(p->K);
+  for (int k = 0; k < p->K; ++k) {
+    const std::string pre = "k" + std::to_string(k) + ".";
+    BlockParams& bp = par.block[k];
+    bp.film.d1 = add_dense(p, pre + "film.d1.", kFilmEmb, kFilmHid);
+    bp.film.d2 = add_dense(p, pre + "film.d2.", kFilmHid, kFilmHid);
+    bp.film.ss = add_dense(p, pre + "film.ss.", kFilmHid, 2 * Md);
+    bp.ln_a = add_norm(p, pre + "res.ln_a.", Md);
+    bp.a = add_dense(p, pre + "res.a.", Md, Md);
+    bp.ln_b = add_norm(p, pre + "res.ln_b.", Md);
+    bp.b = add_dense(p, pre + "res.b.", Md, Md);
+  }
+  par.out_ln = add_norm(p, "out_ln.", Md);
+  par.out = add_dense(p, "out.", Md, C);
 }
 
-static size_t ws_add(smd_plan* p, const std::string& name, size_t bytes) {
+// Reserves a 1024-byte aligned workspace region and returns its byte offset.
+static size_t ws_add(smd_plan* p, std::string name, size_t bytes) {
   const size_t off = p->ws_bytes;
-  p->ws_off[name] = off;
-  p->ws_bytes += (bytes + 1023) / 1024 * 1024;
+  bytes = (bytes + 1023) / 1024 * 1024;
+  p->regions.push_back({std::move(name), off, bytes});
+  p->ws_bytes += bytes;
   return off;
 }
 
 static void build_workspace(smd_plan* p) {
   const smd_config& c = p->cfg;
   const size_t Mp = p->Mp, Md = c.mlp_dims, C = c.channels, B = c.max_batch, K = p->K;
-  const bool tr = c.arch == SMD_ARCH_TRANSFORMER_DDPM;
+  const size_t Cp = (C + 63) / 64 * 64;
+  const int L = p->L;
+  const bool strict = c.precision == SMD_PRECISION_BF16X3;
+  WorkspaceLayout& w = p->reg;
   // bf16 shadow of the whole parameter arena (same offsets): every GEMM weight operand is read from it in place --
   // forward as an MN-major B operand ((in,out) = [K][N]), dX as a K-major B operand ([N=in][K=out]) -- so there
   // are no transposed copies and the optimizer refreshes it in the same pass that updates the fp32 masters.
-  ws_add(p, "wshadow", static_cast<size_t>(p->arena) * 2);
+  w.wshadow = ws_add(p, "wshadow", static_cast<size_t>(p->arena) * 2);
   // out.kernel is (Md, C) with C = 42 / 146: its 2C-byte row pitch is not TMA-addressable, so it gets a copy
   // zero-padded to a multiple of 64 columns
-  ws_add(p, "w.out_pad", Md * ((C + 63) / 64 * 64) * 2);
-  // activations
-  if (tr) {
-    ws_add(p, "h", Mp * kE * 4);
-    ws_add(p, "a", Mp * kE * 2);
-    ws_add(p, "qkv", Mp * 3 * kE * 4);
-    ws_add(p, "o", Mp * kE * 2);
-    ws_add(p, "hidden", Mp * Md * 2);
+  w.out_pad = ws_add(p, "w.out_pad", Md * Cp * 2);
+  // forward activations, n indices per family: a training plan keeps every index for the backward pass, an inference
+  // plan overwrites one region in place
+  auto family = [&](int n, size_t bytes, auto name) {
+    std::vector<size_t> v;
+    for (int i = 0; i < n; ++i) v.push_back(i == 0 || c.training ? ws_add(p, name(i), bytes) : v[0]);
+    return v;
+  };
+  auto idx = [](const char* base) { return [base](int i) { return base + std::to_string(i); }; };
+  if (L > 0) {
+    w.h = family(2 * L + 1, Mp * kE * 4, idx("t.h"));
+    w.a = family(2 * L + 1, Mp * kE * 2, [L](int i) {
+      return i == 2 * L ? std::string("t.a_post") : (i % 2 ? "t.a2_" : "t.a1_") + std::to_string(i / 2);
+    });
+    w.qkv = family(L, Mp * 3 * kE * 4, idx("t.qkv"));
+    w.o = family(L, Mp * kE * 2, idx("t.o"));
+    w.hidden = family(L, Mp * Md * 2, idx("t.hid"));
+    if (c.training) {
+      w.hidden_pre = family(L, Mp * Md * 2, idx("t.hpre"));
+      w.probs = family(L, B * c.num_heads * 32 * 32 * 4, idx("t.probs"));
+    }
   } else {
-    ws_add(p, "xb", Mp * ((C + 63) / 64 * 64) * 2);
+    w.xb = ws_add(p, "xb", Mp * Cp * 2);
   }
-  ws_add(p, "u", Mp * Md * 4);
-  ws_add(p, "r1", Mp * Md * 4);
-  ws_add(p, "act", Mp * Md * 2);
+  w.u = family(K + 1, Mp * Md * 4, idx("t.u"));
+  w.r1 = family(K, Mp * Md * (strict ? 4 : 2), idx("t.r1_"));
+  w.act = family(2 * K + 1, Mp * Md * 2, [K](int i) {
+    return i == static_cast<int>(2 * K) ? std::string("t.act_out") : (i % 2 ? "t.actb" : "t.acta") + std::to_string(i / 2);
+  });
   // per-row LayerNorm (sum, sumsq) of the 2K+1 wide LayerNorms; zeroed once per forward
-  ws_add(p, "stats", (2 * K + 1) * Mp * 2 * 4);
+  w.stats = ws_add(p, "stats", (2 * K + 1) * Mp * 2 * 4);
   // per-tile partial sums of the GEMM feeding the next wide LayerNorm: [row][n_tile * (2 or 3) + column group][2]
-  ws_add(p, "stats_part", Mp * ((Md + kBNMax - 1) / kBNMax * 3) * 2 * 4);
+  w.stats_part = ws_add(p, "stats_part", Mp * ((Md + kBNMax - 1) / kBNMax * 3) * 2 * 4);
   // FiLM generator
-  ws_add(p, "tvec", B * 4);
-  ws_add(p, "enc", B * kFilmEmb * 4);
-  ws_add(p, "e1", B * kFilmHid * 4);
-  ws_add(p, "e2", B * kFilmHid * 4);
-  ws_add(p, "ss", K * B * 2 * Md * 4);
-  ws_add(p, "posenc", static_cast<size_t>(c.seq_len) * kE * 4);
-  ws_add(p, "freqs", 64 * 4);
+  w.tvec = ws_add(p, "tvec", B * 4);
+  w.enc = ws_add(p, "enc", B * kFilmEmb * 4);
+  w.e1 = family(K, B * kFilmHid * 4, idx("t.e1_"));
+  w.e2 = family(K, B * kFilmHid * 4, idx("t.e2_"));
+  if (c.training) w.e1pre = family(K, B * kFilmHid * 4, idx("t.e1pre"));
+  w.ss = ws_add(p, "ss", K * B * 2 * Md * 4);
+  w.posenc = ws_add(p, "posenc", static_cast<size_t>(c.seq_len) * kE * 4);
+  w.freqs = ws_add(p, "freqs", 64 * 4);
   // objective / sampler scratch
-  ws_add(p, "xt", B * c.seq_len * C * 4);
-  ws_add(p, "eps_hat", B * c.seq_len * C * 4);
-  ws_add(p, "coef", kMaxT * 8 * 4);
-  ws_add(p, "keys", kMaxT * 4 * 4);
-  ws_add(p, "slots", kMaxT * 4);
-  ws_add(p, "t_ptr", 64);
-  ws_add(p, "abar", (kMaxT + 1) * 4);
-  ws_add(p, "sigmas", kMaxT * 4);
-  ws_add(p, "packjobs", 256 * sizeof(PackJob));
-  ws_add(p, "packmap", 65536 * 8);
+  w.xt = ws_add(p, "xt", B * c.seq_len * C * 4);
+  w.eps_hat = ws_add(p, "eps_hat", B * c.seq_len * C * 4);
+  w.coef = ws_add(p, "coef", kMaxT * 8 * 4);
+  w.keys = ws_add(p, "keys", kMaxT * 4 * 4);
+  w.slots = ws_add(p, "slots", kMaxT * 4);
+  w.t_ptr = ws_add(p, "t_ptr", 64);
+  w.abar = ws_add(p, "abar", (kMaxT + 1) * 4);
+  w.sigmas = ws_add(p, "sigmas", kMaxT * 4);
   if (c.sampler_T > 0) {
     const size_t T = c.sampler_T;
-    ws_add(p, "ftab.t", T * 4);
-    ws_add(p, "ftab.enc", T * kFilmEmb * 4);
-    ws_add(p, "ftab.e1", T * kFilmHid * 4);
-    ws_add(p, "ftab.e2", T * kFilmHid * 4);
-    ws_add(p, "ftab", K * T * 2 * Md * 4);
+    w.ftab_t = ws_add(p, "ftab.t", T * 4);
+    w.ftab_enc = ws_add(p, "ftab.enc", T * kFilmEmb * 4);
+    w.ftab_e1 = ws_add(p, "ftab.e1", T * kFilmHid * 4);
+    w.ftab_e2 = ws_add(p, "ftab.e2", T * kFilmHid * 4);
+    w.ftab = ws_add(p, "ftab", K * T * 2 * Md * 4);
   }
-  if (c.training) train_workspace(p->train, c, p->Mp, p->K, [&](const std::string& n, size_t b) { return ws_add(p, n, b); });
-  if (c.precision == SMD_PRECISION_BF16X3) {
-    ws_add(p, "x3.scratch", Mp * Md * 4);     // fp32 cross-term accumulator of the three-pass GEMMs
+  if (c.training) {
+    TrainState& t = p->train;
+    t.g16 = ws_add(p, "t.g16", Mp * Md * 2);
+    t.du32 = ws_add(p, "t.du32", Mp * Md * 4);
+    t.du16 = family(K + 1, Mp * Md * 2, idx("t.du16_"));
+    t.dr16t = family(K, Mp * Md * 2, idx("t.dr16t_"));
+    t.dh = ws_add(p, "t.dh", Mp * kE * 4);
+    t.dh2 = ws_add(p, "t.dh2", Mp * kE * 4);
+    t.dh16a = family(L, Mp * kE * 2, idx("t.dh16a"));
+    t.dh16b = family(L, Mp * kE * 2, idx("t.dh16b"));
+    t.dr16 = family(L, Mp * Md * 2, idx("t.dr16_"));
+    t.dqkv16 = family(L, Mp * 3 * kE * 2, idx("t.dqkv16_"));
+    t.dpred16 = ws_add(p, "t.dpred16", Mp * Cp * 2);
+    t.dpred32 = ws_add(p, "t.dpred32", Mp * C * 4);
+    t.dss = ws_add(p, "t.dss", K * B * 2 * Md * 4);   // one [B][2Md] block per FiLM pair
+    t.de = ws_add(p, "t.de", B * kFilmHid * 4);
+    t.de2 = ws_add(p, "t.de2", B * kFilmHid * 4);
+    t.loss = ws_add(p, "t.loss", B * 4);
+    t.loss_ctr = ws_add(p, "t.loss_ctr", 64);
+    t.ind = ws_add(p, "t.ind", 64);
+    const size_t Bp = (B + 127) / 128 * 128;
+    t.e2_16 = ws_add(p, "t.e2_16", Bp * kFilmHid * 2);
+    t.dss16 = ws_add(p, "t.dss16", Bp * 2 * Md * 2);
+  }
+  if (strict) {
+    w.x3_scratch = ws_add(p, "x3.scratch", Mp * Md * 4);   // fp32 cross-term accumulator of the three-pass GEMMs
     p->lo_bytes = p->ws_bytes;                // second copy of the workspace: the lo halves, at the same offsets
     p->lo_elems = static_cast<long long>(p->lo_bytes / 2);
     p->ws_bytes *= 2;
@@ -169,45 +208,42 @@ static int build_ops(smd_plan* p) {
   const int Md = c.mlp_dims, C = c.channels;
   const int Cp = (C + 63) / 64 * 64;
   const uint64_t Mp = p->Mp;
-  auto A = [&](const std::string& n) { return p->buf<void>(n); };
-  auto Wsh = [&](const std::string& n) { return static_cast<const void*>(p->buf<__nv_bfloat16>("wshadow") + p->off.at(n)); };
-  // forward GEMM: A K-major activations [Mp][K], B = (in,out) weight read MN-major ([K][N]) from the shadow arena
-  auto fwd = [&](GemmOp* op, const std::string& a, const std::string& w, int K, int N, int BN) {
-    return make_gemm_op(op, A(a), Mp, Wsh(w), static_cast<uint64_t>(N), N, K, BN, 0, 1, 0, 0, p->lo_bytes);
+  const WorkspaceLayout& w = p->reg;
+  // forward GEMM: A K-major activations [Mp][K], B = (in,out) weight read MN-major ([K][N]) from the shadow arena; every
+  // forward GEMM has N >= 128 and uses the widest tile
+  auto fwd = [&](GemmOp* op, size_t a, long long wt, int K, int N) {
+    return make_gemm_op(op, p->ws + a, Mp, p->wsh(wt), static_cast<uint64_t>(N), N, K, kBNMax, 0, 1, 0, 0, p->lo_bytes);
   };
-  if (c.arch == SMD_ARCH_TRANSFORMER_DDPM) {
-    p->op_qkv.resize(c.num_layers); p->op_o.resize(c.num_layers);
-    p->op_ffn1.resize(c.num_layers); p->op_ffn2.resize(c.num_layers);
-    p->op_ffn.resize(c.num_layers);
-    p->op_attn.resize(c.num_layers);
-    for (int l = 0; l < c.num_layers; ++l) {
-      const std::string pre = "l" + std::to_string(l) + ".";
-      if (!fwd(&p->op_qkv[l], "a", pre + "attn.qkv.kernel", kE, 3 * kE, 128)) return SMD_ERR_CUDA;
-      if (!fwd(&p->op_o[l], "o", pre + "attn.out.kernel", kE, kE, 128)) return SMD_ERR_CUDA;
-      if (!fwd(&p->op_ffn1[l], "a", pre + "ffn1.kernel", kE, Md, 256)) return SMD_ERR_CUDA;
-      if (!fwd(&p->op_ffn2[l], "hidden", pre + "ffn2.kernel", Md, kE, 128)) return SMD_ERR_CUDA;
-      if (Md % 128 == 0 &&
-          !make_ffn_op(&p->op_ffn[l], A("a"), Mp, Wsh(pre + "ffn1.kernel"), Wsh(pre + "ffn2.kernel"), Md)) return SMD_ERR_CUDA;
-      if ((c.num_heads == 8 || c.num_heads == 16) &&
-          !make_attn_op(&p->op_attn[l], A("a"), Mp, Wsh(pre + "attn.qkv.kernel"), Wsh(pre + "attn.out.kernel"))) return SMD_ERR_CUDA;
-    }
-    if (!fwd(&p->op_post, "a", "post.kernel", kE, Md, 256)) return SMD_ERR_CUDA;
+  p->op_qkv.resize(p->L); p->op_o.resize(p->L);
+  p->op_ffn1.resize(p->L); p->op_ffn2.resize(p->L);
+  p->op_ffn.resize(p->L);
+  p->op_attn.resize(p->L);
+  for (int l = 0; l < p->L; ++l) {
+    const LayerParams& lp = p->par.layer[l];
+    const size_t a1 = w.a[2 * l], a2 = w.a[2 * l + 1];
+    if (!fwd(&p->op_qkv[l], a1, lp.qkv.kernel, kE, 3 * kE)) return SMD_ERR_CUDA;
+    if (!fwd(&p->op_o[l], w.o[l], lp.out.kernel, kE, kE)) return SMD_ERR_CUDA;
+    if (!fwd(&p->op_ffn1[l], a2, lp.ffn1.kernel, kE, Md)) return SMD_ERR_CUDA;
+    if (!fwd(&p->op_ffn2[l], w.hidden[l], lp.ffn2.kernel, Md, kE)) return SMD_ERR_CUDA;
+    if (Md % 128 == 0 &&
+        !make_ffn_op(&p->op_ffn[l], p->ws + a2, Mp, p->wsh(lp.ffn1.kernel), p->wsh(lp.ffn2.kernel), Md)) return SMD_ERR_CUDA;
+    if ((c.num_heads == 8 || c.num_heads == 16) &&
+        !make_attn_op(&p->op_attn[l], p->ws + a1, Mp, p->wsh(lp.qkv.kernel), p->wsh(lp.out.kernel))) return SMD_ERR_CUDA;
+  }
+  if (p->L > 0) {
+    if (!fwd(&p->op_post, w.a[2 * p->L], p->par.post.kernel, kE, Md)) return SMD_ERR_CUDA;
   } else {
-    if (!fwd(&p->op_in, "xb", "in.kernel", C, Md, 256)) return SMD_ERR_CUDA;
+    if (!fwd(&p->op_in, w.xb, p->par.in.kernel, C, Md)) return SMD_ERR_CUDA;
   }
   p->op_a.resize(p->K); p->op_b.resize(p->K);
   for (int k = 0; k < p->K; ++k) {
-    const std::string pre = "k" + std::to_string(k) + ".res.";
-    if (!fwd(&p->op_a[k], "act", pre + "a.kernel", Md, Md, 256)) return SMD_ERR_CUDA;
-    if (!fwd(&p->op_b[k], "act", pre + "b.kernel", Md, Md, 256)) return SMD_ERR_CUDA;
+    if (!fwd(&p->op_a[k], w.act[2 * k], p->par.block[k].a.kernel, Md, Md)) return SMD_ERR_CUDA;
+    if (!fwd(&p->op_b[k], w.act[2 * k + 1], p->par.block[k].b.kernel, Md, Md)) return SMD_ERR_CUDA;
   }
-  // output projection from the padded copy [Md][Cp]: N = C columns are valid, the tile is Cp (<= 256) wide
-  {
-    const int BN = Cp >= 256 ? 256 : Cp;
-    if (!make_gemm_op(&p->op_out, A("act"), Mp, A("w.out_pad"), static_cast<uint64_t>(Cp), C, Md, BN, 0, 1, 0, 0,
-                      p->lo_bytes))
-      return SMD_ERR_CUDA;
-  }
+  // output projection from the padded copy [Md][Cp]: N = C columns are valid
+  if (!make_gemm_op(&p->op_out, p->ws + w.act[2 * p->K], Mp, p->ws + w.out_pad, static_cast<uint64_t>(Cp), C, Md,
+                    std::min(Cp, kBNMax), 0, 1, 0, 0, p->lo_bytes))
+    return SMD_ERR_CUDA;
   return SMD_OK;
 }
 
@@ -219,12 +255,12 @@ static int build_ops(smd_plan* p) {
 static cudaError_t gemm(smd_plan* p, const GemmOp& op, int M, GemmEpilogue e, cudaStream_t st, int ln_slot = -1) {
   auto arm_stats = [&](GemmEpilogue& ef) {
     if (ln_slot < 0 || ef.row_stats == nullptr) return;
-    ef.stats_part = p->buf<float>("stats_part");
+    ef.stats_part = p->at<float>(p->reg.stats_part);
     p->stat_slots[ln_slot] = stats_slots_for(op, M, ef);
   };
   if (p->lo_bytes == 0) { arm_stats(e); return launch_gemm(op, M, e, st); }
   if (!op.has_lo) return cudaErrorInvalidValue;
-  float* scratch = p->buf<float>("x3.scratch");
+  float* scratch = p->at<float>(p->reg.x3_scratch);
   GemmOp o1 = op; o1.tmA = op.tmA_lo;
   GemmEpilogue e1 = epi();
   e1.residual = e.residual; e1.ld_res = e.ld_res;
@@ -245,25 +281,26 @@ static cudaError_t gemm(smd_plan* p, const GemmOp& op, int M, GemmEpilogue e, cu
 // ln_film_act arguments for the statistics of wide LayerNorm `ln_slot` (partials + slot count, or totals)
 struct LnStats { const float* part; int nslots; float* totals; };
 static LnStats ln_stats(smd_plan* p, int ln_slot) {
-  float* totals = p->buf<float>("stats") + static_cast<size_t>(ln_slot) * p->Mp * 2;
+  float* totals = p->at<float>(p->reg.stats) + static_cast<size_t>(ln_slot) * p->Mp * 2;
   const int n = p->stat_slots[ln_slot];
-  return n > 0 ? LnStats{p->buf<float>("stats_part"), n, totals} : LnStats{nullptr, 0, totals};
+  return n > 0 ? LnStats{p->at<float>(p->reg.stats_part), n, totals} : LnStats{nullptr, 0, totals};
 }
 
 // FiLM generator for all K blocks: t (R values) -> ss[k][R][2*Md]   (models/ncsn.py:47-61)
-static int run_film(smd_plan* p, const float* params, const float* t, int R, cudaStream_t st, TrainState* save) {
+static int run_film(smd_plan* p, const float* params, const float* t, int R, cudaStream_t st, bool save) {
   const int Md = p->cfg.mlp_dims;
-  float* enc = p->buf<float>("enc");
-  float* ss = p->buf<float>("ss");
-  launch_noise_encoding(t, p->buf<float>("freqs"), enc, R, st); CNT();
+  const WorkspaceLayout& w = p->reg;
+  float* enc = p->at<float>(w.enc);
+  float* ss = p->at<float>(w.ss);
+  launch_noise_encoding(t, p->at<float>(w.freqs), enc, R, st); CNT();
   for (int k = 0; k < p->K; ++k) {
-    const std::string pre = "k" + std::to_string(k) + ".film.";
-    float* e1 = save ? save->at<float>(p->ws, save->off_e1[k]) : p->buf<float>("e1");
-    float* e2 = save ? save->at<float>(p->ws, save->off_e2[k]) : p->buf<float>("e2");
-    float* e1pre = save ? save->at<float>(p->ws, save->off_e1pre[k]) : nullptr;
-    launch_small_linear(enc, p->P(params, pre + "d1.kernel"), p->P(params, pre + "d1.bias"), e1, R, kFilmEmb, kFilmHid, 2, st, e1pre); CNT();
-    launch_small_linear(e1, p->P(params, pre + "d2.kernel"), p->P(params, pre + "d2.bias"), e2, R, kFilmHid, kFilmHid, 0, st); CNT();
-    launch_small_linear(e2, p->P(params, pre + "ss.kernel"), p->P(params, pre + "ss.bias"),
+    const FilmParams& f = p->par.block[k].film;
+    float* e1 = p->at<float>(w.e1[k]);
+    float* e2 = p->at<float>(w.e2[k]);
+    float* e1pre = save ? p->at<float>(w.e1pre[k]) : nullptr;
+    launch_small_linear(enc, params + f.d1.kernel, params + f.d1.bias, e1, R, kFilmEmb, kFilmHid, 2, st, e1pre); CNT();
+    launch_small_linear(e1, params + f.d2.kernel, params + f.d2.bias, e2, R, kFilmHid, kFilmHid, 0, st); CNT();
+    launch_small_linear(e2, params + f.ss.kernel, params + f.ss.bias,
                         ss + static_cast<size_t>(k) * p->cfg.max_batch * 2 * Md, R, kFilmHid, 2 * Md, 0, st); CNT();
   }
   SMD_LAUNCH_CHECK("film");
@@ -289,83 +326,72 @@ int ensure_side_stream(smd_plan* p) {
 
 // The FiLM'd residual tail shared by both architectures (models/ncsn.py:173-178, models/shared.py:61-75).
 // On entry u (fp32 [M][Md]) and stats[0] hold the block input and its row statistics.
-static int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, float* y, cudaStream_t st,
-                    smd::TrainState* save) {
+static int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, float* y, cudaStream_t st) {
   const int Md = p->cfg.mlp_dims, C = p->cfg.channels;
-  float* u = p->buf<float>("u");
-  float* r1 = p->buf<float>("r1");
-  __nv_bfloat16* act = p->buf<__nv_bfloat16>("act");
-  float* stats = p->buf<float>("stats");
+  const WorkspaceLayout& w = p->reg;
+  float* stats = p->at<float>(w.stats);
   const size_t sstride = static_cast<size_t>(p->Mp) * 2;
-  float* ss = p->buf<float>("ss");
+  float* ss = p->at<float>(w.ss);
+  const bool strict = p->lo_bytes != 0;
   for (int k = 0; k < p->K; ++k) {
-    const std::string pre = "k" + std::to_string(k) + ".res.";
+    const BlockParams& bp = p->par.block[k];
     const float* scale = ss + static_cast<size_t>(k) * p->cfg.max_batch * 2 * Md;
     const int* frow_dev = nullptr;
     if (p->film_tab_on) {
-      scale = p->buf<float>("ftab") + static_cast<size_t>(k) * p->T * 2 * Md;
+      scale = p->at<float>(w.ftab) + static_cast<size_t>(k) * p->T * 2 * Md;
       if (p->film_row_dev) frow_dev = p->film_row_dev; else scale += static_cast<size_t>(p->film_row) * 2 * Md;
     }
     const float* shift = scale + Md;
-    float* u_in = u;
-    __nv_bfloat16* r1_out = reinterpret_cast<__nv_bfloat16*>(r1);   // r1 only feeds a LayerNorm: bf16 is enough
-    __nv_bfloat16* act_a = act;
-    __nv_bfloat16* act_b = act;
-    float* u_out = u;
-    if (save) {  // training keeps every block's tensors
-      u_in = save->u(p->ws, k); r1_out = reinterpret_cast<__nv_bfloat16*>(save->r1(p->ws, k)); act_a = save->act_a(p->ws, k);
-      act_b = save->act_b(p->ws, k); u_out = save->u(p->ws, k + 1);
-    }
-    const bool strict = p->lo_bytes != 0;
+    float* u_in = p->at<float>(w.u[k]);
+    float* u_out = p->at<float>(w.u[k + 1]);
+    __nv_bfloat16* act_a = p->at<__nv_bfloat16>(w.act[2 * k]);
+    __nv_bfloat16* act_b = p->at<__nv_bfloat16>(w.act[2 * k + 1]);
     LnStats ls = ln_stats(p, 2 * k);
-    launch_ln_film_act(u_in, ls.totals, p->P(params, pre + "ln_a.scale"), p->P(params, pre + "ln_a.bias"),
+    launch_ln_film_act(u_in, ls.totals, params + bp.ln_a.scale, params + bp.ln_a.bias,
                        scale, shift, 2 * Md, t_broadcast, 2, act_a, M, Md, S, st, frow_dev, nullptr, p->lo_elems,
                        ls.part, ls.nslots, ls.totals); CNT();
     GemmEpilogue e = epi();
-    e.bias = p->P(params, pre + "a.bias");
-    if (strict) { e.out_f32 = r1; e.ld_f32 = Md; }       // (strict mode keeps the pre-LayerNorm intermediate in fp32)
-    else { e.out_bf16 = r1_out; e.ld_bf16 = Md; }
+    e.bias = params + bp.a.bias;
+    // r1 only feeds a LayerNorm: bf16 is enough (strict mode keeps the pre-LayerNorm intermediate in fp32)
+    float* r1 = strict ? p->at<float>(w.r1[k]) : nullptr;
+    __nv_bfloat16* r1_16 = strict ? nullptr : p->at<__nv_bfloat16>(w.r1[k]);
+    if (strict) { e.out_f32 = r1; e.ld_f32 = Md; }
+    else { e.out_bf16 = r1_16; e.ld_bf16 = Md; }
     e.row_stats = stats + (2 * k + 1) * sstride;
-    GemmOp opa = p->op_a[k];
-    GemmOp opb = p->op_b[k];
-    if (save) { if (!retarget_a(&opa, act_a, p->Mp) || !retarget_a(&opb, act_b, p->Mp)) return SMD_ERR_CUDA; }
-    SMD_CUDA(gemm(p, opa, M, e, st, 2 * k + 1));
+    SMD_CUDA(gemm(p, p->op_a[k], M, e, st, 2 * k + 1));
     ls = ln_stats(p, 2 * k + 1);
-    launch_ln_film_act(strict ? r1 : nullptr, ls.totals, p->P(params, pre + "ln_b.scale"),
-                       p->P(params, pre + "ln_b.bias"), scale, shift, 2 * Md, t_broadcast, 2, act_b, M, Md, S, st, frow_dev,
-                       strict ? nullptr : r1_out, p->lo_elems, ls.part, ls.nslots, ls.totals); CNT();
+    launch_ln_film_act(r1, ls.totals, params + bp.ln_b.scale, params + bp.ln_b.bias, scale, shift, 2 * Md,
+                       t_broadcast, 2, act_b, M, Md, S, st, frow_dev, r1_16, p->lo_elems, ls.part, ls.nslots,
+                       ls.totals); CNT();
     e = epi();
-    e.bias = p->P(params, pre + "b.bias");
+    e.bias = params + bp.b.bias;
     e.residual = u_in; e.ld_res = Md;
     e.out_f32 = u_out; e.ld_f32 = Md;
     e.row_stats = stats + (2 * k + 2) * sstride;
-    SMD_CUDA(gemm(p, opb, M, e, st, 2 * k + 2));
+    SMD_CUDA(gemm(p, p->op_b[k], M, e, st, 2 * k + 2));
   }
-  float* u_last = save ? save->u(p->ws, p->K) : u;
-  __nv_bfloat16* act_o = save ? save->act_out(p->ws) : act;
   const LnStats lo_ = ln_stats(p, 2 * p->K);
-  launch_ln_film_act(u_last, lo_.totals, p->P(params, "out_ln.scale"), p->P(params, "out_ln.bias"),
-                     nullptr, nullptr, 0, 0, 0, act_o, M, Md, S, st, nullptr, nullptr, p->lo_elems, lo_.part, lo_.nslots,
-                     lo_.totals); CNT();
+  launch_ln_film_act(p->at<float>(w.u[p->K]), lo_.totals, params + p->par.out_ln.scale, params + p->par.out_ln.bias,
+                     nullptr, nullptr, 0, 0, 0, p->at<__nv_bfloat16>(w.act[2 * p->K]), M, Md, S, st, nullptr, nullptr,
+                     p->lo_elems, lo_.part, lo_.nslots, lo_.totals); CNT();
   GemmEpilogue e = epi();
-  e.bias = p->P(params, "out.bias");
+  e.bias = params + p->par.out.bias;
   e.out_f32 = y; e.ld_f32 = C;
-  GemmOp opo = p->op_out;
-  if (save) { if (!retarget_a(&opo, act_o, p->Mp)) return SMD_ERR_CUDA; }
-  SMD_CUDA(gemm(p, opo, M, e, st));
+  SMD_CUDA(gemm(p, p->op_out, M, e, st));
   SMD_LAUNCH_CHECK("tail");
   return SMD_OK;
 }
 
 int run_forward(smd_plan* p, const float* params, const float* x, const float* t, int t_broadcast, int batch,
-                float* y, cudaStream_t st, smd::TrainState* save, bool raw_out) {
+                float* y, cudaStream_t st, bool save, bool raw_out) {
   const smd_config& c = p->cfg;
   if (!p->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
   if (!p->packed) { set_error("smd_pack_weights has not been called"); return SMD_ERR_STATE; }
   if (batch < 1 || batch > c.max_batch) { set_error("batch out of range"); return SMD_ERR_INVALID; }
   const int S = c.seq_len, C = c.channels, Md = c.mlp_dims;
   const int M = batch * S;
-  float* stats = p->buf<float>("stats");
+  const WorkspaceLayout& w = p->reg;
+  float* stats = p->at<float>(w.stats);
   p->stat_slots.assign(static_cast<size_t>(2 * p->K + 1), 0);
   SMD_CUDA(cudaMemsetAsync(stats, 0, static_cast<size_t>(2 * p->K + 1) * p->Mp * 2 * 4, st));
   int rc = SMD_OK;
@@ -386,103 +412,88 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
     }
   }
   if (rc) return rc;
-  float* u0 = save ? save->u(p->ws, 0) : p->buf<float>("u");
-  if (c.arch == SMD_ARCH_TRANSFORMER_DDPM) {
-    float* h = p->buf<float>("h");
-    __nv_bfloat16* a = p->buf<__nv_bfloat16>("a");
-    float* qkv = p->buf<float>("qkv");
-    __nv_bfloat16* o = p->buf<__nv_bfloat16>("o");
-    __nv_bfloat16* hidden = p->buf<__nv_bfloat16>("hidden");
-    if (save) { h = save->h(p->ws, 0); a = save->a1(p->ws, 0); }
-    launch_embed(x, p->P(params, "in.kernel"), p->P(params, "in.bias"), p->buf<float>("posenc"),
-                 p->P(params, "l0.ln1.scale"), p->P(params, "l0.ln1.bias"), h, a, M, C, S, st, p->lo_elems); CNT();
-    for (int l = 0; l < c.num_layers; ++l) {
-      const std::string pre = "l" + std::to_string(l) + ".";
-      GemmOp oq = p->op_qkv[l], oo = p->op_o[l], o1 = p->op_ffn1[l], o2 = p->op_ffn2[l];
-      float* h_in = h; float* h_mid = h; float* h_out = h;
-      __nv_bfloat16* a1 = a; __nv_bfloat16* a2 = a; __nv_bfloat16* a_next = a;
-      float* probs = nullptr;
-      __nv_bfloat16* hid_pre = nullptr;
-      if (save) {
-        h_in = save->h(p->ws, 2 * l); h_mid = save->h(p->ws, 2 * l + 1); h_out = save->h(p->ws, 2 * l + 2);
-        a1 = save->a1(p->ws, l); a2 = save->a2(p->ws, l);
-        a_next = (l + 1 < c.num_layers) ? save->a1(p->ws, l + 1) : save->a_post(p->ws);
-        qkv = save->qkv(p->ws, l); o = save->o(p->ws, l); hidden = save->hidden(p->ws, l);
-        hid_pre = save->hidden_pre(p->ws, l); probs = save->probs(p->ws, l);
-        if (!retarget_a(&oq, a1, p->Mp) || !retarget_a(&oo, o, p->Mp) || !retarget_a(&o1, a2, p->Mp) ||
-            !retarget_a(&o2, hidden, p->Mp)) return SMD_ERR_CUDA;
-      }
+  float* u0 = p->at<float>(w.u[0]);
+  if (p->L > 0) {
+    const ParamLayout& par = p->par;
+    auto h = [&](int i) { return p->at<float>(w.h[i]); };
+    auto a = [&](int i) { return p->at<__nv_bfloat16>(w.a[i]); };
+    launch_embed(x, params + par.in.kernel, params + par.in.bias, p->at<float>(w.posenc),
+                 params + par.layer[0].ln1.scale, params + par.layer[0].ln1.bias, h(0), a(0), M, C, S, st,
+                 p->lo_elems); CNT();
+    for (int l = 0; l < p->L; ++l) {
+      const LayerParams& lp = par.layer[l];
+      const Norm& next_ln = (l + 1 < p->L) ? par.layer[l + 1].ln1 : par.post_ln;
+      float* h_in = h(2 * l); float* h_mid = h(2 * l + 1); float* h_out = h(2 * l + 2);
+      __nv_bfloat16* a2 = a(2 * l + 1); __nv_bfloat16* a_next = a(2 * l + 2);
       GemmEpilogue e = epi();
       if (!save && p->op_attn[l].ok && p->lo_bytes == 0) {
         // QKV GEMM -> attention -> out-projection + residual + LayerNorm in ONE launch; q / k / v stay on chip
         AttnBlockArgs aa;
-        aa.b_qkv = p->P(params, pre + "attn.qkv.bias"); aa.b_o = p->P(params, pre + "attn.out.bias");
+        aa.b_qkv = params + lp.qkv.bias; aa.b_o = params + lp.out.bias;
         aa.residual = h_in; aa.out_f32 = h_mid;
-        aa.ln_gamma = p->P(params, pre + "ln2.scale"); aa.ln_beta = p->P(params, pre + "ln2.bias");
+        aa.ln_gamma = params + lp.ln2.scale; aa.ln_beta = params + lp.ln2.bias;
         aa.out_bf16 = a2;
         aa.M = M; aa.H = c.num_heads;
         SMD_CUDA(launch_attn_block(p->op_attn[l], aa, st));
       } else {
-      e.bias = p->P(params, pre + "attn.qkv.bias");
+      float* qkv = p->at<float>(w.qkv[l]);
+      e.bias = params + lp.qkv.bias;
       e.out_f32 = qkv; e.ld_f32 = 3 * kE;
-      SMD_CUDA(gemm(p, oq, M, e, st));
-      launch_attention(qkv, o, probs, batch, c.num_heads, st, p->lo_elems); CNT();
+      SMD_CUDA(gemm(p, p->op_qkv[l], M, e, st));
+      launch_attention(qkv, p->at<__nv_bfloat16>(w.o[l]), save ? p->at<float>(w.probs[l]) : nullptr, batch,
+                       c.num_heads, st, p->lo_elems); CNT();
       e = epi();
-      e.bias = p->P(params, pre + "attn.out.bias");
+      e.bias = params + lp.out.bias;
       e.residual = h_in; e.ld_res = kE;
       e.out_f32 = h_mid; e.ld_f32 = kE;
       e.out_bf16 = a2; e.ld_bf16 = kE;
-      e.ln_gamma = p->P(params, pre + "ln2.scale"); e.ln_beta = p->P(params, pre + "ln2.bias");
-      SMD_CUDA(gemm(p, oo, M, e, st));
+      e.ln_gamma = params + lp.ln2.scale; e.ln_beta = params + lp.ln2.bias;
+      SMD_CUDA(gemm(p, p->op_o[l], M, e, st));
       }
-      const std::string nl = (l + 1 < c.num_layers) ? ("l" + std::to_string(l + 1) + ".ln1.") : std::string("post_ln.");
       // worth it once the token count fills the machine; training keeps the two-GEMM path: it has to write the hidden
       // activations anyway
       if (!save && M >= 32 * 256 && p->op_ffn[l].ok && p->lo_bytes == 0) {
         // FFN up + GELU + FFN down + residual + next LayerNorm in one launch; the hidden activation stays on chip
         FfnFusedArgs fa;
-        fa.b1 = p->P(params, pre + "ffn1.bias"); fa.b2 = p->P(params, pre + "ffn2.bias");
+        fa.b1 = params + lp.ffn1.bias; fa.b2 = params + lp.ffn2.bias;
         fa.residual = h_mid; fa.out_f32 = h_out;
-        fa.ln_gamma = p->P(params, nl + "scale"); fa.ln_beta = p->P(params, nl + "bias");
+        fa.ln_gamma = params + next_ln.scale; fa.ln_beta = params + next_ln.bias;
         fa.out_bf16 = a_next;
         fa.M = M; fa.Md = Md;
         SMD_CUDA(launch_ffn_fused(p->op_ffn[l], fa, st));
         continue;
       }
       e = epi();
-      e.bias = p->P(params, pre + "ffn1.bias");
-      e.out_bf16 = hidden; e.ld_bf16 = Md; e.act = ACT_GELU_TANH;
-      e.out_bf16_pre = hid_pre;
-      SMD_CUDA(gemm(p, o1, M, e, st));
+      e.bias = params + lp.ffn1.bias;
+      e.out_bf16 = p->at<__nv_bfloat16>(w.hidden[l]); e.ld_bf16 = Md; e.act = ACT_GELU_TANH;
+      e.out_bf16_pre = save ? p->at<__nv_bfloat16>(w.hidden_pre[l]) : nullptr;
+      SMD_CUDA(gemm(p, p->op_ffn1[l], M, e, st));
       e = epi();
-      e.bias = p->P(params, pre + "ffn2.bias");
+      e.bias = params + lp.ffn2.bias;
       e.residual = h_mid; e.ld_res = kE;
       e.out_f32 = h_out; e.ld_f32 = kE;
       e.out_bf16 = a_next; e.ld_bf16 = kE;
-      e.ln_gamma = p->P(params, nl + "scale"); e.ln_beta = p->P(params, nl + "bias");
-      SMD_CUDA(gemm(p, o2, M, e, st));
+      e.ln_gamma = params + next_ln.scale; e.ln_beta = params + next_ln.bias;
+      SMD_CUDA(gemm(p, p->op_ffn2[l], M, e, st));
     }
     GemmEpilogue e = epi();
-    e.bias = p->P(params, "post.bias");
+    e.bias = params + par.post.bias;
     e.out_f32 = u0; e.ld_f32 = Md;
     e.row_stats = stats;
-    GemmOp op = p->op_post;
-    if (save) { if (!retarget_a(&op, save->a_post(p->ws), p->Mp)) return SMD_ERR_CUDA; }
-    SMD_CUDA(gemm(p, op, M, e, st, 0));
+    SMD_CUDA(gemm(p, p->op_post, M, e, st, 0));
   } else {
-    __nv_bfloat16* xb = p->buf<__nv_bfloat16>("xb");
     const int Cp = (C + 63) / 64 * 64;
     if (Cp != C) { set_error("DenseDDPM on the CUDA path needs channels % 64 == 0"); return SMD_ERR_INVALID; }
-    launch_cast_bf16(x, xb, static_cast<size_t>(M) * C, st, p->lo_elems); CNT();
+    launch_cast_bf16(x, p->at<__nv_bfloat16>(w.xb), static_cast<size_t>(M) * C, st, p->lo_elems); CNT();
     GemmEpilogue e = epi();
-    e.bias = p->P(params, "in.bias");
+    e.bias = params + p->par.in.bias;
     e.out_f32 = u0; e.ld_f32 = Md;
     e.row_stats = stats;
     SMD_CUDA(gemm(p, p->op_in, M, e, st, 0));
   }
   SMD_LAUNCH_CHECK("trunk");
   if (film_on_side) SMD_CUDA(cudaStreamWaitEvent(st, p->ev_film, 0));
-  rc = run_tail(p, params, M, S, t_broadcast, y, st, save);
+  rc = run_tail(p, params, M, S, t_broadcast, y, st);
   if (rc) return rc;
   if (c.arch == SMD_ARCH_DENSE_NCSN && !raw_out) {   // models/ncsn.py:97: output = x / sigmas
     launch_scale_rows(y, t, t_broadcast, batch, S * C, st); CNT();
@@ -559,34 +570,6 @@ __global__ void threefry_uniform_kernel(uint32_t k0, uint32_t k1, float* out, ui
 __global__ void threefry_normal_kernel(uint32_t k0, uint32_t k1, float* out, uint32_t n, uint32_t first, uint32_t total) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
     out[i] = jax_normal_from_bits(jax_random_bits(k0, k1, first + i, total));
-}
-
-void add_pack_job_ptr(smd_plan* p, const std::string& src, void* dst, int K, int N, int mode, int ld) {
-  PackJob j;
-  j.src_off = p->off.at(src); j.dst = dst; j.K = K; j.N = N; j.mode = mode; j.ld = ld;
-  j.tiles_n = (N + 63) / 64;
-  j.tile0 = p->pack_tiles;
-  p->pack_tiles += ((K + 63) / 64) * j.tiles_n;
-  p->pack_jobs.push_back(j);
-}
-
-// the only repack job left: out.kernel -> zero-padded [Md][Cp] copy (everything else is read from the bf16 shadow)
-static int build_pack_jobs(smd_plan* plan) {
-  const smd_config& c = plan->cfg;
-  const int Md = c.mlp_dims, C = c.channels, Cp = (C + 63) / 64 * 64;
-  plan->pack_jobs.clear();
-  plan->pack_tiles = 0;
-  add_pack_job_ptr(plan, "out.kernel", plan->buf<void>("w.out_pad"), Md, C, 1, Cp);
-  SMD_CUDA(cudaMemcpy(plan->buf<PackJob>("packjobs"), plan->pack_jobs.data(), plan->pack_jobs.size() * sizeof(PackJob),
-                      cudaMemcpyHostToDevice));
-  std::vector<int> bm(static_cast<size_t>(plan->pack_tiles) * 2);
-  for (size_t j = 0; j < plan->pack_jobs.size(); ++j) {
-    const PackJob& pj = plan->pack_jobs[j];
-    const int nt = ((pj.K + 63) / 64) * pj.tiles_n;
-    for (int t = 0; t < nt; ++t) { bm[2 * (pj.tile0 + t)] = static_cast<int>(j); bm[2 * (pj.tile0 + t) + 1] = t; }
-  }
-  SMD_CUDA(cudaMemcpy(plan->buf<int>("packmap"), bm.data(), bm.size() * sizeof(int), cudaMemcpyHostToDevice));
-  return SMD_OK;
 }
 
 }  // namespace smd
@@ -674,7 +657,7 @@ int smd_bind_workspace(smd_plan* plan, void* workspace, size_t bytes) {
   if (rc) return rc;
   float f[64];
   host_freqs(f);
-  SMD_CUDA(cudaMemcpy(plan->buf<float>("freqs"), f, sizeof(f), cudaMemcpyHostToDevice));
+  SMD_CUDA(cudaMemcpy(plan->at<float>(plan->reg.freqs), f, sizeof(f), cudaMemcpyHostToDevice));
   // positional table (models/shared.py:33-48), float32 like jnp
   std::vector<float> pe(static_cast<size_t>(plan->cfg.seq_len) * kE);
   for (int s = 0; s < plan->cfg.seq_len; ++s)
@@ -683,19 +666,20 @@ int smd_bind_workspace(smd_plan* plan, void* workspace, size_t bytes) {
       pe[s * kE + j] = sinf(arg);
       pe[s * kE + 64 + j] = cosf(arg);
     }
-  SMD_CUDA(cudaMemcpy(plan->buf<float>("posenc"), pe.data(), pe.size() * 4, cudaMemcpyHostToDevice));
+  SMD_CUDA(cudaMemcpy(plan->at<float>(plan->reg.posenc), pe.data(), pe.size() * 4, cudaMemcpyHostToDevice));
   if (plan->cfg.training) { rc = train_bind(plan); if (rc) return rc; }
-  rc = build_pack_jobs(plan);
-  if (rc) return rc;
   return SMD_OK;
 }
 
 static int refresh_operands(smd_plan* plan, const float* params, bool shadow_is_fresh, cudaStream_t st) {
   if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
   if (!shadow_is_fresh) {
-    launch_cast_bf16(params, plan->buf<__nv_bfloat16>("wshadow"), static_cast<size_t>(plan->arena), st, plan->lo_elems); CNT();
+    launch_cast_bf16(params, plan->wsh(0), static_cast<size_t>(plan->arena), st, plan->lo_elems); CNT();
   }
-  launch_pack_multi(params, plan->buf<PackJob>("packjobs"), plan->buf<void>("packmap"), plan->pack_tiles, st, plan->lo_elems); CNT();
+  // out.kernel is the one GEMM weight not read from the shadow: its zero-padded copy (pad columns stay zero from bind)
+  const int C = plan->cfg.channels;
+  launch_pad_cast_bf16(params + plan->par.out.kernel, plan->at<__nv_bfloat16>(plan->reg.out_pad), plan->cfg.mlp_dims, C,
+                       (C + 63) / 64 * 64, st, plan->lo_elems); CNT();
   SMD_LAUNCH_CHECK("pack_weights");
   plan->packed = true;
   plan->film_tab_ready = false;   // parameters changed
@@ -710,13 +694,12 @@ int smd_pack_weights_after_adam(smd_plan* plan, const float* params, smd_stream_
   return refresh_operands(plan, params, true, static_cast<cudaStream_t>(stream));
 }
 
-void* smd_shadow_arena(smd_plan* plan) { return plan->ws ? plan->buf<void>("wshadow") : nullptr; }
+void* smd_shadow_arena(smd_plan* plan) { return plan->ws ? plan->wsh(0) : nullptr; }
 
 int smd_grads_tail_range(const smd_plan* plan, long long* first_float, long long* num_floats) {
   if (!plan || !first_float || !num_floats) { set_error("null argument"); return SMD_ERR_INVALID; }
-  auto it = plan->off.find("k0.film.d1.kernel");   // first tensor of the FiLM'd tail; out_ln / out follow it
-  if (it == plan->off.end()) { set_error("plan has no FiLM'd residual tail"); return SMD_ERR_STATE; }
-  *first_float = static_cast<long long>(it->second);
+  if (plan->par.block.empty()) { set_error("plan has no FiLM'd residual tail"); return SMD_ERR_STATE; }
+  *first_float = plan->par.block[0].film.d1.kernel;   // first tensor of the FiLM'd tail; out_ln / out follow it
   *num_floats = static_cast<long long>(plan->arena) - *first_float;
   return SMD_OK;
 }
@@ -733,7 +716,7 @@ int smd_wait_tail_grads(smd_plan* plan, smd_stream_t stream) {
 
 int smd_forward(smd_plan* plan, const float* params, const float* x, const float* t, int t_broadcast, int batch,
                 float* y, smd_stream_t stream) {
-  return run_forward(plan, params, x, t, t_broadcast, batch, y, static_cast<cudaStream_t>(stream), nullptr);
+  return run_forward(plan, params, x, t, t_broadcast, batch, y, static_cast<cudaStream_t>(stream), false);
 }
 
 int smd_ddpm_loss(smd_plan* plan, const float* params, const float* x0, const float* used_alpha, const float* eps,
@@ -742,11 +725,11 @@ int smd_ddpm_loss(smd_plan* plan, const float* params, const float* x0, const fl
   if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
   if (batch < 1 || batch > plan->cfg.max_batch) { set_error("batch out of range"); return SMD_ERR_INVALID; }
   const int per = plan->cfg.seq_len * plan->cfg.channels;
-  float* xt = plan->buf<float>("xt");
-  float* cond = plan->buf<float>("tvec");
-  float* pred = pred_or_null ? pred_or_null : plan->buf<float>("eps_hat");
+  float* xt = plan->at<float>(plan->reg.xt);
+  float* cond = plan->at<float>(plan->reg.tvec);
+  float* pred = pred_or_null ? pred_or_null : plan->at<float>(plan->reg.eps_hat);
   launch_q_sample(x0, eps, used_alpha, xt, cond, batch, per, st); CNT();
-  int rc = run_forward(plan, params, xt, cond, 0, batch, pred, st, nullptr);
+  int rc = run_forward(plan, params, xt, cond, 0, batch, pred, st, false);
   if (rc) return rc;
   launch_ddpm_loss(eps, pred, loss_per_example, nullptr, 0.f, batch, per, st); CNT();
   SMD_LAUNCH_CHECK("ddpm_loss");
@@ -760,11 +743,11 @@ int smd_dsm_loss(smd_plan* plan, const float* params, const float* x0, const flo
   if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
   if (batch < 1 || batch > plan->cfg.max_batch) { set_error("batch out of range"); return SMD_ERR_INVALID; }
   const int per = plan->cfg.seq_len * plan->cfg.channels;
-  float* xt = plan->buf<float>("xt");
-  float* cond = plan->buf<float>("tvec");
-  float* pred = pred_or_null ? pred_or_null : plan->buf<float>("eps_hat");
+  float* xt = plan->at<float>(plan->reg.xt);
+  float* cond = plan->at<float>(plan->reg.tvec);
+  float* pred = pred_or_null ? pred_or_null : plan->at<float>(plan->reg.eps_hat);
   launch_q_sample(x0, eps, used_sigma, xt, cond, batch, per, st, nullptr, 1); CNT();
-  int rc = run_forward(plan, params, xt, cond, 0, batch, pred, st, nullptr);
+  int rc = run_forward(plan, params, xt, cond, 0, batch, pred, st, false);
   if (rc) return rc;
   launch_ddpm_loss(eps, pred, loss_per_example, nullptr, 0.f, batch, per, st, used_sigma); CNT();
   SMD_LAUNCH_CHECK("dsm_loss");
@@ -775,7 +758,7 @@ int smd_dsm_setup(smd_plan* plan, const float* host_sigmas, int L, smd_stream_t 
   if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
   if (L < 2 || L > kMaxT) { set_error("schedule length out of range"); return SMD_ERR_INVALID; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  SMD_CUDA(cudaMemcpyAsync(plan->buf<float>("sigmas"), host_sigmas, static_cast<size_t>(L) * 4, cudaMemcpyHostToDevice, st));
+  SMD_CUDA(cudaMemcpyAsync(plan->at<float>(plan->reg.sigmas), host_sigmas, static_cast<size_t>(L) * 4, cudaMemcpyHostToDevice, st));
   SMD_CUDA(cudaStreamSynchronize(st));
   plan->L_dsm = L;
   return SMD_OK;
@@ -793,7 +776,7 @@ int smd_dsm_draws(smd_plan* plan, const uint32_t host_key[2], int global_batch, 
   h_split(host_key, 3, k3);               // rng, label_rng, sample_rng          (utils/losses.py:146)
   if (cn) { const uint32_t rng[2] = {k3[0], k3[1]}; h_split(rng, 2, k2); }        // rng, noise_rng (:152-153)
   // labels = randint(label_rng, minval = int(continuous), maxval = L): span L - cn; table index label - 1 wraps for 0
-  draws_kernel<<<(batch + 127) / 128, 128, 0, st>>>(k3[2], k3[3], k2[2], k2[3], plan->buf<float>("sigmas"), L - 1, L - cn,
+  draws_kernel<<<(batch + 127) / 128, 128, 0, st>>>(k3[2], k3[3], k2[2], k2[3], plan->at<float>(plan->reg.sigmas), L - 1, L - cn,
                                                     global_batch, first_row, batch, cn, cn, used_sigma, labels_or_null);
   CNT();
   const long long n = static_cast<long long>(batch) * per;
@@ -835,7 +818,7 @@ int smd_objective_setup(smd_plan* plan, const float* host_betas, int T, smd_stre
   ap[0] = 1.0f;
   float run = 1.0f;
   for (int i = 0; i < T; ++i) { const float a = 1.0f - host_betas[i]; run = (i == 0) ? a : run * a; ap[i + 1] = run; }
-  SMD_CUDA(cudaMemcpyAsync(plan->buf<float>("abar"), ap.data(), ap.size() * 4, cudaMemcpyHostToDevice, st));
+  SMD_CUDA(cudaMemcpyAsync(plan->at<float>(plan->reg.abar), ap.data(), ap.size() * 4, cudaMemcpyHostToDevice, st));
   SMD_CUDA(cudaStreamSynchronize(st));
   plan->T_obj = T;
   return SMD_OK;
@@ -854,7 +837,7 @@ int smd_ddpm_draws_sharded(smd_plan* plan, const uint32_t host_key[2], int globa
   const uint32_t rng[2] = {k3[0], k3[1]};
   h_split(rng, 2, k2);                    // rng, noise_rng
   // ddpm: labels = randint(int(continuous), T + int(continuous)) -> span T; alphas_prod has T + 1 entries (leading 1)
-  draws_kernel<<<(batch + 127) / 128, 128, 0, st>>>(k3[2], k3[3], k2[2], k2[3], plan->buf<float>("abar"), plan->T_obj,
+  draws_kernel<<<(batch + 127) / 128, 128, 0, st>>>(k3[2], k3[3], k2[2], k2[3], plan->at<float>(plan->reg.abar), plan->T_obj,
                                                     plan->T_obj, global_batch, first_row, batch, continuous_noise ? 1 : 0, 1,
                                                     used_alpha, labels_or_null);
   CNT();
@@ -926,9 +909,9 @@ int smd_sampler_setup(smd_plan* plan, const float* host_betas, int T, const uint
     for (int j = 0; j < 40; ++j) if (idx_tab[j] == image_idx) { sum += j; any = true; }
     if (any) slots[t] = sum + 1;
   }
-  SMD_CUDA(cudaMemcpyAsync(plan->buf<float>("coef"), coef.data(), coef.size() * 4, cudaMemcpyHostToDevice, st));
-  SMD_CUDA(cudaMemcpyAsync(plan->buf<uint32_t>("keys"), keys.data(), keys.size() * 4, cudaMemcpyHostToDevice, st));
-  SMD_CUDA(cudaMemcpyAsync(plan->buf<int>("slots"), slots.data(), slots.size() * 4, cudaMemcpyHostToDevice, st));
+  SMD_CUDA(cudaMemcpyAsync(plan->at<float>(plan->reg.coef), coef.data(), coef.size() * 4, cudaMemcpyHostToDevice, st));
+  SMD_CUDA(cudaMemcpyAsync(plan->at<uint32_t>(plan->reg.keys), keys.data(), keys.size() * 4, cudaMemcpyHostToDevice, st));
+  SMD_CUDA(cudaMemcpyAsync(plan->at<int>(plan->reg.slots), slots.data(), slots.size() * 4, cudaMemcpyHostToDevice, st));
   SMD_CUDA(cudaStreamSynchronize(st));  // host vectors go out of scope
   plan->T = T;
   plan->sampler_ready = true;
@@ -948,18 +931,18 @@ static int ensure_film_table(smd_plan* plan, const float* params, cudaStream_t s
   if (plan->cfg.sampler_T <= 0 || plan->T > plan->cfg.sampler_T) return SMD_OK;   // per-step generator instead
   if (plan->film_tab_ready && plan->film_tab_params == params) return SMD_OK;
   const int T = plan->T, Md = plan->cfg.mlp_dims;
-  float* tv = plan->buf<float>("ftab.t");
-  float* enc = plan->buf<float>("ftab.enc");
-  float* e1 = plan->buf<float>("ftab.e1");
-  float* e2 = plan->buf<float>("ftab.e2");
-  float* tab = plan->buf<float>("ftab");
-  gather_cond_kernel<<<(T + 255) / 256, 256, 0, st>>>(plan->buf<float>("coef"), tv, T); CNT();
-  launch_noise_encoding(tv, plan->buf<float>("freqs"), enc, T, st); CNT();
+  float* tv = plan->at<float>(plan->reg.ftab_t);
+  float* enc = plan->at<float>(plan->reg.ftab_enc);
+  float* e1 = plan->at<float>(plan->reg.ftab_e1);
+  float* e2 = plan->at<float>(plan->reg.ftab_e2);
+  float* tab = plan->at<float>(plan->reg.ftab);
+  gather_cond_kernel<<<(T + 255) / 256, 256, 0, st>>>(plan->at<float>(plan->reg.coef), tv, T); CNT();
+  launch_noise_encoding(tv, plan->at<float>(plan->reg.freqs), enc, T, st); CNT();
   for (int k = 0; k < plan->K; ++k) {
-    const std::string pre = "k" + std::to_string(k) + ".film.";
-    launch_small_linear(enc, plan->P(params, pre + "d1.kernel"), plan->P(params, pre + "d1.bias"), e1, T, kFilmEmb, kFilmHid, 2, st); CNT();
-    launch_small_linear(e1, plan->P(params, pre + "d2.kernel"), plan->P(params, pre + "d2.bias"), e2, T, kFilmHid, kFilmHid, 0, st); CNT();
-    launch_small_linear(e2, plan->P(params, pre + "ss.kernel"), plan->P(params, pre + "ss.bias"),
+    const FilmParams& f = plan->par.block[k].film;
+    launch_small_linear(enc, params + f.d1.kernel, params + f.d1.bias, e1, T, kFilmEmb, kFilmHid, 2, st); CNT();
+    launch_small_linear(e1, params + f.d2.kernel, params + f.d2.bias, e2, T, kFilmHid, kFilmHid, 0, st); CNT();
+    launch_small_linear(e2, params + f.ss.kernel, params + f.ss.bias,
                         tab + static_cast<size_t>(k) * T * 2 * Md, T, kFilmHid, 2 * Md, 0, st); CNT();
   }
   SMD_LAUNCH_CHECK("film table");
@@ -972,9 +955,9 @@ static int ensure_film_table(smd_plan* plan, const float* params, cudaStream_t s
 static int reverse_step_impl(smd_plan* plan, const float* params, const float* x, int n, int t, const float* z,
                              const float* infill_x, const float* infill_mask, const float* infill_z, float* x_next,
                              float* eps_hat, float* collection, float* metrics, cudaStream_t st) {
-  float* tvec = plan->buf<float>("tvec");
-  int* t_ptr = plan->buf<int>("t_ptr");
-  const float* coef = plan->buf<float>("coef");
+  float* tvec = plan->at<float>(plan->reg.tvec);
+  int* t_ptr = plan->at<int>(plan->reg.t_ptr);
+  const float* coef = plan->at<float>(plan->reg.coef);
   const bool use_tab = plan->film_tab_ready && plan->film_tab_params == params;
   if (use_tab) {
     plan->film_tab_on = true;
@@ -986,17 +969,17 @@ static int reverse_step_impl(smd_plan* plan, const float* params, const float* x
   } else {
     launch_fill_cond(coef, t_ptr, tvec, 1, st); CNT();
   }
-  float* eh = eps_hat ? eps_hat : plan->buf<float>("eps_hat");
-  int rc = run_forward(plan, params, x, tvec, 1, n, eh, st, nullptr);
+  float* eh = eps_hat ? eps_hat : plan->at<float>(plan->reg.eps_hat);
+  int rc = run_forward(plan, params, x, tvec, 1, n, eh, st, false);
   plan->film_tab_on = false;
   plan->film_row_dev = nullptr;
   if (rc) return rc;
   ReverseStepArgs a;
   memset(&a, 0, sizeof(a));
   a.x = x; a.eps_hat = eh; a.z = z;
-  a.key_tab = plan->buf<uint32_t>("keys");
+  a.key_tab = plan->at<uint32_t>(plan->reg.keys);
   a.coef = coef;
-  a.slot_tab = plan->buf<int>("slots");
+  a.slot_tab = plan->at<int>(plan->reg.slots);
   a.t_ptr = (t >= 0) ? nullptr : t_ptr;
   a.t = t;
   a.infill_x = infill_x; a.infill_mask = infill_mask; a.infill_z = infill_z;
@@ -1065,7 +1048,7 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
     SMD_CUDA(cudaStreamWaitEvent(plan->own_stream, plan->own_event, 0));
     cs = plan->own_stream;
   }
-  int* t_ptr = plan->buf<int>("t_ptr");
+  int* t_ptr = plan->at<int>(plan->reg.t_ptr);
   const int t0 = T - 1;
   SMD_CUDA(cudaMemcpyAsync(t_ptr, &t0, sizeof(int), cudaMemcpyHostToDevice, cs));
   SMD_CUDA(cudaStreamSynchronize(cs));  // t0 is a stack variable
@@ -1148,18 +1131,19 @@ int smd_threefry_split(const uint32_t host_key[2], int num, uint32_t* host_out_k
 int smd_debug_forward_save(smd_plan* plan, const float* params, const float* x, const float* t, int batch, float* y,
                            smd_stream_t stream) {
   if (!plan->cfg.training) { set_error("plan was not created with training = 1"); return SMD_ERR_STATE; }
-  return run_forward(plan, params, x, t, 0, batch, y, static_cast<cudaStream_t>(stream), &plan->train);
+  return run_forward(plan, params, x, t, 0, batch, y, static_cast<cudaStream_t>(stream), true);
 }
 
 int smd_debug_buffer(smd_plan* plan, const char* name, void** dev_ptr, size_t* bytes) {
   if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
-  auto it = plan->ws_off.find(name);
-  if (it == plan->ws_off.end()) { set_error(std::string("no workspace region named ") + name); return SMD_ERR_INVALID; }
-  size_t end = plan->ws_bytes;
-  for (const auto& kv : plan->ws_off) if (kv.second > it->second && kv.second < end) end = kv.second;
-  if (dev_ptr) *dev_ptr = plan->ws + it->second;
-  if (bytes) *bytes = end - it->second;
-  return SMD_OK;
+  for (const WsRegion& r : plan->regions) {
+    if (r.name != name) continue;
+    if (dev_ptr) *dev_ptr = plan->ws + r.offset;
+    if (bytes) *bytes = r.bytes;
+    return SMD_OK;
+  }
+  set_error(std::string("no workspace region named ") + name);
+  return SMD_ERR_INVALID;
 }
 
 int smd_gemm_bf16(const void* A, const void* B, int M, int N, int K, int a_mn, int b_mn, int BN, int cta_group,

@@ -1,66 +1,8 @@
-// Training-side pieces of libsmd: saved-activation workspace, fused clip + Adam (+EMA), EMA update.
+// Training-side pieces of libsmd: fused clip + Adam (+EMA), EMA update.
 // (The backward pass itself lives in backward.cu.)
-#include "train.cuh"
-#include "kernels.cuh"
+#include "plan.cuh"
 
 namespace smd {
-
-void train_workspace(TrainState& ts, const smd_config& c, int Mp, int K,
-                     const std::function<size_t(const std::string&, size_t)>& add) {
-  ts.enabled = true;
-  ts.L = (c.arch == SMD_ARCH_TRANSFORMER_DDPM) ? c.num_layers : 0;
-  ts.K = K; ts.H = c.num_heads; ts.Md = c.mlp_dims; ts.C = c.channels; ts.S = c.seq_len; ts.B = c.max_batch;
-  ts.Mp = static_cast<size_t>(Mp);
-  const size_t M = ts.Mp, Md = c.mlp_dims, B = c.max_batch;
-  const size_t Cp = (static_cast<size_t>(c.channels) + 63) / 64 * 64;
-  auto nm = [](const char* base, int i) { return std::string("t.") + base + std::to_string(i); };
-  for (int i = 0; i < 2 * ts.L + 1; ++i) ts.off_h.push_back(add(nm("h", i), M * kEt * 4));
-  for (int l = 0; l < ts.L; ++l) {
-    ts.off_a1.push_back(add(nm("a1_", l), M * kEt * 2));
-    ts.off_a2.push_back(add(nm("a2_", l), M * kEt * 2));
-    ts.off_qkv.push_back(add(nm("qkv", l), M * 3 * kEt * 4));
-    ts.off_probs.push_back(add(nm("probs", l), B * c.num_heads * 32 * 32 * 4));
-    ts.off_o.push_back(add(nm("o", l), M * kEt * 2));
-    ts.off_hidden_pre.push_back(add(nm("hpre", l), M * Md * 2));
-    ts.off_hidden.push_back(add(nm("hid", l), M * Md * 2));
-  }
-  if (ts.L) ts.off_a_post = add("t.a_post", M * kEt * 2);
-  for (int k = 0; k < K + 1; ++k) ts.off_u.push_back(add(nm("u", k), M * Md * 4));
-  for (int k = 0; k < K; ++k) {
-    ts.off_r1.push_back(add(nm("r1_", k), M * Md * 4));
-    ts.off_act_a.push_back(add(nm("acta", k), M * Md * 2));
-    ts.off_act_b.push_back(add(nm("actb", k), M * Md * 2));
-    ts.off_e1pre.push_back(add(nm("e1pre", k), B * 512 * 4));
-    ts.off_e1.push_back(add(nm("e1_", k), B * 512 * 4));
-    ts.off_e2.push_back(add(nm("e2_", k), B * 512 * 4));
-  }
-  ts.off_act_out = add("t.act_out", M * Md * 2);
-  ts.off_g32a = add("t.g32a", M * Md * 4);
-  ts.off_g32b = add("t.g32b", M * Md * 4);
-  for (int k = 0; k < K + 1; ++k) ts.off_du16.push_back(add(nm("du16_", k), M * Md * 2));
-  for (int k = 0; k < K; ++k) ts.off_dr16t.push_back(add(nm("dr16t_", k), M * Md * 2));
-  ts.off_dh = add("t.dh", M * kEt * 4);
-  ts.off_dh2 = add("t.dh2", M * kEt * 4);
-  for (int l = 0; l < ts.L; ++l) {
-    ts.off_dh16a.push_back(add(nm("dh16a", l), M * kEt * 2));
-    ts.off_dh16b.push_back(add(nm("dh16b", l), M * kEt * 2));
-    ts.off_dr16.push_back(add(nm("dr16_", l), M * Md * 2));
-    ts.off_dqkv16.push_back(add(nm("dqkv16_", l), M * 3 * kEt * 2));
-  }
-  ts.off_dh16_in = add("t.dh16_in", M * kEt * 2);
-  ts.off_dqkv32 = add("t.dqkv32", M * 3 * kEt * 4);
-  ts.off_dpred16 = add("t.dpred16", M * Cp * 2);
-  ts.off_dpred32 = add("t.dpred32", M * c.channels * 4);
-  ts.off_dss = add("t.dss", static_cast<size_t>(K > 0 ? K : 1) * B * 2 * Md * 4);   // one [B][2Md] block per FiLM pair
-  ts.off_de = add("t.de", B * 512 * 4);
-  ts.off_de2 = add("t.de2", B * 512 * 4);
-  ts.off_loss = add("t.loss", B * 4);
-  ts.off_loss_ctr = add("t.loss_ctr", 64);
-  add("t.ind", 64);   // device table {x0, used_alpha, eps} of the graph-replayed step   // block-completion counter of the loss kernel (zeroed at bind, self-resetting)
-  const size_t Bp = (B + 127) / 128 * 128;
-  ts.off_e2_16 = add("t.e2_16", Bp * 512 * 2);
-  ts.off_dss16 = add("t.dss16", Bp * 2 * Md * 2);
-}
 
 // ---------------------------------------------------------------------------------------------------
 // fused global-norm clip + Adam (+ EMA)        (train_ncsn.py:284-287, flax.optim.Adam, train_utils.py:73-78)
