@@ -52,7 +52,7 @@ typedef struct smd_config {
   int num_heads;       /* --num_heads    (train_ncsn.py:70)  ignored by DenseDDPM */
   int num_mlp_layers;  /* --num_mlp_layers (train_ncsn.py:71) FiLM res-blocks K, ignored by DenseDDPM */
   int mlp_dims;        /* --mlp_dims     (train_ncsn.py:72) */
-  int seq_len;         /* S: data_shape[0] (32) for TransformerDDPM, 1 for DenseDDPM */
+  int seq_len;         /* S: data_shape[0] for TransformerDDPM, one of 32, 64, 128 (else SMD_ERR_INVALID); 1 for DenseDDPM */
   int channels;        /* C: data_shape[-1] after --slice_ckpt (42 / 146 / 512) */
   int max_batch;       /* largest number of examples one call may pass */
   int cta_group;       /* 1 or 2 (accepted for compatibility; sm_90a GEMMs use one CTA per tile) */

@@ -352,7 +352,7 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     e.out_f32 = da32; e.ld_f32 = 128;
     SMD_CUDA(launch_gemm(ts.dXo[l], M, e, st));
     SMD_CUDA(launch_attention_bwd(F32(w.qkv[l]), F32(w.probs[l]), da32, B16(ts.dqkv16[l]), grads + lp.qkv.bias,
-                                  batch, c.num_heads, st));
+                                  batch, S, c.num_heads, st));
     CNT();
     SMD_CUDA(fork_dw());
     e = epi();

@@ -29,7 +29,7 @@ struct LnFilmBwdArgs {
   float* dss;            // [nsamples][2N] gradient of [scale | shift], or null
   int dss_accum;         // 0: overwrite, 1: add (second use of the same FiLM pair).  The sequence fast path always
                          // ADDS: the caller zero-fills dss once per backward pass
-  int M, N, S;           // S in {1, 32}: rows per sample
+  int M, N, S;           // rows per sample: 1, or a multiple of 32 (32, 64, 128)
 };
 
 // blockDim.x = N / 4 threads (N <= 4096): each thread owns one float4 column group; 4 rows per iteration so
@@ -48,7 +48,7 @@ ln_film_act_bwd_kernel(const LnFilmBwdArgs a) {
   const int c = tid * 4;
   const float inv_n = 1.0f / static_cast<float>(N);
   const bool film = a.ss != nullptr;
-  const bool per_block_sample = (a.S == 32);
+  const bool per_block_sample = (a.S % 32 == 0);   // the CTA's 32 rows lie inside sample r0 / S
   float gam[4], bet[4], sc[4] = {1.f, 1.f, 1.f, 1.f}, sh[4] = {0.f, 0.f, 0.f, 0.f};
   float acc_dg[4] = {0, 0, 0, 0}, acc_db[4] = {0, 0, 0, 0}, acc_bias[4] = {0, 0, 0, 0};
   float acc_dsc[4] = {0, 0, 0, 0}, acc_dsh[4] = {0, 0, 0, 0};
@@ -59,7 +59,7 @@ ln_film_act_bwd_kernel(const LnFilmBwdArgs a) {
     bet[0] = b4.x; bet[1] = b4.y; bet[2] = b4.z; bet[3] = b4.w;
   }
   if (film && per_block_sample && r0 < a.M) {
-    const float* sp = a.ss + static_cast<size_t>(r0 / 32) * 2 * N;
+    const float* sp = a.ss + static_cast<size_t>(r0 / a.S) * 2 * N;
     const float4 s4 = *reinterpret_cast<const float4*>(sp + c);
     const float4 h4 = *reinterpret_cast<const float4*>(sp + N + c);
     sc[0] = s4.x; sc[1] = s4.y; sc[2] = s4.z; sc[3] = s4.w;
@@ -199,7 +199,7 @@ ln_film_act_bwd_kernel(const LnFilmBwdArgs a) {
     if (a.dbias) atomicAdd(a.dbias + c + i, acc_bias[i]);
   }
   if (film && per_block_sample && a.dss && r0 < a.M) {
-    float* dp = a.dss + static_cast<size_t>(r0 / 32) * 2 * N;
+    float* dp = a.dss + static_cast<size_t>(r0 / a.S) * 2 * N;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       if (a.dss_accum) { dp[c + i] += acc_dsc[i]; dp[N + c + i] += acc_dsh[i]; }
@@ -209,13 +209,13 @@ ln_film_act_bwd_kernel(const LnFilmBwdArgs a) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Fast path of the same backward for the sequence model (32 rows per sample, all rows valid, bf16 incoming
-// gradient): 16 rows per CTA, two CTAs resident per SM (<= 64 registers), two rows per iteration.  The FiLM pair is
+// Fast path of the same backward for the sequence model (a multiple of 32 rows per sample, all rows valid, bf16
+// incoming gradient): 16 rows per CTA, all inside sample r0 / S, two CTAs resident per SM (<= 64 registers), two rows per iteration.  The FiLM pair is
 // constant over the CTA, so per column only A1 = sum(dact) and A2 = sum(dact * xhat) are accumulated:
 //   dbeta = sc A1, dgamma = sc A2, dshift = A1, dscale = gamma A2 + beta A1.
 // Row reductions: 4 values per thread -> 6-shuffle multi-value butterfly -> [value][warp] smem -> one
 // __syncthreads -> every warp folds the 16 partials itself (no second barrier; smem is double buffered).
-// dss must be zero-initialised by the caller: the two CTAs of a sample add into it.
+// dss must be zero-initialised by the caller: the S / 16 CTAs of a sample add into it.
 // ---------------------------------------------------------------------------------------------------
 template <int BYTES>
 __device__ __forceinline__ void cp_async_own(void* smem_dst, const void* gsrc) {   // per-thread LDGSTS, 8 or 16 bytes
@@ -257,7 +257,7 @@ ln_film_bwd_fast_kernel(const LnFilmBwdArgs a) {
     A[0] = g4.x; A[1] = g4.y; A[2] = g4.z; A[3] = g4.w;
     if constexpr (FILM) {
       const float4 b4 = *reinterpret_cast<const float4*>(a.beta + c);
-      const float* sp = a.ss + static_cast<size_t>(r0 / 32) * 2 * N;
+      const float* sp = a.ss + static_cast<size_t>(r0 / a.S) * 2 * N;
       const float4 s4 = *reinterpret_cast<const float4*>(sp + c);
       const float4 h4 = *reinterpret_cast<const float4*>(sp + N + c);
       Bc[0] = fmaf(b4.x, s4.x, h4.x); Bc[1] = fmaf(b4.y, s4.y, h4.y);
@@ -391,7 +391,7 @@ ln_film_bwd_fast_kernel(const LnFilmBwdArgs a) {
     gam[0] = g4.x; gam[1] = g4.y; gam[2] = g4.z; gam[3] = g4.w;
     if constexpr (FILM) {
       const float4 b4 = *reinterpret_cast<const float4*>(a.beta + c);
-      const float4 s4 = *reinterpret_cast<const float4*>(a.ss + static_cast<size_t>(r0 / 32) * 2 * N + c);
+      const float4 s4 = *reinterpret_cast<const float4*>(a.ss + static_cast<size_t>(r0 / a.S) * 2 * N + c);
       bet[0] = b4.x; bet[1] = b4.y; bet[2] = b4.z; bet[3] = b4.w;
       sc[0] = s4.x; sc[1] = s4.y; sc[2] = s4.z; sc[3] = s4.w;
     }
@@ -404,7 +404,7 @@ ln_film_bwd_fast_kernel(const LnFilmBwdArgs a) {
   }
   if constexpr (FILM) {
     if (a.dss) {
-      float* dp = a.dss + static_cast<size_t>(r0 / 32) * 2 * N;
+      float* dp = a.dss + static_cast<size_t>(r0 / a.S) * 2 * N;
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         atomicAdd(dp + c + i, fmaf(gam[i], A2[i], bet[i] * A1[i]));
@@ -417,7 +417,7 @@ ln_film_bwd_fast_kernel(const LnFilmBwdArgs a) {
 inline void launch_ln_film_act_bwd(const LnFilmBwdArgs& a, cudaStream_t st) {
   const int threads = a.N / 4;
   const bool film = a.ss != nullptr;
-  if (a.S == 32 && a.g16 && !a.g && threads <= 512 && threads % 32 == 0 && a.M % 32 == 0 &&
+  if (a.S % 32 == 0 && a.g16 && !a.g && threads <= 512 && threads % 32 == 0 && a.M % 32 == 0 &&
       ((film && a.act == 2) || (!film && a.act == 0))) {
     const int fb = a.M / 16;
     const int key = (a.u16 ? 4 : 0) | (a.dres ? 2 : 0) | (film ? 1 : 0);
@@ -587,7 +587,7 @@ inline void launch_colsum(const T* in, int ld, float* out, int M, int N, cudaStr
 }
 
 // ---------------------------------------------------------------------------------------------------
-// attention backward (SURVEY Appendix E): one CTA per sample, one warp per head, lane = query / key index
+// attention backward at S = 32 (SURVEY Appendix E): one CTA per sample, one warp per head, lane = query / key index
 // ---------------------------------------------------------------------------------------------------
 template <int DH>
 __global__ void attention_bwd_kernel(const float* __restrict__ qkv, const float* __restrict__ probs,
@@ -918,8 +918,183 @@ attention_bwd_mma_kernel(const float* __restrict__ qkv, const float* __restrict_
   emit(dv, 256, 1.0f);
 }
 
+// ---------------------------------------------------------------------------------------------------
+// Attention backward for S in {64, 128} (any head dim): P and dS of 32 queries x S keys do not fit a warp's registers,
+// so a CTA (one sample, HPB heads) walks the S / 32 query blocks of its sample and, inside each, the S / 32 key blocks.
+//   query block qb (lane = query i):  rs_i = sum_j dP_ij P_ij ;  dS_ij = P_ij (dP_ij - rs_i) ;  dq_i = sum_j dS_ij k_j
+//   per key block (lane = key j):     dv_j += sum_{i in qb} P_ij dO_i ;  dk_j += sum_{i in qb} dS_ij q~_i
+// dP_ij = dO_i . v_j is recomputed in the second sweep instead of being kept.  dq is written once per query block;
+// dk and dv accumulate in fp32 shared memory (a warp owns its head's columns) and are written once at the end.  The
+// bias gradients are the same column sums, added with one atomic per column and block.
+// ---------------------------------------------------------------------------------------------------
+template <int DH, int S>
+__global__ void __launch_bounds__(128)
+attention_bwd_long_kernel(const float* __restrict__ qkv, const float* __restrict__ probs, const float* __restrict__ dO,
+                          __nv_bfloat16* __restrict__ dqkv16, float* __restrict__ dbias, int H) {
+  pdl_trigger();
+  pdl_wait();
+  extern __shared__ __align__(16) float attl_sm[];
+  const int HPB = blockDim.x >> 5, W = HPB * DH, W4 = W / 4;
+  const int hb = blockIdx.y * HPB;
+  float* sQ = attl_sm;             // [S][W] q / sqrt(dh)
+  float* sK = sQ + S * W;
+  float* sV = sK + S * W;
+  float* sD = sV + S * W;          // dO
+  float* sdK = sD + S * W;         // [S][W] fp32 accumulators
+  float* sdV = sdK + S * W;
+  float* scr = sdV + S * W;        // [HPB][2][32][33]: P and dS of one (query block, key block) tile
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const float qs = rsqrtf(static_cast<float>(DH));
+  const float* base = qkv + static_cast<size_t>(b) * S * 384;
+  const float* dob = dO + static_cast<size_t>(b) * S * 128;
+  for (int i = tid; i < S * W4; i += blockDim.x) {
+    const int row = i / W4, c4 = (i % W4) * 4, gc = hb * DH + c4;
+    float4 q4 = *reinterpret_cast<const float4*>(base + row * 384 + gc);
+    q4.x *= qs; q4.y *= qs; q4.z *= qs; q4.w *= qs;
+    *reinterpret_cast<float4*>(&sQ[row * W + c4]) = q4;
+    *reinterpret_cast<float4*>(&sK[row * W + c4]) = *reinterpret_cast<const float4*>(base + row * 384 + 128 + gc);
+    *reinterpret_cast<float4*>(&sV[row * W + c4]) = *reinterpret_cast<const float4*>(base + row * 384 + 256 + gc);
+    *reinterpret_cast<float4*>(&sD[row * W + c4]) = *reinterpret_cast<const float4*>(dob + row * 128 + gc);
+    *reinterpret_cast<float4*>(&sdK[row * W + c4]) = make_float4(0.f, 0.f, 0.f, 0.f);
+    *reinterpret_cast<float4*>(&sdV[row * W + c4]) = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  __syncthreads();
+  const int hl = tid >> 5, lane = tid & 31;
+  const int h = hb + hl;
+  if (h >= H) return;
+  float* tP = scr + hl * 2 * 32 * 33;
+  float* tS = tP + 32 * 33;
+  const int hc = hl * DH;      // column offset inside the staged tiles
+  const int gh = h * DH;       // column offset in global memory
+  auto dot_dO_v = [&](const float (&d_i)[DH], int j) {
+    float s = 0.f;
+#pragma unroll
+    for (int d = 0; d < DH; d += 4) {   // broadcast 16-byte reads
+      const float4 t = *reinterpret_cast<const float4*>(&sV[j * W + hc + d]);
+      s = fmaf(d_i[d], t.x, fmaf(d_i[d + 1], t.y, fmaf(d_i[d + 2], t.z, fmaf(d_i[d + 3], t.w, s))));
+    }
+    return s;
+  };
+  for (int qb = 0; qb < S / 32; ++qb) {
+    const int qi = qb * 32 + lane;
+    const float* pr = probs + ((static_cast<size_t>(b) * H + h) * S + qi) * S;
+    float dO_i[DH];
+#pragma unroll
+    for (int d = 0; d < DH; d += 4) {
+      const float4 t = *reinterpret_cast<const float4*>(&sD[qi * W + hc + d]);
+      dO_i[d] = t.x; dO_i[d + 1] = t.y; dO_i[d + 2] = t.z; dO_i[d + 3] = t.w;
+    }
+    float rs = 0.f;
+    for (int j = 0; j < S; j += 4) {
+      const float4 p4 = *reinterpret_cast<const float4*>(pr + j);
+      rs = fmaf(dot_dO_v(dO_i, j), p4.x, rs); rs = fmaf(dot_dO_v(dO_i, j + 1), p4.y, rs);
+      rs = fmaf(dot_dO_v(dO_i, j + 2), p4.z, rs); rs = fmaf(dot_dO_v(dO_i, j + 3), p4.w, rs);
+    }
+    float dq[DH];
+#pragma unroll
+    for (int d = 0; d < DH; ++d) dq[d] = 0.f;
+    for (int kb = 0; kb < S / 32; ++kb) {
+      // lane = query: this tile's P and dS rows, and dq
+#pragma unroll 4
+      for (int jj = 0; jj < 32; jj += 4) {
+        const int j0 = kb * 32 + jj;
+        const float4 p4 = *reinterpret_cast<const float4*>(pr + j0);
+        const float pv[4] = {p4.x, p4.y, p4.z, p4.w};
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const int j = j0 + u;
+          const float ds = pv[u] * (dot_dO_v(dO_i, j) - rs);
+          tP[lane * 33 + jj + u] = pv[u];
+          tS[lane * 33 + jj + u] = ds;
+#pragma unroll
+          for (int d = 0; d < DH; d += 4) {
+            const float4 t = *reinterpret_cast<const float4*>(&sK[j * W + hc + d]);
+            dq[d] = fmaf(ds, t.x, dq[d]); dq[d + 1] = fmaf(ds, t.y, dq[d + 1]);
+            dq[d + 2] = fmaf(ds, t.z, dq[d + 2]); dq[d + 3] = fmaf(ds, t.w, dq[d + 3]);
+          }
+        }
+      }
+      __syncwarp();
+      // lane = key kb * 32 + lane: contributions of this query block to dv and dk
+      float dv[DH], dk[DH];
+#pragma unroll
+      for (int d = 0; d < DH; ++d) { dv[d] = 0.f; dk[d] = 0.f; }
+#pragma unroll 4
+      for (int i = 0; i < 32; ++i) {
+        const float p = tP[i * 33 + lane], s = tS[i * 33 + lane];
+        const int row = (qb * 32 + i) * W + hc;
+#pragma unroll
+        for (int d = 0; d < DH; d += 4) {
+          const float4 td = *reinterpret_cast<const float4*>(&sD[row + d]);
+          const float4 tq = *reinterpret_cast<const float4*>(&sQ[row + d]);
+          dv[d] = fmaf(p, td.x, dv[d]); dv[d + 1] = fmaf(p, td.y, dv[d + 1]);
+          dv[d + 2] = fmaf(p, td.z, dv[d + 2]); dv[d + 3] = fmaf(p, td.w, dv[d + 3]);
+          dk[d] = fmaf(s, tq.x, dk[d]); dk[d + 1] = fmaf(s, tq.y, dk[d + 1]);
+          dk[d + 2] = fmaf(s, tq.z, dk[d + 2]); dk[d + 3] = fmaf(s, tq.w, dk[d + 3]);
+        }
+      }
+      const int krow = (kb * 32 + lane) * W + hc;
+#pragma unroll
+      for (int d = 0; d < DH; ++d) { sdV[krow + d] += dv[d]; sdK[krow + d] += dk[d]; }
+      __syncwarp();
+    }
+    __nv_bfloat16* orow = dqkv16 + (static_cast<size_t>(b) * S + qi) * 384 + gh;
+#pragma unroll
+    for (int d = 0; d < DH; d += 2)
+      *reinterpret_cast<__nv_bfloat162*>(orow + d) = __floats2bfloat162_rn(dq[d] * qs, dq[d + 1] * qs);
+#pragma unroll
+    for (int d = 0; d < DH; ++d) {
+      const float v = warp_sum(dq[d] * qs);
+      if (lane == 0) atomicAdd(dbias + gh + d, v);
+    }
+  }
+  // dk, dv: lane = key, one pass per key block (the warp wrote these rows itself: __syncwarp suffices)
+  for (int kb = 0; kb < S / 32; ++kb) {
+    const int kj = kb * 32 + lane;
+    __nv_bfloat16* orow = dqkv16 + (static_cast<size_t>(b) * S + kj) * 384 + gh;
+#pragma unroll
+    for (int d = 0; d < DH; d += 2) {
+      const float k0 = sdK[kj * W + hc + d], k1 = sdK[kj * W + hc + d + 1];
+      const float v0 = sdV[kj * W + hc + d], v1 = sdV[kj * W + hc + d + 1];
+      *reinterpret_cast<__nv_bfloat162*>(orow + 128 + d) = __floats2bfloat162_rn(k0, k1);
+      *reinterpret_cast<__nv_bfloat162*>(orow + 256 + d) = __floats2bfloat162_rn(v0, v1);
+    }
+#pragma unroll
+    for (int d = 0; d < DH; ++d) {
+      const float ksum = warp_sum(sdK[kj * W + hc + d]), vsum = warp_sum(sdV[kj * W + hc + d]);
+      if (lane == 0) { atomicAdd(dbias + 128 + gh + d, ksum); atomicAdd(dbias + 256 + gh + d, vsum); }
+    }
+  }
+}
+
+template <int S>
+inline cudaError_t launch_attention_bwd_long(const float* qkv, const float* probs, const float* dO,
+                                             __nv_bfloat16* dqkv16, float* dbias, int B, int H, cudaStream_t st) {
+  const int dh = 128 / H;
+  int hpb = H;
+  while (hpb > 4 && hpb % 2 == 0) hpb /= 2;
+  while (hpb > 1 && hpb * dh * S > 4096) hpb /= 2;   // <= 4096 staged elements per tile: ~100 KB, two CTAs per SM
+  const size_t smem = (6 * static_cast<size_t>(S) * hpb * dh + static_cast<size_t>(hpb) * 2 * 32 * 33) * sizeof(float);
+  const dim3 grid(B, H / hpb);
+#define SMD_ATT_BWD_LONG(DHV)                                                                                        \
+  {                                                                                                                  \
+    cudaError_t e = cudaFuncSetAttribute(attention_bwd_long_kernel<DHV, S>,                                          \
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));       \
+    if (e != cudaSuccess) return e;                                                                                  \
+    attention_bwd_long_kernel<DHV, S><<<grid, hpb * 32, smem, st>>>(qkv, probs, dO, dqkv16, dbias, H);               \
+    return cudaPeekAtLastError();                                                                                    \
+  }
+  if (dh == 16) SMD_ATT_BWD_LONG(16)
+  else if (dh == 8) SMD_ATT_BWD_LONG(8)
+  else if (dh == 32) SMD_ATT_BWD_LONG(32)
+  else SMD_ATT_BWD_LONG(4)
+#undef SMD_ATT_BWD_LONG
+}
+
 inline cudaError_t launch_attention_bwd(const float* qkv, const float* probs, const float* dO, __nv_bfloat16* dqkv16,
-                                        float* dbias, int B, int H, cudaStream_t st) {
+                                        float* dbias, int B, int S, int H, cudaStream_t st) {
+  if (S == 64) return launch_attention_bwd_long<64>(qkv, probs, dO, dqkv16, dbias, B, H, st);
+  if (S == 128) return launch_attention_bwd_long<128>(qkv, probs, dO, dqkv16, dbias, B, H, st);
   const int dh = 128 / H;
   int hpb = H;                       // heads per CTA: <= 4 so that several CTAs are resident per SM
   while (hpb > 4 && hpb % 2 == 0) hpb /= 2;

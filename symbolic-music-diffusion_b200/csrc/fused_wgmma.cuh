@@ -224,7 +224,8 @@ struct AttnBlockArgs {
   const float* ln_gamma;         // [128] LayerNorm of the new residual stream -> out_bf16
   const float* ln_beta;
   __nv_bfloat16* out_bf16;       // bf16 [M][128]
-  int M, H;                      // tokens (a multiple of 32); heads (dh = 128 / H in {8, 16})
+  int M, H;                      // tokens (a multiple of S); heads (dh = 128 / H in {8, 16})
+  int S;                         // sequence length: 32 (two samples per 64-row tile) or 64 (one)
 };
 
 struct AttnSmem {
@@ -245,7 +246,7 @@ struct AttnSmem {
   static_assert(offO % 1024 == 0, "O operand must be 1024-byte aligned");
 };
 
-template <int DH>
+template <int DH, int SEQ>
 __global__ void __launch_bounds__(AttnSmem::kThreads, 1)
 attn_block_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmWqkv,
                   const __grid_constant__ CUtensorMap tmWo, const AttnBlockArgs p) {
@@ -321,19 +322,22 @@ attn_block_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
       asm volatile("bar.sync 1, 128;" ::: "memory");
       // ---------------- attention: warp = head, lane = query (attention_kernel's arithmetic) ----------------
-      for (int s = 0; s < 2; ++s) {
-        const int smp = m0 / 32 + s;
-        if (smp * 32 >= p.M) break;
-        const float* base = qkv_s + (32 * s) * S::kQkvPitch;
-        for (int h = static_cast<int>(wl); h < p.H; h += 4) {
+      // the tile holds 64 / SEQ whole samples; a lane takes queries lane, lane + 32, ... of its sample
+      for (int s = 0; s < 64 / SEQ; ++s) {
+        const int smp = m0 / SEQ + s;
+        if (smp * SEQ >= p.M) break;
+        const float* base = qkv_s + (SEQ * s) * S::kQkvPitch;
+        for (int h = static_cast<int>(wl); h < p.H; h += 4)
+        for (int qh = 0; qh < SEQ / 32; ++qh) {
+          const int qrow = 32 * qh + static_cast<int>(lane);
           float q[DH];
           const float qs = rsqrtf(static_cast<float>(DH));
 #pragma unroll
-          for (int d = 0; d < DH; ++d) q[d] = base[lane * S::kQkvPitch + h * DH + d] * qs;   // flax: query / sqrt(depth)
-          float sc[32];
+          for (int d = 0; d < DH; ++d) q[d] = base[qrow * S::kQkvPitch + h * DH + d] * qs;   // flax: query / sqrt(depth)
+          float sc[SEQ];
           float mx = -INFINITY;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
+          for (int j = 0; j < SEQ; ++j) {
             float sj = 0.f;
             const float4* kr = reinterpret_cast<const float4*>(base + j * S::kQkvPitch + 128 + h * DH);
 #pragma unroll
@@ -347,13 +351,13 @@ attn_block_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           }
           float sum = 0.f;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) { sc[j] = expf(sc[j] - mx); sum += sc[j]; }
+          for (int j = 0; j < SEQ; ++j) { sc[j] = expf(sc[j] - mx); sum += sc[j]; }
           const float inv = 1.0f / sum;
           float o[DH];
 #pragma unroll
           for (int d = 0; d < DH; ++d) o[d] = 0.f;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
+          for (int j = 0; j < SEQ; ++j) {
             const float pj = sc[j] * inv;
             const float4* vr = reinterpret_cast<const float4*>(base + j * S::kQkvPitch + 256 + h * DH);
 #pragma unroll
@@ -363,7 +367,7 @@ attn_block_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
               o[4 * d4 + 2] = fmaf(pj, v4.z, o[4 * d4 + 2]); o[4 * d4 + 3] = fmaf(pj, v4.w, o[4 * d4 + 3]);
             }
           }
-          const int orow = 32 * s + static_cast<int>(lane);
+          const int orow = SEQ * s + qrow;
 #pragma unroll
           for (int d = 0; d < DH; d += 2) {
             const int col = h * DH + d;

@@ -272,19 +272,20 @@ inline bool make_attn_op(AttnOp* op, const void* A, uint64_t rows, const void* W
 }
 inline cudaError_t launch_attn_block(const AttnOp& op, const AttnBlockArgs& a, cudaStream_t st) {
   const int dh = 128 / a.H;
-  if ((dh != 8 && dh != 16) || a.M % 32 != 0) return cudaErrorInvalidValue;
+  if ((dh != 8 && dh != 16) || (a.S != 32 && a.S != 64) || a.M % a.S != 0) return cudaErrorInvalidValue;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_block_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem::kTotal);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(attn_block_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem::kTotal);
-    if (e != cudaSuccess) return e;
+    for (auto k : {attn_block_kernel<16, 32>, attn_block_kernel<8, 32>, attn_block_kernel<16, 64>, attn_block_kernel<8, 64>}) {
+      const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem::kTotal);
+      if (e != cudaSuccess) return e;
+    }
     attr_set = true;
   }
   const int tiles = (a.M + 63) / 64;
   const int T = AttnSmem::kThreads, B = AttnSmem::kTotal;
-  if (dh == 16) return launch_persistent(attn_block_kernel<16>, tiles, T, B, st, op.tmA, op.tmWqkv, op.tmWo, a);
-  return launch_persistent(attn_block_kernel<8>, tiles, T, B, st, op.tmA, op.tmWqkv, op.tmWo, a);
+  auto kernel = a.S == 64 ? (dh == 16 ? attn_block_kernel<16, 64> : attn_block_kernel<8, 64>)
+                          : (dh == 16 ? attn_block_kernel<16, 32> : attn_block_kernel<8, 32>);
+  return launch_persistent(kernel, tiles, T, B, st, op.tmA, op.tmWqkv, op.tmWo, a);
 }
 
 }  // namespace smd

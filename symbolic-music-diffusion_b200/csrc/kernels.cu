@@ -176,23 +176,29 @@ void launch_embed(const float* x, const float* W_in, const float* b_in, const fl
 }
 
 // ---------------------------------------------------------------------------------------------------
-// attention: one CTA per sample, one warp per head, lane = query position (S = 32)
+// attention: one CTA per (sample, head group, 32-query block), one warp per head, lane = query position
+// (S in {32, 64, 128}: the CTA stages all S rows of k and v and its 32 rows of q)
 // ---------------------------------------------------------------------------------------------------
-template <int DH>
+template <int DH, int S>
 __global__ void attention_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ o,
                                  float* __restrict__ probs, int B, int H, long long lo_delta) {
   pdl_trigger();
   pdl_wait();
   // a CTA owns HPB = blockDim.x / 32 heads of one sample (W = HPB * DH columns of k and v): small CTAs, several
-  // resident per SM, so one CTA's global->shared fill overlaps another's math
-  __shared__ __align__(16) float sK[32 * 128];
-  __shared__ __align__(16) float sV[32 * 128];
+  // resident per SM, so one CTA's global->shared fill overlaps another's math.  S = 32 keeps static tiles; longer
+  // sequences stage S rows of k and v in dynamic shared memory (2 S W floats: over the 48 KB static limit at S = 128)
+  __shared__ __align__(16) float sK32[S == 32 ? 32 * 128 : 1];
+  __shared__ __align__(16) float sV32[S == 32 ? 32 * 128 : 1];
+  extern __shared__ __align__(16) float att_kv[];
   const int b = blockIdx.x;
   const int tid = threadIdx.x;
   const int HPB = blockDim.x >> 5, W = HPB * DH, W4 = W / 4;
   const int hb = blockIdx.y * HPB;
-  const float* base = qkv + static_cast<size_t>(b) * 32 * 384;
-  for (int i = tid; i < 32 * W4; i += blockDim.x) {
+  const int q0 = S == 32 ? 0 : blockIdx.z * 32;   // first query row of this CTA
+  float* sK = S == 32 ? sK32 : att_kv;
+  float* sV = S == 32 ? sV32 : att_kv + S * W;
+  const float* base = qkv + static_cast<size_t>(b) * S * 384;
+  for (int i = tid; i < S * W4; i += blockDim.x) {
     const int row = i / W4, c4 = (i % W4) * 4, gc = hb * DH + c4;
     *reinterpret_cast<float4*>(&sK[row * W + c4]) = *reinterpret_cast<const float4*>(base + row * 384 + 128 + gc);
     *reinterpret_cast<float4*>(&sV[row * W + c4]) = *reinterpret_cast<const float4*>(base + row * 384 + 256 + gc);
@@ -203,13 +209,13 @@ __global__ void attention_kernel(const float* __restrict__ qkv, __nv_bfloat16* _
   if (h >= H) return;
   float q[DH];
   const float qs = rsqrtf(static_cast<float>(DH));
-  const float* qr = base + lane * 384 + h * DH;
+  const float* qr = base + (q0 + lane) * 384 + h * DH;
 #pragma unroll
   for (int d = 0; d < DH; ++d) q[d] = qr[d] * qs;   // flax: query / sqrt(depth) before the dot
-  float sc[32];
+  float sc[S];
   float mx = -INFINITY;
 #pragma unroll
-  for (int j = 0; j < 32; ++j) {
+  for (int j = 0; j < S; ++j) {
     float s = 0.f;
     const float4* kr = reinterpret_cast<const float4*>(&sK[j * W + hl * DH]);
 #pragma unroll
@@ -223,13 +229,13 @@ __global__ void attention_kernel(const float* __restrict__ qkv, __nv_bfloat16* _
   }
   float sum = 0.f;
 #pragma unroll
-  for (int j = 0; j < 32; ++j) { sc[j] = expf(sc[j] - mx); sum += sc[j]; }
+  for (int j = 0; j < S; ++j) { sc[j] = expf(sc[j] - mx); sum += sc[j]; }
   const float inv = 1.0f / sum;
   float acc[DH];
 #pragma unroll
   for (int d = 0; d < DH; ++d) acc[d] = 0.f;
 #pragma unroll
-  for (int j = 0; j < 32; ++j) {
+  for (int j = 0; j < S; ++j) {
     const float p = sc[j] * inv;
     sc[j] = p;
     const float4* vr = reinterpret_cast<const float4*>(&sV[j * W + hl * DH]);
@@ -240,28 +246,29 @@ __global__ void attention_kernel(const float* __restrict__ qkv, __nv_bfloat16* _
       acc[4 * d4 + 2] = fmaf(p, v4.z, acc[4 * d4 + 2]); acc[4 * d4 + 3] = fmaf(p, v4.w, acc[4 * d4 + 3]);
     }
   }
-  __nv_bfloat16* orow = o + (static_cast<size_t>(b) * 32 + lane) * 128 + h * DH;
+  __nv_bfloat16* orow = o + (static_cast<size_t>(b) * S + q0 + lane) * 128 + h * DH;
 #pragma unroll
   for (int d = 0; d < DH; d += 2) {
     *reinterpret_cast<__nv_bfloat162*>(orow + d) = __floats2bfloat162_rn(acc[d], acc[d + 1]);
     if (lo_delta) { orow[d + lo_delta] = bf16_lo_part(acc[d]); orow[d + 1 + lo_delta] = bf16_lo_part(acc[d + 1]); }
   }
   if (probs != nullptr) {
-    float* pr = probs + ((static_cast<size_t>(b) * H + h) * 32 + lane) * 32;
+    float* pr = probs + ((static_cast<size_t>(b) * H + h) * S + q0 + lane) * S;
 #pragma unroll
-    for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(pr + j) = make_float4(sc[j], sc[j + 1], sc[j + 2], sc[j + 3]);
+    for (int j = 0; j < S; j += 4) *reinterpret_cast<float4*>(pr + j) = make_float4(sc[j], sc[j + 1], sc[j + 2], sc[j + 3]);
   }
 }
 // ---------------------------------------------------------------------------------------------------
 // Tensor-core variant (DH % 8 == 0): same CTA / warp mapping, but Q K^T and P V run on mma.sync m16n8k8 tf32
-// (a 32x32x16 problem per head is far below a wgmma tile; ~350 instructions per warp instead of ~2000).
+// (a 32xSx16 problem per head is far below a wgmma tile; ~350 instructions per warp instead of ~2000 at S = 32):
+// S / 8 n-tiles for Q K^T and S / 8 k-steps for P V.
 // q, k, v are rounded to tf32 once while the CTA stages them in shared memory (row pitch = W + 4 words, so every
 // fragment read is bank-conflict free); scores, softmax and the P V accumulation stay fp32.  The softmax output is
 // fed to the second MMA straight from the accumulator registers: within each block of 8 keys, k-slot t holds key 2t
 // and k-slot t+4 holds key 2t+1, and the V fragment is read with the same permutation (a sum over keys does not
 // care about their order), so no shuffles are needed between the two products.
 // ---------------------------------------------------------------------------------------------------
-template <int DH>
+template <int DH, int S>
 __global__ void __launch_bounds__(128)
 attention_mma_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ o, float* __restrict__ probs, int B, int H) {
   pdl_trigger();
@@ -269,18 +276,20 @@ attention_mma_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ 
   extern __shared__ __align__(16) uint32_t att_sm[];
   const int tid = threadIdx.x;
   const int HPB = blockDim.x >> 5, W = HPB * DH, W4 = W / 4, P = W + 4;
-  uint32_t* sQ = att_sm;
-  uint32_t* sK = sQ + 32 * P;
-  uint32_t* sV = sK + 32 * P;
-  const int b = blockIdx.x, hb = blockIdx.y * HPB;
+  uint32_t* sQ = att_sm;          // [32][P]: this CTA's query block
+  uint32_t* sK = sQ + 32 * P;     // [S][P]
+  uint32_t* sV = sK + S * P;      // [S][P]
+  const int b = blockIdx.x, hb = blockIdx.y * HPB, q0 = S == 32 ? 0 : blockIdx.z * 32;
   const float qs = rsqrtf(static_cast<float>(DH));   // flax: query / sqrt(depth) before the dot
-  const float* base = qkv + static_cast<size_t>(b) * 32 * 384;
-  for (int i = tid; i < 32 * W4; i += blockDim.x) {
+  const float* base = qkv + static_cast<size_t>(b) * S * 384;
+  for (int i = tid; i < S * W4; i += blockDim.x) {
     const int row = i / W4, c4 = (i % W4) * 4, gc = hb * DH + c4;
-    const float4 q4 = *reinterpret_cast<const float4*>(base + row * 384 + gc);
+    if (S == 32 || row < 32) {
+      const float4 q4 = *reinterpret_cast<const float4*>(base + (q0 + row) * 384 + gc);
+      *reinterpret_cast<uint4*>(&sQ[row * P + c4]) = make_uint4(to_tf32(q4.x * qs), to_tf32(q4.y * qs), to_tf32(q4.z * qs), to_tf32(q4.w * qs));
+    }
     const float4 k4 = *reinterpret_cast<const float4*>(base + row * 384 + 128 + gc);
     const float4 v4 = *reinterpret_cast<const float4*>(base + row * 384 + 256 + gc);
-    *reinterpret_cast<uint4*>(&sQ[row * P + c4]) = make_uint4(to_tf32(q4.x * qs), to_tf32(q4.y * qs), to_tf32(q4.z * qs), to_tf32(q4.w * qs));
     *reinterpret_cast<uint4*>(&sK[row * P + c4]) = make_uint4(to_tf32(k4.x), to_tf32(k4.y), to_tf32(k4.z), to_tf32(k4.w));
     *reinterpret_cast<uint4*>(&sV[row * P + c4]) = make_uint4(to_tf32(v4.x), to_tf32(v4.y), to_tf32(v4.z), to_tf32(v4.w));
   }
@@ -290,12 +299,13 @@ attention_mma_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ 
   if (h >= H) return;
   const int g = lane >> 2, t = lane & 3;
   const int hc = hl * DH;
-  // ---- S = (Q / sqrt(dh)) K^T : 2 m-tiles x 4 n-tiles, DH / 8 k-steps
-  float sc[2][4][4];
+  constexpr int NT = S / 8;   // key tiles
+  // ---- scores = (Q / sqrt(dh)) K^T : 2 m-tiles x S / 8 n-tiles, DH / 8 k-steps
+  float sc[2][NT][4];
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-    for (int nt = 0; nt < 4; ++nt)
+    for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
       for (int i = 0; i < 4; ++i) sc[mt][nt][i] = 0.f;
 #pragma unroll
@@ -307,26 +317,26 @@ attention_mma_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ 
       a[mt][0] = q0[0]; a[mt][1] = q0[8 * P]; a[mt][2] = q0[4]; a[mt][3] = q0[8 * P + 4];
     }
 #pragma unroll
-    for (int nt = 0; nt < 4; ++nt) {
+    for (int nt = 0; nt < NT; ++nt) {
       const uint32_t* k0 = sK + (8 * nt + g) * P + hc + 8 * ks + t;
       const uint32_t b0 = k0[0], b1 = k0[4];
       mma_tf32_16x8x8(sc[0][nt], a[0], b0, b1);
       mma_tf32_16x8x8(sc[1][nt], a[1], b0, b1);
     }
   }
-  // ---- row softmax: a row lives in the 4 lanes of a quad (t = 0..3), 8 values per lane
+  // ---- row softmax: a row lives in the 4 lanes of a quad (t = 0..3), S / 4 values per lane
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt) {
 #pragma unroll
     for (int hr = 0; hr < 2; ++hr) {   // hr = 0: row 16 mt + g (c0, c1); hr = 1: row 16 mt + g + 8 (c2, c3)
       float mx = -INFINITY;
 #pragma unroll
-      for (int nt = 0; nt < 4; ++nt) mx = fmaxf(mx, fmaxf(sc[mt][nt][2 * hr], sc[mt][nt][2 * hr + 1]));
+      for (int nt = 0; nt < NT; ++nt) mx = fmaxf(mx, fmaxf(sc[mt][nt][2 * hr], sc[mt][nt][2 * hr + 1]));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
       float sum = 0.f;
 #pragma unroll
-      for (int nt = 0; nt < 4; ++nt) {
+      for (int nt = 0; nt < NT; ++nt) {
         const float e0 = expf(sc[mt][nt][2 * hr] - mx), e1 = expf(sc[mt][nt][2 * hr + 1] - mx);
         sc[mt][nt][2 * hr] = e0; sc[mt][nt][2 * hr + 1] = e1;
         sum += e0 + e1;
@@ -335,20 +345,20 @@ attention_mma_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ 
       sum += __shfl_xor_sync(0xffffffffu, sum, 2);
       const float inv = 1.0f / sum;
 #pragma unroll
-      for (int nt = 0; nt < 4; ++nt) { sc[mt][nt][2 * hr] *= inv; sc[mt][nt][2 * hr + 1] *= inv; }
+      for (int nt = 0; nt < NT; ++nt) { sc[mt][nt][2 * hr] *= inv; sc[mt][nt][2 * hr + 1] *= inv; }
     }
   }
   if (probs != nullptr) {
-    float* pr = probs + (static_cast<size_t>(b) * H + h) * 32 * 32;
+    float* pr = probs + ((static_cast<size_t>(b) * H + h) * S + q0) * S;
 #pragma unroll
     for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-      for (int nt = 0; nt < 4; ++nt) {
-        *reinterpret_cast<float2*>(pr + (16 * mt + g) * 32 + 8 * nt + 2 * t) = make_float2(sc[mt][nt][0], sc[mt][nt][1]);
-        *reinterpret_cast<float2*>(pr + (16 * mt + g + 8) * 32 + 8 * nt + 2 * t) = make_float2(sc[mt][nt][2], sc[mt][nt][3]);
+      for (int nt = 0; nt < NT; ++nt) {
+        *reinterpret_cast<float2*>(pr + (16 * mt + g) * S + 8 * nt + 2 * t) = make_float2(sc[mt][nt][0], sc[mt][nt][1]);
+        *reinterpret_cast<float2*>(pr + (16 * mt + g + 8) * S + 8 * nt + 2 * t) = make_float2(sc[mt][nt][2], sc[mt][nt][3]);
       }
   }
-  // ---- O = P V : 2 m-tiles x DH / 8 n-tiles, 4 k-steps (one per block of 8 keys, permuted as described above)
+  // ---- O = P V : 2 m-tiles x DH / 8 n-tiles, S / 8 k-steps (one per block of 8 keys, permuted as described above)
   float acc[2][DH / 8][4];
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt)
@@ -357,7 +367,7 @@ attention_mma_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ 
 #pragma unroll
       for (int i = 0; i < 4; ++i) acc[mt][n2][i] = 0.f;
 #pragma unroll
-  for (int kb = 0; kb < 4; ++kb) {
+  for (int kb = 0; kb < NT; ++kb) {
     uint32_t a[2][4];
 #pragma unroll
     for (int mt = 0; mt < 2; ++mt) {
@@ -374,7 +384,7 @@ attention_mma_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ 
       mma_tf32_16x8x8(acc[1][n2], a[1], b0, b1);
     }
   }
-  __nv_bfloat16* ob = o + static_cast<size_t>(b) * 32 * 128 + h * DH;
+  __nv_bfloat16* ob = o + (static_cast<size_t>(b) * S + q0) * 128 + h * DH;
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
@@ -384,23 +394,25 @@ attention_mma_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ 
     }
 }
 
-void launch_attention(const float* qkv, __nv_bfloat16* o, float* probs_or_null, int B, int H, cudaStream_t st,
-                      long long lo_delta) {
+template <int S>
+static void launch_attention_s(const float* qkv, __nv_bfloat16* o, float* probs_or_null, int B, int H, cudaStream_t st,
+                               long long lo_delta) {
   const int dh = 128 / H;
   int hpb = H;
   while (hpb > 4 && hpb % 2 == 0) hpb /= 2;
-  const dim3 grid(B, H / hpb);
+  const dim3 grid(B, H / hpb, S / 32);
   const int threads = hpb * 32;
   if (lo_delta == 0 && dh % 8 == 0 && dh <= 32) {   // (strict mode: fp32 SIMT attention, no tf32 rounding)
-    const size_t smem = 3 * 32 * static_cast<size_t>(hpb * dh + 4) * sizeof(uint32_t);
+    const size_t smem = (32 + 2 * S) * static_cast<size_t>(hpb * dh + 4) * sizeof(uint32_t);
 #define SMD_ATT_MMA(DHV)                                                                                          \
   {                                                                                                               \
     static bool attr = false;                                                                                     \
     if (!attr) {                                                                                                  \
-      cudaFuncSetAttribute(attention_mma_kernel<DHV>, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * 32 * 132 * 4); \
+      cudaFuncSetAttribute(attention_mma_kernel<DHV, S>, cudaFuncAttributeMaxDynamicSharedMemorySize,             \
+                           (32 + 2 * S) * 132 * 4);                                                               \
       attr = true;                                                                                                \
     }                                                                                                             \
-    attention_mma_kernel<DHV><<<grid, threads, smem, st>>>(qkv, o, probs_or_null, B, H);                          \
+    attention_mma_kernel<DHV, S><<<grid, threads, smem, st>>>(qkv, o, probs_or_null, B, H);                       \
   }
     if (dh == 16) SMD_ATT_MMA(16)
     else if (dh == 8) SMD_ATT_MMA(8)
@@ -408,14 +420,33 @@ void launch_attention(const float* qkv, __nv_bfloat16* o, float* probs_or_null, 
 #undef SMD_ATT_MMA
     return;
   }
-  if (dh == 16) attention_kernel<16><<<grid, threads, 0, st>>>(qkv, o, probs_or_null, B, H, lo_delta);
-  else if (dh == 8) attention_kernel<8><<<grid, threads, 0, st>>>(qkv, o, probs_or_null, B, H, lo_delta);
-  else if (dh == 32) attention_kernel<32><<<grid, threads, 0, st>>>(qkv, o, probs_or_null, B, H, lo_delta);
-  else if (dh == 4) attention_kernel<4><<<grid, threads, 0, st>>>(qkv, o, probs_or_null, B, H, lo_delta);
+  // S = 32: static shared memory; longer sequences: k and v for S rows in dynamic shared memory
+  const size_t smem = S == 32 ? 0 : 2 * S * static_cast<size_t>(hpb * dh) * sizeof(float);
+#define SMD_ATT_SIMT(DHV)                                                                                         \
+  {                                                                                                               \
+    static bool attr = false;                                                                                     \
+    if (S != 32 && !attr) {                                                                                       \
+      cudaFuncSetAttribute(attention_kernel<DHV, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * S * 128 * 4); \
+      attr = true;                                                                                                \
+    }                                                                                                             \
+    attention_kernel<DHV, S><<<grid, threads, smem, st>>>(qkv, o, probs_or_null, B, H, lo_delta);                 \
+  }
+  if (dh == 16) SMD_ATT_SIMT(16)
+  else if (dh == 8) SMD_ATT_SIMT(8)
+  else if (dh == 32) SMD_ATT_SIMT(32)
+  else if (dh == 4) SMD_ATT_SIMT(4)
+#undef SMD_ATT_SIMT
+}
+
+void launch_attention(const float* qkv, __nv_bfloat16* o, float* probs_or_null, int B, int S, int H, cudaStream_t st,
+                      long long lo_delta) {
+  if (S == 32) launch_attention_s<32>(qkv, o, probs_or_null, B, H, st, lo_delta);
+  else if (S == 64) launch_attention_s<64>(qkv, o, probs_or_null, B, H, st, lo_delta);
+  else if (S == 128) launch_attention_s<128>(qkv, o, probs_or_null, B, H, st, lo_delta);
 }
 
 // ---------------------------------------------------------------------------------------------------
-// LayerNorm-apply + FiLM + activation -> bf16.  HBM-bound: the CTA streams its 32 rows (one sample when S == 32)
+// LayerNorm-apply + FiLM + activation -> bf16.  HBM-bound: the CTA streams its 32 rows (inside one sample when 32 | S)
 // through a double-buffered shared-memory ring with bulk async copies (cp.async.bulk + mbarrier), 4 rows = up to
 // 32 KB per copy, so ~64 KB per CTA are in flight without tying up registers.  Column-stationary compute:
 // blockDim.x = N / 4 threads, each owning one float4 column group whose gamma / beta / scale / shift stay in
@@ -507,7 +538,8 @@ ln_film_act_kernel(const void* __restrict__ uin, const float* __restrict__ stats
   const float4 g4 = *reinterpret_cast<const float4*>(g + c);
   const float4 b4 = *reinterpret_cast<const float4*>(bta + c);
   const bool film = scale != nullptr;
-  const bool row_const_film = film && (film_row_dev != nullptr || film_bcast || S == 32);
+  // a 32-row block lies inside one sample when S is a multiple of 32: its FiLM row is r0 / S
+  const bool row_const_film = film && (film_row_dev != nullptr || film_bcast || S % 32 == 0);
   float4 s4 = make_float4(1.f, 1.f, 1.f, 1.f), h4 = make_float4(0.f, 0.f, 0.f, 0.f);
   if (row_const_film) {
     const size_t frow = film_row_dev ? static_cast<size_t>(*film_row_dev) : (film_bcast ? 0 : static_cast<size_t>(r0 / S));

@@ -150,9 +150,9 @@ void launch_embed(const float* x, const float* W_in, const float* b_in, const fl
                   const float* ln_b, float* h, __nv_bfloat16* a, int M, int C, int S, cudaStream_t st,
                   long long lo_delta = 0);
 
-// unmasked multi-head self-attention over S = 32 positions (flax.nn.SelfAttention core, models/ncsn.py:161)
-// qkv fp32 [M][3E] -> o bf16 [M][E];  optionally saves the probabilities P [B][H][32][32] fp32 for backward
-void launch_attention(const float* qkv, __nv_bfloat16* o, float* probs_or_null, int B, int H, cudaStream_t st,
+// unmasked multi-head self-attention over S in {32, 64, 128} positions (flax.nn.SelfAttention core, models/ncsn.py:161)
+// qkv fp32 [M][3E] -> o bf16 [M][E];  optionally saves the probabilities P [B][H][S][S] fp32 for backward
+void launch_attention(const float* qkv, __nv_bfloat16* o, float* probs_or_null, int B, int S, int H, cudaStream_t st,
                       long long lo_delta = 0);
 
 // out[m,:] = bf16( act( film( LN(u[m,:]; stats, g, b) ) ) )                        (models/shared.py:62-64,66-68)

@@ -125,7 +125,7 @@ static void build_workspace(smd_plan* p) {
     w.hidden = family(L, Mp * Md * 2, idx("t.hid"));
     if (c.training) {
       w.hidden_pre = family(L, Mp * Md * 2, idx("t.hpre"));
-      w.probs = family(L, B * c.num_heads * 32 * 32 * 4, idx("t.probs"));
+      w.probs = family(L, B * c.num_heads * c.seq_len * c.seq_len * 4, idx("t.probs"));   // [B][H][S][S]
     }
   } else {
     w.xb = ws_add(p, "xb", Mp * Cp * 2);
@@ -426,21 +426,22 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
       float* h_in = h(2 * l); float* h_mid = h(2 * l + 1); float* h_out = h(2 * l + 2);
       __nv_bfloat16* a2 = a(2 * l + 1); __nv_bfloat16* a_next = a(2 * l + 2);
       GemmEpilogue e = epi();
-      if (!save && p->op_attn[l].ok && p->lo_bytes == 0) {
+      // the fused block's 64-row tile holds whole samples up to S = 64; S = 128 takes the unfused path
+      if (!save && S <= 64 && p->op_attn[l].ok && p->lo_bytes == 0) {
         // QKV GEMM -> attention -> out-projection + residual + LayerNorm in ONE launch; q / k / v stay on chip
         AttnBlockArgs aa;
         aa.b_qkv = params + lp.qkv.bias; aa.b_o = params + lp.out.bias;
         aa.residual = h_in; aa.out_f32 = h_mid;
         aa.ln_gamma = params + lp.ln2.scale; aa.ln_beta = params + lp.ln2.bias;
         aa.out_bf16 = a2;
-        aa.M = M; aa.H = c.num_heads;
+        aa.M = M; aa.H = c.num_heads; aa.S = S;
         SMD_CUDA(launch_attn_block(p->op_attn[l], aa, st));
       } else {
       float* qkv = p->at<float>(w.qkv[l]);
       e.bias = params + lp.qkv.bias;
       e.out_f32 = qkv; e.ld_f32 = 3 * kE;
       SMD_CUDA(gemm(p, p->op_qkv[l], M, e, st));
-      launch_attention(qkv, p->at<__nv_bfloat16>(w.o[l]), save ? p->at<float>(w.probs[l]) : nullptr, batch,
+      launch_attention(qkv, p->at<__nv_bfloat16>(w.o[l]), save ? p->at<float>(w.probs[l]) : nullptr, batch, S,
                        c.num_heads, st, p->lo_elems); CNT();
       e = epi();
       e.bias = params + lp.out.bias;
@@ -594,7 +595,8 @@ int smd_plan_create(const smd_config* cfg, smd_plan** out) {
   if (c.precision != SMD_PRECISION_BF16 && c.precision != SMD_PRECISION_BF16X3) { set_error("unknown precision"); return SMD_ERR_INVALID; }
   if (c.precision == SMD_PRECISION_BF16X3 && c.training) { set_error("precision bf16x3 covers the forward pass / sampler only (training = 0)"); return SMD_ERR_INVALID; }
   if (c.arch == SMD_ARCH_TRANSFORMER_DDPM) {
-    if (c.seq_len != 32) { set_error("TransformerDDPM CUDA path supports seq_len == 32 only (all reference configs)"); return SMD_ERR_INVALID; }
+    // each length divides the 128-row GEMM / LayerNorm tile and is a multiple of the 32-row blocks inside one sample
+    if (c.seq_len != 32 && c.seq_len != 64 && c.seq_len != 128) { set_error("TransformerDDPM CUDA path supports seq_len in {32, 64, 128}"); return SMD_ERR_INVALID; }
     if (c.num_heads != 4 && c.num_heads != 8 && c.num_heads != 16 && c.num_heads != 32) { set_error("num_heads must be 4, 8, 16 or 32"); return SMD_ERR_INVALID; }
     if (c.num_mlp_layers < 1) { set_error("num_mlp_layers must be >= 1"); return SMD_ERR_INVALID; }
   } else {
