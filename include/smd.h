@@ -155,6 +155,25 @@ int smd_dsm_grads(smd_plan* plan, const float* params, const float* x0, const fl
 int smd_dsm_setup(smd_plan* plan, const float* host_sigmas, int L, smd_stream_t stream);
 int smd_dsm_draws(smd_plan* plan, const uint32_t host_key[2], int global_batch, int first_row, int batch,
                   int continuous_noise, float* used_sigma, float* eps, int* labels_or_null, smd_stream_t stream);
+/* sliced_score_matching_loss (utils/losses.py:182-247, one particle) with the draws supplied, SMD_ARCH_DENSE_NCSN only
+ * (other plans: SMD_ERR_INVALID): x~ = x0 + used_sigma * eps, s = model(x~, used_sigma), v: (batch, C) of +-1,
+ * loss[b] = (0.5 |s_b|^2 + v_b . (J_s v)_b) * sigma_b^2.  The Hessian term is a forward-mode Jacobian-vector product
+ * through the network (a tangent pass next to the primal one).  score_or_null <- s; hvp_or_null (batch) <- v.J_s v.
+ * A bf16x3 plan runs the tangent GEMMs in three passes as well. */
+int smd_ssm_loss(smd_plan* plan, const float* params, const float* x0, const float* used_sigma, const float* eps,
+                 const float* v, int batch, float* loss_per_example, float* score_or_null, float* hvp_or_null,
+                 smd_stream_t stream);
+/* gradients of mean_{global batch}(that loss) -- the primal and tangent passes differentiated together in reverse
+ * mode; same contract as smd_dsm_grads (loss_sum: 2 floats) */
+int smd_ssm_grads(smd_plan* plan, const float* params, const float* x0, const float* used_sigma, const float* eps,
+                  const float* v, int batch, int global_batch, float* grads, float* loss_sum, smd_stream_t stream);
+/* its random draws (utils/losses.py:203-223): rng, label_rng, sample_rng, score_rng = split(key, 4); labels and
+ * used_sigma as smd_dsm_draws (noise_rng from split(rng) when continuous), eps = normal(sample_rng),
+ * v = rademacher(score_rng) = +1 where the threefry word is < 2^31, else -1.  Schedule: smd_dsm_setup.  Rows
+ * [first_row, first_row + batch) of a global batch, as smd_dsm_draws. */
+int smd_ssm_draws(smd_plan* plan, const uint32_t host_key[2], int global_batch, int first_row, int batch,
+                  int continuous_noise, float* used_sigma, float* eps, float* v, int* labels_or_null,
+                  smd_stream_t stream);
 /* One Langevin update after a network call (annealed_langevin_dynamics utils/ebm_utils.py:139-175, consistent_... :231-253):
  *   x_next = x + alpha * grad + noise_coef * z;  with a mask: x_next = x_next (1 - mask) + (infill_x + infill_sigma z') mask.
  * z / infill_z: supplied N(0,1) tensors or NULL -> jax.random.normal(step_key / infill_key).  metrics4 (device, 4 floats,

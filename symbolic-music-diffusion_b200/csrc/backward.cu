@@ -73,6 +73,22 @@ int train_bind(smd_plan* p) {
   } else {
     if (!make_dw(&ts.dWin, B16(w.xb), C, B16(ts.du16[0]), Md, Md, Mp)) return SMD_ERR_CUDA;
   }
+  if (c.arch == SMD_ARCH_DENSE_NCSN) {   // tangent halves of the sliced-score-matching backward
+    ts.tdWb.resize(K); ts.tdXb.resize(K); ts.tdWa.resize(K); ts.tdXa.resize(K);
+    for (int k = 0; k < K; ++k) {
+      const BlockParams& bp = par.block[k];
+      if (!make_dw(&ts.tdWb[k], B16(w.actt[2 * k + 1]), Md, B16(ts.dut16[k + 1]), Md, Md, Mp)) return SMD_ERR_CUDA;
+      if (!make_dx(&ts.tdXb[k], B16(ts.dut16[k + 1]), Md, p->wsh(bp.b.kernel), Md, Mp)) return SMD_ERR_CUDA;
+      if (!make_dw(&ts.tdWa[k], B16(w.actt[2 * k]), Md, B16(ts.drt16[k]), Md, Md, Mp)) return SMD_ERR_CUDA;
+      if (!make_dx(&ts.tdXa[k], B16(ts.drt16[k]), Md, p->wsh(bp.a.kernel), Md, Mp)) return SMD_ERR_CUDA;
+    }
+    if (!make_gemm_op(&ts.tdWout, B16(w.actt[2 * K]), static_cast<uint64_t>(Md), B16(ts.dpredt16), static_cast<uint64_t>(Cp),
+                      C, static_cast<int>(Mp), std::min(Cp, kBNMax), 1, 1))
+      return SMD_ERR_CUDA;
+    if (!make_gemm_op(&ts.tdXout, B16(ts.dpredt16), Mp, B16(w.out_pad), static_cast<uint64_t>(Md), Md, Cp,
+                      choose_bn(Md), 0, 0)) return SMD_ERR_CUDA;
+    if (!make_dw(&ts.tdWin, B16(w.xbt), C, B16(ts.dut16[0]), Md, Md, Mp)) return SMD_ERR_CUDA;
+  }
   return SMD_OK;
 }
 
@@ -81,6 +97,46 @@ static cudaError_t gemm_k(const GemmOp& op0, int rows, int K, int splits, const 
   op.K = K;
   op.k_splits = splits;
   return launch_gemm(op, rows, e, st);
+}
+
+// FiLM generator backward of block k (models/ncsn.py:47-61); no gradient flows into t.  Independent of the rest of the
+// backward pass: runs on the side stream once this block's dss (complete on `st`) is.
+static cudaError_t film_generator_bwd(smd_plan* p, const float* params, int k, int batch, float* grads, cudaStream_t st) {
+  TrainState& ts = p->train;
+  const WorkspaceLayout& w = p->reg;
+  const BlockParams& bp = p->par.block[k];
+  const int Md = p->cfg.mlp_dims;
+  const int Bk = (batch + 63) / 64 * 64;
+  cudaStream_t side = p->side_stream;
+  auto B16 = [&](size_t off) { return p->at<__nv_bfloat16>(off); };
+  auto F32 = [&](size_t off) { return p->at<float>(off); };
+  float* dss = F32(ts.dss) + static_cast<size_t>(k) * p->cfg.max_batch * 2 * Md;
+  cudaError_t err = cudaEventRecord(p->ev_dss, st);
+  if (err == cudaSuccess) err = cudaStreamWaitEvent(side, p->ev_dss, 0);
+  if (err != cudaSuccess) return err;
+  float* enc = F32(w.enc);
+  float* e1pre = F32(w.e1pre[k]);
+  float* e1 = F32(w.e1[k]);
+  float* e2 = F32(w.e2[k]);
+  float* de2 = F32(ts.de2);
+  float* de1 = F32(ts.de);
+  launch_colsum<float>(dss, 2 * Md, grads + bp.film.ss.bias, batch, 2 * Md, side); CNT();
+  launch_cast_bf16(dss, B16(ts.dss16), static_cast<size_t>(batch) * 2 * Md, side); CNT();
+  launch_cast_bf16(e2, B16(ts.e2_16), static_cast<size_t>(batch) * 512, side); CNT();
+  GemmEpilogue e = epi();
+  e.out_f32 = grads + bp.film.ss.kernel; e.ld_f32 = 2 * Md;
+  err = gemm_k(ts.dWss[k], 512, Bk, 1, e, side);
+  if (err != cudaSuccess) return err;
+  e = epi();
+  e.out_f32 = de2; e.ld_f32 = 512;
+  err = launch_gemm(ts.dXss[k], batch, e, side);
+  if (err != cudaSuccess) return err;
+  launch_colsum<float>(de2, 512, grads + bp.film.d2.bias, batch, 512, side); CNT();
+  launch_small_linear_bwd_w(e1, de2, grads + bp.film.d2.kernel, batch, 512, 512, side); CNT();
+  launch_small_linear_bwd_x(de2, params + bp.film.d2.kernel, e1pre, de1, batch, 512, 512, side); CNT();
+  launch_colsum<float>(de1, 512, grads + bp.film.d1.bias, batch, 512, side); CNT();
+  launch_small_linear_bwd_w(enc, de1, grads + bp.film.d1.kernel, batch, 128, 512, side); CNT();
+  return cudaSuccess;
 }
 
 }  // namespace smd
@@ -239,30 +295,7 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     a.M = M; a.N = Md; a.S = S;
     launch_ln_film_act_bwd(a, st); CNT();
 
-    // ---- FiLM generator backward (models/ncsn.py:47-61); no gradient flows into t ----
-    // independent of the rest of the backward pass: runs on the side stream once this block's dss is complete
-    SMD_CUDA(cudaEventRecord(p->ev_dss, st));
-    SMD_CUDA(cudaStreamWaitEvent(side, p->ev_dss, 0));
-    float* enc = F32(w.enc);
-    float* e1pre = F32(w.e1pre[k]);
-    float* e1 = F32(w.e1[k]);
-    float* e2 = F32(w.e2[k]);
-    float* de2 = F32(ts.de2);
-    float* de1 = F32(ts.de);
-    launch_colsum<float>(dss, 2 * Md, grads + bp.film.ss.bias, batch, 2 * Md, side); CNT();
-    launch_cast_bf16(dss, B16(ts.dss16), static_cast<size_t>(batch) * 2 * Md, side); CNT();
-    launch_cast_bf16(e2, B16(ts.e2_16), static_cast<size_t>(batch) * 512, side); CNT();
-    e = epi();
-    e.out_f32 = grads + bp.film.ss.kernel; e.ld_f32 = 2 * Md;
-    SMD_CUDA(gemm_k(ts.dWss[k], 512, Bk, 1, e, side));
-    e = epi();
-    e.out_f32 = de2; e.ld_f32 = 512;
-    SMD_CUDA(launch_gemm(ts.dXss[k], batch, e, side));
-    launch_colsum<float>(de2, 512, grads + bp.film.d2.bias, batch, 512, side); CNT();
-    launch_small_linear_bwd_w(e1, de2, grads + bp.film.d2.kernel, batch, 512, 512, side); CNT();
-    launch_small_linear_bwd_x(de2, params + bp.film.d2.kernel, e1pre, de1, batch, 512, 512, side); CNT();
-    launch_colsum<float>(de1, 512, grads + bp.film.d1.bias, batch, 512, side); CNT();
-    launch_small_linear_bwd_w(enc, de1, grads + bp.film.d1.kernel, batch, 128, 512, side); CNT();
+    SMD_CUDA(film_generator_bwd(p, params, k, batch, grads, st));
   }
   // every k*. / out_ln / out gradient is final once these three have fired (smd_wait_tail_grads)
   SMD_CUDA(cudaEventRecordWithFlags(p->evx_join, side, ext));
@@ -380,6 +413,166 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
   return SMD_OK;
 }
 
+// Sliced score matching (utils/losses.py:182-247) on DenseNCSN: loss_b = 0.5 |f|^2 + sigma v.(J_f v) with f the raw
+// network output.  The primal pass and its tangent along v (run_forward with tangent) are differentiated together in
+// reverse mode ("reverse over forward"): every dX GEMM runs once on the primal and once on the tangent adjoint, every
+// dW GEMM accumulates the primal and the tangent products, and the LayerNorm / FiLM / swish steps use ssm_ln_bwd.
+// ind: device table {x0, used_sigma, eps, v} (graph replay) or null.
+static int ssm_grads_impl(smd_plan* p, const float* params, const float* x0, const float* used_sigma, const float* eps,
+                          const float* v, const float* const* ind, int batch, int global_batch, float* grads,
+                          float* loss_sum, cudaStream_t st, bool capturing) {
+  const unsigned ext = capturing ? cudaEventRecordExternal : cudaEventRecordDefault;
+  TrainState& ts = p->train;
+  const smd_config& c = p->cfg;
+  const int C = c.channels, Md = c.mlp_dims;
+  const int Cp = (C + 63) / 64 * 64;
+  const int M = batch;
+  const int Mk = (M + 63) / 64 * 64;
+  const int Bk = (batch + 63) / 64 * 64;
+  const WorkspaceLayout& w = p->reg;
+  const ParamLayout& par = p->par;
+  const int K = p->K;
+  auto B16 = [&](size_t off) { return p->at<__nv_bfloat16>(off); };
+  auto F32 = [&](size_t off) { return p->at<float>(off); };
+  { int rcs = ensure_side_stream(p); if (rcs) return rcs; }
+  cudaStream_t side = p->side_stream;
+  cudaStream_t dws = p->dw_stream;
+  auto fork_dw = [&]() -> cudaError_t {
+    cudaError_t e1 = cudaEventRecord(p->ev_dw, st);
+    if (e1 != cudaSuccess) return e1;
+    return cudaStreamWaitEvent(dws, p->ev_dw, 0);
+  };
+  // weight gradient = primal product + tangent product (reduction over both sets of rows), on the weight-gradient stream
+  auto dw2 = [&](const GemmOp& op, const GemmOp& top, int rows, float* out, int ld) -> cudaError_t {
+    GemmEpilogue e = epi();
+    e.out_f32 = out; e.ld_f32 = ld;
+    cudaError_t err = gemm_k(op, rows, Mk, 1, e, dws);
+    if (err != cudaSuccess) return err;
+    e.residual = out; e.ld_res = ld;
+    return gemm_k(top, rows, Mk, 1, e, dws);
+  };
+  auto dx = [&](const GemmOp& op, __nv_bfloat16* out) -> cudaError_t {
+    GemmEpilogue e = epi();
+    e.out_bf16 = out; e.ld_bf16 = Md;
+    return launch_gemm(op, M, e, st);
+  };
+  __nv_bfloat16* g16 = B16(ts.g16);
+  __nv_bfloat16* gt16 = B16(ts.gt16);
+  float* du32 = F32(ts.du32);
+  float* dut32 = F32(ts.dut32);
+  float* stats = F32(w.stats);
+  const size_t sstride = static_cast<size_t>(p->Mp) * 2;
+
+  SMD_CUDA(fork_dw());
+  SMD_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * p->arena, dws));
+  SMD_CUDA(cudaEventRecord(p->ev_gz, dws));
+  SMD_CUDA(cudaMemsetAsync(F32(ts.dss), 0, sizeof(float) * static_cast<size_t>(K) * c.max_batch * 2 * Md, st));
+  if (Mk != M) {  // zero the reduction-tail rows of every MN-major gradient operand
+    const size_t tail = static_cast<size_t>(Mk - M);
+    for (const std::vector<size_t>* fam : {&ts.du16, &ts.dr16t, &ts.dut16, &ts.drt16})
+      for (size_t off : *fam) SMD_CUDA(cudaMemsetAsync(B16(off) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
+    SMD_CUDA(cudaMemsetAsync(B16(ts.dpred16) + static_cast<size_t>(M) * Cp, 0, tail * Cp * 2, st));
+    SMD_CUDA(cudaMemsetAsync(B16(ts.dpredt16) + static_cast<size_t>(M) * Cp, 0, tail * Cp * 2, st));
+  }
+  if (Bk != batch) {
+    SMD_CUDA(cudaMemsetAsync(B16(ts.dss16) + static_cast<size_t>(batch) * 2 * Md, 0,
+                             static_cast<size_t>(Bk - batch) * 2 * Md * 2, st));
+    SMD_CUDA(cudaMemsetAsync(B16(ts.e2_16) + static_cast<size_t>(batch) * 512, 0,
+                             static_cast<size_t>(Bk - batch) * 512 * 2, st));
+  }
+
+  // ---------------- forward: primal (keeps every activation) and tangent along v ----------------
+  float* xt = F32(w.xt);
+  float* cond = F32(w.tvec);
+  float* f = F32(w.eps_hat);
+  launch_q_sample(x0, eps, used_sigma, xt, cond, batch, C, st, ind, 1); CNT();
+  launch_tangent_input(v, ind, B16(w.xbt), static_cast<size_t>(M) * C, st, 0); CNT();
+  int rc = run_forward(p, params, xt, cond, 0, batch, f, st, /*save=*/true, /*raw_out=*/true, /*tangent=*/true);
+  if (rc) return rc;
+  SMD_CUDA(cudaStreamWaitEvent(st, p->ev_gz, 0));
+
+  // ---------------- objective and its two adjoint seeds ----------------
+  float* dpred32 = F32(ts.dpred32);
+  launch_ssm_loss(f, F32(w.yt), v, used_sigma, ind, F32(ts.loss), nullptr, nullptr, loss_sum,
+                  p->at<unsigned int>(ts.loss_ctr), 1.0f / static_cast<float>(global_batch), dpred32, B16(ts.dpred16),
+                  B16(ts.dpredt16), batch, C, Cp, st); CNT();
+  SMD_CUDA(fork_dw());
+  launch_colsum<float>(dpred32, C, grads + par.out.bias, M, C, dws); CNT();
+
+  // ---------------- output projection + final LayerNorm ----------------
+  SMD_CUDA(dw2(ts.dWout, ts.tdWout, Md, grads + par.out.kernel, C));
+  SMD_CUDA(dx(ts.dXout, g16));
+  SMD_CUDA(dx(ts.tdXout, gt16));
+  SsmLnBwdArgs a;
+  memset(&a, 0, sizeof(a));
+  a.x32 = F32(w.u[K]); a.xt = F32(w.ut[K]); a.stats = stats + (2 * K) * sstride;
+  a.gamma = params + par.out_ln.scale; a.beta = params + par.out_ln.bias;
+  a.g16 = g16; a.gt16 = gt16;
+  a.dx32 = du32; a.dx16 = B16(ts.du16[K]); a.dxt32 = dut32; a.dxt16 = B16(ts.dut16[K]);
+  a.dgamma = grads + par.out_ln.scale; a.dbeta = grads + par.out_ln.bias;
+  a.dbias = grads + par.block[K - 1].b.bias;
+  a.M = M; a.N = Md; a.S = 1;
+  launch_ssm_ln_bwd(a, st); CNT();
+
+  // ---------------- FiLM'd residual blocks ----------------
+  for (int k = K - 1; k >= 0; --k) {
+    const BlockParams& bp = par.block[k];
+    const float* ss_k = F32(w.ss) + static_cast<size_t>(k) * c.max_batch * 2 * Md;
+    float* dss = F32(ts.dss) + static_cast<size_t>(k) * c.max_batch * 2 * Md;
+    SMD_CUDA(fork_dw());
+    SMD_CUDA(dw2(ts.dWb[k], ts.tdWb[k], Md, grads + bp.b.kernel, Md));
+    SMD_CUDA(dx(ts.dXb[k], g16));
+    SMD_CUDA(dx(ts.tdXb[k], gt16));
+    memset(&a, 0, sizeof(a));
+    a.x16 = B16(w.r1[k]); a.xt = F32(w.r1t[k]); a.stats = stats + (2 * k + 1) * sstride;
+    a.gamma = params + bp.ln_b.scale; a.beta = params + bp.ln_b.bias;
+    a.ss = ss_k; a.act = 2;
+    a.g16 = g16; a.gt16 = gt16;
+    a.dx16 = B16(ts.dr16t[k]); a.dxt16 = B16(ts.drt16[k]);
+    a.dgamma = grads + bp.ln_b.scale; a.dbeta = grads + bp.ln_b.bias;
+    a.dbias = grads + bp.a.bias;
+    a.dss = dss;
+    a.M = M; a.N = Md; a.S = 1;
+    launch_ssm_ln_bwd(a, st); CNT();
+    SMD_CUDA(fork_dw());
+    SMD_CUDA(dw2(ts.dWa[k], ts.tdWa[k], Md, grads + bp.a.kernel, Md));
+    SMD_CUDA(dx(ts.dXa[k], g16));
+    SMD_CUDA(dx(ts.tdXa[k], gt16));
+    memset(&a, 0, sizeof(a));
+    a.x32 = F32(w.u[k]); a.xt = F32(w.ut[k]); a.stats = stats + (2 * k) * sstride;
+    a.gamma = params + bp.ln_a.scale; a.beta = params + bp.ln_a.bias;
+    a.ss = ss_k; a.act = 2;
+    a.g16 = g16; a.gt16 = gt16;
+    a.dres = du32; a.dres_t = dut32;
+    a.dx32 = du32; a.dx16 = B16(ts.du16[k]); a.dxt32 = dut32; a.dxt16 = B16(ts.dut16[k]);
+    a.dgamma = grads + bp.ln_a.scale; a.dbeta = grads + bp.ln_a.bias;
+    a.dbias = grads + (k > 0 ? par.block[k - 1].b.bias : par.in.bias);
+    a.dss = dss;
+    a.M = M; a.N = Md; a.S = 1;
+    launch_ssm_ln_bwd(a, st); CNT();
+    SMD_CUDA(film_generator_bwd(p, params, k, batch, grads, st));
+  }
+  SMD_CUDA(cudaEventRecordWithFlags(p->evx_join, side, ext));
+  SMD_CUDA(cudaEventRecord(p->ev_join, side));
+  SMD_CUDA(cudaEventRecordWithFlags(p->ev_tail, st, ext));
+  SMD_CUDA(cudaEventRecordWithFlags(p->ev_dwtail, dws, ext));
+  SMD_LAUNCH_CHECK("ssm backward tail");
+
+  // ---------------- input projection (models/ncsn.py:129): x~ and v rows ----------------
+  {
+    GemmEpilogue e = epi();
+    e.out_f32 = grads + par.in.kernel; e.ld_f32 = Md;
+    SMD_CUDA(gemm_k(ts.dWin, C, Mk, 1, e, st));
+    e.residual = grads + par.in.kernel; e.ld_res = Md;
+    SMD_CUDA(gemm_k(ts.tdWin, C, Mk, 1, e, st));
+  }
+  SMD_CUDA(cudaEventRecord(p->ev_dwjoin, dws));
+  SMD_CUDA(cudaStreamWaitEvent(st, p->ev_dwjoin, 0));
+  SMD_CUDA(cudaStreamWaitEvent(st, p->ev_join, 0));
+  SMD_LAUNCH_CHECK("ssm backward");
+  return SMD_OK;
+}
+
 // SMD_TRAIN_GRAPH=0 switches the graph replay of the train step off (eager launches, 3 streams, as in round 1)
 static bool train_graph_enabled() {
   static const bool on = [] { const char* v = getenv("SMD_TRAIN_GRAPH"); return !(v && v[0] == '0'); }();
@@ -391,16 +584,22 @@ static void drop_train_graph(smd_plan* p) {
   p->tg_valid = false;
 }
 
+// objective 0: ddpm, 1: denoising score matching, 2: sliced score matching (v: its projection vectors; else null)
 static int grads_entry(smd_plan* p, const float* params, const float* x0, const float* used_alpha,
-                       const float* eps, int batch, int global_batch, float* grads, float* loss_sum,
+                       const float* eps, const float* v, int batch, int global_batch, float* grads, float* loss_sum,
                        smd_stream_t stream, int objective) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!p->cfg.training) { set_error("plan was not created with training = 1"); return SMD_ERR_STATE; }
   if (!p->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
   if (batch < 1 || batch > p->cfg.max_batch || global_batch < batch) { set_error("batch out of range"); return SMD_ERR_INVALID; }
   const bool capturable = st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread;
-  if (!train_graph_enabled() || !capturable)
-    return grads_impl(p, params, x0, used_alpha, eps, nullptr, batch, global_batch, grads, loss_sum, st, false, objective);
+  auto impl = [&](const float* x0_, const float* ua_, const float* eps_, const float* v_, const float* const* ind_,
+                  bool capturing) {
+    if (objective == 2)
+      return ssm_grads_impl(p, params, x0_, ua_, eps_, v_, ind_, batch, global_batch, grads, loss_sum, st, capturing);
+    return grads_impl(p, params, x0_, ua_, eps_, ind_, batch, global_batch, grads, loss_sum, st, capturing, objective);
+  };
+  if (!train_graph_enabled() || !capturable) return impl(x0, used_alpha, eps, v, nullptr, false);
   // Graph replay: the pass's ~150 launches on three streams (dX chain, weight-gradient GEMMs, FiLM generator) are
   // captured once into one CUDA graph with the same fork / join structure.  The per-step inputs (x0, used_alpha, eps)
   // reach the kernels through a 3-pointer device table, so new input tensors do not force a re-capture; the events a
@@ -417,12 +616,12 @@ static int grads_entry(smd_plan* p, const float* params, const float* x0, const 
       // first use of this configuration runs eagerly: lazy one-time calls (function attributes, stream / event
       // creation) stay out of the capture
       p->tg_warm = true;
-      return grads_impl(p, params, x0, used_alpha, eps, nullptr, batch, global_batch, grads, loss_sum, st, false, objective);
+      return impl(x0, used_alpha, eps, v, nullptr, false);
     }
     cudaGraph_t graph = nullptr;
     const long long before = g_launches.load();
     SMD_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    int rc = grads_impl(p, params, nullptr, nullptr, nullptr, ind, batch, global_batch, grads, loss_sum, st, true, objective);
+    int rc = impl(nullptr, nullptr, nullptr, nullptr, ind, true);
     cudaError_t ce = cudaStreamEndCapture(st, &graph);
     p->tg_nodes = g_launches.load() - before;
     g_launches.store(before);   // captured launches are counted per replay
@@ -433,8 +632,8 @@ static int grads_entry(smd_plan* p, const float* params, const float* x0, const 
     if (ce != cudaSuccess) { set_error(std::string("train graph instantiate: ") + cudaGetErrorString(ce)); return SMD_ERR_CUDA; }
     p->tg_valid = true;
   }
-  // (pageable source: the driver stages these 24 bytes before returning, so the host array may die with this frame)
-  const float* host_ind[3] = {x0, used_alpha, eps};
+  // (pageable source: the driver stages these 32 bytes before returning, so the host array may die with this frame)
+  const float* host_ind[4] = {x0, used_alpha, eps, v};
   SMD_CUDA(cudaMemcpyAsync(ind, host_ind, sizeof(host_ind), cudaMemcpyHostToDevice, st));
   SMD_CUDA(cudaGraphLaunch(p->tg_exec, st));
   g_launches.fetch_add(p->tg_nodes, std::memory_order_relaxed);
@@ -444,7 +643,7 @@ static int grads_entry(smd_plan* p, const float* params, const float* x0, const 
 extern "C" int smd_ddpm_grads(smd_plan* p, const float* params, const float* x0, const float* used_alpha,
                               const float* eps, int batch, int global_batch, float* grads, float* loss_sum,
                               smd_stream_t stream) {
-  return grads_entry(p, params, x0, used_alpha, eps, batch, global_batch, grads, loss_sum, stream, 0);
+  return grads_entry(p, params, x0, used_alpha, eps, nullptr, batch, global_batch, grads, loss_sum, stream, 0);
 }
 
 // denoising score matching (utils/losses.py:129-179): the same pass with x~ = x0 + sigma eps, the network conditioned on
@@ -453,5 +652,13 @@ extern "C" int smd_dsm_grads(smd_plan* p, const float* params, const float* x0, 
                              const float* eps, int batch, int global_batch, float* grads, float* loss_sum,
                              smd_stream_t stream) {
   if (p->cfg.arch != SMD_ARCH_DENSE_NCSN) { set_error("smd_dsm_grads needs a score network (SMD_ARCH_DENSE_NCSN)"); return SMD_ERR_INVALID; }
-  return grads_entry(p, params, x0, used_sigma, eps, batch, global_batch, grads, loss_sum, stream, 1);
+  return grads_entry(p, params, x0, used_sigma, eps, nullptr, batch, global_batch, grads, loss_sum, stream, 1);
+}
+
+// sliced score matching (utils/losses.py:182-247) with the draws of smd_ssm_draws supplied (SMD_ARCH_DENSE_NCSN)
+extern "C" int smd_ssm_grads(smd_plan* p, const float* params, const float* x0, const float* used_sigma,
+                             const float* eps, const float* v, int batch, int global_batch, float* grads,
+                             float* loss_sum, smd_stream_t stream) {
+  if (p->cfg.arch != SMD_ARCH_DENSE_NCSN) { set_error("smd_ssm_grads needs a score network (SMD_ARCH_DENSE_NCSN)"); return SMD_ERR_INVALID; }
+  return grads_entry(p, params, x0, used_sigma, eps, v, batch, global_batch, grads, loss_sum, stream, 2);
 }

@@ -461,6 +461,160 @@ inline void launch_ln_film_act_bwd(const LnFilmBwdArgs& a, cudaStream_t st) {
 }
 
 // ---------------------------------------------------------------------------------------------------
+// sliced score matching: reverse pass through a wide LayerNorm + FiLM + swish AND its tangent (launch_ln_film_tangent).
+// Per row, with xh = (x - mean) r, xc' = x' - mean(x'), q = r mean(xh x'), xh' = r xc' - xh q, z = s (gamma xh + beta) + h,
+// z' = s gamma xh', out = swish(z), out' = swish'(z) z' and the incoming adjoints (g, g'):
+//   gz = g swish'(z) + g' swish''(z) z',  gz' = g' swish'(z);   dscale += gz y + gz' y',  dshift += gz
+//   tangent adjoint:  dx' = r (gxh' - mean(gxh') - xh mean(xh gxh'))          with gxh' = gamma s gz'
+//   primal adjoint:   dx  = LN-backward(gxh - q gxh') - (r^2 xh / N) gr + (xc' / N) gP
+//                     with gr = sum(gxh' xc') - 2 mean(xh x') sum(gxh' xh),  gP = -r^2 sum(gxh' xh)
+// (the last two terms are the dependence of the tangent on x through r and mean(xh x')).  kSsmRows rows per CTA,
+// the column sums (gamma, beta, bias) leave through one atomic per column and CTA.
+// ---------------------------------------------------------------------------------------------------
+struct SsmLnBwdArgs {
+  const float* x32;           // [M][N] primal LayerNorm input (fp32), or null ->
+  const __nv_bfloat16* x16;   // the same stored as bf16
+  const float* xt;            // [M][N] its tangent (fp32)
+  const float* stats;         // [M][2] (sum, sumsq) of the primal rows
+  const float* gamma;
+  const float* beta;
+  const float* ss;            // FiLM [nsamples][2N] = [scale | shift], or null (plain LayerNorm)
+  int act;                    // 2: swish, 0: none
+  const __nv_bfloat16* g16;   // [M][N] adjoint of the primal output
+  const __nv_bfloat16* gt16;  // [M][N] adjoint of the tangent output
+  const float* dres;          // residual adjoints added to dx / dx' (may alias dx32 / dxt32), or null
+  const float* dres_t;
+  float* dx32; __nv_bfloat16* dx16;    // primal input adjoint (either may be null)
+  float* dxt32; __nv_bfloat16* dxt16;  // tangent input adjoint
+  float* dgamma; float* dbeta;         // [N] (atomics)
+  float* dbias;                        // [N] += column sums of dx, or null
+  float* dss;                          // [nsamples][2N] += gradient of [scale | shift] (zeroed by the caller)
+  int M, N, S;
+};
+static constexpr int kSsmRows = 4;
+
+__device__ __forceinline__ void store_bf16x4(__nv_bfloat16* p, const float (&v)[4]) {
+  __nv_bfloat162 q0 = __floats2bfloat162_rn(v[0], v[1]);
+  __nv_bfloat162 q1 = __floats2bfloat162_rn(v[2], v[3]);
+  uint2 pk;
+  pk.x = *reinterpret_cast<uint32_t*>(&q0);
+  pk.y = *reinterpret_cast<uint32_t*>(&q1);
+  *reinterpret_cast<uint2*>(p) = pk;
+}
+
+// CPT adjacent columns per thread, at most 512 threads (<= 128 registers, no spills): CPT = 4 up to N = 2048, 8 above
+template <int CPT>
+__global__ void __launch_bounds__(512) ssm_ln_bwd_kernel(const SsmLnBwdArgs a) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ float red2[2][32];
+  __shared__ float red5[5][32];
+  const int N = a.N, c = threadIdx.x * CPT;
+  const float inv_n = 1.0f / static_cast<float>(N);
+  float adg[CPT], adb[CPT], abias[CPT];
+#pragma unroll
+  for (int i = 0; i < CPT; ++i) { adg[i] = 0.f; adb[i] = 0.f; abias[i] = 0.f; }
+  auto ld4 = [](float* dst, const float4 v) { dst[0] = v.x; dst[1] = v.y; dst[2] = v.z; dst[3] = v.w; };
+  for (int r = 0; r < kSsmRows; ++r) {
+    const int row = blockIdx.x * kSsmRows + r;
+    if (row >= a.M) break;   // uniform over the CTA
+    const size_t off = static_cast<size_t>(row) * N + c;
+    float x[CPT], d[CPT], g[CPT], gt[CPT];
+#pragma unroll
+    for (int j = 0; j < CPT; j += 4) {
+      ld4(x + j, a.x16 ? unpack_bf16x4(*reinterpret_cast<const uint2*>(a.x16 + off + j))
+                       : *reinterpret_cast<const float4*>(a.x32 + off + j));
+      ld4(d + j, *reinterpret_cast<const float4*>(a.xt + off + j));
+      ld4(g + j, unpack_bf16x4(*reinterpret_cast<const uint2*>(a.g16 + off + j)));
+      ld4(gt + j, unpack_bf16x4(*reinterpret_cast<const uint2*>(a.gt16 + off + j)));
+    }
+    const float mean = a.stats[2 * static_cast<size_t>(row)] * inv_n;
+    const float rstd = rsqrtf(a.stats[2 * static_cast<size_t>(row) + 1] * inv_n - mean * mean + 1e-6f);
+    float xh[CPT], s2[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < CPT; ++i) {
+      xh[i] = (x[i] - mean) * rstd;
+      s2[0] += d[i];
+      s2[1] += xh[i] * d[i];
+    }
+    block_sums<2>(s2, red2);
+    const float m1 = s2[0] * inv_n, m2 = s2[1] * inv_n;
+    const float q = rstd * m2;
+    const float* sp = a.ss ? a.ss + static_cast<size_t>(row / a.S) * 2 * N : nullptr;
+    float* dp = (sp && a.dss) ? a.dss + static_cast<size_t>(row / a.S) * 2 * N : nullptr;
+    float* xc = d;   // d is dead once centred
+    float gxd[CPT], h[CPT], s5[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < CPT; ++i) {
+      const float gm = a.gamma[c + i];
+      xc[i] = d[i] - m1;
+      const float xhd = rstd * (xc[i] - xh[i] * m2);
+      const float y = fmaf(gm, xh[i], a.beta[c + i]), yd = gm * xhd;
+      const float sc = sp ? sp[c + i] : 1.0f;
+      const float z = sp ? fmaf(sc, y, sp[N + c + i]) : y, zd = sc * yd;
+      float gz = g[i], gzd = gt[i];
+      if (a.act == 2) {
+        const float sg = sigmoid_exact(z);
+        const float d1 = sg * fmaf(z, 1.0f - sg, 1.0f);
+        const float d2 = sg * (1.0f - sg) * fmaf(z, 1.0f - 2.0f * sg, 2.0f);
+        gz = fmaf(g[i], d1, gt[i] * d2 * zd);
+        gzd = gt[i] * d1;
+      }
+      if (dp) { dp[c + i] += fmaf(gz, y, gzd * yd); dp[N + c + i] += gz; }
+      const float gy = gz * sc, gyd = gzd * sc;
+      adg[i] += fmaf(gy, xh[i], gyd * xhd);
+      adb[i] += gy;
+      gxd[i] = gyd * gm;
+      h[i] = fmaf(-q, gxd[i], gy * gm);
+      s5[0] += gxd[i];
+      s5[1] += xh[i] * gxd[i];
+      s5[2] += gxd[i] * xc[i];
+      s5[3] += h[i];
+      s5[4] += xh[i] * h[i];
+    }
+    block_sums<5>(s5, red5);
+    const float gr = s5[2] - 2.0f * m2 * s5[1];
+    const float gP = -rstd * rstd * s5[1];
+#pragma unroll
+    for (int j = 0; j < CPT; j += 4) {
+      float dx[4], dxt[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int i = j + u;
+        dx[u] = rstd * (h[i] - s5[3] * inv_n - xh[i] * s5[4] * inv_n) - rstd * rstd * xh[i] * inv_n * gr +
+                xc[i] * inv_n * gP;
+        dxt[u] = rstd * (gxd[i] - s5[0] * inv_n - xh[i] * s5[1] * inv_n);
+      }
+      if (a.dres) {
+        const float4 r4 = *reinterpret_cast<const float4*>(a.dres + off + j);
+        dx[0] += r4.x; dx[1] += r4.y; dx[2] += r4.z; dx[3] += r4.w;
+      }
+      if (a.dres_t) {
+        const float4 r4 = *reinterpret_cast<const float4*>(a.dres_t + off + j);
+        dxt[0] += r4.x; dxt[1] += r4.y; dxt[2] += r4.z; dxt[3] += r4.w;
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) abias[j + u] += dx[u];
+      if (a.dx32) *reinterpret_cast<float4*>(a.dx32 + off + j) = make_float4(dx[0], dx[1], dx[2], dx[3]);
+      if (a.dxt32) *reinterpret_cast<float4*>(a.dxt32 + off + j) = make_float4(dxt[0], dxt[1], dxt[2], dxt[3]);
+      if (a.dx16) store_bf16x4(a.dx16 + off + j, dx);
+      if (a.dxt16) store_bf16x4(a.dxt16 + off + j, dxt);
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < CPT; ++i) {
+    atomicAdd(a.dgamma + c + i, adg[i]);
+    atomicAdd(a.dbeta + c + i, adb[i]);
+    if (a.dbias) atomicAdd(a.dbias + c + i, abias[i]);
+  }
+}
+inline void launch_ssm_ln_bwd(const SsmLnBwdArgs& a, cudaStream_t st) {
+  const int blocks = (a.M + kSsmRows - 1) / kSsmRows;
+  if (a.N <= 2048) ssm_ln_bwd_kernel<4><<<blocks, a.N / 4, 0, st>>>(a);
+  else ssm_ln_bwd_kernel<8><<<blocks, a.N / 8, 0, st>>>(a);
+}
+
+// ---------------------------------------------------------------------------------------------------
 // narrow (128-wide) LayerNorm backward, one warp per row; statistics recomputed from the saved input
 // ---------------------------------------------------------------------------------------------------
 struct Ln128BwdArgs {

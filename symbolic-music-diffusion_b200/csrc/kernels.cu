@@ -908,6 +908,149 @@ void launch_scale_rows(float* y, const float* sigma, int bcast, int B, int per, 
   scale_rows_kernel<<<blocks, 256, 0, st>>>(y, sigma, bcast, B, per);
 }
 
+// ---------------------------------------------------------------------------------------------------
+// sliced score matching: tangent pass and objective (utils/losses.py:182-247)
+// ---------------------------------------------------------------------------------------------------
+// one CTA per row, N / 4 threads, four columns each
+__global__ void __launch_bounds__(1024)
+ln_film_tangent_kernel(const float* __restrict__ x32, const __nv_bfloat16* __restrict__ x16,
+                       const float* __restrict__ stats, const float* __restrict__ xt, const float* __restrict__ g,
+                       const float* __restrict__ bta, const float* __restrict__ ss, int film_ld, int act,
+                       __nv_bfloat16* __restrict__ out, int N, int S, long long lo_delta) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ float red[2][32];
+  const int row = blockIdx.x, c = threadIdx.x * 4;
+  const size_t off = static_cast<size_t>(row) * N + c;
+  const float inv_n = 1.0f / static_cast<float>(N);
+  float x[4], d[4];
+  if (x16) {
+    const uint2 raw = *reinterpret_cast<const uint2*>(x16 + off);
+    const float2 lo = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&raw.x));
+    const float2 hi = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&raw.y));
+    x[0] = lo.x; x[1] = lo.y; x[2] = hi.x; x[3] = hi.y;
+  } else {
+    const float4 q = *reinterpret_cast<const float4*>(x32 + off);
+    x[0] = q.x; x[1] = q.y; x[2] = q.z; x[3] = q.w;
+  }
+  {
+    const float4 q = *reinterpret_cast<const float4*>(xt + off);
+    d[0] = q.x; d[1] = q.y; d[2] = q.z; d[3] = q.w;
+  }
+  const float mean = stats[2 * static_cast<size_t>(row)] * inv_n;
+  const float rstd = rsqrtf(stats[2 * static_cast<size_t>(row) + 1] * inv_n - mean * mean + 1e-6f);
+  float xh[4], s[2] = {0.f, 0.f};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    xh[i] = (x[i] - mean) * rstd;
+    s[0] += d[i];
+    s[1] += xh[i] * d[i];
+  }
+  block_sums<2>(s, red);
+  const float m1 = s[0] * inv_n, m2 = s[1] * inv_n;
+  const float* sc = ss ? ss + static_cast<size_t>(row / S) * film_ld : nullptr;
+  float o[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float gm = g[c + i];
+    const float yd = gm * (rstd * (d[i] - m1 - xh[i] * m2));
+    float z = fmaf(gm, xh[i], bta[c + i]), zd = yd;
+    if (sc) { z = fmaf(sc[c + i], z, sc[N + c + i]); zd = sc[c + i] * yd; }
+    if (act == 2) {
+      const float sg = sigmoid_exact(z);
+      zd *= sg * fmaf(z, 1.0f - sg, 1.0f);
+    }
+    o[i] = zd;
+  }
+  __nv_bfloat162 p0 = __floats2bfloat162_rn(o[0], o[1]);
+  __nv_bfloat162 p1 = __floats2bfloat162_rn(o[2], o[3]);
+  uint2 pk;
+  pk.x = *reinterpret_cast<uint32_t*>(&p0);
+  pk.y = *reinterpret_cast<uint32_t*>(&p1);
+  *reinterpret_cast<uint2*>(out + off) = pk;
+  if (lo_delta) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) out[off + i + lo_delta] = bf16_lo_part(o[i]);
+  }
+}
+void launch_ln_film_tangent(const float* x32, const __nv_bfloat16* x16, const float* stats, const float* xt,
+                            const float* g, const float* b, const float* ss, int film_ld, int act, __nv_bfloat16* out,
+                            int M, int N, int S, cudaStream_t st, long long lo_delta) {
+  ln_film_tangent_kernel<<<M, N / 4, 0, st>>>(x32, x16, stats, xt, g, b, ss, film_ld, act, out, N, S, lo_delta);
+}
+
+__global__ void tangent_input_kernel(const float* __restrict__ v, const float* const* __restrict__ ind,
+                                     __nv_bfloat16* __restrict__ out, size_t n, long long lo_delta) {
+  pdl_trigger();
+  pdl_wait();
+  if (ind) v = ind[3];
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    out[i] = __float2bfloat16_rn(v[i]);
+    if (lo_delta) out[i + lo_delta] = bf16_lo_part(v[i]);
+  }
+}
+void launch_tangent_input(const float* v, const float* const* ind, __nv_bfloat16* out, size_t n, cudaStream_t st,
+                          long long lo_delta) {
+  int blocks = static_cast<int>((n + 255) / 256);
+  if (blocks > 148 * 8) blocks = 148 * 8;
+  tangent_input_kernel<<<blocks, 256, 0, st>>>(v, ind, out, n, lo_delta);
+}
+
+__global__ void __launch_bounds__(256)
+ssm_loss_kernel(const float* __restrict__ f, const float* __restrict__ ft, const float* __restrict__ v,
+                const float* __restrict__ sigma, const float* const* __restrict__ ind, float* __restrict__ loss,
+                float* __restrict__ score, float* __restrict__ hvp, float* __restrict__ loss_sum,
+                unsigned int* __restrict__ done_counter, float inv_gb, float* __restrict__ df32,
+                __nv_bfloat16* __restrict__ df16, __nv_bfloat16* __restrict__ dft16, int C, int Cp) {
+  pdl_trigger();
+  pdl_wait();
+  if (ind) { sigma = ind[1]; v = ind[3]; }
+  const int b = blockIdx.x;
+  const size_t base = static_cast<size_t>(b) * C;
+  const float sg = sigma[b];
+  float s[2] = {0.f, 0.f};
+  for (int i = threadIdx.x; i < C; i += blockDim.x) {
+    const float fv = f[base + i], vv = v[base + i];
+    s[0] += fv * fv;
+    s[1] += vv * ft[base + i];
+    if (score) score[base + i] = __fdiv_rn(fv, sg);
+    if (df32) {
+      const float gf = fv * inv_gb;
+      df32[base + i] = gf;
+      df16[static_cast<size_t>(b) * Cp + i] = __float2bfloat16_rn(gf);
+      dft16[static_cast<size_t>(b) * Cp + i] = __float2bfloat16_rn(sg * vv * inv_gb);
+    }
+  }
+  __shared__ float red[2][32];
+  __shared__ bool last;
+  block_sums<2>(s, red);
+  if (threadIdx.x == 0) {
+    loss[b] = fmaf(sg, s[1], 0.5f * s[0]);
+    if (hvp) hvp[b] = __fdiv_rn(s[1], sg);
+    last = false;
+    if (loss_sum) {
+      // as ddpm_loss_bwd_kernel: the last block adds the per-example losses in index order (bit-reproducible)
+      __threadfence();
+      last = atomicInc(done_counter, gridDim.x - 1) == gridDim.x - 1;
+    }
+  }
+  __syncthreads();
+  if (last && threadIdx.x < 32) {
+    __threadfence();
+    float acc = 0.f;
+    for (int i = threadIdx.x; i < static_cast<int>(gridDim.x); i += 32) acc += __ldcg(loss + i);
+    acc = warp_sum(acc);
+    if (threadIdx.x == 0) { loss_sum[0] = acc; loss_sum[1] = acc * inv_gb; }
+  }
+}
+void launch_ssm_loss(const float* f, const float* ft, const float* v, const float* sigma, const float* const* ind,
+                     float* loss, float* score, float* hvp, float* loss_sum, unsigned int* done_counter, float inv_gb,
+                     float* df32, __nv_bfloat16* df16, __nv_bfloat16* dft16, int B, int C, int Cp, cudaStream_t st) {
+  ssm_loss_kernel<<<B, 256, 0, st>>>(f, ft, v, sigma, ind, loss, score, hvp, loss_sum, done_counter, inv_gb, df32,
+                                     df16, dft16, C, Cp);
+}
+
 // One Langevin update after the network call (annealed: utils/ebm_utils.py:139-175; consistent: :231-253):
 //   next = x + alpha * grad + noise_coef * z ;  infill blend with y = infill_x + infill_sigma * z_infill ;
 //   metrics (mean over samples of sqrt(sum_axis1(.)^2 + 1e-10)): grad, alpha * grad, noise ; alpha itself.

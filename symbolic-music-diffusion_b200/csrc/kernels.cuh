@@ -217,6 +217,44 @@ void launch_ddpm_loss(const float* eps, const float* pred, float* loss_per_examp
 
 void launch_scale_rows(float* y, const float* sigma, int bcast, int B, int per, cudaStream_t st);
 
+// ---- sliced score matching (utils/losses.py:182-247): tangent (Jacobian-vector product) pass of DenseNCSN ----
+// d/dz swish(z) and d2/dz2 swish(z) with an exact sigmoid (s): s (1 + z (1 - s)) and s (1 - s) (2 + z (1 - 2 s))
+__device__ __forceinline__ float sigmoid_exact(float z) { return 1.0f / (1.0f + expf(-z)); }
+// NV sums over the CTA (blockDim.x a multiple of 32); every thread receives the totals
+template <int NV>
+__device__ __forceinline__ void block_sums(float (&v)[NV], float (&red)[NV][32]) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+#pragma unroll
+  for (int j = 0; j < NV; ++j) {
+    v[j] = warp_sum(v[j]);
+    if (lane == 0) red[j][warp] = v[j];
+  }
+  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < NV; ++j) {
+    float t = 0.f;
+    for (int w = 0; w < nw; ++w) t += red[j][w];
+    v[j] = t;
+  }
+  __syncthreads();
+}
+// Tangent of out = act(film(LN(x))) along xt: with xh = (x - mean) rstd from the PRIMAL row statistics (sum, sumsq),
+//   xh' = rstd (xt - mean(xt) - xh mean(xh xt)),  y' = gamma xh',  z' = scale y',  out' = swish'(z) z'  (bf16).
+// x: the primal LayerNorm input, fp32 (x32) or bf16 (x16); ss: FiLM [rows / S][film_ld] = [scale | shift] or null.
+void launch_ln_film_tangent(const float* x32, const __nv_bfloat16* x16, const float* stats, const float* xt,
+                            const float* g, const float* b, const float* ss, int film_ld, int act, __nv_bfloat16* out,
+                            int M, int N, int S, cudaStream_t st, long long lo_delta);
+// out = bf16(v) (+ lo halves); ind (graph replay) overrides v with ind[3]
+void launch_tangent_input(const float* v, const float* const* ind, __nv_bfloat16* out, size_t n, cudaStream_t st,
+                          long long lo_delta);
+// Per example b (f = raw network output, ft its tangent along v, sg = sigma[b]):
+//   loss[b] = 0.5 |f|^2 + sg v.ft  (= (0.5 |s|^2 + v.J_s v) sg^2 with s = f / sg);  score <- f / sg;  hvp[b] <- v.ft / sg.
+// Training (df32 != null): the adjoint seeds df = f / global_batch (fp32 + bf16 padded to Cp) and dft = sg v / global_batch
+// (bf16 padded), and loss_sum[0..1] as smd_ddpm_grads (summed in example order by the last block).
+void launch_ssm_loss(const float* f, const float* ft, const float* v, const float* sigma, const float* const* ind,
+                     float* loss, float* score, float* hvp, float* loss_sum, unsigned int* done_counter, float inv_gb,
+                     float* df32, __nv_bfloat16* df16, __nv_bfloat16* dft16, int B, int C, int Cp, cudaStream_t st);
+
 struct LangevinStepArgs {
   const float* x; const float* grad; const float* z;   // z: supplied N(0,1) or null -> threefry(key)
   uint32_t key0, key1, ikey0, ikey1;

@@ -76,6 +76,10 @@ struct WorkspaceLayout {
   // index (the backward pass reads them all); an inference plan gives every index of a family the same region.
   std::vector<size_t> h, a, qkv, o, hidden, u, r1, act, e1, e2;
   std::vector<size_t> hidden_pre, probs, e1pre;   // written by the training forward only; empty in an inference plan
+  // DenseNCSN only -- tangent (Jacobian-vector product) pass of sliced score matching, same indexing as the primal
+  // families: xbt (bf16 input tangent v), ut[0..K] (fp32), r1t per block (fp32), actt[0..2K] (bf16), yt (output tangent)
+  size_t xbt = 0, yt = 0;
+  std::vector<size_t> ut, r1t, actt;
 };
 
 // Named workspace region, for smd_debug_buffer.
@@ -106,6 +110,12 @@ struct TrainState {
   std::vector<GemmOp> dWb, dXb, dWa, dXa, dWss, dXss;
   std::vector<GemmOp> dW2, dX2, dW1, dX1, dWo, dXo, dWqkv, dXqkv;
   GemmOp dWout, dXout, dWpost, dXpost, dWin;
+  // DenseNCSN only -- adjoints of the tangent pass (sliced score matching): gt16 / dut32 mirror g16 / du32, dut16 /
+  // drt16 / dpredt16 mirror du16 / dr16t / dpred16, and the t* GEMMs are the tangent halves of the dW / dX GEMMs
+  size_t gt16 = 0, dut32 = 0, dpredt16 = 0;
+  std::vector<size_t> dut16, drt16;
+  std::vector<GemmOp> tdWb, tdXb, tdWa, tdXa;
+  GemmOp tdWout, tdXout, tdWin;
 };
 
 }  // namespace smd
@@ -136,6 +146,8 @@ struct smd_plan {
   std::vector<FfnOp> op_ffn;   // fused FFN (mlp_dims % 128 == 0)
   std::vector<AttnOp> op_attn; // fused attention block (head dim 8 / 16)
   GemmOp op_post, op_out, op_in;
+  std::vector<GemmOp> op_ta, op_tb;   // DenseNCSN tangent pass: same weights, tangent activations, no bias
+  GemmOp op_tin, op_tout;
   // sampler
   int T = 0;
   int T_obj = 0;  // schedule length of the training objective
@@ -189,8 +201,10 @@ inline GemmEpilogue epi() {
 }
 // raw_out: DenseNCSN only -- leave out the final division by sigma (the training path differentiates through it itself)
 // save: training forward -- keep the unfused kernels and write the save-only outputs the backward pass reads
+// tangent: DenseNCSN only -- also push the tangent already cast into reg.xbt through the network (Jacobian-vector
+// product, raw output tangent into reg.yt); it reads the primal row statistics of each LayerNorm
 int run_forward(smd_plan* p, const float* params, const float* x, const float* t, int t_broadcast, int batch,
-                float* y, cudaStream_t st, bool save, bool raw_out = false);
+                float* y, cudaStream_t st, bool save, bool raw_out = false, bool tangent = false);
 int train_bind(smd_plan* p);
 int ensure_side_stream(smd_plan* p);
 }  // namespace smd

@@ -189,6 +189,22 @@ static void build_workspace(smd_plan* p) {
     t.e2_16 = ws_add(p, "t.e2_16", Bp * kFilmHid * 2);
     t.dss16 = ws_add(p, "t.dss16", Bp * 2 * Md * 2);
   }
+  if (c.arch == SMD_ARCH_DENSE_NCSN) {
+    // tangent pass of sliced score matching, after every other region so the primal offsets stay where they are
+    w.xbt = ws_add(p, "xbt", Mp * Cp * 2);
+    w.ut = family(K + 1, Mp * Md * 4, idx("t.ut"));
+    w.r1t = family(K, Mp * Md * 4, idx("t.r1t"));
+    w.actt = family(2 * K + 1, Mp * Md * 2, idx("t.actt"));
+    w.yt = ws_add(p, "yt", B * C * 4);
+    if (c.training) {
+      TrainState& t = p->train;
+      t.gt16 = ws_add(p, "t.gt16", Mp * Md * 2);
+      t.dut32 = ws_add(p, "t.dut32", Mp * Md * 4);
+      t.dut16 = family(K + 1, Mp * Md * 2, idx("t.dut16_"));
+      t.drt16 = family(K, Mp * Md * 2, idx("t.drt16_"));
+      t.dpredt16 = ws_add(p, "t.dpredt16", Mp * Cp * 2);
+    }
+  }
   if (strict) {
     w.x3_scratch = ws_add(p, "x3.scratch", Mp * Md * 4);   // fp32 cross-term accumulator of the three-pass GEMMs
     p->lo_bytes = p->ws_bytes;                // second copy of the workspace: the lo halves, at the same offsets
@@ -244,6 +260,17 @@ static int build_ops(smd_plan* p) {
   if (!make_gemm_op(&p->op_out, p->ws + w.act[2 * p->K], Mp, p->ws + w.out_pad, static_cast<uint64_t>(Cp), C, Md,
                     std::min(Cp, kBNMax), 0, 1, 0, 0, p->lo_bytes))
     return SMD_ERR_CUDA;
+  if (c.arch == SMD_ARCH_DENSE_NCSN) {
+    if (!fwd(&p->op_tin, w.xbt, p->par.in.kernel, C, Md)) return SMD_ERR_CUDA;
+    p->op_ta.resize(p->K); p->op_tb.resize(p->K);
+    for (int k = 0; k < p->K; ++k) {
+      if (!fwd(&p->op_ta[k], w.actt[2 * k], p->par.block[k].a.kernel, Md, Md)) return SMD_ERR_CUDA;
+      if (!fwd(&p->op_tb[k], w.actt[2 * k + 1], p->par.block[k].b.kernel, Md, Md)) return SMD_ERR_CUDA;
+    }
+    if (!make_gemm_op(&p->op_tout, p->ws + w.actt[2 * p->K], Mp, p->ws + w.out_pad, static_cast<uint64_t>(Cp), C, Md,
+                      std::min(Cp, kBNMax), 0, 1, 0, 0, p->lo_bytes))
+      return SMD_ERR_CUDA;
+  }
   return SMD_OK;
 }
 
@@ -326,7 +353,9 @@ int ensure_side_stream(smd_plan* p) {
 
 // The FiLM'd residual tail shared by both architectures (models/ncsn.py:173-178, models/shared.py:61-75).
 // On entry u (fp32 [M][Md]) and stats[0] hold the block input and its row statistics.
-static int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, float* y, cudaStream_t st) {
+// tangent: run the tangent pass next to it (ut[0] and the primal statistics are ready; see run_forward).
+static int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, float* y, cudaStream_t st,
+                    bool tangent) {
   const int Md = p->cfg.mlp_dims, C = p->cfg.channels;
   const WorkspaceLayout& w = p->reg;
   float* stats = p->at<float>(w.stats);
@@ -350,6 +379,11 @@ static int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadc
     launch_ln_film_act(u_in, ls.totals, params + bp.ln_a.scale, params + bp.ln_a.bias,
                        scale, shift, 2 * Md, t_broadcast, 2, act_a, M, Md, S, st, frow_dev, nullptr, p->lo_elems,
                        ls.part, ls.nslots, ls.totals); CNT();
+    if (tangent) {
+      launch_ln_film_tangent(u_in, nullptr, ls.totals, p->at<float>(w.ut[k]), params + bp.ln_a.scale,
+                             params + bp.ln_a.bias, scale, 2 * Md, 2, p->at<__nv_bfloat16>(w.actt[2 * k]), M, Md, S, st,
+                             p->lo_elems); CNT();
+    }
     GemmEpilogue e = epi();
     e.bias = params + bp.a.bias;
     // r1 only feeds a LayerNorm: bf16 is enough (strict mode keeps the pre-LayerNorm intermediate in fp32)
@@ -359,16 +393,32 @@ static int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadc
     else { e.out_bf16 = r1_16; e.ld_bf16 = Md; }
     e.row_stats = stats + (2 * k + 1) * sstride;
     SMD_CUDA(gemm(p, p->op_a[k], M, e, st, 2 * k + 1));
+    if (tangent) {
+      e = epi();
+      e.out_f32 = p->at<float>(w.r1t[k]); e.ld_f32 = Md;
+      SMD_CUDA(gemm(p, p->op_ta[k], M, e, st));
+    }
     ls = ln_stats(p, 2 * k + 1);
     launch_ln_film_act(r1, ls.totals, params + bp.ln_b.scale, params + bp.ln_b.bias, scale, shift, 2 * Md,
                        t_broadcast, 2, act_b, M, Md, S, st, frow_dev, r1_16, p->lo_elems, ls.part, ls.nslots,
                        ls.totals); CNT();
+    if (tangent) {
+      launch_ln_film_tangent(r1, r1_16, ls.totals, p->at<float>(w.r1t[k]), params + bp.ln_b.scale,
+                             params + bp.ln_b.bias, scale, 2 * Md, 2, p->at<__nv_bfloat16>(w.actt[2 * k + 1]), M, Md, S,
+                             st, p->lo_elems); CNT();
+    }
     e = epi();
     e.bias = params + bp.b.bias;
     e.residual = u_in; e.ld_res = Md;
     e.out_f32 = u_out; e.ld_f32 = Md;
     e.row_stats = stats + (2 * k + 2) * sstride;
     SMD_CUDA(gemm(p, p->op_b[k], M, e, st, 2 * k + 2));
+    if (tangent) {   // u' <- act_b' W_b + u'  (no bias)
+      e = epi();
+      e.residual = p->at<float>(w.ut[k]); e.ld_res = Md;
+      e.out_f32 = p->at<float>(w.ut[k + 1]); e.ld_f32 = Md;
+      SMD_CUDA(gemm(p, p->op_tb[k], M, e, st));
+    }
   }
   const LnStats lo_ = ln_stats(p, 2 * p->K);
   launch_ln_film_act(p->at<float>(w.u[p->K]), lo_.totals, params + p->par.out_ln.scale, params + p->par.out_ln.bias,
@@ -378,12 +428,20 @@ static int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadc
   e.bias = params + p->par.out.bias;
   e.out_f32 = y; e.ld_f32 = C;
   SMD_CUDA(gemm(p, p->op_out, M, e, st));
+  if (tangent) {
+    launch_ln_film_tangent(p->at<float>(w.u[p->K]), nullptr, lo_.totals, p->at<float>(w.ut[p->K]),
+                           params + p->par.out_ln.scale, params + p->par.out_ln.bias, nullptr, 0, 0,
+                           p->at<__nv_bfloat16>(w.actt[2 * p->K]), M, Md, S, st, p->lo_elems); CNT();
+    e = epi();
+    e.out_f32 = p->at<float>(w.yt); e.ld_f32 = C;
+    SMD_CUDA(gemm(p, p->op_tout, M, e, st));
+  }
   SMD_LAUNCH_CHECK("tail");
   return SMD_OK;
 }
 
 int run_forward(smd_plan* p, const float* params, const float* x, const float* t, int t_broadcast, int batch,
-                float* y, cudaStream_t st, bool save, bool raw_out) {
+                float* y, cudaStream_t st, bool save, bool raw_out, bool tangent) {
   const smd_config& c = p->cfg;
   if (!p->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
   if (!p->packed) { set_error("smd_pack_weights has not been called"); return SMD_ERR_STATE; }
@@ -491,10 +549,15 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
     e.out_f32 = u0; e.ld_f32 = Md;
     e.row_stats = stats;
     SMD_CUDA(gemm(p, p->op_in, M, e, st, 0));
+    if (tangent) {   // u0' = v W_in (the caller cast v into xbt)
+      e = epi();
+      e.out_f32 = p->at<float>(w.ut[0]); e.ld_f32 = Md;
+      SMD_CUDA(gemm(p, p->op_tin, M, e, st));
+    }
   }
   SMD_LAUNCH_CHECK("trunk");
   if (film_on_side) SMD_CUDA(cudaStreamWaitEvent(st, p->ev_film, 0));
-  rc = run_tail(p, params, M, S, t_broadcast, y, st);
+  rc = run_tail(p, params, M, S, t_broadcast, y, st, tangent);
   if (rc) return rc;
   if (c.arch == SMD_ARCH_DENSE_NCSN && !raw_out) {   // models/ncsn.py:97: output = x / sigmas
     launch_scale_rows(y, t, t_broadcast, batch, S * C, st); CNT();
@@ -571,6 +634,14 @@ __global__ void threefry_uniform_kernel(uint32_t k0, uint32_t k1, float* out, ui
 __global__ void threefry_normal_kernel(uint32_t k0, uint32_t k1, float* out, uint32_t n, uint32_t first, uint32_t total) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
     out[i] = jax_normal_from_bits(jax_random_bits(k0, k1, first + i, total));
+}
+
+// out[j] = element (first + j) of jax.random.rademacher(key, (total,)) as of jax 0.2.8: 2 bernoulli(key, 0.5) - 1 with
+// bernoulli = uniform01 < 0.5, i.e. +1 exactly when the threefry word is below 2^31
+__global__ void threefry_rademacher_kernel(uint32_t k0, uint32_t k1, float* out, uint32_t n, uint32_t first,
+                                           uint32_t total) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    out[i] = jax_random_bits(k0, k1, first + i, total) < 0x80000000u ? 1.0f : -1.0f;
 }
 
 }  // namespace smd
@@ -789,6 +860,56 @@ int smd_dsm_draws(smd_plan* plan, const uint32_t host_key[2], int global_batch, 
                                                  static_cast<uint32_t>(global_batch * per));
   CNT();
   SMD_LAUNCH_CHECK("dsm_draws");
+  return SMD_OK;
+}
+
+int smd_ssm_draws(smd_plan* plan, const uint32_t host_key[2], int global_batch, int first_row, int batch,
+                  int continuous_noise, float* used_sigma, float* eps, float* v, int* labels_or_null,
+                  smd_stream_t stream) {
+  if (plan->cfg.arch != SMD_ARCH_DENSE_NCSN) { set_error("smd_ssm_draws needs a score network (SMD_ARCH_DENSE_NCSN)"); return SMD_ERR_INVALID; }
+  if (plan->L_dsm <= 0) { set_error("smd_dsm_setup has not been called"); return SMD_ERR_STATE; }
+  if (batch < 1 || first_row < 0 || global_batch < first_row + batch) { set_error("batch out of range"); return SMD_ERR_INVALID; }
+  const long long per = static_cast<long long>(plan->cfg.seq_len) * plan->cfg.channels;
+  if (static_cast<long long>(global_batch) * per > 0xFFFFFFFFll) { set_error("global batch too large"); return SMD_ERR_INVALID; }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int L = plan->L_dsm, cn = continuous_noise ? 1 : 0;
+  uint32_t k4[8], k2[4] = {0, 0, 0, 0};
+  h_split(host_key, 4, k4);               // rng, label_rng, sample_rng, score_rng   (utils/losses.py:203)
+  if (cn) { const uint32_t rng[2] = {k4[0], k4[1]}; h_split(rng, 2, k2); }        // rng, noise_rng (:210)
+  draws_kernel<<<(batch + 127) / 128, 128, 0, st>>>(k4[2], k4[3], k2[2], k2[3], plan->at<float>(plan->reg.sigmas), L - 1, L - cn,
+                                                    global_batch, first_row, batch, cn, cn, used_sigma, labels_or_null);
+  CNT();
+  const long long n = static_cast<long long>(batch) * per;
+  int blocks = static_cast<int>((n + 255) / 256);
+  if (blocks > 148 * 8) blocks = 148 * 8;
+  const uint32_t first = static_cast<uint32_t>(first_row * per), total = static_cast<uint32_t>(global_batch * per);
+  threefry_normal_kernel<<<blocks, 256, 0, st>>>(k4[4], k4[5], eps, static_cast<uint32_t>(n), first, total);
+  CNT();
+  threefry_rademacher_kernel<<<blocks, 256, 0, st>>>(k4[6], k4[7], v, static_cast<uint32_t>(n), first, total);
+  CNT();
+  SMD_LAUNCH_CHECK("ssm_draws");
+  return SMD_OK;
+}
+
+int smd_ssm_loss(smd_plan* plan, const float* params, const float* x0, const float* used_sigma, const float* eps,
+                 const float* v, int batch, float* loss_per_example, float* score_or_null, float* hvp_or_null,
+                 smd_stream_t stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (plan->cfg.arch != SMD_ARCH_DENSE_NCSN) { set_error("smd_ssm_loss needs a score network (SMD_ARCH_DENSE_NCSN)"); return SMD_ERR_INVALID; }
+  if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
+  if (batch < 1 || batch > plan->cfg.max_batch) { set_error("batch out of range"); return SMD_ERR_INVALID; }
+  const int C = plan->cfg.channels;
+  float* xt = plan->at<float>(plan->reg.xt);
+  float* cond = plan->at<float>(plan->reg.tvec);
+  float* f = plan->at<float>(plan->reg.eps_hat);
+  launch_q_sample(x0, eps, used_sigma, xt, cond, batch, C, st, nullptr, 1); CNT();
+  launch_tangent_input(v, nullptr, plan->at<__nv_bfloat16>(plan->reg.xbt), static_cast<size_t>(batch) * C, st,
+                       plan->lo_elems); CNT();
+  int rc = run_forward(plan, params, xt, cond, 0, batch, f, st, false, /*raw_out=*/true, /*tangent=*/true);
+  if (rc) return rc;
+  launch_ssm_loss(f, plan->at<float>(plan->reg.yt), v, used_sigma, nullptr, loss_per_example, score_or_null,
+                  hvp_or_null, nullptr, nullptr, 1.0f, nullptr, nullptr, nullptr, batch, C, C, st); CNT();
+  SMD_LAUNCH_CHECK("ssm_loss");
   return SMD_OK;
 }
 

@@ -269,6 +269,43 @@ class Engine:
                                           batch, int(global_batch or batch), self.grads.data_ptr(),
                                           self._grads_buf[self.arena_floats:].data_ptr(), self._stream()))
 
+    def ssm_draws(self, key, batch: int, want_labels: bool = False, global_batch: Optional[int] = None,
+                  first_row: int = 0, continuous_noise: bool = False):
+        """(used_sigma (B,), eps, v[, labels]) of sliced_score_matching_loss (utils/losses.py:203-223) on device; v holds
+        the Rademacher (+-1) projection vectors.  Schedule: dsm_setup."""
+        dev = self._ws.device
+        shape = (batch, self.seq_len, self.cfg.channels) if ARCHS[self.cfg.arch] == 0 else (batch, self.cfg.channels)
+        used = torch.empty((batch,), dtype=torch.float32, device=dev)
+        eps = torch.empty(shape, dtype=torch.float32, device=dev)
+        v = torch.empty(shape, dtype=torch.float32, device=dev)
+        labels = torch.empty((batch,), dtype=torch.int32, device=dev) if want_labels else None
+        k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
+        _lib.check(self.lib.smd_ssm_draws(self._plan, k, int(global_batch or batch), int(first_row), batch,
+                                          1 if continuous_noise else 0, used.data_ptr(), eps.data_ptr(), v.data_ptr(),
+                                          _ptr(labels), self._stream()))
+        return (used, eps, v, labels) if want_labels else (used, eps, v)
+
+    def ssm_loss(self, x0: torch.Tensor, used_sigma: torch.Tensor, eps: torch.Tensor, v: torch.Tensor,
+                 want_terms: bool = False):
+        """Per-example sliced score matching loss; with want_terms also (score (B, C), v.J_s v (B,))."""
+        x0 = _f32c(x0, "x0"); eps = _f32c(eps, "eps"); v = _f32c(v, "v")
+        us = _f32c(used_sigma.reshape(-1), "used_sigma")
+        batch = x0.shape[0]
+        loss = torch.empty((batch,), dtype=torch.float32, device=x0.device)
+        score = torch.empty_like(x0) if want_terms else None
+        hvp = torch.empty((batch,), dtype=torch.float32, device=x0.device) if want_terms else None
+        _lib.check(self.lib.smd_ssm_loss(self._plan, self.params.data_ptr(), x0.data_ptr(), us.data_ptr(), eps.data_ptr(),
+                                         v.data_ptr(), batch, loss.data_ptr(), _ptr(score), _ptr(hvp), self._stream()))
+        return (loss, score, hvp) if want_terms else loss
+
+    def compute_ssm_grads(self, x0, used_sigma, eps, v, global_batch: Optional[int] = None) -> None:
+        x0 = _f32c(x0, "x0"); eps = _f32c(eps, "eps"); v = _f32c(v, "v")
+        us = _f32c(used_sigma.reshape(-1), "used_sigma")
+        batch = x0.shape[0]
+        _lib.check(self.lib.smd_ssm_grads(self._plan, self.params.data_ptr(), x0.data_ptr(), us.data_ptr(), eps.data_ptr(),
+                                          v.data_ptr(), batch, int(global_batch or batch), self.grads.data_ptr(),
+                                          self._grads_buf[self.arena_floats:].data_ptr(), self._stream()))
+
     def langevin_step(self, x, grad, alpha: float, noise_coef: float, step_key=None, z=None, infill_x=None,
                       infill_mask=None, infill_sigma: float = 0.0, infill_key=None, infill_z=None, x_next=None,
                       collection_slot=None, metrics4=None):

@@ -50,6 +50,9 @@ _SIGNATURES = {
     "smd_dsm_grads": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
     "smd_dsm_setup": (C.c_int, [_P, C.POINTER(C.c_float), C.c_int, _P]),
     "smd_dsm_draws": (C.c_int, [_P, C.POINTER(C.c_uint32), C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P]),
+    "smd_ssm_loss": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, _P, _P, _P, _P]),
+    "smd_ssm_grads": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "smd_ssm_draws": (C.c_int, [_P, C.POINTER(C.c_uint32), C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
     "smd_langevin_step": (C.c_int, [_P, _P, _P, C.c_int, C.c_float, C.c_float, C.POINTER(C.c_uint32), _P, _P, _P,
                                     C.c_float, C.POINTER(C.c_uint32), _P, _P, _P, _P, _P]),
     "smd_sampler_setup": (C.c_int, [_P, C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_uint32), _P]),

@@ -1,5 +1,5 @@
-"""Objectives with the reference signatures (utils/losses.py): the DDPM objective (the hot path) and denoising score
-matching for the NCSN family (SURVEY 8(f4))."""
+"""Objectives with the reference signatures (utils/losses.py): the DDPM objective (the hot path) and denoising / sliced
+score matching for the NCSN family (SURVEY 8(f4))."""
 from __future__ import annotations
 
 import numpy as np
@@ -47,3 +47,23 @@ def denoising_score_matching_loss(batch, model, sigmas, rng, continuous_noise=Fa
         eng._dsm_sigmas = sig.copy()
     used, eps = eng.dsm_draws((int(rng[0]), int(rng[1])), x0.shape[0], continuous_noise=bool(continuous_noise))
     return reduce_fn(eng.dsm_loss(x0, used, eps), reduction)
+
+
+def _score_engine(batch, model, sigmas):
+    from .nn import _as_device_f32
+    x0 = _as_device_f32(batch)
+    eng = model.engine(x0.shape[0])
+    sig = np.asarray(sigmas, np.float32)
+    if getattr(eng, "_dsm_sigmas", None) is None or not np.array_equal(eng._dsm_sigmas, sig):
+        eng.dsm_setup(sig)
+        eng._dsm_sigmas = sig.copy()
+    return x0, eng
+
+
+def sliced_score_matching_loss(batch, model, sigmas, rng, continuous_noise=False, reduction="mean"):
+    """utils/losses.py:182-247 (one particle): sigma labels, noise and Rademacher vectors v from `rng` (jax threefry
+    semantics, on device), x~ = x + sigma eps, s = model(x~, sigma), (0.5 |s|^2 + v.J_s v) sigma^2 per example.  The
+    Hessian term v.J_s v is a Jacobian-vector product through the network.  `model` must be ncsn.DenseNCSN."""
+    x0, eng = _score_engine(batch, model, sigmas)
+    used, eps, v = eng.ssm_draws((int(rng[0]), int(rng[1])), x0.shape[0], continuous_noise=bool(continuous_noise))
+    return reduce_fn(eng.ssm_loss(x0, used, eps, v), reduction)

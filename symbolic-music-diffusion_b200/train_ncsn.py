@@ -1,8 +1,8 @@
 """Training entry point with the reference's flag surface (train_ncsn.py:48-128), so configs/ddpm-*.cfg run
 unchanged:  python -m smd_b200.train_ncsn --flagfile=configs/ddpm-mel-32seq-512.cfg [--synthetic]
 
-Only the DDPM family is on the GPU hot path: --loss=ddpm, --sampling=ddpm, --architecture in
-{TransformerDDPM, TransformerDDPM4, DenseDDPM}.  Other values raise ValueError exactly where the reference would
+Objectives: --loss=ddpm (TransformerDDPM, TransformerDDPM4, DenseDDPM), --loss=dsm and --loss=ssm (DenseNCSN; ssm
+with any other architecture raises ValueError).  Other values raise ValueError exactly where the reference would
 dispatch on them.  Data-parallel: launch with torchrun (one process per GPU); the batch is sharded across ranks
 and gradients are summed with one NCCL all-reduce over the flat arena (SURVEY section 8(e)).
 """
@@ -16,7 +16,7 @@ import torch
 from absl import app, flags, logging
 
 from smd_b200 import checkpoints, ebm_utils, input_pipeline, jrandom as random, ncsn, nn, optim, parallel, train_utils
-from smd_b200.losses import denoising_score_matching_loss, diffusion_loss
+from smd_b200.losses import denoising_score_matching_loss, diffusion_loss, sliced_score_matching_loss
 
 FLAGS = flags.FLAGS
 _D = flags.DEFINE_integer, flags.DEFINE_float, flags.DEFINE_bool, flags.DEFINE_string, flags.DEFINE_enum
@@ -102,9 +102,11 @@ def _objective():
     if FLAGS.loss == "dsm":
         return denoising_score_matching_loss
     if FLAGS.loss == "ssm":
-        # sliced score matching (utils/losses.py:182-247) differentiates through the score network's Jacobian-vector
-        # product: it needs a second-order backward pass that is not written
-        raise ValueError("--loss=ssm needs a double-backward pass that is not implemented (use dsm or ddpm)")
+        # sliced score matching (utils/losses.py:182-247): its Jacobian-vector product and second-order backward are
+        # written for the dense score network only
+        if FLAGS.architecture != "DenseNCSN":
+            raise ValueError(f"--loss=ssm needs --architecture=DenseNCSN (got {FLAGS.architecture})")
+        return sliced_score_matching_loss
     raise ValueError(f"Unsupported objective {FLAGS.loss}")
 
 
@@ -133,8 +135,9 @@ def lr_at(step: int) -> float:
 
 def train_step(objective, batch, optimizer, sigmas, rng, learning_rate, ema=None):
     """train_ncsn.py:260-288 on this rank's shard: grads -> all-reduce -> clip -> Adam (one fused pass)."""
-    if objective not in (diffusion_loss, denoising_score_matching_loss):
-        raise ValueError("only the ddpm and dsm objectives have a hand-written backward")
+    if objective not in (diffusion_loss, denoising_score_matching_loss, sliced_score_matching_loss):
+        raise ValueError("only the ddpm, dsm and ssm objectives have a hand-written backward")
+    ssm = objective is sliced_score_matching_loss
     dsm = objective is denoising_score_matching_loss
     model = optimizer.target
     world, rank = parallel.world_size(), parallel.rank()
@@ -142,7 +145,7 @@ def train_step(objective, batch, optimizer, sigmas, rng, learning_rate, ema=None
     local = x0.shape[0]
     eng = model.engine(local, training=True)
     betas = np.asarray(sigmas, np.float32)
-    if dsm:
+    if dsm or ssm:
         if getattr(eng, "_dsm_sigmas", None) is None or not np.array_equal(eng._dsm_sigmas, betas):
             eng.dsm_setup(betas)
             eng._dsm_sigmas = betas.copy()
@@ -153,7 +156,11 @@ def train_step(objective, batch, optimizer, sigmas, rng, learning_rate, ema=None
         eng.init_train_state(ema=False)
     # every rank holds the SAME key and consumes rows [rank*local, (rank+1)*local) of the global batch's threefry
     # streams (labels, alpha-bar, eps): an N-GPU run with seed s sees exactly the noise of the 1-GPU run with seed s
-    if dsm:
+    if ssm:
+        used, eps, v = eng.ssm_draws((int(rng[0]), int(rng[1])), local, global_batch=local * world,
+                                     first_row=rank * local, continuous_noise=FLAGS.continuous_noise)
+        eng.compute_ssm_grads(x0, used, eps, v, global_batch=local * world)
+    elif dsm:
         used, eps = eng.dsm_draws((int(rng[0]), int(rng[1])), local, global_batch=local * world, first_row=rank * local,
                                   continuous_noise=FLAGS.continuous_noise)
         eng.compute_dsm_grads(x0, used, eps, global_batch=local * world)
