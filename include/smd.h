@@ -43,7 +43,11 @@ enum smd_arch {
   SMD_ARCH_DENSE_DDPM = 1,
   /* models/ncsn.py:83-98 (DenseNCSN) with its undefined `t` read as `sigmas`: the DenseDDPM stack conditioned on sigma,
    * output divided by sigma (a score).  Same parameter layout as SMD_ARCH_DENSE_DDPM. */
-  SMD_ARCH_DENSE_NCSN = 2
+  SMD_ARCH_DENSE_NCSN = 2,
+  /* models/autoregressive.py:37-82 (TransformerMDN): the TransformerDDPM trunk on the input shifted right by one position,
+   * causal self-attention, res-blocks without FiLM and a mixture-density head.  Created with smd_mdn_plan_create only
+   * (seq_len 32, precision bf16). */
+  SMD_ARCH_TRANSFORMER_MDN = 3
 };
 
 typedef struct smd_config {
@@ -204,6 +208,30 @@ int smd_ddpm_reverse_step(smd_plan* plan, const float* params, const float* x, i
 int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int steps, const float* infill_x,
                     const float* infill_mask, float* collection, float* metrics, int use_graph,
                     smd_stream_t stream);
+
+/* ---- autoregressive baseline (TransformerMDN, train_mdn.py) -------------------------------------------------- */
+/* cfg->arch must be SMD_ARCH_TRANSFORMER_MDN; num_components = --mdn_components (Kc).  SMD_ERR_INVALID for
+ * seq_len != 32, precision bf16x3 or num_components < 1.  Parameters: the TransformerDDPM trunk, k{i}.res.* without
+ * film, out_ln, then mdn.mu / mdn.log_sigma (Md, Kc*C) and mdn.pi (Md, Kc); column k*C + c of mu / log_sigma is
+ * component k, channel c.  smd_forward, the DDPM / NCSN objectives and the sampler return SMD_ERR_INVALID on such a
+ * plan. */
+int smd_mdn_plan_create(const smd_config* cfg, int num_components, smd_plan** out);
+/* (pi, mu, log_sigma) = model(x, shift)   (models/autoregressive.py:40-82).  x: (batch, S, C) fp32; pi (batch, S, Kc),
+ * mu and log_sigma (batch, S, Kc*C) fp32.  shift = 0 feeds x to the trunk as it is (autoregressive decoding). */
+int smd_mdn_forward(smd_plan* plan, const float* params, const float* x, int batch, int shift, float* pi, float* mu,
+                    float* log_sigma, smd_stream_t stream);
+/* mdn_loss(pi, mu, log_sigma, x, 'none') (train_mdn.py:100-133), no plan needed: loss[r] = -log sum_k softmax(pi_r)_k
+ * N(x_r; mu_rk, diag(exp(log_sigma_rk))^2) for rows r < rows; pi (rows, Kc), mu / log_sigma (rows, Kc*C), x (rows, C). */
+int smd_mdn_nll(const float* pi, const float* mu, const float* log_sigma, const float* x, int rows, int C, int Kc,
+                float* loss, smd_stream_t stream);
+/* eval_step's loss (train_mdn.py:154-168): the model on shift_right(x), scored against x; one loss per token (batch*S). */
+int smd_mdn_loss(smd_plan* plan, const float* params, const float* x, int batch, float* loss_per_token,
+                 smd_stream_t stream);
+/* gradients of the mean of that loss over global_batch * S tokens; same contract as smd_ddpm_grads (loss_sum[0] = this
+ * shard's token-loss sum, loss_sum[1] = loss_sum[0] / (global_batch * S)), CUDA-graph replay and
+ * smd_grads_tail_range / smd_wait_tail_grads (the k*, out_ln and mdn.* slice) included. */
+int smd_mdn_grads(smd_plan* plan, const float* params, const float* x, int batch, int global_batch, float* grads,
+                  float* loss_sum, smd_stream_t stream);
 
 /* ---- jax.random (threefry2x32) on device ------------------------------------------------------------------ */
 int smd_threefry_normal(const uint32_t host_key[2], float* out, long long n, smd_stream_t stream);

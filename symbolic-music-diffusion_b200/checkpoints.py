@@ -1,7 +1,8 @@
 """Checkpoint save / restore with the call shape of flax.training.checkpoints (train_ncsn.py:395-399,
 sample_ncsn.py:341-342): save_checkpoint(dir, (optimizer, ema, early_stop), step, keep=N) writes
 ``checkpoint_<step>`` atomically and prunes to the newest `keep`; restore_checkpoint(dir, target) loads the
-latest into the template objects.
+latest into the template objects.  train_mdn.py:305-307 saves the 2-tuple (optimizer, early_stop) instead: its
+state dict is {'0': optimizer, '1': early_stop}, as flax's to_state_dict writes any tuple.
 
 Default format: msgpack of a state dict {'0': optimizer, '1': ema, '2': early_stop} with the flat arenas as ndarray
 leaves encoded as {'__nd__': True, 'dtype', 'shape', 'data'} plus the arena layout (self-describing).
@@ -29,12 +30,25 @@ def _un_nd(d) -> np.ndarray:
     return np.frombuffer(d["data"], dtype=np.dtype(d["dtype"])).reshape(d["shape"]).copy()
 
 
+def split_target(target):
+    """(optimizer, ema, early_stop) or train_mdn's (optimizer, early_stop) -> (optimizer, ema or None, early_stop)"""
+    if len(target) == 2:
+        return target[0], None, target[1]
+    return tuple(target)
+
+
+def join_target(target, optimizer, ema, early_stop):
+    return (optimizer, early_stop) if len(target) == 2 else (optimizer, ema, early_stop)
+
+
 def _state(target) -> dict:
-    optimizer, ema, early_stop = target
+    optimizer, ema, early_stop = split_target(target)
     opt = {"state": {"step": int(optimizer.step), "grad_ema": _nd(optimizer.grad_ema.cpu().numpy()),
                      "grad_sq_ema": _nd(optimizer.grad_sq_ema.cpu().numpy())},
            "target": {"params": _nd(optimizer.target.arena.flat.cpu().numpy()),
                       "layout": [[n, int(o), list(s)] for n, o, s in optimizer.target.arena.layout]}}
+    if len(target) == 2:
+        return {"0": opt, "1": early_stop.state_dict()}
     e = None if ema is None else {"mu": float(ema.mu), "params": _nd(ema.params.flat.cpu().numpy())}
     return {"0": opt, "1": e, "2": early_stop.state_dict()}
 
@@ -84,7 +98,7 @@ def restore_checkpoint(ckpt_dir: str, target, step: int = None, prefix: str = PR
         st = flax_compat.msgpack_restore(f.read())       # plain msgpack plus flax's ndarray ext types
     if flax_compat.is_flax_state(st):
         return flax_compat.load_flax_state(st, target)
-    optimizer, ema, early_stop = target
+    optimizer, ema, early_stop = split_target(target)
     o = st["0"]
     flat = _un_nd(o["target"]["params"])
     arena = optimizer.target.arena
@@ -100,5 +114,6 @@ def restore_checkpoint(ckpt_dir: str, target, step: int = None, prefix: str = PR
         ema.params.bump()
         ema.mu = float(st["1"]["mu"])
     from .train_utils import EarlyStopping
-    es = EarlyStopping(**st["2"]) if st.get("2") else early_stop
-    return optimizer, ema, es
+    es_key = "1" if len(target) == 2 else "2"
+    es = EarlyStopping(**st[es_key]) if st.get(es_key) else early_stop
+    return join_target(target, optimizer, ema, es)

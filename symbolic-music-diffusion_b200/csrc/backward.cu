@@ -8,7 +8,7 @@
 namespace smd {
 
 // Split count for a dW GEMM that runs beside the dX chain: ~48 CTAs, leaving two thirds of the SMs to `st`.
-static int pick_splits_side(int m_rows, int n_cols, int BN, int num_kb) {
+int pick_splits_side(int m_rows, int n_cols, int BN, int num_kb) {
   const int tiles = ((m_rows + 127) / 128) * ((n_cols + BN - 1) / BN);
   int s = 48 / tiles;
   if (s < 1) s = 1;
@@ -45,14 +45,17 @@ int train_bind(smd_plan* p) {
     if (!make_dx(&ts.dXb[k], B16(ts.du16[k + 1]), Md, p->wsh(bp.b.kernel), Md, Mp)) return SMD_ERR_CUDA;
     if (!make_dw(&ts.dWa[k], B16(w.act[2 * k]), Md, B16(ts.dr16t[k]), Md, Md, Mp)) return SMD_ERR_CUDA;
     if (!make_dx(&ts.dXa[k], B16(ts.dr16t[k]), Md, p->wsh(bp.a.kernel), Md, Mp)) return SMD_ERR_CUDA;
+    if (p->mdn()) continue;   // no FiLM generator
     if (!make_dw(&ts.dWss[k], B16(ts.e2_16), 512, B16(ts.dss16), 2 * Md, 2 * Md, Bp)) return SMD_ERR_CUDA;
     if (!make_dx(&ts.dXss[k], B16(ts.dss16), 2 * Md, p->wsh(bp.film.ss.kernel), 512, Bp)) return SMD_ERR_CUDA;
   }
-  // output projection: dpred16 is zero-padded to Cp columns; the plain weight copy is [Md][Cp]
-  if (!make_gemm_op(&ts.dWout, B16(w.act[2 * K]), static_cast<uint64_t>(Md), B16(ts.dpred16), static_cast<uint64_t>(Cp),
+  // output projection: dpred16 is zero-padded to Cp columns; the plain weight copy is [Md][Cp] (TransformerMDN: dZ and
+  // the packed head weight, both Np wide; its dW GEMMs are built by mdn_train_bind)
+  if (!p->mdn() &&
+      !make_gemm_op(&ts.dWout, B16(w.act[2 * K]), static_cast<uint64_t>(Md), B16(ts.dpred16), static_cast<uint64_t>(Cp),
                     C, static_cast<int>(Mp), std::min(Cp, kBNMax), 1, 1))
     return SMD_ERR_CUDA;
-  if (!make_gemm_op(&ts.dXout, B16(ts.dpred16), Mp, B16(w.out_pad), static_cast<uint64_t>(Md), Md, Cp,
+  if (!make_gemm_op(&ts.dXout, B16(ts.dpred16), Mp, B16(w.out_pad), static_cast<uint64_t>(Md), Md, p->head_ld,
                     choose_bn(Md), 0, 0)) return SMD_ERR_CUDA;
   if (L > 0) {
     if (!make_dw(&ts.dWpost, B16(w.a[2 * L]), 128, B16(ts.du16[0]), Md, Md, Mp)) return SMD_ERR_CUDA;
@@ -89,10 +92,11 @@ int train_bind(smd_plan* p) {
                       choose_bn(Md), 0, 0)) return SMD_ERR_CUDA;
     if (!make_dw(&ts.tdWin, B16(w.xbt), C, B16(ts.dut16[0]), Md, Md, Mp)) return SMD_ERR_CUDA;
   }
+  if (p->mdn()) return mdn_train_bind(p);
   return SMD_OK;
 }
 
-static cudaError_t gemm_k(const GemmOp& op0, int rows, int K, int splits, const GemmEpilogue& e, cudaStream_t st) {
+cudaError_t gemm_k(const GemmOp& op0, int rows, int K, int splits, const GemmEpilogue& e, cudaStream_t st) {
   GemmOp op = op0;
   op.K = K;
   op.k_splits = splits;
@@ -139,58 +143,33 @@ static cudaError_t film_generator_bwd(smd_plan* p, const float* params, int k, i
   return cudaSuccess;
 }
 
-}  // namespace smd
+void launch_colsum_bf16(const __nv_bfloat16* in, int ld, float* out, int M, int N, cudaStream_t st) {
+  launch_colsum<__nv_bfloat16>(in, ld, out, M, N, st);
+}
 
-using namespace smd;
-
-// ind: device table {x0, used_alpha, eps} read by the kernels instead of the pointer arguments (graph replay), or null.
-// capturing: the call is being recorded into a CUDA graph -- the three "tail gradients are final" events that
-// smd_wait_tail_grads hands to the caller's communication stream are then recorded as EXTERNAL event nodes, so a stream
-// outside the graph can wait on them after the graph has been launched.
-static int grads_impl(smd_plan* p, const float* params, const float* x0, const float* used_alpha, const float* eps,
-                      const float* const* ind, int batch, int global_batch, float* grads, float* loss_sum,
-                      cudaStream_t st, bool capturing, int objective) {
-  const unsigned ext = capturing ? cudaEventRecordExternal : cudaEventRecordDefault;
-  TrainState& ts = p->train;
-  const smd_config& c = p->cfg;
-  const int S = c.seq_len, C = c.channels, Md = c.mlp_dims;
-  const int Cp = (C + 63) / 64 * 64;
-  const int M = batch * S;
-  const int Mk = (M + 63) / 64 * 64;           // reduction length of the dW GEMMs
-  const int Bk = (batch + 63) / 64 * 64;
-  const int per = S * C;
-  const WorkspaceLayout& w = p->reg;
-  const ParamLayout& par = p->par;
-  const int K = p->K, L = p->L;
-  auto B16 = [&](size_t off) { return p->at<__nv_bfloat16>(off); };
-  auto F32 = [&](size_t off) { return p->at<float>(off); };
-
-  { int rcs = ensure_side_stream(p); if (rcs) return rcs; }
-  cudaStream_t side = p->side_stream;
-  cudaStream_t dws = p->dw_stream;
+cudaError_t fork_dw(smd_plan* p, cudaStream_t st) {
   // Weight-gradient GEMMs are leaves of the backward graph: they run on dw_stream next to the dX chain; every gradient
   // operand they read has its own buffer, so nothing they read is rewritten within this backward pass.
-  auto fork_dw = [&]() -> cudaError_t {
-    cudaError_t e1 = cudaEventRecord(p->ev_dw, st);
-    if (e1 != cudaSuccess) return e1;
-    return cudaStreamWaitEvent(dws, p->ev_dw, 0);
-  };
-  // dX GEMM outputs (gradient wrt a bf16 activation), stored as bf16: half the epilogue / LayerNorm-backward bytes
-  __nv_bfloat16* g16 = B16(ts.g16);
-  float* du32 = F32(ts.du32);   // gradient of the fp32 residual stream u
-  float* stats = F32(w.stats);
-  const size_t sstride = static_cast<size_t>(p->Mp) * 2;
-  const int nkb = Mk / 64;
-  float* xt = F32(w.xt);
+  cudaError_t e1 = cudaEventRecord(p->ev_dw, st);
+  if (e1 != cudaSuccess) return e1;
+  return cudaStreamWaitEvent(p->dw_stream, p->ev_dw, 0);
+}
 
+int bwd_begin(smd_plan* p, int M, int batch, float* grads, cudaStream_t st) {
+  TrainState& ts = p->train;
+  const smd_config& c = p->cfg;
+  const int Md = c.mlp_dims, K = p->K, L = p->L;
+  const int Mk = (M + 63) / 64 * 64;           // reduction length of the dW GEMMs
+  const int Bk = (batch + 63) / 64 * 64;
+  auto B16 = [&](size_t off) { return p->at<__nv_bfloat16>(off); };
   // Zeroing the 100 MB gradient arena (~20 us) goes to the weight-gradient stream: the forward pass does not touch it
   // and every writer either runs on that stream or is ordered after ev_gz below.
-  SMD_CUDA(fork_dw());
-  SMD_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * p->arena, dws));
-  SMD_CUDA(cudaEventRecord(p->ev_gz, dws));
+  SMD_CUDA(fork_dw(p, st));
+  SMD_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * p->arena, p->dw_stream));
+  SMD_CUDA(cudaEventRecord(p->ev_gz, p->dw_stream));
   // FiLM (scale|shift) gradients are accumulated with atomics by the two CTAs of a sample and by both uses of a pair
-  SMD_CUDA(cudaMemsetAsync(F32(ts.dss), 0,
-                           sizeof(float) * static_cast<size_t>(K) * c.max_batch * 2 * Md, st));
+  if (!p->mdn())
+    SMD_CUDA(cudaMemsetAsync(p->at<float>(ts.dss), 0, sizeof(float) * static_cast<size_t>(K) * c.max_batch * 2 * Md, st));
   if (Mk != M) {  // zero the reduction-tail rows of every MN-major gradient operand
     const size_t tail = static_cast<size_t>(Mk - M);
     for (size_t off : ts.du16) SMD_CUDA(cudaMemsetAsync(B16(off) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
@@ -201,65 +180,66 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
       SMD_CUDA(cudaMemsetAsync(B16(ts.dr16[l]) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
       SMD_CUDA(cudaMemsetAsync(B16(ts.dqkv16[l]) + static_cast<size_t>(M) * 384, 0, tail * 384 * 2, st));
     }
-    SMD_CUDA(cudaMemsetAsync(B16(ts.dpred16) + static_cast<size_t>(M) * Cp, 0, tail * Cp * 2, st));
+    SMD_CUDA(cudaMemsetAsync(B16(ts.dpred16) + static_cast<size_t>(M) * p->head_ld, 0, tail * p->head_ld * 2, st));
   }
-  if (Bk != batch) {
+  if (Bk != batch && !p->mdn()) {
     SMD_CUDA(cudaMemsetAsync(B16(ts.dss16) + static_cast<size_t>(batch) * 2 * Md, 0,
                              static_cast<size_t>(Bk - batch) * 2 * Md * 2, st));
     SMD_CUDA(cudaMemsetAsync(B16(ts.e2_16) + static_cast<size_t>(batch) * 512, 0,
                              static_cast<size_t>(Bk - batch) * 512 * 2, st));
   }
+  return SMD_OK;
+}
 
-  // ---------------- forward (keeps every activation) ----------------
-  float* cond = F32(w.tvec);
-  float* pred = F32(w.eps_hat);
-  launch_q_sample(x0, eps, used_alpha, xt, cond, batch, per, st, ind, objective); CNT();
-  int rc = run_forward(p, params, xt, cond, 0, batch, pred, st, /*save=*/true, /*raw_out=*/true);
-  if (rc) return rc;
-  SMD_CUDA(cudaStreamWaitEvent(st, p->ev_gz, 0));   // gradient arena zeroed (long done by now)
+int bwd_out_ln(smd_plan* p, const float* params, int M, float* grads, cudaStream_t st) {
+  TrainState& ts = p->train;
+  const ParamLayout& par = p->par;
+  const int K = p->K;
+  GemmEpilogue e = epi();
+  e.out_bf16 = p->at<__nv_bfloat16>(ts.g16); e.ld_bf16 = p->cfg.mlp_dims;
+  SMD_CUDA(launch_gemm(ts.dXout, M, e, st));
+  LnFilmBwdArgs a;
+  memset(&a, 0, sizeof(a));
+  a.g16 = p->at<__nv_bfloat16>(ts.g16); a.u = p->at<float>(p->reg.u[K]);
+  a.stats = p->at<float>(p->reg.stats) + (2 * K) * static_cast<size_t>(p->Mp) * 2;
+  a.gamma = params + par.out_ln.scale; a.beta = params + par.out_ln.bias;
+  a.dx32 = p->at<float>(ts.du32); a.dx16 = p->at<__nv_bfloat16>(ts.du16[K]);
+  a.dgamma = grads + par.out_ln.scale; a.dbeta = grads + par.out_ln.bias;
+  a.dbias = grads + par.block[K - 1].b.bias;
+  a.M = M; a.N = p->cfg.mlp_dims; a.S = p->cfg.seq_len;
+  launch_ln_film_act_bwd(a, st); CNT();
+  return SMD_OK;
+}
 
-  // ---------------- objective ----------------
-  // ddpm: mean over (S, C) and the global batch; dsm: sum over (S, C) (x 0.5), mean over the global batch
-  const float gscale = objective == 1 ? 1.0f / static_cast<float>(global_batch)
-                                      : 1.0f / (static_cast<float>(global_batch) * static_cast<float>(per));
-  float* dpred32 = F32(ts.dpred32);
-  __nv_bfloat16* dpred16 = B16(ts.dpred16);
-  ddpm_loss_bwd_kernel<<<batch, 256, 0, st>>>(eps, pred, F32(ts.loss), loss_sum, p->at<unsigned int>(ts.loss_ctr),
-                                              1.0f / static_cast<float>(global_batch), dpred32, dpred16, gscale, S, C, Cp,
-                                              ind, objective);
-  CNT();
-  SMD_CUDA(fork_dw());
-  launch_colsum<float>(dpred32, C, grads + par.out.bias, M, C, dws); CNT();
-
-  // ---------------- output projection + final LayerNorm ----------------
-  {
-    GemmEpilogue e = epi();
-    e.out_f32 = grads + par.out.kernel; e.ld_f32 = C;
-    const int sp = pick_splits_side(Md, C, ts.dWout.BN, nkb);
-    e.atomic_out = sp > 1;
-    SMD_CUDA(gemm_k(ts.dWout, Md, Mk, sp, e, dws));
-    e = epi();
-    e.out_bf16 = g16; e.ld_bf16 = Md;
-    SMD_CUDA(launch_gemm(ts.dXout, M, e, st));
-    LnFilmBwdArgs a;
-    memset(&a, 0, sizeof(a));
-    a.g16 = g16; a.u = F32(w.u[K]); a.stats = stats + (2 * K) * sstride;
-    a.gamma = params + par.out_ln.scale; a.beta = params + par.out_ln.bias;
-    a.dx32 = du32; a.dx16 = B16(ts.du16[K]);
-    a.dgamma = grads + par.out_ln.scale; a.dbeta = grads + par.out_ln.bias;
-    a.dbias = grads + par.block[K - 1].b.bias;
-    a.M = M; a.N = Md; a.S = S;
-    launch_ln_film_act_bwd(a, st); CNT();
-  }
-
-  // ---------------- FiLM'd residual blocks ----------------
+// capturing: the call is being recorded into a CUDA graph -- the three "tail gradients are final" events that
+// smd_wait_tail_grads hands to the caller's communication stream are then recorded as EXTERNAL event nodes, so a stream
+// outside the graph can wait on them after the graph has been launched.
+int bwd_tail(smd_plan* p, const float* params, int batch, float* grads, cudaStream_t st, bool capturing) {
+  const unsigned ext = capturing ? cudaEventRecordExternal : cudaEventRecordDefault;
+  TrainState& ts = p->train;
+  const smd_config& c = p->cfg;
+  const int S = c.seq_len, Md = c.mlp_dims;
+  const int M = batch * S;
+  const int Mk = (M + 63) / 64 * 64;
+  const WorkspaceLayout& w = p->reg;
+  const ParamLayout& par = p->par;
+  const int K = p->K, L = p->L;
+  const bool film = !p->mdn();
+  auto B16 = [&](size_t off) { return p->at<__nv_bfloat16>(off); };
+  auto F32 = [&](size_t off) { return p->at<float>(off); };
+  cudaStream_t dws = p->dw_stream;
+  __nv_bfloat16* g16 = B16(ts.g16);
+  float* du32 = F32(ts.du32);
+  float* stats = F32(w.stats);
+  const size_t sstride = static_cast<size_t>(p->Mp) * 2;
   float* ssbuf = F32(w.ss);
   float* dss_all = F32(ts.dss);
   for (int k = K - 1; k >= 0; --k) {
     const BlockParams& bp = par.block[k];
-    const float* ss_k = ssbuf + static_cast<size_t>(k) * c.max_batch * 2 * Md;
-    float* dss = dss_all + static_cast<size_t>(k) * c.max_batch * 2 * Md;
-    SMD_CUDA(fork_dw());
+    // (TransformerMDN: the identity FiLM rows smd_bind_workspace wrote into block 0, no FiLM gradient)
+    const float* ss_k = film ? ssbuf + static_cast<size_t>(k) * c.max_batch * 2 * Md : ssbuf;
+    float* dss = film ? dss_all + static_cast<size_t>(k) * c.max_batch * 2 * Md : nullptr;
+    SMD_CUDA(fork_dw(p, st));
     GemmEpilogue e = epi();
     e.out_f32 = grads + bp.b.kernel; e.ld_f32 = Md;
     SMD_CUDA(gemm_k(ts.dWb[k], Md, Mk, 1, e, dws));
@@ -277,7 +257,7 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     a.dss = dss; a.dss_accum = 0;
     a.M = M; a.N = Md; a.S = S;
     launch_ln_film_act_bwd(a, st); CNT();
-    SMD_CUDA(fork_dw());
+    SMD_CUDA(fork_dw(p, st));
     e = epi();
     e.out_f32 = grads + bp.a.kernel; e.ld_f32 = Md;
     SMD_CUDA(gemm_k(ts.dWa[k], Md, Mk, 1, e, dws));
@@ -295,27 +275,36 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     a.M = M; a.N = Md; a.S = S;
     launch_ln_film_act_bwd(a, st); CNT();
 
-    SMD_CUDA(film_generator_bwd(p, params, k, batch, grads, st));
+    if (film) SMD_CUDA(film_generator_bwd(p, params, k, batch, grads, st));
   }
-  // every k*. / out_ln / out gradient is final once these three have fired (smd_wait_tail_grads)
-  SMD_CUDA(cudaEventRecordWithFlags(p->evx_join, side, ext));
-  SMD_CUDA(cudaEventRecord(p->ev_join, side));   // internal join marker (last node of the side stream: `st` waits on it)
+  // every k*. / out_ln / output-layer gradient is final once these three have fired (smd_wait_tail_grads); without a
+  // FiLM generator the side stream has no work of its own and joins here (a captured graph records events only on
+  // streams that take part in the capture)
+  if (!film) {
+    SMD_CUDA(cudaEventRecord(p->ev_fork, st));
+    SMD_CUDA(cudaStreamWaitEvent(p->side_stream, p->ev_fork, 0));
+  }
+  SMD_CUDA(cudaEventRecordWithFlags(p->evx_join, p->side_stream, ext));
+  SMD_CUDA(cudaEventRecord(p->ev_join, p->side_stream));   // internal join marker (last node of the side stream: `st` waits on it)
   SMD_CUDA(cudaEventRecordWithFlags(p->ev_tail, st, ext));
   SMD_CUDA(cudaEventRecordWithFlags(p->ev_dwtail, dws, ext));
   SMD_LAUNCH_CHECK("backward tail");
+  return SMD_OK;
+}
 
-  if (L == 0) {
-    // DenseDDPM: input projection weight gradient (models/ncsn.py:129)
-    GemmEpilogue e = epi();
-    e.out_f32 = grads + par.in.kernel; e.ld_f32 = Md;
-    SMD_CUDA(gemm_k(ts.dWin, C, Mk, 1, e, st));
-    SMD_CUDA(cudaEventRecord(p->ev_dwjoin, dws));
-    SMD_CUDA(cudaStreamWaitEvent(st, p->ev_dwjoin, 0));
-    SMD_CUDA(cudaStreamWaitEvent(st, p->ev_join, 0));
-    SMD_LAUNCH_CHECK("backward dense");
-    return SMD_OK;
-  }
-
+int bwd_trunk(smd_plan* p, const float* params, int batch, float* grads, cudaStream_t st) {
+  TrainState& ts = p->train;
+  const smd_config& c = p->cfg;
+  const int S = c.seq_len, C = c.channels, Md = c.mlp_dims;
+  const int M = batch * S;
+  const int Mk = (M + 63) / 64 * 64;
+  const int nkb = Mk / 64;
+  const WorkspaceLayout& w = p->reg;
+  const ParamLayout& par = p->par;
+  const int L = p->L;
+  auto B16 = [&](size_t off) { return p->at<__nv_bfloat16>(off); };
+  auto F32 = [&](size_t off) { return p->at<float>(off); };
+  cudaStream_t dws = p->dw_stream;
   // ---------------- post dense + post LayerNorm ----------------
   float* da32 = F32(ts.dh2);
   float* dh32 = F32(ts.dh);
@@ -326,7 +315,7 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     e.out_f32 = grads + par.post.kernel; e.ld_f32 = Md;
     const int sp = pick_splits_side(128, Md, ts.dWpost.BN, nkb);
     e.atomic_out = sp > 1;
-    SMD_CUDA(fork_dw());
+    SMD_CUDA(fork_dw(p, st));
     SMD_CUDA(gemm_k(ts.dWpost, 128, Mk, sp, e, dws));
     e = epi();
     e.out_f32 = da32; e.ld_f32 = 128;
@@ -350,7 +339,7 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     e.out_bf16 = dr16l; e.ld_bf16 = Md;
     e.gelu_grad_of = B16(w.hidden_pre[l]); e.ld_gg = Md;
     SMD_CUDA(launch_gemm(ts.dX2[l], M, e, st));
-    SMD_CUDA(fork_dw());
+    SMD_CUDA(fork_dw(p, st));
     e = epi();
     e.out_f32 = grads + lp.ffn2.kernel; e.ld_f32 = 128;
     int sp = pick_splits_side(Md, 128, ts.dW2[l].BN, nkb);
@@ -375,7 +364,7 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     a.M = M;
     launch_ln128_bwd(a, st); CNT();
     // attention: h_mid = attn(a1) Wo + bo + h_in
-    SMD_CUDA(fork_dw());
+    SMD_CUDA(fork_dw(p, st));
     e = epi();
     e.out_f32 = grads + lp.out.kernel; e.ld_f32 = 128;
     sp = pick_splits_side(128, 128, ts.dWo[l].BN, nkb);
@@ -387,7 +376,7 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
     SMD_CUDA(launch_attention_bwd(F32(w.qkv[l]), F32(w.probs[l]), da32, B16(ts.dqkv16[l]), grads + lp.qkv.bias,
                                   batch, S, c.num_heads, st));
     CNT();
-    SMD_CUDA(fork_dw());
+    SMD_CUDA(fork_dw(p, st));
     e = epi();
     e.out_f32 = grads + lp.qkv.kernel; e.ld_f32 = 384;
     sp = pick_splits_side(128, 384, ts.dWqkv[l].BN, nkb);
@@ -406,11 +395,89 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
   }
   SMD_CUDA(cudaEventRecord(p->ev_dwjoin, dws));
   // ---------------- input projection ----------------
-  launch_embed_bwd(xt, dh32, grads + par.in.kernel, M, C, st); CNT();
+  launch_embed_bwd(F32(w.xt), dh32, grads + par.in.kernel, M, C, st); CNT();
   SMD_CUDA(cudaStreamWaitEvent(st, p->ev_dwjoin, 0));
   SMD_CUDA(cudaStreamWaitEvent(st, p->ev_join, 0));
   SMD_LAUNCH_CHECK("backward trunk");
   return SMD_OK;
+}
+
+}  // namespace smd
+
+using namespace smd;
+
+// ind: device table {x0, used_alpha, eps} read by the kernels instead of the pointer arguments (graph replay), or null.
+static int grads_impl(smd_plan* p, const float* params, const float* x0, const float* used_alpha, const float* eps,
+                      const float* const* ind, int batch, int global_batch, float* grads, float* loss_sum,
+                      cudaStream_t st, bool capturing, int objective) {
+  TrainState& ts = p->train;
+  const smd_config& c = p->cfg;
+  const int S = c.seq_len, C = c.channels, Md = c.mlp_dims;
+  const int Cp = (C + 63) / 64 * 64;
+  const int M = batch * S;
+  const int Mk = (M + 63) / 64 * 64;           // reduction length of the dW GEMMs
+  const int per = S * C;
+  const WorkspaceLayout& w = p->reg;
+  const ParamLayout& par = p->par;
+  const int L = p->L;
+  auto B16 = [&](size_t off) { return p->at<__nv_bfloat16>(off); };
+  auto F32 = [&](size_t off) { return p->at<float>(off); };
+
+  { int rcs = ensure_side_stream(p); if (rcs) return rcs; }
+  cudaStream_t dws = p->dw_stream;
+  const int nkb = Mk / 64;
+  float* xt = F32(w.xt);
+  int rc = bwd_begin(p, M, batch, grads, st);
+  if (rc) return rc;
+
+  // ---------------- forward (keeps every activation) ----------------
+  float* cond = F32(w.tvec);
+  float* pred = F32(w.eps_hat);
+  launch_q_sample(x0, eps, used_alpha, xt, cond, batch, per, st, ind, objective); CNT();
+  rc = run_forward(p, params, xt, cond, 0, batch, pred, st, /*save=*/true, /*raw_out=*/true);
+  if (rc) return rc;
+  SMD_CUDA(cudaStreamWaitEvent(st, p->ev_gz, 0));   // gradient arena zeroed (long done by now)
+
+  // ---------------- objective ----------------
+  // ddpm: mean over (S, C) and the global batch; dsm: sum over (S, C) (x 0.5), mean over the global batch
+  const float gscale = objective == 1 ? 1.0f / static_cast<float>(global_batch)
+                                      : 1.0f / (static_cast<float>(global_batch) * static_cast<float>(per));
+  float* dpred32 = F32(ts.dpred32);
+  __nv_bfloat16* dpred16 = B16(ts.dpred16);
+  ddpm_loss_bwd_kernel<<<batch, 256, 0, st>>>(eps, pred, F32(ts.loss), loss_sum, p->at<unsigned int>(ts.loss_ctr),
+                                              1.0f / static_cast<float>(global_batch), dpred32, dpred16, gscale, S, C, Cp,
+                                              ind, objective);
+  CNT();
+  SMD_CUDA(fork_dw(p, st));
+  launch_colsum<float>(dpred32, C, grads + par.out.bias, M, C, dws); CNT();
+
+  // ---------------- output projection + final LayerNorm ----------------
+  {
+    GemmEpilogue e = epi();
+    e.out_f32 = grads + par.out.kernel; e.ld_f32 = C;
+    const int sp = pick_splits_side(Md, C, ts.dWout.BN, nkb);
+    e.atomic_out = sp > 1;
+    SMD_CUDA(gemm_k(ts.dWout, Md, Mk, sp, e, dws));
+  }
+  rc = bwd_out_ln(p, params, M, grads, st);
+  if (rc) return rc;
+
+  // ---------------- FiLM'd residual blocks ----------------
+  rc = bwd_tail(p, params, batch, grads, st, capturing);
+  if (rc) return rc;
+
+  if (L == 0) {
+    // DenseDDPM: input projection weight gradient (models/ncsn.py:129)
+    GemmEpilogue e = epi();
+    e.out_f32 = grads + par.in.kernel; e.ld_f32 = Md;
+    SMD_CUDA(gemm_k(ts.dWin, C, Mk, 1, e, st));
+    SMD_CUDA(cudaEventRecord(p->ev_dwjoin, dws));
+    SMD_CUDA(cudaStreamWaitEvent(st, p->ev_dwjoin, 0));
+    SMD_CUDA(cudaStreamWaitEvent(st, p->ev_join, 0));
+    SMD_LAUNCH_CHECK("backward dense");
+    return SMD_OK;
+  }
+  return bwd_trunk(p, params, batch, grads, st);
 }
 
 // Sliced score matching (utils/losses.py:182-247) on DenseNCSN: loss_b = 0.5 |f|^2 + sigma v.(J_f v) with f the raw
@@ -584,7 +651,8 @@ static void drop_train_graph(smd_plan* p) {
   p->tg_valid = false;
 }
 
-// objective 0: ddpm, 1: denoising score matching, 2: sliced score matching (v: its projection vectors; else null)
+// objective 0: ddpm, 1: denoising score matching, 2: sliced score matching (v: its projection vectors; else null),
+// 3: the mixture-density NLL of TransformerMDN (x0: the sequences; used_alpha / eps null)
 static int grads_entry(smd_plan* p, const float* params, const float* x0, const float* used_alpha,
                        const float* eps, const float* v, int batch, int global_batch, float* grads, float* loss_sum,
                        smd_stream_t stream, int objective) {
@@ -597,12 +665,13 @@ static int grads_entry(smd_plan* p, const float* params, const float* x0, const 
                   bool capturing) {
     if (objective == 2)
       return ssm_grads_impl(p, params, x0_, ua_, eps_, v_, ind_, batch, global_batch, grads, loss_sum, st, capturing);
+    if (objective == 3) return mdn_grads_impl(p, params, x0_, ind_, batch, global_batch, grads, loss_sum, st, capturing);
     return grads_impl(p, params, x0_, ua_, eps_, ind_, batch, global_batch, grads, loss_sum, st, capturing, objective);
   };
   if (!train_graph_enabled() || !capturable) return impl(x0, used_alpha, eps, v, nullptr, false);
   // Graph replay: the pass's ~150 launches on three streams (dX chain, weight-gradient GEMMs, FiLM generator) are
   // captured once into one CUDA graph with the same fork / join structure.  The per-step inputs (x0, used_alpha, eps)
-  // reach the kernels through a 3-pointer device table, so new input tensors do not force a re-capture; the events a
+  // reach the kernels through a device pointer table, so new input tensors do not force a re-capture; the events a
   // data-parallel caller waits on (smd_wait_tail_grads) are external event-record nodes of the graph.
   const bool same = p->tg_valid && p->tg_params == params && p->tg_grads == grads && p->tg_loss == loss_sum &&
                     p->tg_batch == batch && p->tg_global == global_batch && p->tg_objective == objective;
@@ -643,7 +712,15 @@ static int grads_entry(smd_plan* p, const float* params, const float* x0, const 
 extern "C" int smd_ddpm_grads(smd_plan* p, const float* params, const float* x0, const float* used_alpha,
                               const float* eps, int batch, int global_batch, float* grads, float* loss_sum,
                               smd_stream_t stream) {
+  if (p->mdn()) { set_error("smd_ddpm_grads does not apply to a TransformerMDN plan (use smd_mdn_grads)"); return SMD_ERR_INVALID; }
   return grads_entry(p, params, x0, used_alpha, eps, nullptr, batch, global_batch, grads, loss_sum, stream, 0);
+}
+
+// TransformerMDN (train_mdn.py:180-205): gradient of the mean token NLL; x is the only per-step input
+extern "C" int smd_mdn_grads(smd_plan* p, const float* params, const float* x, int batch, int global_batch,
+                             float* grads, float* loss_sum, smd_stream_t stream) {
+  if (!p || !p->mdn()) { set_error("smd_mdn_grads needs a TransformerMDN plan (smd_mdn_plan_create)"); return SMD_ERR_INVALID; }
+  return grads_entry(p, params, x, nullptr, nullptr, nullptr, batch, global_batch, grads, loss_sum, stream, 3);
 }
 
 // denoising score matching (utils/losses.py:129-179): the same pass with x~ = x0 + sigma eps, the network conditioned on

@@ -26,12 +26,14 @@ inline PFN_cuTensorMapEncodeTiled_v12000 get_encode_fn() {
   return fn;
 }
 
-// bf16 row-major matrix [rows][cols]; box = box_rows x 64 columns (128 bytes, SWIZZLE_128B).
-inline bool make_tmap_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+// bf16 row-major matrix [rows][cols]; box = box_rows x 64 columns (128 bytes, SWIZZLE_128B).  pitch: row pitch in
+// elements when the matrix is a column slice of a wider one (0: cols)
+inline bool make_tmap_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows,
+                           uint64_t pitch = 0) {
   auto fn = get_encode_fn();
   if (!fn) { set_error("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)"); return false; }
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {cols * 2};
+  cuuint64_t strides[1] = {(pitch ? pitch : cols) * 2};
   cuuint32_t box[2] = {64, box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
@@ -59,13 +61,14 @@ inline int choose_bn(int N) {
 
 // A: K-major [a_rows][K] (a_mn=0) or MN-major [K][a_rows] (a_mn=1); same for B with N rows.
 // A requested BN above kBNMax is lowered to kBNMax (the widest accumulator tile).
+// b_pitch: row pitch (elements) of an MN-major B that is a column slice of a wider matrix (0: b_rows_total)
 inline bool make_gemm_op(GemmOp* op, const void* A, uint64_t a_rows, const void* B, uint64_t b_rows_total, int N,
                          int K, int BN, int a_mn, int b_mn, uint64_t k_rows_a = 0, uint64_t k_rows_b = 0,
-                         size_t lo_bytes = 0) {
+                         size_t lo_bytes = 0, uint64_t b_pitch = 0) {
   if (lo_bytes) {
     GemmOp lo;
     if (!make_gemm_op(&lo, static_cast<const uint8_t*>(A) + lo_bytes, a_rows, static_cast<const uint8_t*>(B) + lo_bytes,
-                      b_rows_total, N, K, BN, a_mn, b_mn, k_rows_a, k_rows_b, 0)) return false;
+                      b_rows_total, N, K, BN, a_mn, b_mn, k_rows_a, k_rows_b, 0, b_pitch)) return false;
     op->tmA_lo = lo.tmA; op->tmB_lo = lo.tmB; op->has_lo = true;
   }
   if (BN > kBNMax) BN = kBNMax;
@@ -78,7 +81,7 @@ inline bool make_gemm_op(GemmOp* op, const void* A, uint64_t a_rows, const void*
   else ok = make_tmap_bf16(&op->tmA, A, k_rows_a ? k_rows_a : static_cast<uint64_t>(K), a_rows, 64);
   if (!ok) return false;
   if (!b_mn) ok = make_tmap_bf16(&op->tmB, B, b_rows_total, static_cast<uint64_t>(K), static_cast<uint32_t>(BN));
-  else ok = make_tmap_bf16(&op->tmB, B, k_rows_b ? k_rows_b : static_cast<uint64_t>(K), b_rows_total, 64);
+  else ok = make_tmap_bf16(&op->tmB, B, k_rows_b ? k_rows_b : static_cast<uint64_t>(K), b_rows_total, 64, b_pitch);
   return ok;
 }
 

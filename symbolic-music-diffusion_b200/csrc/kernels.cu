@@ -177,11 +177,13 @@ void launch_embed(const float* x, const float* W_in, const float* b_in, const fl
 
 // ---------------------------------------------------------------------------------------------------
 // attention: one CTA per (sample, head group, 32-query block), one warp per head, lane = query position
-// (S in {32, 64, 128}: the CTA stages all S rows of k and v and its 32 rows of q)
+// (S in {32, 64, 128}: the CTA stages all S rows of k and v and its 32 rows of q).
+// CAUSAL: query i attends to keys j <= i only; the masked probabilities are exactly 0 (flax's -1e10 bias underflows
+// to 0 in the softmax), so the stored-probability backward needs no change
 // ---------------------------------------------------------------------------------------------------
-template <int DH, int S>
-__global__ void attention_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ o,
-                                 float* __restrict__ probs, int B, int H, long long lo_delta) {
+template <int DH, int S, bool CAUSAL>
+__device__ __forceinline__ void attention_simt(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ o,
+                                               float* __restrict__ probs, int B, int H, long long lo_delta) {
   pdl_trigger();
   pdl_wait();
   // a CTA owns HPB = blockDim.x / 32 heads of one sample (W = HPB * DH columns of k and v): small CTAs, several
@@ -224,6 +226,7 @@ __global__ void attention_kernel(const float* __restrict__ qkv, __nv_bfloat16* _
       s = fmaf(q[4 * d4], k4.x, s); s = fmaf(q[4 * d4 + 1], k4.y, s);
       s = fmaf(q[4 * d4 + 2], k4.z, s); s = fmaf(q[4 * d4 + 3], k4.w, s);
     }
+    if (CAUSAL && j > q0 + lane) s = -INFINITY;
     sc[j] = s;
     mx = fmaxf(mx, s);
   }
@@ -258,6 +261,16 @@ __global__ void attention_kernel(const float* __restrict__ qkv, __nv_bfloat16* _
     for (int j = 0; j < S; j += 4) *reinterpret_cast<float4*>(pr + j) = make_float4(sc[j], sc[j + 1], sc[j + 2], sc[j + 3]);
   }
 }
+template <int DH, int S>
+__global__ void attention_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ o,
+                                 float* __restrict__ probs, int B, int H, long long lo_delta) {
+  attention_simt<DH, S, false>(qkv, o, probs, B, H, lo_delta);
+}
+template <int DH>
+__global__ void causal_attention_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ o,
+                                        float* __restrict__ probs, int B, int H, long long lo_delta) {
+  attention_simt<DH, 32, true>(qkv, o, probs, B, H, lo_delta);
+}
 // ---------------------------------------------------------------------------------------------------
 // Tensor-core variant (DH % 8 == 0): same CTA / warp mapping, but Q K^T and P V run on mma.sync m16n8k8 tf32
 // (a 32xSx16 problem per head is far below a wgmma tile; ~350 instructions per warp instead of ~2000 at S = 32):
@@ -268,9 +281,9 @@ __global__ void attention_kernel(const float* __restrict__ qkv, __nv_bfloat16* _
 // and k-slot t+4 holds key 2t+1, and the V fragment is read with the same permutation (a sum over keys does not
 // care about their order), so no shuffles are needed between the two products.
 // ---------------------------------------------------------------------------------------------------
-template <int DH, int S>
-__global__ void __launch_bounds__(128)
-attention_mma_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ o, float* __restrict__ probs, int B, int H) {
+template <int DH, int S, bool CAUSAL>
+__device__ __forceinline__ void attention_mma(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ o,
+                                              float* __restrict__ probs, int B, int H) {
   pdl_trigger();
   pdl_wait();
   extern __shared__ __align__(16) uint32_t att_sm[];
@@ -323,6 +336,15 @@ attention_mma_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ 
       mma_tf32_16x8x8(sc[0][nt], a[0], b0, b1);
       mma_tf32_16x8x8(sc[1][nt], a[1], b0, b1);
     }
+  }
+  if (CAUSAL) {   // key 8 nt + 2 t (+1) against query q0 + 16 mt + g (+8): the diagonal key keeps every row finite
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          if (8 * nt + 2 * t + (i & 1) > q0 + 16 * mt + g + 8 * (i >> 1)) sc[mt][nt][i] = -INFINITY;
   }
   // ---- row softmax: a row lives in the 4 lanes of a quad (t = 0..3), S / 4 values per lane
 #pragma unroll
@@ -393,8 +415,28 @@ attention_mma_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ 
       *reinterpret_cast<__nv_bfloat162*>(ob + (16 * mt + g + 8) * 128 + 8 * n2 + 2 * t) = __floats2bfloat162_rn(acc[mt][n2][2], acc[mt][n2][3]);
     }
 }
+template <int DH, int S>
+__global__ void __launch_bounds__(128)
+attention_mma_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ o, float* __restrict__ probs, int B, int H) {
+  attention_mma<DH, S, false>(qkv, o, probs, B, H);
+}
+template <int DH>
+__global__ void __launch_bounds__(128)
+causal_attention_mma_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ o, float* __restrict__ probs,
+                            int B, int H) {
+  attention_mma<DH, 32, true>(qkv, o, probs, B, H);
+}
+// the kernel a launch runs: the causal variants exist for S = 32 only
+template <int DH, int S, bool CAUSAL>
+constexpr auto attention_simt_fn() {
+  if constexpr (CAUSAL) return &causal_attention_kernel<DH>; else return &attention_kernel<DH, S>;
+}
+template <int DH, int S, bool CAUSAL>
+constexpr auto attention_mma_fn() {
+  if constexpr (CAUSAL) return &causal_attention_mma_kernel<DH>; else return &attention_mma_kernel<DH, S>;
+}
 
-template <int S>
+template <int S, bool CAUSAL>
 static void launch_attention_s(const float* qkv, __nv_bfloat16* o, float* probs_or_null, int B, int H, cudaStream_t st,
                                long long lo_delta) {
   const int dh = 128 / H;
@@ -408,11 +450,11 @@ static void launch_attention_s(const float* qkv, __nv_bfloat16* o, float* probs_
   {                                                                                                               \
     static bool attr = false;                                                                                     \
     if (!attr) {                                                                                                  \
-      cudaFuncSetAttribute(attention_mma_kernel<DHV, S>, cudaFuncAttributeMaxDynamicSharedMemorySize,             \
+      cudaFuncSetAttribute(attention_mma_fn<DHV, S, CAUSAL>(), cudaFuncAttributeMaxDynamicSharedMemorySize,       \
                            (32 + 2 * S) * 132 * 4);                                                               \
       attr = true;                                                                                                \
     }                                                                                                             \
-    attention_mma_kernel<DHV, S><<<grid, threads, smem, st>>>(qkv, o, probs_or_null, B, H);                       \
+    attention_mma_fn<DHV, S, CAUSAL>()<<<grid, threads, smem, st>>>(qkv, o, probs_or_null, B, H);                 \
   }
     if (dh == 16) SMD_ATT_MMA(16)
     else if (dh == 8) SMD_ATT_MMA(8)
@@ -426,10 +468,11 @@ static void launch_attention_s(const float* qkv, __nv_bfloat16* o, float* probs_
   {                                                                                                               \
     static bool attr = false;                                                                                     \
     if (S != 32 && !attr) {                                                                                       \
-      cudaFuncSetAttribute(attention_kernel<DHV, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * S * 128 * 4); \
+      cudaFuncSetAttribute(attention_simt_fn<DHV, S, CAUSAL>(), cudaFuncAttributeMaxDynamicSharedMemorySize,      \
+                           2 * S * 128 * 4);                                                                      \
       attr = true;                                                                                                \
     }                                                                                                             \
-    attention_kernel<DHV, S><<<grid, threads, smem, st>>>(qkv, o, probs_or_null, B, H, lo_delta);                 \
+    attention_simt_fn<DHV, S, CAUSAL>()<<<grid, threads, smem, st>>>(qkv, o, probs_or_null, B, H, lo_delta);      \
   }
   if (dh == 16) SMD_ATT_SIMT(16)
   else if (dh == 8) SMD_ATT_SIMT(8)
@@ -438,11 +481,16 @@ static void launch_attention_s(const float* qkv, __nv_bfloat16* o, float* probs_
 #undef SMD_ATT_SIMT
 }
 
-void launch_attention(const float* qkv, __nv_bfloat16* o, float* probs_or_null, int B, int S, int H, cudaStream_t st,
-                      long long lo_delta) {
-  if (S == 32) launch_attention_s<32>(qkv, o, probs_or_null, B, H, st, lo_delta);
-  else if (S == 64) launch_attention_s<64>(qkv, o, probs_or_null, B, H, st, lo_delta);
-  else if (S == 128) launch_attention_s<128>(qkv, o, probs_or_null, B, H, st, lo_delta);
+cudaError_t launch_attention(const float* qkv, __nv_bfloat16* o, float* probs_or_null, int B, int S, int H,
+                             cudaStream_t st, long long lo_delta, bool causal) {
+  if (causal) {
+    if (S != 32) return cudaErrorInvalidValue;
+    launch_attention_s<32, true>(qkv, o, probs_or_null, B, H, st, lo_delta);
+  } else if (S == 32) launch_attention_s<32, false>(qkv, o, probs_or_null, B, H, st, lo_delta);
+  else if (S == 64) launch_attention_s<64, false>(qkv, o, probs_or_null, B, H, st, lo_delta);
+  else if (S == 128) launch_attention_s<128, false>(qkv, o, probs_or_null, B, H, st, lo_delta);
+  else return cudaErrorInvalidValue;
+  return cudaSuccess;
 }
 
 // ---------------------------------------------------------------------------------------------------

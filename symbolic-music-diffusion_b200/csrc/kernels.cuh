@@ -150,10 +150,12 @@ void launch_embed(const float* x, const float* W_in, const float* b_in, const fl
                   const float* ln_b, float* h, __nv_bfloat16* a, int M, int C, int S, cudaStream_t st,
                   long long lo_delta = 0);
 
-// unmasked multi-head self-attention over S in {32, 64, 128} positions (flax.nn.SelfAttention core, models/ncsn.py:161)
-// qkv fp32 [M][3E] -> o bf16 [M][E];  optionally saves the probabilities P [B][H][S][S] fp32 for backward
-void launch_attention(const float* qkv, __nv_bfloat16* o, float* probs_or_null, int B, int S, int H, cudaStream_t st,
-                      long long lo_delta = 0);
+// multi-head self-attention over S in {32, 64, 128} positions (flax.nn.SelfAttention core, models/ncsn.py:161)
+// qkv fp32 [M][3E] -> o bf16 [M][E];  optionally saves the probabilities P [B][H][S][S] fp32 for backward.
+// causal (S = 32 only; models/autoregressive.py:61, causal_mask=True): query i sees keys j <= i, masked P exactly 0.
+// Returns cudaErrorInvalidValue (and launches nothing) for a length / mask combination without a kernel.
+cudaError_t launch_attention(const float* qkv, __nv_bfloat16* o, float* probs_or_null, int B, int S, int H,
+                             cudaStream_t st, long long lo_delta = 0, bool causal = false);
 
 // out[m,:] = bf16( act( film( LN(u[m,:]; stats, g, b) ) ) )                        (models/shared.py:62-64,66-68)
 // stats[m] = (sum, sumsq) over the N columns; scale/shift rows selected by m / S (or row 0 if film_bcast)

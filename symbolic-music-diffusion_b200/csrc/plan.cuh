@@ -47,13 +47,15 @@ static constexpr int kE = 128;       // embed_channels (models/ncsn.py:151)
 static constexpr int kFilmEmb = 128; // DenseFiLM embedding_channels (models/ncsn.py:174)
 static constexpr int kFilmHid = 512; // embedding_channels * 4
 static constexpr int kMaxT = 8192;
+// TransformerMDN: C + 2 Kc floats of dynamic shared memory per mixture-NLL row (48 KB less the kernel's static part)
+static constexpr int kMdnMaxRowFloats = (48 * 1024 - 256) / 4;
 
 // Parameter arena offsets (in floats).  The same offset indexes the fp32 parameters, the gradients and the bf16 shadow.
 struct Dense { long long kernel = 0, bias = 0; };
 struct Norm { long long scale = 0, bias = 0; };
 struct LayerParams { Norm ln1; Dense qkv, out; Norm ln2; Dense ffn1, ffn2; };
 struct FilmParams { Dense d1, d2, ss; };
-struct BlockParams { FilmParams film; Norm ln_a; Dense a; Norm ln_b; Dense b; };
+struct BlockParams { FilmParams film; Norm ln_a; Dense a; Norm ln_b; Dense b; };   // TransformerMDN: no film
 struct ParamLayout {
   Dense in;
   std::vector<LayerParams> layer;   // TransformerDDPM only
@@ -61,7 +63,8 @@ struct ParamLayout {
   Dense post;                       // TransformerDDPM only
   std::vector<BlockParams> block;   // FiLM'd residual blocks
   Norm out_ln;
-  Dense out;
+  Dense out;                        // all but TransformerMDN
+  Dense mdn_mu, mdn_log_sigma, mdn_pi;   // TransformerMDN: the mixture-density head (models/shared.py MDN)
 };
 
 // Workspace byte offsets of everything the forward pass, the objectives and the sampler use.
@@ -80,6 +83,9 @@ struct WorkspaceLayout {
   // families: xbt (bf16 input tangent v), ut[0..K] (fp32), r1t per block (fp32), actt[0..2K] (bf16), yt (output tangent)
   size_t xbt = 0, yt = 0;
   std::vector<size_t> ut, r1t, actt;
+  // TransformerMDN only: fp32 head output [Mp][Np] = [mu | log_sigma | pi] (each part padded to 64 columns) and the
+  // matching padded fp32 bias [Np]; out_pad then holds the packed bf16 head weight [Md][Np]
+  size_t head = 0, head_bias = 0;
 };
 
 // Named workspace region, for smd_debug_buffer.
@@ -99,17 +105,18 @@ struct TrainState {
   std::vector<size_t> dh16b;           // bf16 [Mp][128] x L: gradient at the attention output (from LN2)
   std::vector<size_t> dr16;            // bf16 [Mp][Md]  x L: gradient at the FFN pre-activation
   std::vector<size_t> dqkv16;          // bf16 [Mp][384] x L
-  size_t dpred16 = 0;                  // bf16 [Mp][Cp64]
+  size_t dpred16 = 0;                  // bf16 [Mp][Cp64] (TransformerMDN: dZ, the head-output gradient [Mp][Np])
   size_t dpred32 = 0;                  // fp32 [Mp][C]
   size_t dss = 0;                      // fp32 [K][B][2Md]
   size_t de = 0, de2 = 0;              // fp32 [B][512] x2
-  size_t loss = 0;                     // fp32 [B]
+  size_t loss = 0;                     // fp32 [B] (TransformerMDN: [B][S], one loss per token)
   size_t loss_ctr = 0;                 // u32: block-completion counter of the loss kernel (zeroed at bind, self-resetting)
   size_t ind = 0;                      // device table {x0, used_alpha, eps} of the graph-replayed step
   size_t e2_16 = 0, dss16 = 0;         // bf16 [Bp][512], [Bp][2Md]
   std::vector<GemmOp> dWb, dXb, dWa, dXa, dWss, dXss;
   std::vector<GemmOp> dW2, dX2, dW1, dX1, dWo, dXo, dWqkv, dXqkv;
   GemmOp dWout, dXout, dWpost, dXpost, dWin;
+  GemmOp dWmdn[3];                     // TransformerMDN: dW of the mu / log_sigma / pi column slices of dZ
   // DenseNCSN only -- adjoints of the tangent pass (sliced score matching): gt16 / dut32 mirror g16 / du32, dut16 /
   // drt16 / dpredt16 mirror du16 / dr16t / dpred16, and the t* GEMMs are the tangent halves of the dW / dX GEMMs
   size_t gt16 = 0, dut32 = 0, dpredt16 = 0;
@@ -133,7 +140,13 @@ struct smd_plan {
   size_t lo_bytes = 0;
   long long lo_elems = 0;
   int L = 0;   // transformer layers (0 for the dense networks)
-  int K = 0;   // number of FiLM res-blocks (num_mlp_layers, or num_layers for DenseDDPM)
+  int K = 0;   // number of (FiLM) res-blocks (num_mlp_layers, or num_layers for DenseDDPM)
+  // output layer width: C (columns of out.kernel, padded to Cp for the bf16 copy), or for TransformerMDN the packed
+  // head, Kc mixture components: [mu | log_sigma | pi] with parts of Kc C, Kc C and Kc columns, each padded to 64
+  int Kc = 0;
+  int KCp = 0, Kcp = 0;          // padded widths of the mu / log_sigma parts and of the pi part (TransformerMDN)
+  int head_n = 0, head_ld = 0;   // valid columns of the output GEMM and the row pitch of its bf16 weight copy
+  bool mdn() const { return cfg.arch == SMD_ARCH_TRANSFORMER_MDN; }
   // ---- workspace ----
   WorkspaceLayout reg;
   std::vector<WsRegion> regions;
@@ -207,4 +220,25 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
                 float* y, cudaStream_t st, bool save, bool raw_out = false, bool tangent = false);
 int train_bind(smd_plan* p);
 int ensure_side_stream(smd_plan* p);
+
+// Pieces of the backward pass shared by the objectives (backward.cu).  bwd_begin zeroes the gradient arena (on the
+// weight-gradient stream) and the reduction-tail rows of every MN-major gradient operand; bwd_out_ln runs the output
+// layer's dX GEMM (operand dpred16) and the out_ln backward; bwd_tail the (FiLM) res-blocks, then records the events
+// of smd_wait_tail_grads; bwd_trunk the post / transformer layers / input projection (input reg.xt) and the joins.
+int bwd_begin(smd_plan* p, int M, int batch, float* grads, cudaStream_t st);
+int bwd_out_ln(smd_plan* p, const float* params, int M, float* grads, cudaStream_t st);
+int bwd_tail(smd_plan* p, const float* params, int batch, float* grads, cudaStream_t st, bool capturing);
+int bwd_trunk(smd_plan* p, const float* params, int batch, float* grads, cudaStream_t st);
+cudaError_t fork_dw(smd_plan* p, cudaStream_t st);
+// out[n] += sum_m in[m * ld + n] (bias gradients from a bf16 gradient operand)
+void launch_colsum_bf16(const __nv_bfloat16* in, int ld, float* out, int M, int N, cudaStream_t st);
+int pick_splits_side(int m_rows, int n_cols, int BN, int num_kb);
+// op with its reduction length set to K and split `splits` ways (the dW GEMMs reduce over the batch's token rows)
+cudaError_t gemm_k(const GemmOp& op0, int rows, int K, int splits, const GemmEpilogue& e, cudaStream_t st);
+
+// TransformerMDN (mdn.cu): packed head refresh, backward GEMM descriptors, and the train step body
+int mdn_pack_head(smd_plan* p, const float* params, cudaStream_t st);
+int mdn_train_bind(smd_plan* p);
+int mdn_grads_impl(smd_plan* p, const float* params, const float* x, const float* const* ind, int batch,
+                   int global_batch, float* grads, float* loss_sum, cudaStream_t st, bool capturing);
 }  // namespace smd

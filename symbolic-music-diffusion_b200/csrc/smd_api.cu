@@ -47,7 +47,8 @@ static void build_layout(smd_plan* p) {
   const smd_config& c = p->cfg;
   const int C = c.channels, Md = c.mlp_dims;
   ParamLayout& par = p->par;
-  if (c.arch == SMD_ARCH_TRANSFORMER_DDPM) {
+  const bool film = !p->mdn();   // TransformerMDN's res-blocks are DenseResBlock(x, mlp_dims) with scale 1, shift 0
+  if (c.arch == SMD_ARCH_TRANSFORMER_DDPM || p->mdn()) {
     par.in = add_dense(p, "in.", C, kE);
     p->L = c.num_layers;
     par.layer.resize(p->L);
@@ -72,16 +73,24 @@ static void build_layout(smd_plan* p) {
   for (int k = 0; k < p->K; ++k) {
     const std::string pre = "k" + std::to_string(k) + ".";
     BlockParams& bp = par.block[k];
-    bp.film.d1 = add_dense(p, pre + "film.d1.", kFilmEmb, kFilmHid);
-    bp.film.d2 = add_dense(p, pre + "film.d2.", kFilmHid, kFilmHid);
-    bp.film.ss = add_dense(p, pre + "film.ss.", kFilmHid, 2 * Md);
+    if (film) {
+      bp.film.d1 = add_dense(p, pre + "film.d1.", kFilmEmb, kFilmHid);
+      bp.film.d2 = add_dense(p, pre + "film.d2.", kFilmHid, kFilmHid);
+      bp.film.ss = add_dense(p, pre + "film.ss.", kFilmHid, 2 * Md);
+    }
     bp.ln_a = add_norm(p, pre + "res.ln_a.", Md);
     bp.a = add_dense(p, pre + "res.a.", Md, Md);
     bp.ln_b = add_norm(p, pre + "res.ln_b.", Md);
     bp.b = add_dense(p, pre + "res.b.", Md, Md);
   }
   par.out_ln = add_norm(p, "out_ln.", Md);
-  par.out = add_dense(p, "out.", Md, C);
+  if (p->mdn()) {   // models/shared.py MDN: three Dense layers, flax order mu, log_sigma, pi
+    par.mdn_mu = add_dense(p, "mdn.mu.", Md, p->Kc * C);
+    par.mdn_log_sigma = add_dense(p, "mdn.log_sigma.", Md, p->Kc * C);
+    par.mdn_pi = add_dense(p, "mdn.pi.", Md, p->Kc);
+  } else {
+    par.out = add_dense(p, "out.", Md, C);
+  }
 }
 
 // Reserves a 1024-byte aligned workspace region and returns its byte offset.
@@ -105,8 +114,9 @@ static void build_workspace(smd_plan* p) {
   // are no transposed copies and the optimizer refreshes it in the same pass that updates the fp32 masters.
   w.wshadow = ws_add(p, "wshadow", static_cast<size_t>(p->arena) * 2);
   // out.kernel is (Md, C) with C = 42 / 146: its 2C-byte row pitch is not TMA-addressable, so it gets a copy
-  // zero-padded to a multiple of 64 columns
-  w.out_pad = ws_add(p, "w.out_pad", Md * Cp * 2);
+  // zero-padded to a multiple of 64 columns (TransformerMDN: the three head kernels packed into [Md][Np])
+  const size_t Hp = p->head_ld;
+  w.out_pad = ws_add(p, "w.out_pad", Md * Hp * 2);
   // forward activations, n indices per family: a training plan keeps every index for the backward pass, an inference
   // plan overwrites one region in place
   auto family = [&](int n, size_t bytes, auto name) {
@@ -177,12 +187,12 @@ static void build_workspace(smd_plan* p) {
     t.dh16b = family(L, Mp * kE * 2, idx("t.dh16b"));
     t.dr16 = family(L, Mp * Md * 2, idx("t.dr16_"));
     t.dqkv16 = family(L, Mp * 3 * kE * 2, idx("t.dqkv16_"));
-    t.dpred16 = ws_add(p, "t.dpred16", Mp * Cp * 2);
+    t.dpred16 = ws_add(p, "t.dpred16", Mp * Hp * 2);
     t.dpred32 = ws_add(p, "t.dpred32", Mp * C * 4);
     t.dss = ws_add(p, "t.dss", K * B * 2 * Md * 4);   // one [B][2Md] block per FiLM pair
     t.de = ws_add(p, "t.de", B * kFilmHid * 4);
     t.de2 = ws_add(p, "t.de2", B * kFilmHid * 4);
-    t.loss = ws_add(p, "t.loss", B * 4);
+    t.loss = ws_add(p, "t.loss", B * (p->mdn() ? c.seq_len : 1) * 4);
     t.loss_ctr = ws_add(p, "t.loss_ctr", 64);
     t.ind = ws_add(p, "t.ind", 64);
     const size_t Bp = (B + 127) / 128 * 128;
@@ -204,6 +214,10 @@ static void build_workspace(smd_plan* p) {
       t.drt16 = family(K, Mp * Md * 2, idx("t.drt16_"));
       t.dpredt16 = ws_add(p, "t.dpredt16", Mp * Cp * 2);
     }
+  }
+  if (p->mdn()) {
+    w.head = ws_add(p, "mdn.head", Mp * Hp * 4);
+    w.head_bias = ws_add(p, "mdn.head_bias", Hp * 4);
   }
   if (strict) {
     w.x3_scratch = ws_add(p, "x3.scratch", Mp * Md * 4);   // fp32 cross-term accumulator of the three-pass GEMMs
@@ -256,9 +270,9 @@ static int build_ops(smd_plan* p) {
     if (!fwd(&p->op_a[k], w.act[2 * k], p->par.block[k].a.kernel, Md, Md)) return SMD_ERR_CUDA;
     if (!fwd(&p->op_b[k], w.act[2 * k + 1], p->par.block[k].b.kernel, Md, Md)) return SMD_ERR_CUDA;
   }
-  // output projection from the padded copy [Md][Cp]: N = C columns are valid
-  if (!make_gemm_op(&p->op_out, p->ws + w.act[2 * p->K], Mp, p->ws + w.out_pad, static_cast<uint64_t>(Cp), C, Md,
-                    std::min(Cp, kBNMax), 0, 1, 0, 0, p->lo_bytes))
+  // output projection from the padded copy [Md][Cp]: N = C columns are valid (TransformerMDN: all Np of [Md][Np])
+  if (!make_gemm_op(&p->op_out, p->ws + w.act[2 * p->K], Mp, p->ws + w.out_pad, static_cast<uint64_t>(p->head_ld),
+                    p->head_n, Md, std::min(p->head_ld, kBNMax), 0, 1, 0, 0, p->lo_bytes))
     return SMD_ERR_CUDA;
   if (c.arch == SMD_ARCH_DENSE_NCSN) {
     if (!fwd(&p->op_tin, w.xbt, p->par.in.kernel, C, Md)) return SMD_ERR_CUDA;
@@ -364,13 +378,13 @@ static int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadc
   const bool strict = p->lo_bytes != 0;
   for (int k = 0; k < p->K; ++k) {
     const BlockParams& bp = p->par.block[k];
-    const float* scale = ss + static_cast<size_t>(k) * p->cfg.max_batch * 2 * Md;
+    const float* scale = p->mdn() ? nullptr : ss + static_cast<size_t>(k) * p->cfg.max_batch * 2 * Md;
     const int* frow_dev = nullptr;
     if (p->film_tab_on) {
       scale = p->at<float>(w.ftab) + static_cast<size_t>(k) * p->T * 2 * Md;
       if (p->film_row_dev) frow_dev = p->film_row_dev; else scale += static_cast<size_t>(p->film_row) * 2 * Md;
     }
-    const float* shift = scale + Md;
+    const float* shift = scale ? scale + Md : nullptr;
     float* u_in = p->at<float>(w.u[k]);
     float* u_out = p->at<float>(w.u[k + 1]);
     __nv_bfloat16* act_a = p->at<__nv_bfloat16>(w.act[2 * k]);
@@ -425,8 +439,8 @@ static int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadc
                      nullptr, nullptr, 0, 0, 0, p->at<__nv_bfloat16>(w.act[2 * p->K]), M, Md, S, st, nullptr, nullptr,
                      p->lo_elems, lo_.part, lo_.nslots, lo_.totals); CNT();
   GemmEpilogue e = epi();
-  e.bias = params + p->par.out.bias;
-  e.out_f32 = y; e.ld_f32 = C;
+  e.bias = p->mdn() ? p->at<float>(w.head_bias) : params + p->par.out.bias;
+  e.out_f32 = y; e.ld_f32 = p->mdn() ? p->head_ld : C;
   SMD_CUDA(gemm(p, p->op_out, M, e, st));
   if (tangent) {
     launch_ln_film_tangent(p->at<float>(w.u[p->K]), nullptr, lo_.totals, p->at<float>(w.ut[p->K]),
@@ -454,7 +468,7 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
   SMD_CUDA(cudaMemsetAsync(stats, 0, static_cast<size_t>(2 * p->K + 1) * p->Mp * 2 * 4, st));
   int rc = SMD_OK;
   bool film_on_side = false;
-  if (!p->film_tab_on) {
+  if (!p->film_tab_on && !p->mdn()) {
     if (save) {
       // training: the FiLM generator only feeds the tail, so it runs on a side stream next to the trunk
       rc = ensure_side_stream(p);
@@ -484,8 +498,9 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
       float* h_in = h(2 * l); float* h_mid = h(2 * l + 1); float* h_out = h(2 * l + 2);
       __nv_bfloat16* a2 = a(2 * l + 1); __nv_bfloat16* a_next = a(2 * l + 2);
       GemmEpilogue e = epi();
-      // the fused block's 64-row tile holds whole samples up to S = 64; S = 128 takes the unfused path
-      if (!save && S <= 64 && p->op_attn[l].ok && p->lo_bytes == 0) {
+      // the fused block's 64-row tile holds whole samples up to S = 64; S = 128 and causal attention take the
+      // unfused path
+      if (!save && S <= 64 && p->op_attn[l].ok && p->lo_bytes == 0 && !p->mdn()) {
         // QKV GEMM -> attention -> out-projection + residual + LayerNorm in ONE launch; q / k / v stay on chip
         AttnBlockArgs aa;
         aa.b_qkv = params + lp.qkv.bias; aa.b_o = params + lp.out.bias;
@@ -499,8 +514,8 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
       e.bias = params + lp.qkv.bias;
       e.out_f32 = qkv; e.ld_f32 = 3 * kE;
       SMD_CUDA(gemm(p, p->op_qkv[l], M, e, st));
-      launch_attention(qkv, p->at<__nv_bfloat16>(w.o[l]), save ? p->at<float>(w.probs[l]) : nullptr, batch, S,
-                       c.num_heads, st, p->lo_elems); CNT();
+      SMD_CUDA(launch_attention(qkv, p->at<__nv_bfloat16>(w.o[l]), save ? p->at<float>(w.probs[l]) : nullptr, batch,
+                                S, c.num_heads, st, p->lo_elems, /*causal=*/p->mdn())); CNT();
       e = epi();
       e.bias = params + lp.out.bias;
       e.residual = h_in; e.ld_res = kE;
@@ -652,20 +667,34 @@ __global__ void threefry_rademacher_kernel(uint32_t k0, uint32_t k1, float* out,
 extern "C" {
 
 const char* smd_last_error(void) { return get_error(); }
+
+// the score-network entry points have no meaning for the autoregressive baseline's plans
+static bool reject_mdn(const smd_plan* plan, const char* fn) {
+  if (!plan || !plan->mdn()) return false;
+  set_error(std::string(fn) + " does not apply to a TransformerMDN plan (use the smd_mdn_* entry points)");
+  return true;
+}
 int smd_version(void) { return 100; }
 long long smd_launch_count(void) { return g_launches.load(); }
 
-int smd_plan_create(const smd_config* cfg, smd_plan** out) {
+static int plan_create(const smd_config* cfg, int num_components, smd_plan** out) {
   if (!cfg || !out) { set_error("null argument"); return SMD_ERR_INVALID; }
   smd_config c = *cfg;
-  if (c.arch != SMD_ARCH_TRANSFORMER_DDPM && c.arch != SMD_ARCH_DENSE_DDPM && c.arch != SMD_ARCH_DENSE_NCSN) { set_error("unknown arch"); return SMD_ERR_INVALID; }
+  const bool mdn = c.arch == SMD_ARCH_TRANSFORMER_MDN;
+  if (c.arch != SMD_ARCH_TRANSFORMER_DDPM && c.arch != SMD_ARCH_DENSE_DDPM && c.arch != SMD_ARCH_DENSE_NCSN && !mdn) { set_error("unknown arch"); return SMD_ERR_INVALID; }
   if (c.cta_group == 0) c.cta_group = 1;
   if (c.cta_group != 1 && c.cta_group != 2) { set_error("cta_group must be 1 or 2"); return SMD_ERR_INVALID; }
   if (c.mlp_dims < 256 || c.mlp_dims % 256 != 0 || c.mlp_dims > 4096) { set_error("mlp_dims must be a multiple of 256 in [256, 4096]"); return SMD_ERR_INVALID; }
   if (c.channels < 1 || c.max_batch < 1 || c.num_layers < 1) { set_error("bad sizes"); return SMD_ERR_INVALID; }
   if (c.precision != SMD_PRECISION_BF16 && c.precision != SMD_PRECISION_BF16X3) { set_error("unknown precision"); return SMD_ERR_INVALID; }
   if (c.precision == SMD_PRECISION_BF16X3 && c.training) { set_error("precision bf16x3 covers the forward pass / sampler only (training = 0)"); return SMD_ERR_INVALID; }
-  if (c.arch == SMD_ARCH_TRANSFORMER_DDPM) {
+  if (mdn) {
+    if (c.seq_len != 32) { set_error("TransformerMDN CUDA path supports seq_len 32 only"); return SMD_ERR_INVALID; }
+    if (c.precision != SMD_PRECISION_BF16) { set_error("TransformerMDN supports precision bf16 only"); return SMD_ERR_INVALID; }
+    if (num_components < 1) { set_error("num_components must be >= 1"); return SMD_ERR_INVALID; }
+    if (c.channels + 2LL * num_components > kMdnMaxRowFloats) { set_error("channels + 2 num_components must be <= " + std::to_string(kMdnMaxRowFloats)); return SMD_ERR_INVALID; }
+  }
+  if (c.arch == SMD_ARCH_TRANSFORMER_DDPM || mdn) {
     // each length divides the 128-row GEMM / LayerNorm tile and is a multiple of the 32-row blocks inside one sample
     if (c.seq_len != 32 && c.seq_len != 64 && c.seq_len != 128) { set_error("TransformerDDPM CUDA path supports seq_len in {32, 64, 128}"); return SMD_ERR_INVALID; }
     if (c.num_heads != 4 && c.num_heads != 8 && c.num_heads != 16 && c.num_heads != 32) { set_error("num_heads must be 4, 8, 16 or 32"); return SMD_ERR_INVALID; }
@@ -676,10 +705,31 @@ int smd_plan_create(const smd_config* cfg, smd_plan** out) {
   smd_plan* p = new smd_plan();
   p->cfg = c;
   p->Mp = (c.max_batch * c.seq_len + 255) / 256 * 256;
+  p->head_n = c.channels;
+  p->head_ld = (c.channels + 63) / 64 * 64;
+  if (mdn) {
+    p->Kc = num_components;
+    p->KCp = (num_components * c.channels + 63) / 64 * 64;
+    p->Kcp = (num_components + 63) / 64 * 64;
+    p->head_n = p->head_ld = 2 * p->KCp + p->Kcp;
+  }
   build_layout(p);
   build_workspace(p);
   *out = p;
   return SMD_OK;
+}
+
+int smd_plan_create(const smd_config* cfg, smd_plan** out) {
+  if (cfg && cfg->arch == SMD_ARCH_TRANSFORMER_MDN) {
+    set_error("SMD_ARCH_TRANSFORMER_MDN plans are created with smd_mdn_plan_create (it takes the component count)");
+    return SMD_ERR_INVALID;
+  }
+  return plan_create(cfg, 0, out);
+}
+
+int smd_mdn_plan_create(const smd_config* cfg, int num_components, smd_plan** out) {
+  if (cfg && cfg->arch != SMD_ARCH_TRANSFORMER_MDN) { set_error("smd_mdn_plan_create needs arch SMD_ARCH_TRANSFORMER_MDN"); return SMD_ERR_INVALID; }
+  return plan_create(cfg, num_components, out);
 }
 
 void smd_plan_destroy(smd_plan* plan) {
@@ -740,6 +790,14 @@ int smd_bind_workspace(smd_plan* plan, void* workspace, size_t bytes) {
       pe[s * kE + 64 + j] = cosf(arg);
     }
   SMD_CUDA(cudaMemcpy(plan->at<float>(plan->reg.posenc), pe.data(), pe.size() * 4, cudaMemcpyHostToDevice));
+  if (plan->mdn() && plan->cfg.training) {
+    // TransformerMDN's res-blocks are DenseResBlock with scale 1, shift 0: its backward passes these identity FiLM rows
+    // ([max_batch][scale 1 | shift 0]) so the LayerNorm-swish backward takes its sequence fast path
+    const size_t Md = plan->cfg.mlp_dims;
+    std::vector<float> ident(plan->cfg.max_batch * 2 * Md, 0.0f);
+    for (int b = 0; b < plan->cfg.max_batch; ++b) std::fill_n(ident.begin() + b * 2 * Md, Md, 1.0f);
+    SMD_CUDA(cudaMemcpy(plan->at<float>(plan->reg.ss), ident.data(), ident.size() * 4, cudaMemcpyHostToDevice));
+  }
   if (plan->cfg.training) { rc = train_bind(plan); if (rc) return rc; }
   return SMD_OK;
 }
@@ -751,8 +809,13 @@ static int refresh_operands(smd_plan* plan, const float* params, bool shadow_is_
   }
   // out.kernel is the one GEMM weight not read from the shadow: its zero-padded copy (pad columns stay zero from bind)
   const int C = plan->cfg.channels;
-  launch_pad_cast_bf16(params + plan->par.out.kernel, plan->at<__nv_bfloat16>(plan->reg.out_pad), plan->cfg.mlp_dims, C,
-                       (C + 63) / 64 * 64, st, plan->lo_elems); CNT();
+  if (plan->mdn()) {
+    const int rc = mdn_pack_head(plan, params, st);
+    if (rc) return rc;
+  } else {
+    launch_pad_cast_bf16(params + plan->par.out.kernel, plan->at<__nv_bfloat16>(plan->reg.out_pad), plan->cfg.mlp_dims,
+                         C, plan->head_ld, st, plan->lo_elems); CNT();
+  }
   SMD_LAUNCH_CHECK("pack_weights");
   plan->packed = true;
   plan->film_tab_ready = false;   // parameters changed
@@ -772,7 +835,8 @@ void* smd_shadow_arena(smd_plan* plan) { return plan->ws ? plan->wsh(0) : nullpt
 int smd_grads_tail_range(const smd_plan* plan, long long* first_float, long long* num_floats) {
   if (!plan || !first_float || !num_floats) { set_error("null argument"); return SMD_ERR_INVALID; }
   if (plan->par.block.empty()) { set_error("plan has no FiLM'd residual tail"); return SMD_ERR_STATE; }
-  *first_float = plan->par.block[0].film.d1.kernel;   // first tensor of the FiLM'd tail; out_ln / out follow it
+  // first tensor of the residual tail; out_ln and the output layer (out, or mdn.*) follow it
+  *first_float = plan->mdn() ? plan->par.block[0].ln_a.scale : plan->par.block[0].film.d1.kernel;
   *num_floats = static_cast<long long>(plan->arena) - *first_float;
   return SMD_OK;
 }
@@ -789,12 +853,14 @@ int smd_wait_tail_grads(smd_plan* plan, smd_stream_t stream) {
 
 int smd_forward(smd_plan* plan, const float* params, const float* x, const float* t, int t_broadcast, int batch,
                 float* y, smd_stream_t stream) {
+  if (reject_mdn(plan, "smd_forward")) return SMD_ERR_INVALID;
   return run_forward(plan, params, x, t, t_broadcast, batch, y, static_cast<cudaStream_t>(stream), false);
 }
 
 int smd_ddpm_loss(smd_plan* plan, const float* params, const float* x0, const float* used_alpha, const float* eps,
                   int batch, float* loss_per_example, float* pred_or_null, smd_stream_t stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (reject_mdn(plan, "smd_ddpm_loss")) return SMD_ERR_INVALID;
   if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
   if (batch < 1 || batch > plan->cfg.max_batch) { set_error("batch out of range"); return SMD_ERR_INVALID; }
   const int per = plan->cfg.seq_len * plan->cfg.channels;
@@ -982,6 +1048,7 @@ int smd_ddpm_draws(smd_plan* plan, const uint32_t host_key[2], int batch, float*
 
 int smd_sampler_setup(smd_plan* plan, const float* host_betas, int T, const uint32_t host_key[2],
                       smd_stream_t stream) {
+  if (reject_mdn(plan, "smd_sampler_setup")) return SMD_ERR_INVALID;
   if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
   if (T < 1 || T > kMaxT) { set_error("T out of range"); return SMD_ERR_INVALID; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1133,6 +1200,7 @@ int smd_sampler_set_shard(smd_plan* plan, long long first_row, long long total_r
 int smd_ddpm_reverse_step(smd_plan* plan, const float* params, const float* x, int n, int t, const float* z,
                           const float* infill_x, const float* infill_mask, const float* infill_z, float* x_next,
                           float* eps_hat_or_null, float* collection, float* metrics, smd_stream_t stream) {
+  if (reject_mdn(plan, "smd_ddpm_reverse_step")) return SMD_ERR_INVALID;
   if (!plan->sampler_ready) { set_error("smd_sampler_setup has not been called"); return SMD_ERR_STATE; }
   if (t < 0 || t >= plan->T) { set_error("t out of range"); return SMD_ERR_INVALID; }
   if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
@@ -1145,6 +1213,7 @@ int smd_ddpm_reverse_step(smd_plan* plan, const float* params, const float* x, i
 int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int steps, const float* infill_x,
                     const float* infill_mask, float* collection, float* metrics, int use_graph,
                     smd_stream_t stream) {
+  if (reject_mdn(plan, "smd_ddpm_sample")) return SMD_ERR_INVALID;
   if (!plan->sampler_ready) { set_error("smd_sampler_setup has not been called"); return SMD_ERR_STATE; }
   if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
   if (steps < 1 || steps > plan->T) { set_error("steps out of range"); return SMD_ERR_INVALID; }
@@ -1253,6 +1322,7 @@ int smd_threefry_split(const uint32_t host_key[2], int num, uint32_t* host_out_k
 
 int smd_debug_forward_save(smd_plan* plan, const float* params, const float* x, const float* t, int batch, float* y,
                            smd_stream_t stream) {
+  if (reject_mdn(plan, "smd_debug_forward_save")) return SMD_ERR_INVALID;
   if (!plan->cfg.training) { set_error("plan was not created with training = 1"); return SMD_ERR_STATE; }
   return run_forward(plan, params, x, t, 0, batch, y, static_cast<cudaStream_t>(stream), true);
 }

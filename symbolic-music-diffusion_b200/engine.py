@@ -15,7 +15,8 @@ import torch
 
 from . import lib as _lib
 
-ARCHS = {"TransformerDDPM": 0, "TransformerDDPM4": 0, "DenseDDPM": 1, "DenseNCSN": 2}
+ARCHS = {"TransformerDDPM": 0, "TransformerDDPM4": 0, "DenseDDPM": 1, "DenseNCSN": 2, "TransformerMDN": 3}
+SEQUENCE_ARCHS = (0, 3)   # (B, S, C) inputs; the dense networks take (B, C)
 PRECISIONS = {"bf16": 0, "bf16x3": 1}
 
 
@@ -29,6 +30,7 @@ class ModelConfig:
     mlp_dims: int = 2048
     seq_len: int = 32
     channels: int = 42
+    mdn_components: int = 100   # TransformerMDN only (train_mdn.py --mdn_components)
 
     def flops_fwd_per_sample(self) -> float:
         """Algorithmic forward FLOPs per sample (SURVEY section 8(d))."""
@@ -66,15 +68,20 @@ class Engine:
         if precision not in PRECISIONS:
             raise ValueError(f"unknown precision {precision!r} (expected one of {sorted(PRECISIONS)})")
         self.precision = precision
+        self.mdn = ARCHS[cfg.arch] == 3
+        if sampler_T is None:
+            sampler_T = 0 if training or self.mdn else 1000
         c = _lib.SmdConfig(ARCHS[cfg.arch], cfg.num_layers, cfg.num_heads, cfg.num_mlp_layers, cfg.mlp_dims,
-                           cfg.seq_len if ARCHS[cfg.arch] == 0 else 1, cfg.channels, self.max_batch,
-                           int(cta_group), int(training),
-                           int((0 if training else 1000) if sampler_T is None else sampler_T), PRECISIONS[precision])
+                           cfg.seq_len if ARCHS[cfg.arch] in SEQUENCE_ARCHS else 1, cfg.channels, self.max_batch,
+                           int(cta_group), int(training), int(sampler_T), PRECISIONS[precision])
         h = C.c_void_p()
-        _lib.check(self.lib.smd_plan_create(C.byref(c), C.byref(h)))
+        if self.mdn:
+            _lib.check(self.lib.smd_mdn_plan_create(C.byref(c), int(cfg.mdn_components), C.byref(h)))
+        else:
+            _lib.check(self.lib.smd_plan_create(C.byref(c), C.byref(h)))
         self._plan = h
         self._comm_stream = None
-        self.seq_len = cfg.seq_len if ARCHS[cfg.arch] == 0 else 1
+        self.seq_len = cfg.seq_len if ARCHS[cfg.arch] in SEQUENCE_ARCHS else 1
         self.training = bool(training)
         self.layout: List[Tuple[str, int, Tuple[int, ...]]] = []
         name = C.create_string_buffer(128)
@@ -317,6 +324,41 @@ class Engine:
                                               float(infill_sigma), mk(infill_key), _ptr(infill_z), x_next.data_ptr(),
                                               _ptr(collection_slot), _ptr(metrics4), self._stream()))
         return x_next
+
+    # ------------------------------------------------------------------ TransformerMDN (train_mdn.py)
+    def _mdn_input(self, x: torch.Tensor) -> torch.Tensor:
+        x = _f32c(x, "x")
+        if x.dim() != 3 or tuple(x.shape[1:]) != (self.seq_len, self.cfg.channels):
+            raise ValueError(f"x must have shape (batch, {self.seq_len}, {self.cfg.channels}), got {tuple(x.shape)}")
+        return x
+
+    def mdn_forward(self, x: torch.Tensor, shift: bool = True):
+        """(pi (B,S,Kc), mu (B,S,Kc*C), log_sigma (B,S,Kc*C)) = model(x, shift) (models/autoregressive.py:40-82)."""
+        x = self._mdn_input(x)
+        B, S, Cc = x.shape
+        kc = self.cfg.mdn_components
+        pi = torch.empty((B, S, kc), dtype=torch.float32, device=x.device)
+        mu = torch.empty((B, S, kc * Cc), dtype=torch.float32, device=x.device)
+        ls = torch.empty_like(mu)
+        _lib.check(self.lib.smd_mdn_forward(self._plan, self.params.data_ptr(), x.data_ptr(), B, 1 if shift else 0,
+                                            pi.data_ptr(), mu.data_ptr(), ls.data_ptr(), self._stream()))
+        return pi, mu, ls
+
+    def mdn_loss(self, x: torch.Tensor) -> torch.Tensor:
+        """Per-token negative log-likelihood (B*S,) of eval_step (train_mdn.py:154-168)."""
+        x = self._mdn_input(x)
+        loss = torch.empty((x.shape[0] * x.shape[1],), dtype=torch.float32, device=x.device)
+        _lib.check(self.lib.smd_mdn_loss(self._plan, self.params.data_ptr(), x.data_ptr(), x.shape[0], loss.data_ptr(),
+                                         self._stream()))
+        return loss
+
+    def compute_mdn_grads(self, x: torch.Tensor, global_batch: Optional[int] = None) -> None:
+        """grads <- d(mean token NLL over the GLOBAL batch)/d params for this shard; loss_sum / loss_mean as
+        compute_grads (loss_mean: the token mean)."""
+        x = self._mdn_input(x)
+        _lib.check(self.lib.smd_mdn_grads(self._plan, self.params.data_ptr(), x.data_ptr(), x.shape[0],
+                                          int(global_batch or x.shape[0]), self.grads.data_ptr(),
+                                          self._grads_buf[self.arena_floats:].data_ptr(), self._stream()))
 
     # ------------------------------------------------------------------ optimizer step (train_ncsn.py:260-288)
     def init_train_state(self, ema: bool = False) -> None:

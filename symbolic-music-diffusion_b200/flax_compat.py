@@ -1,4 +1,8 @@
-"""flax-0.3.0 checkpoint wire format for `(optimizer, ema, early_stop)` (SURVEY section 8, row f1).
+"""flax-0.3.0 checkpoint wire format for `(optimizer, ema, early_stop)` (SURVEY section 8, row f1), and for the
+`(optimizer, early_stop)` 2-tuple of train_mdn.py:305-307 ({'0': optimizer, '1': early_stop}).  TransformerMDN's
+parameter tree (models/autoregressive.py:49-82): the TransformerDDPM trunk indices, DenseResBlock_{4+5L+k},
+LayerNorm_{4+5L+K} and the explicitly named `mdn` module with Dense_0 / Dense_1 / Dense_2 = mu / log_sigma / pi
+(models/shared.py MDN) -- restated like the rest of this module, not verified against flax.
 
 What the reference writes (train_ncsn.py:395-399 -> flax.training.checkpoints.save_checkpoint ->
 flax.serialization.to_bytes): msgpack of `to_state_dict(target)` where
@@ -83,6 +87,7 @@ def _tree_paths(cfg) -> Dict[str, Tuple[Tuple[str, ...], str]]:
         out["out"] = ((f"Dense_{2 + 2 * n}",), "dense")
         return out
     L, K = cfg.num_layers, cfg.num_mlp_layers
+    mdn = cfg.arch == "TransformerMDN"
     out["in"] = (("Dense_1",), "dense")                                  # index 0 is TransformerPositionalEncoding
     for l in range(L):
         b = 2 + 5 * l
@@ -98,6 +103,18 @@ def _tree_paths(cfg) -> Dict[str, Tuple[Tuple[str, ...], str]]:
     b = 2 + 5 * L
     out["post_ln"] = ((f"LayerNorm_{b}",), "ln")
     out["post"] = ((f"Dense_{b + 1}",), "dense")
+    if mdn:   # DenseResBlock(x, mlp_dims) without a FiLM generator: one submodule per block
+        for k in range(K):
+            res = f"DenseResBlock_{b + 2 + k}"
+            out[f"k{k}.res.ln_a"] = ((res, "LayerNorm_0"), "ln")
+            out[f"k{k}.res.a"] = ((res, "Dense_2"), "dense")
+            out[f"k{k}.res.ln_b"] = ((res, "LayerNorm_3"), "ln")
+            out[f"k{k}.res.b"] = ((res, "Dense_5"), "dense")
+        out["out_ln"] = ((f"LayerNorm_{b + 2 + K}",), "ln")
+        out["mdn.mu"] = (("mdn", "Dense_0"), "dense")
+        out["mdn.log_sigma"] = (("mdn", "Dense_1"), "dense")
+        out["mdn.pi"] = (("mdn", "Dense_2"), "dense")
+        return out
     for k in range(K):
         film_res(f"k{k}", f"DenseFiLM_{b + 2 + 2 * k}", f"DenseResBlock_{b + 3 + 2 * k}")
     out["out_ln"] = ((f"LayerNorm_{b + 2 + 2 * K}",), "ln")
@@ -195,8 +212,9 @@ def _named_to_flat(named: Dict[str, np.ndarray], layout, size: int) -> np.ndarra
 
 
 def to_flax_state(target) -> dict:
-    """State dict of (optimizer, ema, early_stop) in flax's layout (numpy leaves)."""
-    optimizer, ema, early_stop = target
+    """State dict of (optimizer, ema, early_stop) -- or (optimizer, early_stop) -- in flax's layout (numpy leaves)."""
+    from .checkpoints import split_target
+    optimizer, ema, early_stop = split_target(target)
     arena = optimizer.target.arena
     cfg = arena.spec.model_config(arena.input_shape)
     layout = arena.layout
@@ -216,6 +234,8 @@ def to_flax_state(target) -> dict:
     if ema is not None:
         e = {"mu": float(ema.mu), "params": params_to_flax(_flat_to_named(npf(ema.params.flat), layout), cfg)}
     es = early_stop.state_dict()
+    if len(target) == 2:
+        return {"0": opt, "1": es}
     return {"0": opt, "1": e, "2": es}
 
 
@@ -229,8 +249,9 @@ def is_flax_state(st) -> bool:
 def load_flax_state(st: dict, target):
     """Fill the template objects from a flax-layout state dict (inverse of to_flax_state)."""
     import torch
+    from .checkpoints import join_target, split_target
     from .train_utils import EarlyStopping
-    optimizer, ema, early_stop = target
+    optimizer, ema, early_stop = split_target(target)
     arena = optimizer.target.arena
     cfg = arena.spec.model_config(arena.input_shape)
     layout, size = arena.layout, arena.flat.numel()
@@ -252,7 +273,8 @@ def load_flax_state(st: dict, target):
         ema.params.bump()
         ema.mu = float(np.asarray(st["1"]["mu"]))
     es = early_stop
-    if st.get("2"):
-        d = {k: (v.item() if isinstance(v, np.generic) else v) for k, v in st["2"].items()}
+    es_key = "1" if len(target) == 2 else "2"
+    if st.get(es_key):
+        d = {k: (v.item() if isinstance(v, np.generic) else v) for k, v in st[es_key].items()}
         es = EarlyStopping(**d)
-    return optimizer, ema, es
+    return join_target(target, optimizer, ema, es)

@@ -405,12 +405,15 @@ class DevicePrefetcher:
                 d.record_stream(torch.cuda.current_stream())
                 yield d
         finally:
+            # closing the iterator early (a step limit mid-epoch) must not leave the worker inside a CUDA call when the
+            # interpreter exits: unblock it from a full queue and wait for it
             stop.set()
-            while not q.empty():
+            while th.is_alive():
                 try:
                     q.get_nowait()
                 except queue.Empty:
-                    break
+                    pass
+                th.join(timeout=0.01)
 
 
 def get_dataset(dataset="", data_shape=(2,), problem="vae", batch_size=128, normalize=True, pca_ckpt="",

@@ -68,6 +68,11 @@ _SIGNATURES = {
     "smd_debug_forward_save": (C.c_int, [_P, _P, _P, _P, C.c_int, _P, _P]),
     "smd_debug_buffer": (C.c_int, [_P, C.c_char_p, C.POINTER(_P), C.POINTER(C.c_size_t)]),
     "smd_launch_count": (C.c_longlong, []),
+    "smd_mdn_plan_create": (C.c_int, [C.POINTER(SmdConfig), C.c_int, C.POINTER(_P)]),
+    "smd_mdn_forward": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P]),
+    "smd_mdn_nll": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "smd_mdn_loss": (C.c_int, [_P, _P, _P, C.c_int, _P, _P]),
+    "smd_mdn_grads": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

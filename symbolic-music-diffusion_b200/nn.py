@@ -44,10 +44,13 @@ class ModuleSpec:
             return ModelConfig(arch=self.arch, num_layers=int(kw.get("num_layers", 3)),
                                mlp_dims=int(kw.get("mlp_dims", 2048)), seq_len=1, channels=int(input_shape[-1]))
         if len(input_shape) != 2:
-            raise ValueError("TransformerDDPM expects inputs of shape (batch, seq_len, channels)")
+            raise ValueError(f"{self.arch} expects inputs of shape (batch, seq_len, channels)")
+        extra = {}
+        if self.arch == "TransformerMDN":   # models/autoregressive.py:40-47 keyword mdn_mixtures
+            extra["mdn_components"] = int(kw.get("mdn_mixtures", 100))
         return ModelConfig(arch=self.arch, num_layers=int(kw.get("num_layers", 6)), num_heads=int(kw.get("num_heads", 8)),
                            num_mlp_layers=int(kw.get("num_mlp_layers", 2)), mlp_dims=int(kw.get("mlp_dims", 2048)),
-                           seq_len=int(input_shape[0]), channels=int(input_shape[1]))
+                           seq_len=int(input_shape[0]), channels=int(input_shape[1]), **extra)
 
     def engine(self, input_shape, max_batch: int, training: bool) -> Engine:
         """Smallest cached engine of this spec that fits (shape, training, batch); created on demand."""
@@ -140,8 +143,14 @@ class Model:
             eng._packed_tag = tag
         return eng
 
-    def __call__(self, inputs, t):
+    def __call__(self, inputs, t=None, shift=True):
+        """Score networks: eps_hat = model(inputs, t).  TransformerMDN: (pi, mu, log_sigma) = model(inputs, shift)
+        (models/autoregressive.py:40), the second positional argument being `shift`."""
         x = _as_device_f32(inputs)
+        if self.module.arch == "TransformerMDN":
+            return self.engine(x.shape[0]).mdn_forward(x, shift=bool(shift if t is None else t))
+        if t is None:
+            raise TypeError("model(inputs, t): the score networks need the noise level t")
         tt = _as_device_f32(t).reshape(-1)
         if tt.numel() != x.shape[0]:
             raise ValueError("t must have one entry per example (rank equal to inputs' rank in the reference)")
