@@ -62,7 +62,8 @@ typedef struct smd_config {
   int cta_group;       /* 1 or 2 (accepted for compatibility; sm_90a GEMMs use one CTA per tile) */
   int training;        /* 1: reserve the saved-activation / gradient buffers of smd_ddpm_grads */
   int sampler_T;       /* > 0: reserve a (K, sampler_T, 2*mlp_dims) FiLM table so the sampler evaluates the FiLM
-                          generator once per schedule instead of once per step (all samples share t) */
+                          generator once per schedule instead of once per step (all samples share t).
+                          TransformerMDN: > 0 reserves the decode state of smd_mdn_sample instead (no FiLM table) */
   int precision;       /* smd_precision.  SMD_PRECISION_BF16X3 (forward / sampling only, ~3x the GEMM time): every
                           tensor-core operand is split into bf16 hi + lo halves and the GEMMs add the cross terms
                           (hi*hi + hi*lo + lo*hi, fp32 accumulate), activations use exact tanhf / expf and attention runs
@@ -214,7 +215,8 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
  * seq_len != 32, precision bf16x3 or num_components < 1.  Parameters: the TransformerDDPM trunk, k{i}.res.* without
  * film, out_ln, then mdn.mu / mdn.log_sigma (Md, Kc*C) and mdn.pi (Md, Kc); column k*C + c of mu / log_sigma is
  * component k, channel c.  smd_forward, the DDPM / NCSN objectives and the sampler return SMD_ERR_INVALID on such a
- * plan. */
+ * plan.  cfg->sampler_T > 0 reserves the decode state of smd_mdn_sample instead of a FiLM table: per layer a
+ * (max_batch, S, 384) fp32 key/value cache ("mdn.kv{l}") and one (max_batch, C) input token ("mdn.tok"). */
 int smd_mdn_plan_create(const smd_config* cfg, int num_components, smd_plan** out);
 /* (pi, mu, log_sigma) = model(x, shift)   (models/autoregressive.py:40-82).  x: (batch, S, C) fp32; pi (batch, S, Kc),
  * mu and log_sigma (batch, S, Kc*C) fp32.  shift = 0 feeds x to the trunk as it is (autoregressive decoding). */
@@ -232,6 +234,31 @@ int smd_mdn_loss(smd_plan* plan, const float* params, const float* x, int batch,
  * smd_grads_tail_range / smd_wait_tail_grads (the k*, out_ln and mdn.* slice) included. */
 int smd_mdn_grads(smd_plan* plan, const float* params, const float* x, int batch, int global_batch, float* grads,
                   float* loss_sum, smd_stream_t stream);
+/* MixtureSameFamily(Categorical(logits=pi), MultivariateNormalDiag(mu, exp(log_sigma))).sample(seed=host_key), no plan
+ * needed: rows [first_row, first_row + rows) of a draw over total_rows rows (0: rows) into out (rows, C), and the
+ * chosen component of each row into components_or_null (rows,) int32.  pi (rows, Kc), mu / log_sigma (rows, Kc*C).
+ * Keys and counters: comp_key, mix_key = split(fold_in(host_key, 0x916f26ab)) (tfp's split_seed with salt
+ * 'MixtureSameFamily'); k* = argmax_k(pi + g), g element r*Kc + k of gumbel(mix_key, (total_rows, Kc)); value
+ * mu + exp(log_sigma) z at k*, z element (r*Kc + k*)*C + c of normal(comp_key, (total_rows, Kc, C)).  This recipe is
+ * an assumption about tfp-nightly 0.12 on jax 0.2.8, which cannot be run to confirm it.  SMD_ERR_INVALID when
+ * total_rows * Kc * C exceeds 2^32 - 1. */
+int smd_mdn_mixture_sample(const float* pi, const float* mu, const float* log_sigma, int rows, int C, int Kc,
+                           const uint32_t host_key[2], long long first_row, long long total_rows, float* out,
+                           int* components_or_null, smd_stream_t stream);
+/* sample(num_samples = n) of sample_mdn.py:54-119 with host_key = the rng left after `rng, model_rng = split(rng)`:
+ * tokens start at zero; step i = 0..S-1 splits rng, embed_rng = split(rng), draws next_tokens from model(tokens,
+ * shift=False) with the smd_mdn_mixture_sample recipe over all N*S rows, and sets tokens[:, i+1] = next_tokens[:, i]
+ * (i < S-1) or tokens = next_tokens (i = S-1, a fresh draw at every position, as the reference does).  Steps 0..S-2
+ * run the network at position i only, on one row per sample, with the keys and values of earlier positions cached in
+ * the plan; the last step is one full forward over the chain.  out (n, S, C) receives the result; chain_or_null (n, S,
+ * C) the tokens before the last step (position 0 zero); components_or_null (n, S) int32 the last step's components.
+ * first_row / total_rows (0: n) place these n samples in a batch of total_rows samples sharded over ranks (every
+ * draw uses global rows, so gathered shards equal one call over the whole batch).  The plan must have been created
+ * with sampler_T > 0 (else SMD_ERR_STATE); SMD_ERR_INVALID for another arch, n > max_batch, first_row + n >
+ * total_rows or total_rows * S * Kc * C > 2^32 - 1. */
+int smd_mdn_sample(smd_plan* plan, const float* params, const uint32_t host_key[2], int n, long long first_row,
+                   long long total_rows, float* out, float* chain_or_null, int* components_or_null,
+                   smd_stream_t stream);
 
 /* ---- jax.random (threefry2x32) on device ------------------------------------------------------------------ */
 int smd_threefry_normal(const uint32_t host_key[2], float* out, long long n, smd_stream_t stream);

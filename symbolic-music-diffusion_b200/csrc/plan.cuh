@@ -86,6 +86,10 @@ struct WorkspaceLayout {
   // TransformerMDN only: fp32 head output [Mp][Np] = [mu | log_sigma | pi] (each part padded to 64 columns) and the
   // matching padded fp32 bias [Np]; out_pad then holds the packed bf16 head weight [Md][Np]
   size_t head = 0, head_bias = 0;
+  // TransformerMDN plans created with sampler_T > 0 (autoregressive decoding, smd_mdn_sample): per layer the fp32 q / k /
+  // v rows of every decoded position, [max_batch][S][384] like qkv, and the fp32 input token of the step [max_batch][C]
+  std::vector<size_t> kv;
+  size_t tok = 0;
 };
 
 // Named workspace region, for smd_debug_buffer.
@@ -220,6 +224,13 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
                 float* y, cudaStream_t st, bool save, bool raw_out = false, bool tangent = false);
 int train_bind(smd_plan* p);
 int ensure_side_stream(smd_plan* p);
+// Every forward GEMM goes through here (bf16x3 passes, and the per-tile row statistics of wide LayerNorm `ln_slot`).
+cudaError_t gemm(smd_plan* p, const GemmOp& op, int M, GemmEpilogue e, cudaStream_t st, int ln_slot = -1);
+// The residual tail from u[0] (row statistics in stats[0]) through out_ln and the output GEMM into y, M rows.
+int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, float* y, cudaStream_t st, bool tangent);
+// host threefry block function and jax.random.split (out: num x 2 words)
+void h_threefry(uint32_t k0, uint32_t k1, uint32_t& x0, uint32_t& x1);
+void h_split(const uint32_t key[2], int num, uint32_t* out);
 
 // Pieces of the backward pass shared by the objectives (backward.cu).  bwd_begin zeroes the gradient arena (on the
 // weight-gradient stream) and the reduction-tail rows of every MN-major gradient operand; bwd_out_ln runs the output

@@ -167,7 +167,7 @@ static void build_workspace(smd_plan* p) {
   w.t_ptr = ws_add(p, "t_ptr", 64);
   w.abar = ws_add(p, "abar", (kMaxT + 1) * 4);
   w.sigmas = ws_add(p, "sigmas", kMaxT * 4);
-  if (c.sampler_T > 0) {
+  if (c.sampler_T > 0 && !p->mdn()) {
     const size_t T = c.sampler_T;
     w.ftab_t = ws_add(p, "ftab.t", T * 4);
     w.ftab_enc = ws_add(p, "ftab.enc", T * kFilmEmb * 4);
@@ -218,6 +218,10 @@ static void build_workspace(smd_plan* p) {
   if (p->mdn()) {
     w.head = ws_add(p, "mdn.head", Mp * Hp * 4);
     w.head_bias = ws_add(p, "mdn.head_bias", Hp * 4);
+    if (c.sampler_T > 0) {   // decode state of smd_mdn_sample (the chain itself lives in xt)
+      for (int l = 0; l < L; ++l) w.kv.push_back(ws_add(p, "mdn.kv" + std::to_string(l), B * c.seq_len * 3 * kE * 4));
+      w.tok = ws_add(p, "mdn.tok", B * C * 4);
+    }
   }
   if (strict) {
     w.x3_scratch = ws_add(p, "x3.scratch", Mp * Md * 4);   // fp32 cross-term accumulator of the three-pass GEMMs
@@ -293,7 +297,7 @@ static int build_ops(smd_plan* p) {
 // A_hi B_hi with the layer's epilogue taking `scratch` as its residual -- all accumulated in fp32.
 // ln_slot >= 0: this GEMM feeds wide LayerNorm `ln_slot` through a stand-alone ln_film_act launch: its row statistics
 // go out as per-tile partials (added in a fixed order by the consumer) instead of atomics.
-static cudaError_t gemm(smd_plan* p, const GemmOp& op, int M, GemmEpilogue e, cudaStream_t st, int ln_slot = -1) {
+cudaError_t gemm(smd_plan* p, const GemmOp& op, int M, GemmEpilogue e, cudaStream_t st, int ln_slot) {
   auto arm_stats = [&](GemmEpilogue& ef) {
     if (ln_slot < 0 || ef.row_stats == nullptr) return;
     ef.stats_part = p->at<float>(p->reg.stats_part);
@@ -368,8 +372,7 @@ int ensure_side_stream(smd_plan* p) {
 // The FiLM'd residual tail shared by both architectures (models/ncsn.py:173-178, models/shared.py:61-75).
 // On entry u (fp32 [M][Md]) and stats[0] hold the block input and its row statistics.
 // tangent: run the tangent pass next to it (ut[0] and the primal statistics are ready; see run_forward).
-static int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, float* y, cudaStream_t st,
-                    bool tangent) {
+int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, float* y, cudaStream_t st, bool tangent) {
   const int Md = p->cfg.mlp_dims, C = p->cfg.channels;
   const WorkspaceLayout& w = p->reg;
   float* stats = p->at<float>(w.stats);
@@ -583,7 +586,7 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
 
 // host threefry (same block function as the device one)
 static inline uint32_t h_rotl(uint32_t x, int r) { return (x << r) | (x >> (32 - r)); }
-static void h_threefry(uint32_t k0, uint32_t k1, uint32_t& x0, uint32_t& x1) {
+void h_threefry(uint32_t k0, uint32_t k1, uint32_t& x0, uint32_t& x1) {
   static const int R[2][4] = {{13, 15, 26, 6}, {17, 29, 16, 24}};
   const uint32_t ks[3] = {k0, k1, k0 ^ k1 ^ 0x1BD11BDAu};
   x0 += ks[0]; x1 += ks[1];
@@ -593,7 +596,7 @@ static void h_threefry(uint32_t k0, uint32_t k1, uint32_t& x0, uint32_t& x1) {
     x1 += ks[(i + 2) % 3] + static_cast<uint32_t>(i + 1);
   }
 }
-static void h_split(const uint32_t key[2], int num, uint32_t* out) {
+void h_split(const uint32_t key[2], int num, uint32_t* out) {
   // jax.random.split: threefry_2x32(key, iota(2*num)).reshape(num, 2); counters split in halves
   std::vector<uint32_t> flat(2 * num);
   for (int i = 0; i < num; ++i) {

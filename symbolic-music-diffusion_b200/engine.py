@@ -71,6 +71,8 @@ class Engine:
         self.mdn = ARCHS[cfg.arch] == 3
         if sampler_T is None:
             sampler_T = 0 if training or self.mdn else 1000
+        elif self.mdn and sampler_T:
+            sampler_T = cfg.seq_len   # an MDN sampler plan: the decode state of mdn_sample (one step per position)
         c = _lib.SmdConfig(ARCHS[cfg.arch], cfg.num_layers, cfg.num_heads, cfg.num_mlp_layers, cfg.mlp_dims,
                            cfg.seq_len if ARCHS[cfg.arch] in SEQUENCE_ARCHS else 1, cfg.channels, self.max_batch,
                            int(cta_group), int(training), int(sampler_T), PRECISIONS[precision])
@@ -351,6 +353,43 @@ class Engine:
         _lib.check(self.lib.smd_mdn_loss(self._plan, self.params.data_ptr(), x.data_ptr(), x.shape[0], loss.data_ptr(),
                                          self._stream()))
         return loss
+
+    def mdn_sample(self, key, n: int, first_row: int = 0, total_rows: int = 0, chain: bool = False,
+                   components: bool = False):
+        """sample(num_samples=n) of sample_mdn.py:54-119 -> (n, S, C), with key the rng left after
+        ``rng, model_rng = split(rng)``.  chain=True also returns the tokens before the last step, components=True the
+        last step's mixture components (n, S) int32.  first_row / total_rows: these n samples are rows
+        [first_row, first_row + n) of a total_rows-sample run (data-parallel shards; 0: n).  Needs an engine created
+        with sampler_T (any value > 0)."""
+        dev = self._ws.device
+        S, Cc = self.seq_len, self.cfg.channels
+        out = torch.empty((n, S, Cc), dtype=torch.float32, device=dev)
+        ch = torch.empty_like(out) if chain else None
+        comp = torch.empty((n, S), dtype=torch.int32, device=dev) if components else None
+        k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
+        _lib.check(self.lib.smd_mdn_sample(self._plan, self.params.data_ptr(), k, int(n), int(first_row),
+                                           int(total_rows), out.data_ptr(), _ptr(ch), _ptr(comp), self._stream()))
+        res = (out,) + ((ch,) if chain else ()) + ((comp,) if components else ())
+        return res if len(res) > 1 else out
+
+    def mdn_mixture_sample(self, pi: torch.Tensor, mu: torch.Tensor, log_sigma: torch.Tensor, key, first_row: int = 0,
+                           total_rows: int = 0, components: bool = False):
+        """MixtureSameFamily(Categorical(pi), MultivariateNormalDiag(mu, exp(log_sigma))).sample(seed=key) per row:
+        pi (..., Kc), mu / log_sigma (..., Kc*C) -> (..., C).  first_row / total_rows: these rows are rows
+        [first_row, ...) of a draw over total_rows rows (0: all of them)."""
+        pi = _f32c(pi, "pi"); mu = _f32c(mu, "mu"); log_sigma = _f32c(log_sigma, "log_sigma")
+        kc, Cc = self.cfg.mdn_components, self.cfg.channels
+        if pi.shape[-1] != kc or tuple(mu.shape[:-1]) != tuple(pi.shape[:-1]) or mu.shape[-1] != kc * Cc \
+                or mu.shape != log_sigma.shape:
+            raise ValueError(f"pi must be (..., {kc}) and mu / log_sigma (..., {kc * Cc}) with the same leading shape")
+        rows = pi.numel() // kc
+        out = torch.empty(tuple(pi.shape[:-1]) + (Cc,), dtype=torch.float32, device=pi.device)
+        comp = torch.empty(tuple(pi.shape[:-1]), dtype=torch.int32, device=pi.device) if components else None
+        k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
+        _lib.check(self.lib.smd_mdn_mixture_sample(pi.data_ptr(), mu.data_ptr(), log_sigma.data_ptr(), rows, Cc, kc, k,
+                                                   int(first_row), int(total_rows), out.data_ptr(), _ptr(comp),
+                                                   self._stream()))
+        return (out, comp) if components else out
 
     def compute_mdn_grads(self, x: torch.Tensor, global_batch: Optional[int] = None) -> None:
         """grads <- d(mean token NLL over the GLOBAL batch)/d params for this shard; loss_sum / loss_mean as

@@ -73,6 +73,9 @@ _SIGNATURES = {
     "smd_mdn_nll": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "smd_mdn_loss": (C.c_int, [_P, _P, _P, C.c_int, _P, _P]),
     "smd_mdn_grads": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "smd_mdn_mixture_sample": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_longlong,
+                                         C.c_longlong, _P, _P, _P]),
+    "smd_mdn_sample": (C.c_int, [_P, _P, C.POINTER(C.c_uint32), C.c_int, C.c_longlong, C.c_longlong, _P, _P, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

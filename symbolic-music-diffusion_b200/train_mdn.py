@@ -49,7 +49,7 @@ flags.DEFINE_boolean("normalize", True, "Normalize dataset to [-1, 1].")
 # --- logging, checkpointing, evaluation --------------------------------------------------------------------
 flags.DEFINE_integer("logging_freq", 100, "Logging frequency.")
 flags.DEFINE_integer("snapshot_freq", 5000, "Evaluation and checkpoint frequency.")
-flags.DEFINE_boolean("snapshot_sampling", True, "Sample during evaluation (no autoregressive sampler here).")
+flags.DEFINE_boolean("snapshot_sampling", True, "Sample during evaluation (as in the reference, train_mdn never samples; sample_mdn does).")
 flags.DEFINE_integer("eval_samples", 3000, "Number of samples to generate.")
 flags.DEFINE_integer("checkpoints_to_keep", 50, "Number of checkpoints to keep.")
 flags.DEFINE_boolean("save_ckpt", True, "Save model checkpoints at each evaluation step.")
@@ -163,7 +163,7 @@ def train(train_batches, valid_batches, output_dir=None, verbose=True):
         except Exception:  # tensorboard is optional
             writer = None
     if FLAGS.snapshot_sampling:
-        logging.warning("--snapshot_sampling: there is no autoregressive sampler on this path; ignored")
+        logging.warning("--snapshot_sampling: train_mdn does not sample during evaluation (use sample_mdn); ignored")
     examples = train_batches.examples
 
     class _LocalRows:                            # rows [rank*B/W, (rank+1)*B/W) of every global batch
