@@ -155,7 +155,7 @@ cudaError_t fork_dw(smd_plan* p, cudaStream_t st) {
   return cudaStreamWaitEvent(p->dw_stream, p->ev_dw, 0);
 }
 
-int bwd_begin(smd_plan* p, int M, int batch, float* grads, cudaStream_t st) {
+int bwd_begin(smd_plan* p, int M, int batch, float* grads, cudaStream_t st, bool tangent) {
   TrainState& ts = p->train;
   const smd_config& c = p->cfg;
   const int Md = c.mlp_dims, K = p->K, L = p->L;
@@ -174,6 +174,10 @@ int bwd_begin(smd_plan* p, int M, int batch, float* grads, cudaStream_t st) {
     const size_t tail = static_cast<size_t>(Mk - M);
     for (size_t off : ts.du16) SMD_CUDA(cudaMemsetAsync(B16(off) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
     for (size_t off : ts.dr16t) SMD_CUDA(cudaMemsetAsync(B16(off) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
+    if (tangent) {
+      for (size_t off : ts.dut16) SMD_CUDA(cudaMemsetAsync(B16(off) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
+      for (size_t off : ts.drt16) SMD_CUDA(cudaMemsetAsync(B16(off) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
+    }
     for (int l = 0; l < L; ++l) {
       SMD_CUDA(cudaMemsetAsync(B16(ts.dh16a[l]) + static_cast<size_t>(M) * 128, 0, tail * 128 * 2, st));
       SMD_CUDA(cudaMemsetAsync(B16(ts.dh16b[l]) + static_cast<size_t>(M) * 128, 0, tail * 128 * 2, st));
@@ -181,6 +185,8 @@ int bwd_begin(smd_plan* p, int M, int batch, float* grads, cudaStream_t st) {
       SMD_CUDA(cudaMemsetAsync(B16(ts.dqkv16[l]) + static_cast<size_t>(M) * 384, 0, tail * 384 * 2, st));
     }
     SMD_CUDA(cudaMemsetAsync(B16(ts.dpred16) + static_cast<size_t>(M) * p->head_ld, 0, tail * p->head_ld * 2, st));
+    if (tangent)
+      SMD_CUDA(cudaMemsetAsync(B16(ts.dpredt16) + static_cast<size_t>(M) * p->head_ld, 0, tail * p->head_ld * 2, st));
   }
   if (Bk != batch && !p->mdn()) {
     SMD_CUDA(cudaMemsetAsync(B16(ts.dss16) + static_cast<size_t>(batch) * 2 * Md, 0,
@@ -211,11 +217,25 @@ int bwd_out_ln(smd_plan* p, const float* params, int M, float* grads, cudaStream
   return SMD_OK;
 }
 
-// capturing: the call is being recorded into a CUDA graph -- the three "tail gradients are final" events that
-// smd_wait_tail_grads hands to the caller's communication stream are then recorded as EXTERNAL event nodes, so a stream
-// outside the graph can wait on them after the graph has been launched.
-int bwd_tail(smd_plan* p, const float* params, int batch, float* grads, cudaStream_t st, bool capturing) {
+// Every k*. / out_ln / output-layer gradient is final once the three events recorded with `ext` have fired
+// (smd_wait_tail_grads).  When the call is being captured into a CUDA graph they are EXTERNAL event nodes, so a stream
+// outside the graph can wait on them.  Without a FiLM generator the side stream has no work of its own and joins here
+// (a captured graph records events only on streams that take part in the capture).
+static int bwd_tail_done(smd_plan* p, cudaStream_t st, bool capturing) {
   const unsigned ext = capturing ? cudaEventRecordExternal : cudaEventRecordDefault;
+  if (p->mdn()) {
+    SMD_CUDA(cudaEventRecord(p->ev_fork, st));
+    SMD_CUDA(cudaStreamWaitEvent(p->side_stream, p->ev_fork, 0));
+  }
+  SMD_CUDA(cudaEventRecordWithFlags(p->evx_join, p->side_stream, ext));
+  SMD_CUDA(cudaEventRecord(p->ev_join, p->side_stream));   // internal join marker (last node of the side stream: `st` waits on it)
+  SMD_CUDA(cudaEventRecordWithFlags(p->ev_tail, st, ext));
+  SMD_CUDA(cudaEventRecordWithFlags(p->ev_dwtail, p->dw_stream, ext));
+  SMD_LAUNCH_CHECK("backward tail");
+  return SMD_OK;
+}
+
+int bwd_tail(smd_plan* p, const float* params, int batch, float* grads, cudaStream_t st, bool capturing) {
   TrainState& ts = p->train;
   const smd_config& c = p->cfg;
   const int S = c.seq_len, Md = c.mlp_dims;
@@ -277,19 +297,7 @@ int bwd_tail(smd_plan* p, const float* params, int batch, float* grads, cudaStre
 
     if (film) SMD_CUDA(film_generator_bwd(p, params, k, batch, grads, st));
   }
-  // every k*. / out_ln / output-layer gradient is final once these three have fired (smd_wait_tail_grads); without a
-  // FiLM generator the side stream has no work of its own and joins here (a captured graph records events only on
-  // streams that take part in the capture)
-  if (!film) {
-    SMD_CUDA(cudaEventRecord(p->ev_fork, st));
-    SMD_CUDA(cudaStreamWaitEvent(p->side_stream, p->ev_fork, 0));
-  }
-  SMD_CUDA(cudaEventRecordWithFlags(p->evx_join, p->side_stream, ext));
-  SMD_CUDA(cudaEventRecord(p->ev_join, p->side_stream));   // internal join marker (last node of the side stream: `st` waits on it)
-  SMD_CUDA(cudaEventRecordWithFlags(p->ev_tail, st, ext));
-  SMD_CUDA(cudaEventRecordWithFlags(p->ev_dwtail, dws, ext));
-  SMD_LAUNCH_CHECK("backward tail");
-  return SMD_OK;
+  return bwd_tail_done(p, st, capturing);
 }
 
 int bwd_trunk(smd_plan* p, const float* params, int batch, float* grads, cudaStream_t st) {
@@ -406,10 +414,31 @@ int bwd_trunk(smd_plan* p, const float* params, int batch, float* grads, cudaStr
 
 using namespace smd;
 
-// ind: device table {x0, used_alpha, eps} read by the kernels instead of the pointer arguments (graph replay), or null.
+// DenseDDPM / DenseNCSN (no trunk): the input projection's weight gradient (models/ncsn.py:129) -- with tangent, plus
+// the product over the tangent rows x~ and v -- then the joins of the weight-gradient and side streams.
+static int bwd_dense_in(smd_plan* p, int M, float* grads, cudaStream_t st, bool tangent) {
+  const int Md = p->cfg.mlp_dims, C = p->cfg.channels;
+  const int Mk = (M + 63) / 64 * 64;
+  float* dw = grads + p->par.in.kernel;
+  GemmEpilogue e = epi();
+  e.out_f32 = dw; e.ld_f32 = Md;
+  SMD_CUDA(gemm_k(p->train.dWin, C, Mk, 1, e, st));
+  if (tangent) {
+    e.residual = dw; e.ld_res = Md;
+    SMD_CUDA(gemm_k(p->train.tdWin, C, Mk, 1, e, st));
+  }
+  SMD_CUDA(cudaEventRecord(p->ev_dwjoin, p->dw_stream));
+  SMD_CUDA(cudaStreamWaitEvent(st, p->ev_dwjoin, 0));
+  SMD_CUDA(cudaStreamWaitEvent(st, p->ev_join, 0));
+  SMD_LAUNCH_CHECK("backward dense");
+  return SMD_OK;
+}
+
+// DDPM or denoising score matching.  ind: device table {x0, used_alpha, eps} read by the kernels instead of the pointer
+// arguments (graph replay), or null.
 static int grads_impl(smd_plan* p, const float* params, const float* x0, const float* used_alpha, const float* eps,
                       const float* const* ind, int batch, int global_batch, float* grads, float* loss_sum,
-                      cudaStream_t st, bool capturing, int objective) {
+                      cudaStream_t st, bool capturing, Objective objective) {
   TrainState& ts = p->train;
   const smd_config& c = p->cfg;
   const int S = c.seq_len, C = c.channels, Md = c.mlp_dims;
@@ -440,8 +469,8 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
 
   // ---------------- objective ----------------
   // ddpm: mean over (S, C) and the global batch; dsm: sum over (S, C) (x 0.5), mean over the global batch
-  const float gscale = objective == 1 ? 1.0f / static_cast<float>(global_batch)
-                                      : 1.0f / (static_cast<float>(global_batch) * static_cast<float>(per));
+  const float gscale = objective == kObjDsm ? 1.0f / static_cast<float>(global_batch)
+                                           : 1.0f / (static_cast<float>(global_batch) * static_cast<float>(per));
   float* dpred32 = F32(ts.dpred32);
   __nv_bfloat16* dpred16 = B16(ts.dpred16);
   ddpm_loss_bwd_kernel<<<batch, 256, 0, st>>>(eps, pred, F32(ts.loss), loss_sum, p->at<unsigned int>(ts.loss_ctr),
@@ -465,19 +494,7 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
   // ---------------- FiLM'd residual blocks ----------------
   rc = bwd_tail(p, params, batch, grads, st, capturing);
   if (rc) return rc;
-
-  if (L == 0) {
-    // DenseDDPM: input projection weight gradient (models/ncsn.py:129)
-    GemmEpilogue e = epi();
-    e.out_f32 = grads + par.in.kernel; e.ld_f32 = Md;
-    SMD_CUDA(gemm_k(ts.dWin, C, Mk, 1, e, st));
-    SMD_CUDA(cudaEventRecord(p->ev_dwjoin, dws));
-    SMD_CUDA(cudaStreamWaitEvent(st, p->ev_dwjoin, 0));
-    SMD_CUDA(cudaStreamWaitEvent(st, p->ev_join, 0));
-    SMD_LAUNCH_CHECK("backward dense");
-    return SMD_OK;
-  }
-  return bwd_trunk(p, params, batch, grads, st);
+  return L == 0 ? bwd_dense_in(p, M, grads, st, false) : bwd_trunk(p, params, batch, grads, st);
 }
 
 // Sliced score matching (utils/losses.py:182-247) on DenseNCSN: loss_b = 0.5 |f|^2 + sigma v.(J_f v) with f the raw
@@ -488,27 +505,19 @@ static int grads_impl(smd_plan* p, const float* params, const float* x0, const f
 static int ssm_grads_impl(smd_plan* p, const float* params, const float* x0, const float* used_sigma, const float* eps,
                           const float* v, const float* const* ind, int batch, int global_batch, float* grads,
                           float* loss_sum, cudaStream_t st, bool capturing) {
-  const unsigned ext = capturing ? cudaEventRecordExternal : cudaEventRecordDefault;
   TrainState& ts = p->train;
   const smd_config& c = p->cfg;
   const int C = c.channels, Md = c.mlp_dims;
   const int Cp = (C + 63) / 64 * 64;
   const int M = batch;
   const int Mk = (M + 63) / 64 * 64;
-  const int Bk = (batch + 63) / 64 * 64;
   const WorkspaceLayout& w = p->reg;
   const ParamLayout& par = p->par;
   const int K = p->K;
   auto B16 = [&](size_t off) { return p->at<__nv_bfloat16>(off); };
   auto F32 = [&](size_t off) { return p->at<float>(off); };
   { int rcs = ensure_side_stream(p); if (rcs) return rcs; }
-  cudaStream_t side = p->side_stream;
   cudaStream_t dws = p->dw_stream;
-  auto fork_dw = [&]() -> cudaError_t {
-    cudaError_t e1 = cudaEventRecord(p->ev_dw, st);
-    if (e1 != cudaSuccess) return e1;
-    return cudaStreamWaitEvent(dws, p->ev_dw, 0);
-  };
   // weight gradient = primal product + tangent product (reduction over both sets of rows), on the weight-gradient stream
   auto dw2 = [&](const GemmOp& op, const GemmOp& top, int rows, float* out, int ld) -> cudaError_t {
     GemmEpilogue e = epi();
@@ -529,32 +538,16 @@ static int ssm_grads_impl(smd_plan* p, const float* params, const float* x0, con
   float* dut32 = F32(ts.dut32);
   float* stats = F32(w.stats);
   const size_t sstride = static_cast<size_t>(p->Mp) * 2;
-
-  SMD_CUDA(fork_dw());
-  SMD_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * p->arena, dws));
-  SMD_CUDA(cudaEventRecord(p->ev_gz, dws));
-  SMD_CUDA(cudaMemsetAsync(F32(ts.dss), 0, sizeof(float) * static_cast<size_t>(K) * c.max_batch * 2 * Md, st));
-  if (Mk != M) {  // zero the reduction-tail rows of every MN-major gradient operand
-    const size_t tail = static_cast<size_t>(Mk - M);
-    for (const std::vector<size_t>* fam : {&ts.du16, &ts.dr16t, &ts.dut16, &ts.drt16})
-      for (size_t off : *fam) SMD_CUDA(cudaMemsetAsync(B16(off) + static_cast<size_t>(M) * Md, 0, tail * Md * 2, st));
-    SMD_CUDA(cudaMemsetAsync(B16(ts.dpred16) + static_cast<size_t>(M) * Cp, 0, tail * Cp * 2, st));
-    SMD_CUDA(cudaMemsetAsync(B16(ts.dpredt16) + static_cast<size_t>(M) * Cp, 0, tail * Cp * 2, st));
-  }
-  if (Bk != batch) {
-    SMD_CUDA(cudaMemsetAsync(B16(ts.dss16) + static_cast<size_t>(batch) * 2 * Md, 0,
-                             static_cast<size_t>(Bk - batch) * 2 * Md * 2, st));
-    SMD_CUDA(cudaMemsetAsync(B16(ts.e2_16) + static_cast<size_t>(batch) * 512, 0,
-                             static_cast<size_t>(Bk - batch) * 512 * 2, st));
-  }
+  int rc = bwd_begin(p, M, batch, grads, st, /*tangent=*/true);
+  if (rc) return rc;
 
   // ---------------- forward: primal (keeps every activation) and tangent along v ----------------
   float* xt = F32(w.xt);
   float* cond = F32(w.tvec);
   float* f = F32(w.eps_hat);
-  launch_q_sample(x0, eps, used_sigma, xt, cond, batch, C, st, ind, 1); CNT();
+  launch_q_sample(x0, eps, used_sigma, xt, cond, batch, C, st, ind, kObjDsm); CNT();   // x~ = x0 + sigma eps
   launch_tangent_input(v, ind, B16(w.xbt), static_cast<size_t>(M) * C, st, 0); CNT();
-  int rc = run_forward(p, params, xt, cond, 0, batch, f, st, /*save=*/true, /*raw_out=*/true, /*tangent=*/true);
+  rc = run_forward(p, params, xt, cond, 0, batch, f, st, /*save=*/true, /*raw_out=*/true, /*tangent=*/true);
   if (rc) return rc;
   SMD_CUDA(cudaStreamWaitEvent(st, p->ev_gz, 0));
 
@@ -563,7 +556,7 @@ static int ssm_grads_impl(smd_plan* p, const float* params, const float* x0, con
   launch_ssm_loss(f, F32(w.yt), v, used_sigma, ind, F32(ts.loss), nullptr, nullptr, loss_sum,
                   p->at<unsigned int>(ts.loss_ctr), 1.0f / static_cast<float>(global_batch), dpred32, B16(ts.dpred16),
                   B16(ts.dpredt16), batch, C, Cp, st); CNT();
-  SMD_CUDA(fork_dw());
+  SMD_CUDA(fork_dw(p, st));
   launch_colsum<float>(dpred32, C, grads + par.out.bias, M, C, dws); CNT();
 
   // ---------------- output projection + final LayerNorm ----------------
@@ -586,7 +579,7 @@ static int ssm_grads_impl(smd_plan* p, const float* params, const float* x0, con
     const BlockParams& bp = par.block[k];
     const float* ss_k = F32(w.ss) + static_cast<size_t>(k) * c.max_batch * 2 * Md;
     float* dss = F32(ts.dss) + static_cast<size_t>(k) * c.max_batch * 2 * Md;
-    SMD_CUDA(fork_dw());
+    SMD_CUDA(fork_dw(p, st));
     SMD_CUDA(dw2(ts.dWb[k], ts.tdWb[k], Md, grads + bp.b.kernel, Md));
     SMD_CUDA(dx(ts.dXb[k], g16));
     SMD_CUDA(dx(ts.tdXb[k], gt16));
@@ -601,7 +594,7 @@ static int ssm_grads_impl(smd_plan* p, const float* params, const float* x0, con
     a.dss = dss;
     a.M = M; a.N = Md; a.S = 1;
     launch_ssm_ln_bwd(a, st); CNT();
-    SMD_CUDA(fork_dw());
+    SMD_CUDA(fork_dw(p, st));
     SMD_CUDA(dw2(ts.dWa[k], ts.tdWa[k], Md, grads + bp.a.kernel, Md));
     SMD_CUDA(dx(ts.dXa[k], g16));
     SMD_CUDA(dx(ts.tdXa[k], gt16));
@@ -619,43 +612,16 @@ static int ssm_grads_impl(smd_plan* p, const float* params, const float* x0, con
     launch_ssm_ln_bwd(a, st); CNT();
     SMD_CUDA(film_generator_bwd(p, params, k, batch, grads, st));
   }
-  SMD_CUDA(cudaEventRecordWithFlags(p->evx_join, side, ext));
-  SMD_CUDA(cudaEventRecord(p->ev_join, side));
-  SMD_CUDA(cudaEventRecordWithFlags(p->ev_tail, st, ext));
-  SMD_CUDA(cudaEventRecordWithFlags(p->ev_dwtail, dws, ext));
-  SMD_LAUNCH_CHECK("ssm backward tail");
-
-  // ---------------- input projection (models/ncsn.py:129): x~ and v rows ----------------
-  {
-    GemmEpilogue e = epi();
-    e.out_f32 = grads + par.in.kernel; e.ld_f32 = Md;
-    SMD_CUDA(gemm_k(ts.dWin, C, Mk, 1, e, st));
-    e.residual = grads + par.in.kernel; e.ld_res = Md;
-    SMD_CUDA(gemm_k(ts.tdWin, C, Mk, 1, e, st));
-  }
-  SMD_CUDA(cudaEventRecord(p->ev_dwjoin, dws));
-  SMD_CUDA(cudaStreamWaitEvent(st, p->ev_dwjoin, 0));
-  SMD_CUDA(cudaStreamWaitEvent(st, p->ev_join, 0));
-  SMD_LAUNCH_CHECK("ssm backward");
-  return SMD_OK;
+  rc = bwd_tail_done(p, st, capturing);
+  if (rc) return rc;
+  return bwd_dense_in(p, M, grads, st, /*tangent=*/true);
 }
 
-// SMD_TRAIN_GRAPH=0 switches the graph replay of the train step off (eager launches, 3 streams, as in round 1)
-static bool train_graph_enabled() {
-  static const bool on = [] { const char* v = getenv("SMD_TRAIN_GRAPH"); return !(v && v[0] == '0'); }();
-  return on;
-}
-
-static void drop_train_graph(smd_plan* p) {
-  if (p->tg_exec) { cudaGraphExecDestroy(p->tg_exec); p->tg_exec = nullptr; }
-  p->tg_valid = false;
-}
-
-// objective 0: ddpm, 1: denoising score matching, 2: sliced score matching (v: its projection vectors; else null),
-// 3: the mixture-density NLL of TransformerMDN (x0: the sequences; used_alpha / eps null)
+// v: the projection vectors of sliced score matching, else null.  TransformerMDN: x0 holds the sequences, used_alpha /
+// eps are null.
 static int grads_entry(smd_plan* p, const float* params, const float* x0, const float* used_alpha,
                        const float* eps, const float* v, int batch, int global_batch, float* grads, float* loss_sum,
-                       smd_stream_t stream, int objective) {
+                       smd_stream_t stream, Objective objective) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!p->cfg.training) { set_error("plan was not created with training = 1"); return SMD_ERR_STATE; }
   if (!p->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
@@ -663,22 +629,22 @@ static int grads_entry(smd_plan* p, const float* params, const float* x0, const 
   const bool capturable = st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread;
   auto impl = [&](const float* x0_, const float* ua_, const float* eps_, const float* v_, const float* const* ind_,
                   bool capturing) {
-    if (objective == 2)
+    if (objective == kObjSsm)
       return ssm_grads_impl(p, params, x0_, ua_, eps_, v_, ind_, batch, global_batch, grads, loss_sum, st, capturing);
-    if (objective == 3) return mdn_grads_impl(p, params, x0_, ind_, batch, global_batch, grads, loss_sum, st, capturing);
+    if (objective == kObjMdn) return mdn_grads_impl(p, params, x0_, ind_, batch, global_batch, grads, loss_sum, st, capturing);
     return grads_impl(p, params, x0_, ua_, eps_, ind_, batch, global_batch, grads, loss_sum, st, capturing, objective);
   };
-  if (!train_graph_enabled() || !capturable) return impl(x0, used_alpha, eps, v, nullptr, false);
+  if (!capturable) return impl(x0, used_alpha, eps, v, nullptr, false);
   // Graph replay: the pass's ~150 launches on three streams (dX chain, weight-gradient GEMMs, FiLM generator) are
   // captured once into one CUDA graph with the same fork / join structure.  The per-step inputs (x0, used_alpha, eps)
   // reach the kernels through a device pointer table, so new input tensors do not force a re-capture; the events a
   // data-parallel caller waits on (smd_wait_tail_grads) are external event-record nodes of the graph.
-  const bool same = p->tg_valid && p->tg_params == params && p->tg_grads == grads && p->tg_loss == loss_sum &&
+  const bool same = p->train_graph.exec && p->tg_params == params && p->tg_grads == grads && p->tg_loss == loss_sum &&
                     p->tg_batch == batch && p->tg_global == global_batch && p->tg_objective == objective;
   const float** ind = p->at<const float*>(p->train.ind);
   if (!same) {
     const bool warm = p->tg_warm && p->tg_params == params && p->tg_batch == batch && p->tg_objective == objective;
-    drop_train_graph(p);
+    p->train_graph.drop();
     p->tg_params = params; p->tg_grads = grads; p->tg_loss = loss_sum; p->tg_batch = batch; p->tg_global = global_batch;
     p->tg_objective = objective;
     if (!warm) {
@@ -687,40 +653,28 @@ static int grads_entry(smd_plan* p, const float* params, const float* x0, const 
       p->tg_warm = true;
       return impl(x0, used_alpha, eps, v, nullptr, false);
     }
-    cudaGraph_t graph = nullptr;
-    const long long before = g_launches.load();
-    SMD_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    int rc = impl(nullptr, nullptr, nullptr, nullptr, ind, true);
-    cudaError_t ce = cudaStreamEndCapture(st, &graph);
-    p->tg_nodes = g_launches.load() - before;
-    g_launches.store(before);   // captured launches are counted per replay
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (ce != cudaSuccess) { set_error(std::string("train graph capture: ") + cudaGetErrorString(ce)); return SMD_ERR_CUDA; }
-    ce = cudaGraphInstantiate(&p->tg_exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (ce != cudaSuccess) { set_error(std::string("train graph instantiate: ") + cudaGetErrorString(ce)); return SMD_ERR_CUDA; }
-    p->tg_valid = true;
+    const int rc = p->train_graph.capture(st, [&] { return impl(nullptr, nullptr, nullptr, nullptr, ind, true); },
+                                          "train graph");
+    if (rc) return rc;
   }
   // (pageable source: the driver stages these 32 bytes before returning, so the host array may die with this frame)
   const float* host_ind[4] = {x0, used_alpha, eps, v};
   SMD_CUDA(cudaMemcpyAsync(ind, host_ind, sizeof(host_ind), cudaMemcpyHostToDevice, st));
-  SMD_CUDA(cudaGraphLaunch(p->tg_exec, st));
-  g_launches.fetch_add(p->tg_nodes, std::memory_order_relaxed);
-  return SMD_OK;
+  return p->train_graph.launch(st);
 }
 
 extern "C" int smd_ddpm_grads(smd_plan* p, const float* params, const float* x0, const float* used_alpha,
                               const float* eps, int batch, int global_batch, float* grads, float* loss_sum,
                               smd_stream_t stream) {
   if (p->mdn()) { set_error("smd_ddpm_grads does not apply to a TransformerMDN plan (use smd_mdn_grads)"); return SMD_ERR_INVALID; }
-  return grads_entry(p, params, x0, used_alpha, eps, nullptr, batch, global_batch, grads, loss_sum, stream, 0);
+  return grads_entry(p, params, x0, used_alpha, eps, nullptr, batch, global_batch, grads, loss_sum, stream, kObjDdpm);
 }
 
 // TransformerMDN (train_mdn.py:180-205): gradient of the mean token NLL; x is the only per-step input
 extern "C" int smd_mdn_grads(smd_plan* p, const float* params, const float* x, int batch, int global_batch,
                              float* grads, float* loss_sum, smd_stream_t stream) {
   if (!p || !p->mdn()) { set_error("smd_mdn_grads needs a TransformerMDN plan (smd_mdn_plan_create)"); return SMD_ERR_INVALID; }
-  return grads_entry(p, params, x, nullptr, nullptr, nullptr, batch, global_batch, grads, loss_sum, stream, 3);
+  return grads_entry(p, params, x, nullptr, nullptr, nullptr, batch, global_batch, grads, loss_sum, stream, kObjMdn);
 }
 
 // denoising score matching (utils/losses.py:129-179): the same pass with x~ = x0 + sigma eps, the network conditioned on
@@ -729,7 +683,7 @@ extern "C" int smd_dsm_grads(smd_plan* p, const float* params, const float* x0, 
                              const float* eps, int batch, int global_batch, float* grads, float* loss_sum,
                              smd_stream_t stream) {
   if (p->cfg.arch != SMD_ARCH_DENSE_NCSN) { set_error("smd_dsm_grads needs a score network (SMD_ARCH_DENSE_NCSN)"); return SMD_ERR_INVALID; }
-  return grads_entry(p, params, x0, used_sigma, eps, nullptr, batch, global_batch, grads, loss_sum, stream, 1);
+  return grads_entry(p, params, x0, used_sigma, eps, nullptr, batch, global_batch, grads, loss_sum, stream, kObjDsm);
 }
 
 // sliced score matching (utils/losses.py:182-247) with the draws of smd_ssm_draws supplied (SMD_ARCH_DENSE_NCSN)
@@ -737,5 +691,5 @@ extern "C" int smd_ssm_grads(smd_plan* p, const float* params, const float* x0, 
                              const float* eps, const float* v, int batch, int global_batch, float* grads,
                              float* loss_sum, smd_stream_t stream) {
   if (p->cfg.arch != SMD_ARCH_DENSE_NCSN) { set_error("smd_ssm_grads needs a score network (SMD_ARCH_DENSE_NCSN)"); return SMD_ERR_INVALID; }
-  return grads_entry(p, params, x0, used_sigma, eps, v, batch, global_batch, grads, loss_sum, stream, 2);
+  return grads_entry(p, params, x0, used_sigma, eps, v, batch, global_batch, grads, loss_sum, stream, kObjSsm);
 }

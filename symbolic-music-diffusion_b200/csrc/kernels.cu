@@ -40,9 +40,7 @@ __global__ void q_sample_kernel(const float* __restrict__ x0, const float* __res
 void launch_q_sample(const float* x0, const float* eps, const float* used_alpha, float* xt, float* cond, int B,
                      int per_sample, cudaStream_t st, const float* const* ind, int mode) {
   const size_t total = static_cast<size_t>(B) * per_sample;
-  int blocks = static_cast<int>((total + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
-  q_sample_kernel<<<blocks, 256, 0, st>>>(x0, eps, used_alpha, xt, cond, B, per_sample, ind, mode);
+  q_sample_kernel<<<grid_stride_blocks(total), 256, 0, st>>>(x0, eps, used_alpha, xt, cond, B, per_sample, ind, mode);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -951,9 +949,7 @@ __global__ void scale_rows_kernel(float* __restrict__ y, const float* __restrict
 }
 void launch_scale_rows(float* y, const float* sigma, int bcast, int B, int per, cudaStream_t st) {
   const size_t total = static_cast<size_t>(B) * per;
-  int blocks = static_cast<int>((total + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
-  scale_rows_kernel<<<blocks, 256, 0, st>>>(y, sigma, bcast, B, per);
+  scale_rows_kernel<<<grid_stride_blocks(total), 256, 0, st>>>(y, sigma, bcast, B, per);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1040,9 +1036,7 @@ __global__ void tangent_input_kernel(const float* __restrict__ v, const float* c
 }
 void launch_tangent_input(const float* v, const float* const* ind, __nv_bfloat16* out, size_t n, cudaStream_t st,
                           long long lo_delta) {
-  int blocks = static_cast<int>((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
-  tangent_input_kernel<<<blocks, 256, 0, st>>>(v, ind, out, n, lo_delta);
+  tangent_input_kernel<<<grid_stride_blocks(n), 256, 0, st>>>(v, ind, out, n, lo_delta);
 }
 
 __global__ void __launch_bounds__(256)

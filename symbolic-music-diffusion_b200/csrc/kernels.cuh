@@ -137,6 +137,14 @@ __device__ __forceinline__ float jax_normal_from_bits(uint32_t bits) {
   return 1.41421356237f * erfinv_giles(u);
 }
 
+// Grid cap of the grid-stride kernels (256-thread CTAs): 8 CTAs per SM of a 148-SM part, which still covers every SM of
+// an H100.  Every timing of these kernels was taken with this cap, so changing it is a performance change of its own.
+static constexpr int kGridStrideMaxBlocks = 148 * 8;
+inline int grid_stride_blocks(size_t n) {
+  const size_t blocks = (n + 255) / 256;
+  return static_cast<int>(blocks < kGridStrideMaxBlocks ? blocks : kGridStrideMaxBlocks);
+}
+
 // ---------------------------------------------------------------------------------------------------
 // kernels (definitions in kernels.cu)
 // ---------------------------------------------------------------------------------------------------

@@ -139,9 +139,7 @@ static cudaError_t launch_mdn_nll(const MdnNllArgs& a, cudaStream_t st) {
 
 static void launch_mdn_shift(const float* x, const float* const* ind, float* xs, int B, int S, int C, cudaStream_t st) {
   const size_t n = static_cast<size_t>(B) * S * C;
-  int blocks = static_cast<int>((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
-  mdn_shift_kernel<<<blocks, 256, 0, st>>>(x, ind, xs, B, S, C); CNT();
+  mdn_shift_kernel<<<grid_stride_blocks(n), 256, 0, st>>>(x, ind, xs, B, S, C); CNT();
 }
 
 // head-output columns of the three parts (offsets into the packed [mu | log_sigma | pi] width)

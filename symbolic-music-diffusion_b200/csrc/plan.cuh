@@ -129,6 +129,48 @@ struct TrainState {
   GemmOp tdWout, tdXout, tdWin;
 };
 
+// Training objectives of the grads entry points (backward.cu); the value is the `mode` / `objective` the q_sample and
+// loss kernels receive.
+enum Objective : int { kObjDdpm = 0, kObjDsm = 1, kObjSsm = 2, kObjMdn = 3 };
+
+// A launch sequence captured once and replayed as one CUDA graph.  g_launches counts the captured launches once per
+// replay (launch), not at capture.
+struct CapturedGraph {
+  cudaGraphExec_t exec = nullptr;
+  long long nodes = 0;   // launches recorded by the capture
+
+  void drop() {
+    if (exec) cudaGraphExecDestroy(exec);
+    exec = nullptr;
+  }
+  // Replaces the graph by what body() enqueues on st (a capturable stream); returns body's error code or SMD_ERR_CUDA,
+  // leaving no graph behind on failure.
+  template <typename Body>
+  int capture(cudaStream_t st, Body&& body, const char* what) {
+    drop();
+    cudaGraph_t graph = nullptr;
+    const long long before = g_launches.load();
+    SMD_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    const int rc = body();
+    cudaError_t ce = cudaStreamEndCapture(st, &graph);
+    nodes = g_launches.load() - before;
+    g_launches.store(before);
+    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
+    if (ce != cudaSuccess) { set_error(std::string(what) + " capture: " + cudaGetErrorString(ce)); return SMD_ERR_CUDA; }
+    ce = cudaGraphInstantiate(&exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (ce == cudaSuccess) return SMD_OK;
+    exec = nullptr;
+    set_error(std::string(what) + " instantiate: " + cudaGetErrorString(ce));
+    return SMD_ERR_CUDA;
+  }
+  int launch(cudaStream_t st) {
+    SMD_CUDA(cudaGraphLaunch(exec, st));
+    g_launches.fetch_add(nodes, std::memory_order_relaxed);
+    return SMD_OK;
+  }
+};
+
 }  // namespace smd
 
 using namespace smd;
@@ -177,7 +219,8 @@ struct smd_plan {
   const float* film_tab_params = nullptr;
   bool sampler_ready = false;
   long long shard_first_row = 0, shard_total_rows = 0;   // smd_sampler_set_shard
-  cudaGraphExec_t graph_exec = nullptr;
+  // graph replay of one smd_ddpm_sample step, and the arguments it was captured with
+  smd::CapturedGraph sample_graph;
   int graph_n = -1;
   const float* graph_params = nullptr;
   float* graph_x = nullptr;
@@ -185,7 +228,6 @@ struct smd_plan {
   const float* graph_infill_mask = nullptr;
   float* graph_collection = nullptr;
   float* graph_metrics = nullptr;
-  long long graph_nodes = 0;
   cudaStream_t own_stream = nullptr;
   cudaEvent_t own_event = nullptr;
   // training: the FiLM generator (forward and backward) runs on a side stream, concurrently with the trunk
@@ -193,16 +235,16 @@ struct smd_plan {
   cudaStream_t dw_stream = nullptr;     // trunk weight-gradient GEMMs (leaves of the backward graph)
   cudaEvent_t ev_fork = nullptr, ev_film = nullptr, ev_dss = nullptr, ev_join = nullptr, ev_dw = nullptr, ev_dwjoin = nullptr, ev_tail = nullptr, ev_dwtail = nullptr;
   smd::TrainState train;
-  // graph replay of smd_ddpm_grads (backward.cu)
-  cudaGraphExec_t tg_exec = nullptr;
-  long long tg_nodes = 0;
-  bool tg_valid = false, tg_warm = false;
   cudaEvent_t ev_gz = nullptr;      // gradient arena zeroed (on the weight-gradient stream)
   cudaEvent_t evx_join = nullptr;   // "FiLM generator gradients final", waitable from outside the graph
+  // graph replay of the grads entry points (backward.cu), and the arguments it was captured with
+  smd::CapturedGraph train_graph;
+  bool tg_warm = false;
   const float* tg_params = nullptr;
   float* tg_grads = nullptr;
   float* tg_loss = nullptr;
-  int tg_batch = 0, tg_global = 0, tg_objective = 0;
+  int tg_batch = 0, tg_global = 0;
+  smd::Objective tg_objective = smd::kObjDdpm;
 
   template <typename Tp>
   Tp* at(size_t off) const { return reinterpret_cast<Tp*>(ws + off); }
@@ -233,10 +275,11 @@ void h_threefry(uint32_t k0, uint32_t k1, uint32_t& x0, uint32_t& x1);
 void h_split(const uint32_t key[2], int num, uint32_t* out);
 
 // Pieces of the backward pass shared by the objectives (backward.cu).  bwd_begin zeroes the gradient arena (on the
-// weight-gradient stream) and the reduction-tail rows of every MN-major gradient operand; bwd_out_ln runs the output
-// layer's dX GEMM (operand dpred16) and the out_ln backward; bwd_tail the (FiLM) res-blocks, then records the events
-// of smd_wait_tail_grads; bwd_trunk the post / transformer layers / input projection (input reg.xt) and the joins.
-int bwd_begin(smd_plan* p, int M, int batch, float* grads, cudaStream_t st);
+// weight-gradient stream) and the reduction-tail rows of every MN-major gradient operand (with tangent, also those of
+// the sliced-score-matching tangent adjoints); bwd_out_ln runs the output layer's dX GEMM (operand dpred16) and the
+// out_ln backward; bwd_tail the (FiLM) res-blocks, then records the events of smd_wait_tail_grads; bwd_trunk the
+// post / transformer layers / input projection (input reg.xt) and the joins.
+int bwd_begin(smd_plan* p, int M, int batch, float* grads, cudaStream_t st, bool tangent = false);
 int bwd_out_ln(smd_plan* p, const float* params, int M, float* grads, cudaStream_t st);
 int bwd_tail(smd_plan* p, const float* params, int batch, float* grads, cudaStream_t st, bool capturing);
 int bwd_trunk(smd_plan* p, const float* params, int batch, float* grads, cudaStream_t st);

@@ -662,6 +662,35 @@ __global__ void threefry_rademacher_kernel(uint32_t k0, uint32_t k1, float* out,
     out[i] = jax_random_bits(k0, k1, first + i, total) < 0x80000000u ? 1.0f : -1.0f;
 }
 
+static void launch_threefry_normal(const uint32_t key[2], float* out, uint32_t n, uint32_t first, uint32_t total,
+                                   cudaStream_t st) {
+  threefry_normal_kernel<<<grid_stride_blocks(n), 256, 0, st>>>(key[0], key[1], out, n, first, total); CNT();
+}
+
+// The draws of a training objective for rows [first_row, first_row + batch) of a global batch: key -> `nsplit` keys
+// (rng, label_rng, sample_rng[, score_rng]) and rng -> (rng, noise_rng); labels and used from `table` (draws_kernel),
+// eps = normal(sample_rng) and, when v is given, v = rademacher(score_rng).
+static int objective_draws(const smd_plan* plan, const uint32_t host_key[2], int nsplit, const float* table,
+                           int wrap_index, int span, int minlabel, int continuous, int global_batch, int first_row,
+                           int batch, float* used, float* eps, float* v, int* labels, cudaStream_t st, const char* what) {
+  if (batch < 1 || first_row < 0 || global_batch < first_row + batch) { set_error("batch out of range"); return SMD_ERR_INVALID; }
+  const long long per = static_cast<long long>(plan->cfg.seq_len) * plan->cfg.channels;
+  if (static_cast<long long>(global_batch) * per > 0xFFFFFFFFll) { set_error("global batch too large"); return SMD_ERR_INVALID; }
+  uint32_t k[8], k2[4];
+  h_split(host_key, nsplit, k);
+  const uint32_t rng[2] = {k[0], k[1]};
+  h_split(rng, 2, k2);
+  draws_kernel<<<(batch + 127) / 128, 128, 0, st>>>(k[2], k[3], k2[2], k2[3], table, wrap_index, span, global_batch,
+                                                    first_row, batch, minlabel, continuous, used, labels);
+  CNT();
+  const uint32_t n = static_cast<uint32_t>(batch * per), first = static_cast<uint32_t>(first_row * per),
+                 total = static_cast<uint32_t>(global_batch * per);
+  launch_threefry_normal(k + 4, eps, n, first, total, st);
+  if (v) { threefry_rademacher_kernel<<<grid_stride_blocks(n), 256, 0, st>>>(k[6], k[7], v, n, first, total); CNT(); }
+  SMD_LAUNCH_CHECK(what);
+  return SMD_OK;
+}
+
 }  // namespace smd
 
 // =====================================================================================================
@@ -737,8 +766,8 @@ int smd_mdn_plan_create(const smd_config* cfg, int num_components, smd_plan** ou
 
 void smd_plan_destroy(smd_plan* plan) {
   if (!plan) return;
-  if (plan->graph_exec) cudaGraphExecDestroy(plan->graph_exec);
-  if (plan->tg_exec) cudaGraphExecDestroy(plan->tg_exec);
+  plan->sample_graph.drop();
+  plan->train_graph.drop();
   if (plan->evx_join) cudaEventDestroy(plan->evx_join);
   if (plan->ev_gz) cudaEventDestroy(plan->ev_gz);
   if (plan->own_event) cudaEventDestroy(plan->own_event);
@@ -777,8 +806,8 @@ int smd_bind_workspace(smd_plan* plan, void* workspace, size_t bytes) {
   SMD_CUDA(cudaMemset(workspace, 0, plan->ws_bytes));  // padded rows / columns of every operand start finite
   plan->packed = false;
   plan->sampler_ready = false;
-  if (plan->tg_exec) { cudaGraphExecDestroy(plan->tg_exec); plan->tg_exec = nullptr; }
-  plan->tg_valid = false; plan->tg_warm = false;
+  plan->train_graph.drop();
+  plan->tg_warm = false;
   int rc = build_ops(plan);
   if (rc) return rc;
   float f[64];
@@ -909,27 +938,12 @@ int smd_dsm_setup(smd_plan* plan, const float* host_sigmas, int L, smd_stream_t 
 int smd_dsm_draws(smd_plan* plan, const uint32_t host_key[2], int global_batch, int first_row, int batch,
                   int continuous_noise, float* used_sigma, float* eps, int* labels_or_null, smd_stream_t stream) {
   if (plan->L_dsm <= 0) { set_error("smd_dsm_setup has not been called"); return SMD_ERR_STATE; }
-  if (batch < 1 || first_row < 0 || global_batch < first_row + batch) { set_error("batch out of range"); return SMD_ERR_INVALID; }
-  const long long per = static_cast<long long>(plan->cfg.seq_len) * plan->cfg.channels;
-  if (static_cast<long long>(global_batch) * per > 0xFFFFFFFFll) { set_error("global batch too large"); return SMD_ERR_INVALID; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // split(key, 3) (utils/losses.py:146), noise_rng (:152-153); labels = randint(label_rng, minval = int(continuous),
+  // maxval = L): span L - cn; table index label - 1 wraps for 0
   const int L = plan->L_dsm, cn = continuous_noise ? 1 : 0;
-  uint32_t k3[6], k2[4] = {0, 0, 0, 0};
-  h_split(host_key, 3, k3);               // rng, label_rng, sample_rng          (utils/losses.py:146)
-  if (cn) { const uint32_t rng[2] = {k3[0], k3[1]}; h_split(rng, 2, k2); }        // rng, noise_rng (:152-153)
-  // labels = randint(label_rng, minval = int(continuous), maxval = L): span L - cn; table index label - 1 wraps for 0
-  draws_kernel<<<(batch + 127) / 128, 128, 0, st>>>(k3[2], k3[3], k2[2], k2[3], plan->at<float>(plan->reg.sigmas), L - 1, L - cn,
-                                                    global_batch, first_row, batch, cn, cn, used_sigma, labels_or_null);
-  CNT();
-  const long long n = static_cast<long long>(batch) * per;
-  int blocks = static_cast<int>((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
-  threefry_normal_kernel<<<blocks, 256, 0, st>>>(k3[4], k3[5], eps, static_cast<uint32_t>(n),
-                                                 static_cast<uint32_t>(first_row * per),
-                                                 static_cast<uint32_t>(global_batch * per));
-  CNT();
-  SMD_LAUNCH_CHECK("dsm_draws");
-  return SMD_OK;
+  return objective_draws(plan, host_key, 3, plan->at<float>(plan->reg.sigmas), L - 1, L - cn, cn, cn, global_batch,
+                         first_row, batch, used_sigma, eps, nullptr, labels_or_null, static_cast<cudaStream_t>(stream),
+                         "dsm_draws");
 }
 
 int smd_ssm_draws(smd_plan* plan, const uint32_t host_key[2], int global_batch, int first_row, int batch,
@@ -937,27 +951,11 @@ int smd_ssm_draws(smd_plan* plan, const uint32_t host_key[2], int global_batch, 
                   smd_stream_t stream) {
   if (plan->cfg.arch != SMD_ARCH_DENSE_NCSN) { set_error("smd_ssm_draws needs a score network (SMD_ARCH_DENSE_NCSN)"); return SMD_ERR_INVALID; }
   if (plan->L_dsm <= 0) { set_error("smd_dsm_setup has not been called"); return SMD_ERR_STATE; }
-  if (batch < 1 || first_row < 0 || global_batch < first_row + batch) { set_error("batch out of range"); return SMD_ERR_INVALID; }
-  const long long per = static_cast<long long>(plan->cfg.seq_len) * plan->cfg.channels;
-  if (static_cast<long long>(global_batch) * per > 0xFFFFFFFFll) { set_error("global batch too large"); return SMD_ERR_INVALID; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // split(key, 4) (utils/losses.py:203), noise_rng (:210); labels as smd_dsm_draws
   const int L = plan->L_dsm, cn = continuous_noise ? 1 : 0;
-  uint32_t k4[8], k2[4] = {0, 0, 0, 0};
-  h_split(host_key, 4, k4);               // rng, label_rng, sample_rng, score_rng   (utils/losses.py:203)
-  if (cn) { const uint32_t rng[2] = {k4[0], k4[1]}; h_split(rng, 2, k2); }        // rng, noise_rng (:210)
-  draws_kernel<<<(batch + 127) / 128, 128, 0, st>>>(k4[2], k4[3], k2[2], k2[3], plan->at<float>(plan->reg.sigmas), L - 1, L - cn,
-                                                    global_batch, first_row, batch, cn, cn, used_sigma, labels_or_null);
-  CNT();
-  const long long n = static_cast<long long>(batch) * per;
-  int blocks = static_cast<int>((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
-  const uint32_t first = static_cast<uint32_t>(first_row * per), total = static_cast<uint32_t>(global_batch * per);
-  threefry_normal_kernel<<<blocks, 256, 0, st>>>(k4[4], k4[5], eps, static_cast<uint32_t>(n), first, total);
-  CNT();
-  threefry_rademacher_kernel<<<blocks, 256, 0, st>>>(k4[6], k4[7], v, static_cast<uint32_t>(n), first, total);
-  CNT();
-  SMD_LAUNCH_CHECK("ssm_draws");
-  return SMD_OK;
+  return objective_draws(plan, host_key, 4, plan->at<float>(plan->reg.sigmas), L - 1, L - cn, cn, cn, global_batch,
+                         first_row, batch, used_sigma, eps, v, labels_or_null, static_cast<cudaStream_t>(stream),
+                         "ssm_draws");
 }
 
 int smd_ssm_loss(smd_plan* plan, const float* params, const float* x0, const float* used_sigma, const float* eps,
@@ -1020,28 +1018,10 @@ int smd_ddpm_draws_sharded(smd_plan* plan, const uint32_t host_key[2], int globa
                            int continuous_noise, float* used_alpha, float* eps, int* labels_or_null,
                            smd_stream_t stream) {
   if (plan->T_obj <= 0) { set_error("smd_objective_setup has not been called"); return SMD_ERR_STATE; }
-  if (batch < 1 || first_row < 0 || global_batch < first_row + batch) { set_error("batch out of range"); return SMD_ERR_INVALID; }
-  const long long per = static_cast<long long>(plan->cfg.seq_len) * plan->cfg.channels;
-  if (static_cast<long long>(global_batch) * per > 0xFFFFFFFFll) { set_error("global batch too large"); return SMD_ERR_INVALID; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  uint32_t k3[6], k2[4];
-  h_split(host_key, 3, k3);               // rng, label_rng, sample_rng
-  const uint32_t rng[2] = {k3[0], k3[1]};
-  h_split(rng, 2, k2);                    // rng, noise_rng
   // ddpm: labels = randint(int(continuous), T + int(continuous)) -> span T; alphas_prod has T + 1 entries (leading 1)
-  draws_kernel<<<(batch + 127) / 128, 128, 0, st>>>(k3[2], k3[3], k2[2], k2[3], plan->at<float>(plan->reg.abar), plan->T_obj,
-                                                    plan->T_obj, global_batch, first_row, batch, continuous_noise ? 1 : 0, 1,
-                                                    used_alpha, labels_or_null);
-  CNT();
-  const long long n = static_cast<long long>(batch) * per;
-  int blocks = static_cast<int>((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
-  threefry_normal_kernel<<<blocks, 256, 0, st>>>(k3[4], k3[5], eps, static_cast<uint32_t>(n),
-                                                 static_cast<uint32_t>(first_row * per),
-                                                 static_cast<uint32_t>(global_batch * per));
-  CNT();
-  SMD_LAUNCH_CHECK("ddpm_draws");
-  return SMD_OK;
+  return objective_draws(plan, host_key, 3, plan->at<float>(plan->reg.abar), plan->T_obj, plan->T_obj,
+                         continuous_noise ? 1 : 0, 1, global_batch, first_row, batch, used_alpha, eps, nullptr,
+                         labels_or_null, static_cast<cudaStream_t>(stream), "ddpm_draws");
 }
 
 int smd_ddpm_draws(smd_plan* plan, const uint32_t host_key[2], int batch, float* used_alpha, float* eps,
@@ -1109,7 +1089,7 @@ int smd_sampler_setup(smd_plan* plan, const float* host_betas, int T, const uint
   plan->T = T;
   plan->sampler_ready = true;
   plan->film_tab_ready = false;
-  if (plan->graph_exec) { cudaGraphExecDestroy(plan->graph_exec); plan->graph_exec = nullptr; }
+  plan->sample_graph.drop();
   return SMD_OK;
 }
 
@@ -1196,7 +1176,7 @@ int smd_sampler_set_shard(smd_plan* plan, long long first_row, long long total_r
       total_rows * plan->cfg.seq_len * plan->cfg.channels > 0xFFFFFFFFll) { set_error("bad shard"); return SMD_ERR_INVALID; }
   plan->shard_first_row = first_row;
   plan->shard_total_rows = total_rows;
-  if (plan->graph_exec) { cudaGraphExecDestroy(plan->graph_exec); plan->graph_exec = nullptr; }  // kernel args changed
+  plan->sample_graph.drop();  // kernel args changed
   return SMD_OK;
 }
 
@@ -1247,30 +1227,23 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
   const int t0 = T - 1;
   SMD_CUDA(cudaMemcpyAsync(t_ptr, &t0, sizeof(int), cudaMemcpyHostToDevice, cs));
   SMD_CUDA(cudaStreamSynchronize(cs));  // t0 is a stack variable
-  const bool same = plan->graph_exec && plan->graph_n == n && plan->graph_params == params && plan->graph_x == x &&
+  const bool same = plan->sample_graph.exec && plan->graph_n == n && plan->graph_params == params && plan->graph_x == x &&
                     plan->graph_infill_x == infill_x && plan->graph_infill_mask == infill_mask &&
                     plan->graph_collection == collection && plan->graph_metrics == metrics;
   if (!same) {
-    if (plan->graph_exec) { cudaGraphExecDestroy(plan->graph_exec); plan->graph_exec = nullptr; }
-    cudaGraph_t graph = nullptr;
-    const long long before = g_launches.load();
-    SMD_CUDA(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-    int rc = reverse_step_impl(plan, params, x, n, -1, nullptr, infill_x, infill_mask, nullptr, x, nullptr,
-                               collection, metrics, cs);
-    if (rc == SMD_OK) { launch_step_advance(t_ptr, cs); CNT(); }
-    cudaError_t ce = cudaStreamEndCapture(cs, &graph);
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (ce != cudaSuccess) { set_error(std::string("graph capture: ") + cudaGetErrorString(ce)); return SMD_ERR_CUDA; }
-    plan->graph_nodes = g_launches.load() - before;
-    g_launches.store(before);  // captured launches are counted per replay below
-    SMD_CUDA(cudaGraphInstantiate(&plan->graph_exec, graph, 0));
-    cudaGraphDestroy(graph);
+    const int rc = plan->sample_graph.capture(cs, [&] {
+      const int r = reverse_step_impl(plan, params, x, n, -1, nullptr, infill_x, infill_mask, nullptr, x, nullptr,
+                                      collection, metrics, cs);
+      if (r == SMD_OK) { launch_step_advance(t_ptr, cs); CNT(); }
+      return r;
+    }, "sampler graph");
+    if (rc) return rc;
     plan->graph_n = n; plan->graph_params = params; plan->graph_x = x; plan->graph_infill_x = infill_x;
     plan->graph_infill_mask = infill_mask; plan->graph_collection = collection; plan->graph_metrics = metrics;
   }
   for (int i = 0; i < steps; ++i) {
-    SMD_CUDA(cudaGraphLaunch(plan->graph_exec, cs));
-    g_launches.fetch_add(plan->graph_nodes, std::memory_order_relaxed);
+    const int rc = plan->sample_graph.launch(cs);
+    if (rc) return rc;
   }
   if (cs != st) {
     SMD_CUDA(cudaEventRecord(plan->own_event, cs));
@@ -1279,40 +1252,24 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
   return SMD_OK;
 }
 
-int smd_threefry_normal(const uint32_t host_key[2], float* out, long long n, smd_stream_t stream) {
-  if (n < 0 || n > 0xFFFFFFFFll) { set_error("n out of range"); return SMD_ERR_INVALID; }
-  if (n == 0) return SMD_OK;
-  int blocks = static_cast<int>((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
-  threefry_normal_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(host_key[0], host_key[1], out,
-                                                                                static_cast<uint32_t>(n), 0u,
-                                                                                static_cast<uint32_t>(n));
-  CNT();
-  SMD_LAUNCH_CHECK("threefry_normal");
-  return SMD_OK;
-}
 int smd_threefry_normal_slice(const uint32_t host_key[2], float* out, long long n, long long first, long long total,
                               smd_stream_t stream) {
   if (n < 0 || first < 0 || first + n > total || total > 0xFFFFFFFFll) { set_error("slice out of range"); return SMD_ERR_INVALID; }
   if (n == 0) return SMD_OK;
-  int blocks = static_cast<int>((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
-  threefry_normal_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(host_key[0], host_key[1], out,
-                                                                                static_cast<uint32_t>(n),
-                                                                                static_cast<uint32_t>(first),
-                                                                                static_cast<uint32_t>(total));
-  CNT();
-  SMD_LAUNCH_CHECK("threefry_normal_slice");
+  launch_threefry_normal(host_key, out, static_cast<uint32_t>(n), static_cast<uint32_t>(first),
+                         static_cast<uint32_t>(total), static_cast<cudaStream_t>(stream));
+  SMD_LAUNCH_CHECK("threefry_normal");
   return SMD_OK;
+}
+int smd_threefry_normal(const uint32_t host_key[2], float* out, long long n, smd_stream_t stream) {
+  return smd_threefry_normal_slice(host_key, out, n, 0, n, stream);
 }
 int smd_threefry_uniform(const uint32_t host_key[2], float* out, long long n, float minval, float maxval,
                          smd_stream_t stream) {
   if (n < 0 || n > 0xFFFFFFFFll) { set_error("n out of range"); return SMD_ERR_INVALID; }
   if (n == 0) return SMD_OK;
-  int blocks = static_cast<int>((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
-  threefry_uniform_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(host_key[0], host_key[1], out,
-                                                                                 static_cast<uint32_t>(n), minval, maxval);
+  threefry_uniform_kernel<<<grid_stride_blocks(n), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      host_key[0], host_key[1], out, static_cast<uint32_t>(n), minval, maxval);
   CNT();
   SMD_LAUNCH_CHECK("threefry_uniform");
   return SMD_OK;

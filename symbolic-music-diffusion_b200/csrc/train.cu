@@ -107,7 +107,7 @@ int smd_clip_adam(float* params, float* grads, float* adam_m, float* adam_v, flo
                   float beta2, float eps, float ema_mu, float* scratch, float* grad_norm_out, smd_stream_t stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (n <= 0 || !scratch) { set_error("bad arguments"); return SMD_ERR_INVALID; }
-  const int blocks = 148 * 8;
+  const int blocks = kGridStrideMaxBlocks;
   auto al = [](const void* q, uintptr_t a) { return q == nullptr || (reinterpret_cast<uintptr_t>(q) % a) == 0; };
   const int vec_ok = al(params, 16) && al(grads, 16) && al(adam_m, 16) && al(adam_v, 16) && al(ema_or_null, 16) &&
                      al(bf16_shadow_or_null, 8);
@@ -126,7 +126,7 @@ int smd_clip_adam(float* params, float* grads, float* adam_m, float* adam_v, flo
 }
 
 int smd_ema_update(float* ema, const float* params, long long n, float mu, smd_stream_t stream) {
-  ema_kernel<<<148 * 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(ema, params, n, mu);
+  ema_kernel<<<kGridStrideMaxBlocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(ema, params, n, mu);
   g_launches.fetch_add(1);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { set_error(std::string("ema: ") + cudaGetErrorString(e)); return SMD_ERR_CUDA; }

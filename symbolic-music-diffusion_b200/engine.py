@@ -231,16 +231,22 @@ class Engine:
 
         With ``global_batch`` / ``first_row`` the result is rows [first_row, first_row + batch) of the draws of a
         global batch (data-parallel ranks consume slices of ONE threefry stream: DP(seed) == single-GPU(seed))."""
+        return self._objective_draws(self.lib.smd_ddpm_draws_sharded, key, batch, want_labels, global_batch, first_row,
+                                     continuous_noise)
+
+    def _objective_draws(self, fn, key, batch, want_labels, global_batch, first_row, continuous_noise,
+                         rademacher=False):
+        """(used (B,), eps[, v][, labels]) from the draws entry point ``fn``; v (the Rademacher projection vectors of
+        sliced score matching) with ``rademacher``."""
         dev = self._ws.device
         shape = (batch, self.seq_len, self.cfg.channels) if ARCHS[self.cfg.arch] == 0 else (batch, self.cfg.channels)
-        used = torch.empty((batch,), dtype=torch.float32, device=dev)
-        eps = torch.empty(shape, dtype=torch.float32, device=dev)
+        out = [torch.empty((batch,), dtype=torch.float32, device=dev)]
+        out += [torch.empty(shape, dtype=torch.float32, device=dev) for _ in range(2 if rademacher else 1)]
         labels = torch.empty((batch,), dtype=torch.int32, device=dev) if want_labels else None
         k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
-        _lib.check(self.lib.smd_ddpm_draws_sharded(self._plan, k, int(global_batch or batch), int(first_row), batch,
-                                                   1 if continuous_noise else 0, used.data_ptr(), eps.data_ptr(),
-                                                   _ptr(labels), self._stream()))
-        return (used, eps, labels) if want_labels else (used, eps)
+        _lib.check(fn(self._plan, k, int(global_batch or batch), int(first_row), batch, 1 if continuous_noise else 0,
+                      *[t.data_ptr() for t in out], _ptr(labels), self._stream()))
+        return tuple(out) + (labels,) if want_labels else tuple(out)
 
     # ------------------------------------------------------------------ NCSN family (SURVEY 8(f4))
     def dsm_setup(self, sigmas: np.ndarray) -> None:
@@ -251,16 +257,8 @@ class Engine:
     def dsm_draws(self, key, batch: int, want_labels: bool = False, global_batch: Optional[int] = None,
                   first_row: int = 0, continuous_noise: bool = False):
         """(used_sigma (B,), eps[, labels]) of denoising_score_matching_loss (utils/losses.py:146-164) on device."""
-        dev = self._ws.device
-        shape = (batch, self.seq_len, self.cfg.channels) if ARCHS[self.cfg.arch] == 0 else (batch, self.cfg.channels)
-        used = torch.empty((batch,), dtype=torch.float32, device=dev)
-        eps = torch.empty(shape, dtype=torch.float32, device=dev)
-        labels = torch.empty((batch,), dtype=torch.int32, device=dev) if want_labels else None
-        k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
-        _lib.check(self.lib.smd_dsm_draws(self._plan, k, int(global_batch or batch), int(first_row), batch,
-                                          1 if continuous_noise else 0, used.data_ptr(), eps.data_ptr(), _ptr(labels),
-                                          self._stream()))
-        return (used, eps, labels) if want_labels else (used, eps)
+        return self._objective_draws(self.lib.smd_dsm_draws, key, batch, want_labels, global_batch, first_row,
+                                     continuous_noise)
 
     def dsm_loss(self, x0: torch.Tensor, used_sigma: torch.Tensor, eps: torch.Tensor, want_pred: bool = False):
         x0 = _f32c(x0, "x0"); eps = _f32c(eps, "eps"); us = _f32c(used_sigma.reshape(-1), "used_sigma")
@@ -282,17 +280,8 @@ class Engine:
                   first_row: int = 0, continuous_noise: bool = False):
         """(used_sigma (B,), eps, v[, labels]) of sliced_score_matching_loss (utils/losses.py:203-223) on device; v holds
         the Rademacher (+-1) projection vectors.  Schedule: dsm_setup."""
-        dev = self._ws.device
-        shape = (batch, self.seq_len, self.cfg.channels) if ARCHS[self.cfg.arch] == 0 else (batch, self.cfg.channels)
-        used = torch.empty((batch,), dtype=torch.float32, device=dev)
-        eps = torch.empty(shape, dtype=torch.float32, device=dev)
-        v = torch.empty(shape, dtype=torch.float32, device=dev)
-        labels = torch.empty((batch,), dtype=torch.int32, device=dev) if want_labels else None
-        k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
-        _lib.check(self.lib.smd_ssm_draws(self._plan, k, int(global_batch or batch), int(first_row), batch,
-                                          1 if continuous_noise else 0, used.data_ptr(), eps.data_ptr(), v.data_ptr(),
-                                          _ptr(labels), self._stream()))
-        return (used, eps, v, labels) if want_labels else (used, eps, v)
+        return self._objective_draws(self.lib.smd_ssm_draws, key, batch, want_labels, global_batch, first_row,
+                                     continuous_noise, rademacher=True)
 
     def ssm_loss(self, x0: torch.Tensor, used_sigma: torch.Tensor, eps: torch.Tensor, v: torch.Tensor,
                  want_terms: bool = False):

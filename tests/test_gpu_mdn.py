@@ -156,32 +156,6 @@ def test_grads_are_reproducible_and_graph_replay_matches_eager(lib):
     assert torch.equal(l1, l2) and all(torch.equal(u, v) for u, v in zip(f1, f2))
 
 
-def test_graph_replay_equals_eager_subprocess(lib, tmp_path):
-    code = f"""
-import sys, numpy as np, torch
-sys.path.insert(0, {ROOT!r})
-from tests.test_gpu_mdn import _engine, _x
-eng, _ = _engine(8, training=True)
-eng.init_train_state()
-x = torch.from_numpy(_x(8, 7)).cuda()
-s = torch.cuda.Stream()
-with torch.cuda.stream(s):
-    for _ in range(3):
-        eng.compute_mdn_grads(x)
-s.synchronize()
-np.save(sys.argv[1], np.concatenate([eng.grads.cpu().numpy(), eng.loss_sum.cpu().numpy()]))
-"""
-    outs = []
-    for flag in ("1", "0"):
-        path = tmp_path / f"g{flag}.npy"
-        r = subprocess.run([sys.executable, "-c", code, str(path)], env=dict(os.environ, SMD_TRAIN_GRAPH=flag),
-                           capture_output=True, text=True, timeout=600, cwd=ROOT)
-        assert r.returncode == 0, r.stderr[-3000:]
-        outs.append(np.load(path))
-    np.testing.assert_allclose(outs[0][:-1], outs[1][:-1], rtol=1e-4, atol=1e-7)
-    assert outs[0][-1] == outs[1][-1]
-
-
 def test_other_entry_points_reject_an_mdn_plan(lib):
     from smd_b200 import Engine, ModelConfig
     eng, _ = _engine(2, training=True)
