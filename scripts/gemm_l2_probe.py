@@ -15,7 +15,10 @@ what this card reaches on the shape.
 Each result line is JSON; `sha` is a hash of the GEMM's fp32 / bf16 outputs (not of the row statistics, whose atomics
 make the last bits order dependent), so two libraries can be compared bit for bit.
 
-  python scripts/gemm_l2_probe.py [--root TREE] [--out FILE] [--iters N] [--tokens 4096 32000] [--bn 128 64]
+  python scripts/gemm_l2_probe.py [--root TREE] [--out FILE] [--iters N] [--tokens 4096 32000] [--bn 128 256]
+
+--bn 256 asks for the wide layout (128 x 256 tiles), which every case here gets; its `sha` must equal the BN = 128
+line's of the same case.
 
 --root imports smd_b200 (and its libsmd.so) from another checkout of this repository, e.g. a build of the parent
 commit, so that two builds are timed by the same script.
@@ -58,7 +61,7 @@ def main():
     ap.add_argument("--out", default=None)
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--tokens", type=int, nargs="+", default=[4096, 32000])
-    ap.add_argument("--bn", type=int, nargs="+", default=[128])
+    ap.add_argument("--bn", type=int, nargs="+", default=[128, 256])
     ap.add_argument("--cases", nargs="+", default=list(CASES))
     args = ap.parse_args()
     sys.path.insert(0, os.path.abspath(args.root))

@@ -10,7 +10,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "symbolic-music-diffusion_b200", "libsmd.so")
-KEYS = ["HGMMA", "UTMALDG", "UTMASTG", "SYNCS", "HMMA", "MUFU.TANH", "LDGSTS", "UBLKCP", "ACQBULK", "RED", "ATOM",
+KEYS = ["HGMMA", "HGMMA.64x256x16", "UTMALDG", "UTMASTG", "SYNCS", "HMMA", "MUFU.TANH", "LDGSTS", "UBLKCP", "ACQBULK", "RED", "ATOM",
         "USETMAXREG", "STL", "LDL"]
 
 
@@ -33,6 +33,8 @@ def main():
         if not m:
             continue
         op = m.group(1)
+        if op.startswith("HGMMA"):   # the mnemonic match stops at the shape's lower-case x: read the whole token
+            op = line[m.start(1):].split()[0]
         for k in KEYS:
             if op == k or op.startswith(k + ".") or (k == "MUFU.TANH" and op.startswith("MUFU.TANH")):
                 counts[cur][k] += 1

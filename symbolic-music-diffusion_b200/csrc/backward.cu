@@ -16,15 +16,17 @@ int pick_splits_side(int m_rows, int n_cols, int BN, int num_kb) {
   return s;
 }
 
-// dW GEMM: A = X (MN-major [tokens][in]), B = G (MN-major [tokens][out]) -> out_f32 [in][out]
-static bool make_dw(GemmOp* op, const void* X, int in_f, const void* G, int g_cols, int out_f, uint64_t rows) {
-  const int BN = std::min((out_f + 63) / 64 * 64, kBNMax);
+// dW GEMM: A = X (MN-major [tokens][in]), B = G (MN-major [tokens][out]) -> out_f32 [in][out].  wide: ask for the
+// 128 x 256 layout (the res-block GEMMs)
+static bool make_dw(GemmOp* op, const void* X, int in_f, const void* G, int g_cols, int out_f, uint64_t rows,
+                    bool wide = false) {
+  const int BN = wide ? kBNWide : std::min((out_f + 63) / 64 * 64, kBNMax);
   return make_gemm_op(op, X, static_cast<uint64_t>(in_f), G, static_cast<uint64_t>(g_cols), out_f,
                       static_cast<int>(rows), BN, 1, 1);
 }
 // dX GEMM: A = G (K-major [tokens][out]), B = W plain (in,out) = [N=in][K=out] -> [tokens][in]
-static bool make_dx(GemmOp* op, const void* G, int out_f, const void* W, int in_f, uint64_t rows) {
-  return make_gemm_op(op, G, rows, W, static_cast<uint64_t>(in_f), in_f, out_f, choose_bn(in_f), 0, 0);
+static bool make_dx(GemmOp* op, const void* G, int out_f, const void* W, int in_f, uint64_t rows, bool wide = false) {
+  return make_gemm_op(op, G, rows, W, static_cast<uint64_t>(in_f), in_f, out_f, wide ? kBNWide : choose_bn(in_f), 0, 0);
 }
 
 int train_bind(smd_plan* p) {
@@ -41,10 +43,10 @@ int train_bind(smd_plan* p) {
   const uint64_t Bp = (static_cast<uint64_t>(c.max_batch) + 127) / 128 * 128;
   for (int k = 0; k < K; ++k) {
     const BlockParams& bp = par.block[k];
-    if (!make_dw(&ts.dWb[k], B16(w.act[2 * k + 1]), Md, B16(ts.du16[k + 1]), Md, Md, Mp)) return SMD_ERR_CUDA;
-    if (!make_dx(&ts.dXb[k], B16(ts.du16[k + 1]), Md, p->wsh(bp.b.kernel), Md, Mp)) return SMD_ERR_CUDA;
-    if (!make_dw(&ts.dWa[k], B16(w.act[2 * k]), Md, B16(ts.dr16t[k]), Md, Md, Mp)) return SMD_ERR_CUDA;
-    if (!make_dx(&ts.dXa[k], B16(ts.dr16t[k]), Md, p->wsh(bp.a.kernel), Md, Mp)) return SMD_ERR_CUDA;
+    if (!make_dw(&ts.dWb[k], B16(w.act[2 * k + 1]), Md, B16(ts.du16[k + 1]), Md, Md, Mp, true)) return SMD_ERR_CUDA;
+    if (!make_dx(&ts.dXb[k], B16(ts.du16[k + 1]), Md, p->wsh(bp.b.kernel), Md, Mp, true)) return SMD_ERR_CUDA;
+    if (!make_dw(&ts.dWa[k], B16(w.act[2 * k]), Md, B16(ts.dr16t[k]), Md, Md, Mp, true)) return SMD_ERR_CUDA;
+    if (!make_dx(&ts.dXa[k], B16(ts.dr16t[k]), Md, p->wsh(bp.a.kernel), Md, Mp, true)) return SMD_ERR_CUDA;
     if (p->mdn()) continue;   // no FiLM generator
     if (!make_dw(&ts.dWss[k], B16(ts.e2_16), 512, B16(ts.dss16), 2 * Md, 2 * Md, Bp)) return SMD_ERR_CUDA;
     if (!make_dx(&ts.dXss[k], B16(ts.dss16), 2 * Md, p->wsh(bp.film.ss.kernel), 512, Bp)) return SMD_ERR_CUDA;
@@ -80,10 +82,10 @@ int train_bind(smd_plan* p) {
     ts.tdWb.resize(K); ts.tdXb.resize(K); ts.tdWa.resize(K); ts.tdXa.resize(K);
     for (int k = 0; k < K; ++k) {
       const BlockParams& bp = par.block[k];
-      if (!make_dw(&ts.tdWb[k], B16(w.actt[2 * k + 1]), Md, B16(ts.dut16[k + 1]), Md, Md, Mp)) return SMD_ERR_CUDA;
-      if (!make_dx(&ts.tdXb[k], B16(ts.dut16[k + 1]), Md, p->wsh(bp.b.kernel), Md, Mp)) return SMD_ERR_CUDA;
-      if (!make_dw(&ts.tdWa[k], B16(w.actt[2 * k]), Md, B16(ts.drt16[k]), Md, Md, Mp)) return SMD_ERR_CUDA;
-      if (!make_dx(&ts.tdXa[k], B16(ts.drt16[k]), Md, p->wsh(bp.a.kernel), Md, Mp)) return SMD_ERR_CUDA;
+      if (!make_dw(&ts.tdWb[k], B16(w.actt[2 * k + 1]), Md, B16(ts.dut16[k + 1]), Md, Md, Mp, true)) return SMD_ERR_CUDA;
+      if (!make_dx(&ts.tdXb[k], B16(ts.dut16[k + 1]), Md, p->wsh(bp.b.kernel), Md, Mp, true)) return SMD_ERR_CUDA;
+      if (!make_dw(&ts.tdWa[k], B16(w.actt[2 * k]), Md, B16(ts.drt16[k]), Md, Md, Mp, true)) return SMD_ERR_CUDA;
+      if (!make_dx(&ts.tdXa[k], B16(ts.drt16[k]), Md, p->wsh(bp.a.kernel), Md, Mp, true)) return SMD_ERR_CUDA;
     }
     if (!make_gemm_op(&ts.tdWout, B16(w.actt[2 * K]), static_cast<uint64_t>(Md), B16(ts.dpredt16), static_cast<uint64_t>(Cp),
                       C, static_cast<int>(Mp), std::min(Cp, kBNMax), 1, 1))

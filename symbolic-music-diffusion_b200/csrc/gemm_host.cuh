@@ -60,7 +60,10 @@ inline int choose_bn(int N) {
 }
 
 // A: K-major [a_rows][K] (a_mn=0) or MN-major [K][a_rows] (a_mn=1); same for B with N rows.
-// A requested BN above kBNMax is lowered to kBNMax (the widest accumulator tile).
+// BN = kBNWide asks for the wide layout (GemmSmemWide).  It is kept for N % 256 == 0 and K > 256, where gemm_kind may
+// run that layout; any other BN above kBNMax is lowered to kBNMax.  The tensor maps do not depend on the choice (B's
+// box is at most 128 rows; the wide kernel loads its 256 rows as two boxes), so a launch that gemm_kind does not give
+// the wide layout runs the same op with 128-wide tiles.
 // b_pitch: row pitch (elements) of an MN-major B that is a column slice of a wider matrix (0: b_rows_total)
 inline bool make_gemm_op(GemmOp* op, const void* A, uint64_t a_rows, const void* B, uint64_t b_rows_total, int N,
                          int K, int BN, int a_mn, int b_mn, uint64_t k_rows_a = 0, uint64_t k_rows_b = 0,
@@ -71,7 +74,7 @@ inline bool make_gemm_op(GemmOp* op, const void* A, uint64_t a_rows, const void*
                       b_rows_total, N, K, BN, a_mn, b_mn, k_rows_a, k_rows_b, 0, b_pitch)) return false;
     op->tmA_lo = lo.tmA; op->tmB_lo = lo.tmB; op->has_lo = true;
   }
-  if (BN > kBNMax) BN = kBNMax;
+  if (BN > kBNMax && !(BN == kBNWide && N % kBNWide == 0 && K > 256)) BN = kBNMax;
   op->N = N; op->K = K; op->BN = BN; op->a_mn = a_mn; op->b_mn = b_mn; op->k_splits = 1;
   if (K % 64 != 0) { set_error("GEMM K must be a multiple of 64"); return false; }
   if (BN % 16 != 0 || BN < 16) { set_error("bad BN " + std::to_string(BN)); return false; }
@@ -80,7 +83,7 @@ inline bool make_gemm_op(GemmOp* op, const void* A, uint64_t a_rows, const void*
   if (!a_mn) ok = make_tmap_bf16(&op->tmA, A, a_rows, static_cast<uint64_t>(K), 128);
   else ok = make_tmap_bf16(&op->tmA, A, k_rows_a ? k_rows_a : static_cast<uint64_t>(K), a_rows, 64);
   if (!ok) return false;
-  if (!b_mn) ok = make_tmap_bf16(&op->tmB, B, b_rows_total, static_cast<uint64_t>(K), static_cast<uint32_t>(BN));
+  if (!b_mn) ok = make_tmap_bf16(&op->tmB, B, b_rows_total, static_cast<uint64_t>(K), static_cast<uint32_t>(BN < kBNMax ? BN : kBNMax));
   else ok = make_tmap_bf16(&op->tmB, B, k_rows_b ? k_rows_b : static_cast<uint64_t>(K), b_rows_total, 64, b_pitch);
   return ok;
 }
@@ -160,12 +163,34 @@ inline cudaError_t launch_persistent(Kern kern, int tiles, int threads, int smem
   return cudaLaunchKernelEx(&cfg, kern, args...);
 }
 
-// The GEMM instantiation a launch runs: epilogue feature set and thread layout (GemmSmem's kEW).
+// The GEMM instantiation a launch runs: epilogue feature set and thread layout (GemmSmem's kEW, or the wide layout).
 struct GemmKind {
   uint32_t flags;
   int ew;
+  bool wide = false;   // 128 x 256 tiles (GemmSmemWide); ew is then unused
 };
+// the 128-wide tiles a launch of an op built with BN = kBNWide runs when gemm_kind does not give it the wide layout
+inline GemmOp narrow_op(const GemmOp& op) {
+  GemmOp o = op;
+  if (o.BN > kBNMax) o.BN = kBNMax;
+  return o;
+}
 inline GemmKind gemm_kind(const GemmOp& op, int M, const GemmEpilogue& ep) {
+  if (op.BN > kBNMax) {
+    // Wide layout: ops built with BN = kBNWide (the res-block GEMMs), long K, one split, and a clean epilogue of one of
+    // two kinds: fp32 out (dW) or bf16 out without activation (res-block a, dX).  Its epilogue runs on the MMA warps
+    // from registers, not overlapped with MMA work.  The residual kind (res-block b) reads 128 KB of fp32 residual per
+    // tile; in the wide layout that latency is exposed and costs more than the faster K loop gains, so it keeps the
+    // dedicated-epilogue layout.  A launch whose 128-wide tiles fit in one round keeps them: halving the CTA count
+    // would leave SMs idle.
+    if (ep.lo_delta == 0 && op.K > 256 && op.N % kBNWide == 0 && gemm_k_splits(op) == 1 && epi_clean(op, ep) &&
+        gemm_tiles(narrow_op(op), M) > device_sm_count()) {
+      const uint32_t need = epi_needs(ep);
+      for (const uint32_t kind : {kEpiF32, kEpiBf16})
+        if ((need & ~kind) == 0) return {kind, 8, true};
+    }
+    return gemm_kind(narrow_op(op), M, ep);
+  }
   if (ep.lo_delta != 0) return {kEpiStrict, 8};   // strict-precision mode (bf16x3)
   const uint32_t need = epi_needs(ep);
   if (epi_clean(op, ep)) {
@@ -189,7 +214,10 @@ inline GemmKind gemm_kind(const GemmOp& op, int M, const GemmEpilogue& ep) {
 // Slots per row of the per-tile statistics partials (GemmEpilogue::stats_part) the launch writes: one per n-tile and
 // column group of its instantiation.
 inline int stats_slots_for(const GemmOp& op, int M, const GemmEpilogue& ep) {
-  return ((op.N + op.BN - 1) / op.BN) * epi_groups(gemm_kind(op, M, ep).ew);
+  const GemmKind k = gemm_kind(op, M, ep);
+  if (k.wide) return (op.N / kBNWide) * GemmSmemWide::kEpiGroups;
+  const GemmOp o = narrow_op(op);
+  return ((o.N + o.BN - 1) / o.BN) * epi_groups(k.ew);
 }
 
 template <uint32_t kF, int kEW = 8>
@@ -215,12 +243,32 @@ inline cudaError_t launch_gemm_ew(int ew, const GemmOp& op, int M, const GemmEpi
                   : ew == 4 ? launch_gemm_inst<kF, 4>(op, M, ep, st) : launch_gemm_inst<kF, 8>(op, M, ep, st);
 }
 
-inline cudaError_t launch_gemm(const GemmOp& op, int M, const GemmEpilogue& ep, cudaStream_t st) {
+template <uint32_t kF>
+inline cudaError_t launch_gemm_wide(const GemmOp& op, int M, const GemmEpilogue& ep, cudaStream_t st) {
+  using SM = GemmSmemWide;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_wide_kernel<kF>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         SM::kTotal);
+    if (e != cudaSuccess) return e;
+    attr_set = true;
+  }
+  GemmShape sh;
+  sh.M = M; sh.N = op.N; sh.K = op.K; sh.BN = kBNWide; sh.a_mn = op.a_mn; sh.b_mn = op.b_mn; sh.k_splits = 1;
+  const int tiles = ((M + kBM - 1) / kBM) * (op.N / kBNWide);
+  return launch_persistent(gemm_bf16_wgmma_wide_kernel<kF>, tiles, SM::kThreads, SM::kTotal, st, op.tmA, op.tmB, sh, ep);
+}
+
+inline cudaError_t launch_gemm(const GemmOp& wop, int M, const GemmEpilogue& ep, cudaStream_t st) {
+  const GemmKind k = gemm_kind(wop, M, ep);
+  if (k.wide) {
+    return k.flags == kEpiF32 ? launch_gemm_wide<kEpiF32>(wop, M, ep, st) : launch_gemm_wide<kEpiBf16>(wop, M, ep, st);
+  }
+  const GemmOp op = narrow_op(wop);
   // full-row LayerNorm needs the whole row in one tile (N <= BN; BN is at most kBNMax)
   if (ep.ln_gamma != nullptr && op.N > op.BN) return cudaErrorInvalidValue;
   // the K splits of a tile add into the same output elements
   if (gemm_k_splits(op) > 1 && !ep.atomic_out) return cudaErrorInvalidValue;
-  const GemmKind k = gemm_kind(op, M, ep);
   switch (k.flags) {
     case kEpiStrict: return launch_gemm_inst<kEpiStrict>(op, M, ep, st);
     case kEpiF32: return launch_gemm_ew<kEpiF32>(k.ew, op, M, ep, st);

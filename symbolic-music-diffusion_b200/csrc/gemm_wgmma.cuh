@@ -5,7 +5,8 @@
 //
 //   D[M,N] = A[M,K] * B[N,K]^T     (both operands may independently be K-major or MN-major in global memory)
 //
-// One CTA per 128 x BN tile (BN <= 128).  Two thread layouts (kEW below):
+// One CTA per 128 x BN tile (BN <= 128; the wide layout at the end of this file, gemm_bf16_wgmma_wide_kernel, runs
+// 128 x 256 tiles for the res-block GEMMs).  Two thread layouts of the 128-wide kernel (kEW below):
 //   * dedicated epilogue (kEW = 4, 512 threads): warpgroup 0 is the TMA producer, warpgroups 1 and 2 only run the K
 //     loops and store their accumulators to `acc_tile`, warpgroup 3 runs the epilogue.  The accumulator hand-off goes
 //     through two mbarriers (acc_full / acc_empty), so the MMA warps start tile i + 1 while the epilogue warps still
@@ -46,6 +47,9 @@ static constexpr uint32_t kEpiAct = F_BIAS | F_ACT | F_BF16 | F_PRE | F_STATS;  
 static constexpr uint32_t kEpiLn = F_BIAS | F_RES | F_F32 | F_LN | F_BF16;        // attention out / FFN down + LayerNorm
 static constexpr uint32_t kEpiGG = F_GG | F_BF16;                                 // FFN backward (x gelu')
 static constexpr uint32_t kEpiAtomic = F_F32 | F_ATOMIC;                          // split-K weight gradients
+// kEpiAct without the activation: the wide layout's bf16 kind (res-block a, dX).  Its epilogue is unrolled over all
+// 128 accumulators of a thread, and a runtime activation switch there would triple the code on the MMA warps.
+static constexpr uint32_t kEpiBf16 = kEpiAct & ~F_ACT;
 
 struct GemmEpilogue {
   const float* bias;            // [N] or null
@@ -83,6 +87,7 @@ struct GemmShape {
 static constexpr int kBM = 128;
 static constexpr int kBK = 64;
 static constexpr int kBNMax = 128;                 // widest n-tile: one m64n128 wgmma per consumer warpgroup
+static constexpr int kBNWide = 256;                // n-tile of the wide layout (GemmSmemWide): one m64n256 wgmma
 // floats per staged accumulator row: unpadded, the 16-byte chunks of each row are XOR-swizzled instead (acc_chunk), which
 // leaves room in shared memory for a fourth operand stage in the 8-epilogue-warp kinds
 static constexpr int kAccPitch = kBNMax;
@@ -350,11 +355,13 @@ __device__ __forceinline__ void ln_pack(const float (&v)[32], float mean, float 
   }
 }
 
-// the K loop of one warpgroup: rows [64 wg, 64 wg + 64) of the tile, all kBNMax columns
-template <int kTA, int kTB>
-__device__ __forceinline__ void gemm_mainloop(float (&d)[64], uint8_t* smem, int stage_bytes, int a_bytes, int stages,
+// the K loop of one warpgroup: rows [64 wg, 64 wg + 64) of the tile, all kN columns (kBNMax, or kBNWide for the
+// wide layout: the B tile is then 256 K-major rows or four 64-column MN blocks, same descriptor strides)
+template <int kTA, int kTB, int kN = kBNMax>
+__device__ __forceinline__ void gemm_mainloop(float (&d)[kN / 2], uint8_t* smem, int stage_bytes, int a_bytes, int stages,
                                               uint64_t* full_bar, uint64_t* empty_bar, int& stage, uint32_t& phase,
                                               int nkb, uint32_t wg, bool releaser) {
+  static_assert(kN == 128 || kN == 256, "one m64nNk16 wgmma per k16 step");
   // per-k16 advance of the descriptor start address (bytes): 32 B inside a K-major row, two 8-row atoms MN-major
   const uint32_t a_kadv = kTA ? 2048u : 32u, b_kadv = kTB ? 2048u : 32u;
   const uint32_t a_lbo = kTA ? 8192u : 0u, b_lbo = kTB ? 8192u : 0u;
@@ -365,9 +372,12 @@ __device__ __forceinline__ void gemm_mainloop(float (&d)[64], uint8_t* smem, int
     const uint32_t sB = smem_u32(smem + stage * stage_bytes + a_bytes);
     wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < kBK / 16; ++k)
-      wgmma_m64n128k16_bf16<kTA, kTB>(d, make_smem_desc_sw128(sA + k * a_kadv, a_lbo, 1024u),
-                                      make_smem_desc_sw128(sB + k * b_kadv, b_lbo, 1024u), (kb | k) != 0 ? 1u : 0u);
+    for (int k = 0; k < kBK / 16; ++k) {
+      const uint64_t ad = make_smem_desc_sw128(sA + k * a_kadv, a_lbo, 1024u);
+      const uint64_t bd = make_smem_desc_sw128(sB + k * b_kadv, b_lbo, 1024u);
+      if constexpr (kN == 256) wgmma_m64n256k16_bf16<kTA, kTB>(d, ad, bd, (kb | k) != 0 ? 1u : 0u);
+      else wgmma_m64n128k16_bf16<kTA, kTB>(d, ad, bd, (kb | k) != 0 ? 1u : 0u);
+    }
     wgmma_commit();
     wgmma_wait<1>();                       // the previous k block's MMAs are done: its slot can be refilled
     if (prev >= 0 && releaser) mbar_arrive(&empty_bar[prev]);
@@ -878,6 +888,222 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 
   // ===================== teardown =====================
   __syncwarp();  // reconverge single-lane roles before the block barrier
+  __syncthreads();
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Wide layout: 128 x 256 tiles for the long-K res-block GEMMs (N % 256 == 0, one K split, the kEpiF32 / kEpiBf16
+// kinds with a clean epilogue).  384 threads: warpgroup 0 is the TMA producer, warpgroups 1 and 2 each issue
+// one m64n256k16 per k16 step into 128 fp32 accumulator registers per thread and then run the epilogue straight from
+// those registers, while the producer streams the next tile's operands into the ring.
+//
+// Against the 128 x 128 layouts: both consumer warpgroups read one shared B tile twice as wide, so a k16 step does
+// twice the MMA work per byte of B read from shared memory (51 instead of 43 FLOP per shared-memory byte), and the CTA
+// moves 87 instead of 64 FLOP per byte from L2.  There is no room to stage a 128 KB fp32 tile next to a useful ring, so
+// nothing is staged: fp32 pairs are stored as the fragment holds them (a quad covers a 32-byte sector), bf16 pairs are
+// first transposed inside the quad of lanes that holds a row, so that each lane stores a whole 16-byte octet.  The epilogue is not overlapped with MMA work, which the long K loop amortises for
+// these kinds; a fp32 residual read (kEpiF32Res) would expose its latency on the MMA warps and stays on the
+// dedicated-epilogue layout.
+struct GemmSmemWide {
+  static constexpr int kABytes = kBM * kBK * 2;            // 16 KB
+  static constexpr int kBBytes = kBNWide * kBK * 2;        // 32 KB
+  static constexpr int kStageBytes = kABytes + kBBytes;    // 48 KB
+  static constexpr int kBarBytes = 256;
+  static constexpr int kMaxSmem = GemmSmem<8>::kMaxSmem;
+  static constexpr int kStages = (kMaxSmem - 1024 - kBarBytes) / kStageBytes;
+  static constexpr int kTotal = kStages * kStageBytes + kBarBytes + 1024;
+  static constexpr int kThreads = 384;
+  static constexpr int kEpiGroups = 1;   // one statistics slot per (row, n-tile): the quad of a row adds its partials
+  // setmaxnreg budgets: the CTA starts with 65536 / 384 = 170 registers per thread (one CTA per SM)
+  static constexpr int kProdRegs = 40, kMmaRegs = 232;
+  static_assert(kProdRegs + 2 * kMmaRegs <= 3 * 170, "register budgets exceed the CTA's file");
+  static_assert(kStages == 4, "the wide GEMM ring should hold four 48 KB stages (as many k blocks as eight 32 KB ones)");
+  static_assert(kTotal <= kMaxSmem, "shared memory");
+  static_assert(2 * kStages <= kBarBytes / 8, "mbarriers do not fit their region");
+};
+
+// 4 x 4 transpose inside each quad of lanes (q = lane & 3): lane q holds x[o], the column pair q of octet o; it gets
+// y[r], the column pair r of octet q (lane r's x[q]).  Three xor shuffles; the indices are selected, not addressed, so
+// everything stays in registers.  Executed by the whole warp.
+__device__ __forceinline__ void quad_transpose(const uint32_t (&x)[4], uint32_t (&y)[4], uint32_t q) {
+  auto pick = [](const uint32_t (&v)[4], uint32_t i) { return i == 0 ? v[0] : i == 1 ? v[1] : i == 2 ? v[2] : v[3]; };
+  uint32_t got[4];
+  got[0] = pick(x, q);
+#pragma unroll
+  for (uint32_t s = 1; s < 4; ++s) got[s] = __shfl_xor_sync(0xffffffffu, pick(x, q ^ s), s);   // lane q ^ s's x[q]
+#pragma unroll
+  for (uint32_t r = 0; r < 4; ++r) y[r] = pick(got, r ^ q);
+}
+
+template <uint32_t kF>
+__global__ void __launch_bounds__(GemmSmemWide::kThreads, 1)
+gemm_bf16_wgmma_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                            const GemmShape sh, const __grid_constant__ GemmEpilogue ep) {
+  using SM = GemmSmemWide;
+  static_assert((kF & ~(kEpiF32 | kEpiBf16)) == 0, "the wide layout runs the kEpiF32 / kEpiBf16 epilogues only");
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SM::kStages * SM::kStageBytes);   // [kStages]
+  uint64_t* empty_bar = full_bar + SM::kStages;                                              // [kStages]
+
+  const uint32_t warp = threadIdx.x >> 5;
+  const uint32_t lane = threadIdx.x & 31;
+  const int num_m = (sh.M + kBM - 1) / kBM;
+  const int num_n = sh.N / kBNWide;
+  const int num_tiles = num_m * num_n;
+  const int nkb = sh.K / kBK;
+
+  pdl_trigger();
+  if (warp == 0 && elect_one()) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+  }
+  if (warp == 1 && elect_one()) {
+    for (int i = 0; i < SM::kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);   // one arrival per MMA warp
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (warp < 4) {
+    // ===================== TMA producer (one lane of warp 0) =====================
+    setmaxnreg_dec<SM::kProdRegs>();
+    if (warp == 0 && elect_one()) {
+      int stage = 0; uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m_row0 = (tile / num_n) * kBM, n_row0 = (tile % num_n) * kBNWide;
+        for (int kb = 0; kb < nkb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1u);
+          uint8_t* sA = smem + stage * SM::kStageBytes;
+          uint8_t* sB = sA + SM::kABytes;
+          const int k0 = kb * kBK;
+          mbar_arrive_expect_tx(&full_bar[stage], static_cast<uint32_t>(SM::kStageBytes));
+          if (!sh.a_mn) tma_load_2d(&tmA, &full_bar[stage], sA, k0, m_row0);
+          else
+            for (int j = 0; j < kBM / 64; ++j) tma_load_2d(&tmA, &full_bar[stage], sA + j * 8192, m_row0 + 64 * j, k0);
+          // B's tensor map has the 128-row (K-major) / 64-column (MN-major) box of the narrow layouts
+          if (!sh.b_mn)
+            for (int j = 0; j < kBNWide / 128; ++j)
+              tma_load_2d(&tmB, &full_bar[stage], sB + j * 16384, k0, n_row0 + 128 * j);
+          else
+            for (int j = 0; j < kBNWide / 64; ++j) tma_load_2d(&tmB, &full_bar[stage], sB + j * 8192, n_row0 + 64 * j, k0);
+          if (++stage == SM::kStages) { stage = 0; phase ^= 1u; }
+        }
+      }
+    }
+  } else {
+    // ===================== MMA + epilogue warpgroups =====================
+    setmaxnreg_inc<SM::kMmaRegs>();
+    constexpr bool H_BIAS = (kF & F_BIAS) != 0, H_F32 = (kF & F_F32) != 0, H_BF16 = (kF & F_BF16) != 0;
+    constexpr bool H_PRE = (kF & F_PRE) != 0, H_STATS = (kF & F_STATS) != 0;
+    const bool has_bias = H_BIAS && ep.bias != nullptr;
+    const bool has_f32 = H_F32 && ep.out_f32 != nullptr;
+    const bool has_bf16 = H_BF16 && ep.out_bf16 != nullptr;
+    const bool has_pre = H_PRE && ep.out_bf16_pre != nullptr;
+    const bool has_stats = H_STATS && ep.row_stats != nullptr;
+    const uint32_t wg = (warp - 4u) >> 2;
+    // this thread's fragment (wgmma_m64n256k16_bf16): rows r_frag and r_frag + 8 of the tile (h = 0, 1), columns
+    // 8 j + c_frag + {0, 1} for the 32 column octets j: d[4 j + 2 h + e]
+    const int r_frag = static_cast<int>(wg * 64u + (warp & 3u) * 16u + (lane >> 2));
+    const int c_frag = 2 * static_cast<int>(lane & 3u);
+    int stage = 0; uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      float d[kBNWide / 2];
+      if (!sh.a_mn && !sh.b_mn) gemm_mainloop<0, 0, kBNWide>(d, smem, SM::kStageBytes, SM::kABytes, SM::kStages, full_bar, empty_bar, stage, phase, nkb, wg, lane == 0);
+      else if (!sh.a_mn) gemm_mainloop<0, 1, kBNWide>(d, smem, SM::kStageBytes, SM::kABytes, SM::kStages, full_bar, empty_bar, stage, phase, nkb, wg, lane == 0);
+      else if (!sh.b_mn) gemm_mainloop<1, 0, kBNWide>(d, smem, SM::kStageBytes, SM::kABytes, SM::kStages, full_bar, empty_bar, stage, phase, nkb, wg, lane == 0);
+      else gemm_mainloop<1, 1, kBNWide>(d, smem, SM::kStageBytes, SM::kABytes, SM::kStages, full_bar, empty_bar, stage, phase, nkb, wg, lane == 0);
+
+      const int n_tile = tile % num_n;
+      const int m0 = (tile / num_n) * kBM, n0 = n_tile * kBNWide;
+      const int row[2] = {m0 + r_frag, m0 + r_frag + 8};
+      const bool ok[2] = {row[0] < sh.M, row[1] < sh.M};
+      // per-element operations in the order of the 128-wide epilogue (acc + bias, then the outputs), so every fp32 /
+      // bf16 output is bit-identical to that layout's.  Four octets at a time; for the bf16 outputs the quad of a row
+      // transposes its packed column pairs (quad_transpose) so that each lane stores one whole octet (16 B) and the
+      // quad 64 contiguous bytes of the row: whole 32-byte sectors instead of 16-byte halves.
+      const uint32_t q = lane & 3u;
+      float s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
+#pragma unroll
+      for (int j0 = 0; j0 < kBNWide / 8; j0 += 4) {
+        float2 b[4];
+#pragma unroll
+        for (int o = 0; o < 4; ++o)
+          b[o] = has_bias ? __ldg(reinterpret_cast<const float2*>(ep.bias + n0 + 8 * (j0 + o) + c_frag))
+                          : make_float2(0.f, 0.f);
+        const int colq = n0 + 8 * (j0 + static_cast<int>(q));   // the octet this lane stores
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float v0[4], v1[4];
+#pragma unroll
+          for (int o = 0; o < 4; ++o) {
+            v0[o] = d[4 * (j0 + o) + 2 * h]; v1[o] = d[4 * (j0 + o) + 2 * h + 1];
+            if (has_bias) add_pair(v0[o], v1[o], b[o].x, b[o].y);
+            if constexpr (H_STATS) {
+              s1[h] += v0[o] + v1[o];
+              s2[h] = fmaf(v1[o], v1[o], fmaf(v0[o], v0[o], s2[h]));
+            }
+          }
+          const size_t ro = static_cast<size_t>(row[h]);
+          if constexpr (H_F32) {
+            // fp32 pairs go out as they are: a quad already covers a whole 32-byte sector per octet
+            if (has_f32 && ok[h]) {
+#pragma unroll
+              for (int o = 0; o < 4; ++o)
+                *reinterpret_cast<float2*>(ep.out_f32 + ro * ep.ld_f32 + n0 + 8 * (j0 + o) + c_frag) = make_float2(v0[o], v1[o]);
+            }
+          }
+          if constexpr (H_PRE) {
+            if (has_pre) {
+              uint32_t x[4], y[4];
+#pragma unroll
+              for (int o = 0; o < 4; ++o) x[o] = pack_bf16x2(v0[o], v1[o]);
+              quad_transpose(x, y, q);
+              if (ok[h]) *reinterpret_cast<uint4*>(ep.out_bf16_pre + ro * ep.ld_bf16 + colq) = make_uint4(y[0], y[1], y[2], y[3]);
+            }
+          }
+          if constexpr (H_BF16) {
+            if (has_bf16) {
+              uint32_t x[4], y[4];
+#pragma unroll
+              for (int o = 0; o < 4; ++o) x[o] = pack_bf16x2(v0[o], v1[o]);
+              quad_transpose(x, y, q);
+              if (ok[h]) *reinterpret_cast<uint4*>(ep.out_bf16 + ro * ep.ld_bf16 + colq) = make_uint4(y[0], y[1], y[2], y[3]);
+            }
+          }
+        }
+      }
+      if constexpr (H_STATS) {
+        if (has_stats) {
+          // the four lanes of a quad hold a row's 256 columns: fixed butterfly, then lane 0 of the quad stores
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            s1[h] += __shfl_xor_sync(0xffffffffu, s1[h], 1);
+            s2[h] += __shfl_xor_sync(0xffffffffu, s2[h], 1);
+            s1[h] += __shfl_xor_sync(0xffffffffu, s1[h], 2);
+            s2[h] += __shfl_xor_sync(0xffffffffu, s2[h], 2);
+          }
+          if ((lane & 3u) == 0) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              if (!ok[h]) continue;
+              if (ep.stats_part != nullptr) {
+                reinterpret_cast<float2*>(ep.stats_part)[static_cast<size_t>(row[h]) * num_n + n_tile] =
+                    make_float2(s1[h], s2[h]);
+              } else {
+                atomicAdd(ep.row_stats + 2 * static_cast<size_t>(row[h]), s1[h]);
+                atomicAdd(ep.row_stats + 2 * static_cast<size_t>(row[h]) + 1, s2[h]);
+              }
+            }
+          }
+        }
+      }
+    }
+  }
+  __syncwarp();
   __syncthreads();
 }
 

@@ -148,6 +148,7 @@ static void build_workspace(smd_plan* p) {
   // per-row LayerNorm (sum, sumsq) of the 2K+1 wide LayerNorms; zeroed once per forward
   w.stats = ws_add(p, "stats", (2 * K + 1) * Mp * 2 * 4);
   // per-tile partial sums of the GEMM feeding the next wide LayerNorm: [row][n_tile * (2 or 3) + column group][2]
+  // (sized for 128-wide tiles with three groups; the wide layout writes one slot per 256-wide tile)
   w.stats_part = ws_add(p, "stats_part", Mp * ((Md + kBNMax - 1) / kBNMax * 3) * 2 * 4);
   // FiLM generator
   w.tvec = ws_add(p, "tvec", B * 4);
@@ -244,9 +245,9 @@ static int build_ops(smd_plan* p) {
   const uint64_t Mp = p->Mp;
   const WorkspaceLayout& w = p->reg;
   // forward GEMM: A K-major activations [Mp][K], B = (in,out) weight read MN-major ([K][N]) from the shadow arena; every
-  // forward GEMM has N >= 128 and uses the widest tile
-  auto fwd = [&](GemmOp* op, size_t a, long long wt, int K, int N) {
-    return make_gemm_op(op, p->ws + a, Mp, p->wsh(wt), static_cast<uint64_t>(N), N, K, kBNMax, 0, 1, 0, 0, p->lo_bytes);
+  // forward GEMM has N >= 128 and uses 128-wide tiles, the res-block GEMMs ask for the wide layout (BN = kBNWide)
+  auto fwd = [&](GemmOp* op, size_t a, long long wt, int K, int N, int BN = kBNMax) {
+    return make_gemm_op(op, p->ws + a, Mp, p->wsh(wt), static_cast<uint64_t>(N), N, K, BN, 0, 1, 0, 0, p->lo_bytes);
   };
   p->op_qkv.resize(p->L); p->op_o.resize(p->L);
   p->op_ffn1.resize(p->L); p->op_ffn2.resize(p->L);
@@ -271,8 +272,8 @@ static int build_ops(smd_plan* p) {
   }
   p->op_a.resize(p->K); p->op_b.resize(p->K);
   for (int k = 0; k < p->K; ++k) {
-    if (!fwd(&p->op_a[k], w.act[2 * k], p->par.block[k].a.kernel, Md, Md)) return SMD_ERR_CUDA;
-    if (!fwd(&p->op_b[k], w.act[2 * k + 1], p->par.block[k].b.kernel, Md, Md)) return SMD_ERR_CUDA;
+    if (!fwd(&p->op_a[k], w.act[2 * k], p->par.block[k].a.kernel, Md, Md, kBNWide)) return SMD_ERR_CUDA;
+    if (!fwd(&p->op_b[k], w.act[2 * k + 1], p->par.block[k].b.kernel, Md, Md, kBNWide)) return SMD_ERR_CUDA;
   }
   // output projection from the padded copy [Md][Cp]: N = C columns are valid (TransformerMDN: all Np of [Md][Np])
   if (!make_gemm_op(&p->op_out, p->ws + w.act[2 * p->K], Mp, p->ws + w.out_pad, static_cast<uint64_t>(p->head_ld),
@@ -282,8 +283,8 @@ static int build_ops(smd_plan* p) {
     if (!fwd(&p->op_tin, w.xbt, p->par.in.kernel, C, Md)) return SMD_ERR_CUDA;
     p->op_ta.resize(p->K); p->op_tb.resize(p->K);
     for (int k = 0; k < p->K; ++k) {
-      if (!fwd(&p->op_ta[k], w.actt[2 * k], p->par.block[k].a.kernel, Md, Md)) return SMD_ERR_CUDA;
-      if (!fwd(&p->op_tb[k], w.actt[2 * k + 1], p->par.block[k].b.kernel, Md, Md)) return SMD_ERR_CUDA;
+      if (!fwd(&p->op_ta[k], w.actt[2 * k], p->par.block[k].a.kernel, Md, Md, kBNWide)) return SMD_ERR_CUDA;
+      if (!fwd(&p->op_tb[k], w.actt[2 * k + 1], p->par.block[k].b.kernel, Md, Md, kBNWide)) return SMD_ERR_CUDA;
     }
     if (!make_gemm_op(&p->op_tout, p->ws + w.actt[2 * p->K], Mp, p->ws + w.out_pad, static_cast<uint64_t>(Cp), C, Md,
                       std::min(Cp, kBNMax), 0, 1, 0, 0, p->lo_bytes))
