@@ -11,6 +11,8 @@
  *   smd_ema_update         <- EMAHelper.update               utils/train_utils.py:73-78
  *   smd_ddpm_reverse_step  <- body of sample_with_beta       utils/ebm_utils.py:327-397
  *   smd_ddpm_sample        <- diffusion_dynamics(...)        utils/ebm_utils.py:274-405 (lax.scan over T steps)
+ *   smd_langevin_setup + smd_langevin_sample <- annealed_langevin_dynamics / consistent_langevin_dynamics
+ *                                                            utils/ebm_utils.py:89-271 (nested lax.scan, L*T steps)
  *   smd_threefry_*         <- jax.random.{split,normal,...}  (jax 0.2.8, call sites utils/losses.py:271-294,
  *                                                            utils/ebm_utils.py:329,342,360)
  *
@@ -210,6 +212,33 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
                     const float* infill_mask, float* collection, float* metrics, int use_graph,
                     smd_stream_t stream);
 
+/* ---- Langevin chains (annealed / consistent Langevin dynamics of the NCSN family) ------------------------------ */
+/* kind 0 = annealed (utils/ebm_utils.py:89-198), 1 = consistent (:201-271).  host_sigmas: HOST, L floats (L >= 2).
+ * steps_per_level: T of the annealed chain (ignored by the consistent one).  host_key: the `rng` the sampler receives.
+ * Builds the per-level table (sigma, alpha = epsilon (sigma / sigma_L)^2, noise coefficient sqrt(2 alpha) or
+ * beta sigma_{l+1}) and the collection indices linspace(1, L*T, 100) in the workspace.  It shares those regions with
+ * smd_sampler_setup: each of the two invalidates the other (the other sampler then returns SMD_ERR_STATE).
+ * SMD_ERR_INVALID for a TransformerMDN plan, L < 2 or L > 8192, an unknown kind or (annealed) T < 1. */
+int smd_langevin_setup(smd_plan* plan, const float* host_sigmas, int L, int steps_per_level, float epsilon, int kind,
+                       const uint32_t host_key[2], smd_stream_t stream);
+/* The whole chain on x (n, S, C) or (n, D) in place: L*T steps (annealed) or L steps (consistent), then the denoising
+ * step x += sigma_L^2 model(x, sigma_L) if denoise.  The step keys follow the reference's scan carry
+ * (rng, step_rng, infill_rng = split(rng, 3), or rng, step_rng = split(rng)) and are derived on the device.
+ * collection (annealed only): (101 + denoise, n, ...) or NULL -- rows 1..100 at the linspace steps, the last one after
+ * the denoising step; row 0 is the caller's.  metrics: (4, L, T) (annealed) or (4, L, 1) (consistent) or NULL:
+ * grad_norm, step_norm, alpha, noise_norm.  infill_x / infill_mask (annealed only) or NULL.  use_graph != 0: one step
+ * captured as a CUDA graph and replayed (re-captured when n, params, x, infill, collection, metrics or denoise change).
+ * smd_sampler_set_shard slices the chain noise as for smd_ddpm_sample.  SMD_ERR_INVALID for n > max_batch, or for
+ * the consistent chain with infill or collection. */
+int smd_langevin_sample(smd_plan* plan, const float* params, float* x, int n, const float* infill_x,
+                        const float* infill_mask, int denoise, float* collection, float* metrics, int use_graph,
+                        smd_stream_t stream);
+/* Host only: the tables smd_langevin_setup uploads.  host_coef (L x 4: sigma, alpha, noise coefficient, 0) and
+ * host_slots (the collection row of each of the L*T steps, or -1, for a collection of collection_rows rows); either
+ * may be NULL.  Same rejections as smd_langevin_setup. */
+int smd_langevin_tables(const float* host_sigmas, int L, int steps_per_level, float epsilon, int kind,
+                        int collection_rows, float* host_coef, int* host_slots);
+
 /* ---- autoregressive baseline (TransformerMDN, train_mdn.py) -------------------------------------------------- */
 /* cfg->arch must be SMD_ARCH_TRANSFORMER_MDN; num_components = --mdn_components (Kc).  SMD_ERR_INVALID for
  * seq_len != 32, precision bf16x3 or num_components < 1.  Parameters: the TransformerDDPM trunk, k{i}.res.* without
@@ -268,6 +297,10 @@ int smd_threefry_normal_slice(const uint32_t host_key[2], float* out, long long 
 /* jax.random.uniform(key, (n,), float32, minval, maxval) as of jax 0.2.8 (sample_ncsn.py:230: the infill initial state) */
 int smd_threefry_uniform(const uint32_t host_key[2], float* out, long long n, float minval, float maxval,
                          smd_stream_t stream);
+/* elements [first, first + n) of jax.random.uniform(key, (total,), float32, minval, maxval) (a rank's rows of the
+ * uniform initial state of the Langevin chains) */
+int smd_threefry_uniform_slice(const uint32_t host_key[2], float* out, long long n, long long first, long long total,
+                               float minval, float maxval, smd_stream_t stream);
 /* host-side split: out_keys = jax.random.split(key, num) (num x 2 uint32) */
 int smd_threefry_split(const uint32_t host_key[2], int num, uint32_t* host_out_keys);
 

@@ -1097,9 +1097,24 @@ void launch_ssm_loss(const float* f, const float* ft, const float* v, const floa
 //   next = x + alpha * grad + noise_coef * z ;  infill blend with y = infill_x + infill_sigma * z_infill ;
 //   metrics (mean over samples of sqrt(sum_axis1(.)^2 + 1e-10)): grad, alpha * grad, noise ; alpha itself.
 // thread = (sample n, channel c) looping over the S positions (axis 1), like the DDPM step kernel.
+// With a.state (graph replay of smd_langevin_sample) the per-step scalars, keys and output rows come from the device.
 __global__ void __launch_bounds__(256) langevin_step_kernel(const LangevinStepArgs a) {
   const int NC = a.N * a.C;
   const uint32_t total = static_cast<uint32_t>(a.N) * a.S * a.C;
+  const uint32_t rtotal = a.rng_total ? a.rng_total : total, rfirst = a.rng_total ? a.rng_first : 0u;
+  float alpha = a.alpha, noise_coef = a.noise_coef, infill_sigma = a.infill_sigma;
+  uint32_t k0 = a.key0, k1 = a.key1, ik0 = a.ikey0, ik1 = a.ikey1;
+  float* coll = a.collection_slot;
+  float* met = a.metrics;
+  size_t mstride = 1;
+  if (a.state) {
+    const LangevinChainState* cs = a.state;
+    const float* cf = a.coef + kLangevinCoef * cs->si;
+    infill_sigma = cf[0]; alpha = cf[1]; noise_coef = cf[2];
+    k0 = cs->skey[0]; k1 = cs->skey[1]; ik0 = cs->ikey[0]; ik1 = cs->ikey[1];
+    coll = (coll && cs->slot >= 0) ? coll + static_cast<size_t>(cs->slot) * total : nullptr;
+    if (met) { met += static_cast<size_t>(cs->si) * a.T + cs->i; mstride = static_cast<size_t>(a.L) * a.T; }
+  }
   float m_g = 0.f, m_s = 0.f, m_n = 0.f;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < NC) {
@@ -1108,23 +1123,23 @@ __global__ void __launch_bounds__(256) langevin_step_kernel(const LangevinStepAr
     for (int s = 0; s < a.S; ++s) {
       const uint32_t idx = (static_cast<uint32_t>(n) * a.S + s) * a.C + c;
       const float x = a.x[idx], g = a.grad[idx];
-      const float z = a.z ? a.z[idx] : jax_normal_from_bits(jax_random_bits(a.key0, a.key1, idx, total));
-      const float noise = __fmul_rn(a.noise_coef, z);
-      const float stp = __fmul_rn(a.alpha, g);
+      const float z = a.z ? a.z[idx] : jax_normal_from_bits(jax_random_bits(k0, k1, rfirst + idx, rtotal));
+      const float noise = __fmul_rn(noise_coef, z);
+      const float stp = __fmul_rn(alpha, g);
       float nx = __fadd_rn(__fadd_rn(x, stp), noise);
       if (a.infill_mask) {
-        const float iz = a.infill_z ? a.infill_z[idx] : jax_normal_from_bits(jax_random_bits(a.ikey0, a.ikey1, idx, total));
-        const float y = __fadd_rn(a.infill_x[idx], __fmul_rn(a.infill_sigma, iz));
+        const float iz = a.infill_z ? a.infill_z[idx] : jax_normal_from_bits(jax_random_bits(ik0, ik1, rfirst + idx, rtotal));
+        const float y = __fadd_rn(a.infill_x[idx], __fmul_rn(infill_sigma, iz));
         const float mk = a.infill_mask[idx];
         nx = nx * (1.0f - mk) + y * mk;
       }
       g2 += g * g; s2 += stp * stp; n2 += noise * noise;
       a.x_next[idx] = nx;
-      if (a.collection_slot) a.collection_slot[idx] = nx;
+      if (coll) coll[idx] = nx;
     }
     m_g = sqrtf(g2 + 1e-10f); m_s = sqrtf(s2 + 1e-10f); m_n = sqrtf(n2 + 1e-10f);
   }
-  if (a.metrics) {
+  if (met) {
     __shared__ float red[3][8];
     m_g = warp_sum(m_g); m_s = warp_sum(m_s); m_n = warp_sum(m_n);
     const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
@@ -1134,14 +1149,43 @@ __global__ void __launch_bounds__(256) langevin_step_kernel(const LangevinStepAr
       float v = 0.f;
       for (int j = 0; j < (blockDim.x >> 5); ++j) v += red[threadIdx.x][j];
       const int rowi = (threadIdx.x == 0) ? 0 : (threadIdx.x == 1 ? 1 : 3);   // grad_norm, step_norm, (alpha), noise_norm
-      atomicAdd(a.metrics + rowi, v / static_cast<float>(NC));
+      atomicAdd(met + rowi * mstride, v / static_cast<float>(NC));
     }
-    if (blockIdx.x == 0 && threadIdx.x == 3) a.metrics[2] = a.alpha;
+    if (blockIdx.x == 0 && threadIdx.x == 3) met[2 * mstride] = alpha;
   }
 }
 void launch_langevin_step(const LangevinStepArgs& a, cudaStream_t st) {
   const int NC = a.N * a.C;
   langevin_step_kernel<<<(NC + 255) / 256, 256, 0, st>>>(a);
+}
+
+// jax.random.split(chain, nsplit) on the device: keys j = words (2j, 2j + 1) of threefry(chain, (i, nsplit + i))
+__global__ void langevin_advance_kernel(LangevinChainState* s, const float* __restrict__ coef,
+                                        const int* __restrict__ idx_tab, float* __restrict__ cond, int L, int T,
+                                        int kind, int rows, int advance) {
+  if (advance) s->step += 1;
+  const int step = s->step;
+  if (step >= L * T) return;   // after the last step: nothing left to prepare
+  const int nsplit = kind == 0 ? 3 : 2;
+  const uint32_t c0 = s->chain[0], c1 = s->chain[1];
+  uint32_t flat[6] = {0u, 0u, 0u, 0u, 0u, 0u};
+  for (int j = 0; j < nsplit; ++j) {
+    uint32_t x0 = static_cast<uint32_t>(j), x1 = static_cast<uint32_t>(nsplit + j);
+    threefry2x32(c0, c1, x0, x1);
+    flat[j] = x0; flat[nsplit + j] = x1;
+  }
+  s->chain[0] = flat[0]; s->chain[1] = flat[1];
+  s->skey[0] = flat[2]; s->skey[1] = flat[3];
+  s->ikey[0] = flat[4]; s->ikey[1] = flat[5];   // zero for kind 1
+  const int si = step / T;
+  s->si = si;
+  s->i = step % T;
+  s->slot = idx_tab ? langevin_slot(idx_tab, step, rows) : -1;
+  cond[0] = coef[kLangevinCoef * si];
+}
+void launch_langevin_advance(LangevinChainState* s, const float* coef, const int* idx_tab, float* cond, int L, int T,
+                             int kind, int rows, int advance, cudaStream_t st) {
+  langevin_advance_kernel<<<1, 1, 0, st>>>(s, coef, idx_tab, cond, L, T, kind, rows, advance);
 }
 
 }  // namespace smd

@@ -265,6 +265,31 @@ void launch_ssm_loss(const float* f, const float* ft, const float* v, const floa
                      float* loss, float* score, float* hvp, float* loss_sum, unsigned int* done_counter, float inv_gb,
                      float* df32, __nv_bfloat16* df16, __nv_bfloat16* dft16, int B, int C, int Cp, cudaStream_t st);
 
+// Device state of the Langevin chain (smd_langevin_sample), in the plan's 64-byte t_ptr region: the step counter,
+// the chain key (the scan carry `rng`) and what langevin_advance derived from them for the current step.
+struct LangevinChainState {
+  int step;                 // global step si * T + i
+  int si, i;                // noise level and step within it
+  int slot;                 // collection row of this step, or -1
+  uint32_t chain[2];        // rng after this step's split
+  uint32_t skey[2], ikey[2];   // step_rng, infill_rng
+};
+static_assert(sizeof(LangevinChainState) <= 64, "LangevinChainState must fit the t_ptr region");
+// Per-level coefficients of the chain: [L][4] = (sigma, alpha, noise_coef, 0)
+static constexpr int kLangevinCoef = 4;
+static constexpr int kLangevinCollect = 100;   // collection_steps (utils/ebm_utils.py:120)
+
+// Collection row written by global step `step` (image_idx = step + 1): the reference's sum of the matching positions
+// of collection_idx plus one (utils/ebm_utils.py:156-163), -1 when none matches or when the summed row lies past the
+// collection's `rows` rows (repeated linspace indices: XLA's scatter drops that update).
+__host__ __device__ inline int langevin_slot(const int* idx_tab, int step, int rows) {
+  int sum = 0;
+  bool any = false;
+  for (int j = 0; j < kLangevinCollect; ++j)
+    if (idx_tab[j] == step + 1) { sum += j; any = true; }
+  return (any && sum + 1 < rows) ? sum + 1 : -1;
+}
+
 struct LangevinStepArgs {
   const float* x; const float* grad; const float* z;   // z: supplied N(0,1) or null -> threefry(key)
   uint32_t key0, key1, ikey0, ikey1;
@@ -272,7 +297,20 @@ struct LangevinStepArgs {
   const float* infill_x; const float* infill_mask; const float* infill_z;
   float* x_next; float* collection_slot; float* metrics;   // metrics: 4 floats (accumulated; zero them first)
   int N, S, C;
+  // Graph-replayable chain step (state != null): keys, alpha, noise_coef, infill_sigma and the collection row come from
+  // *state and coef[state->si]; collection_slot is then the collection's base ((rows, N, S, C)) and metrics the
+  // (4, L, T) table, column (si, i).
+  const LangevinChainState* state;
+  const float* coef;        // [L][kLangevinCoef]
+  int L, T;
+  // sharded sampling as ReverseStepArgs: samples [rng_first / (S*C), ...) of rng_total / (S*C) (0 / 0: off)
+  uint32_t rng_first, rng_total;
 };
 void launch_langevin_step(const LangevinStepArgs& a, cudaStream_t st);
+// One thread: (advance != 0) bumps the step counter, then, while step < L*T, derives the step's keys from the chain key
+// (`rng, step_rng, infill_rng = split(rng, 3)` for kind 0, `rng, step_rng = split(rng)` for kind 1), the noise level,
+// the collection row (of `rows`, see langevin_slot) and the conditioning value cond[0] = sigma.
+void launch_langevin_advance(LangevinChainState* s, const float* coef, const int* idx_tab, float* cond, int L, int T,
+                             int kind, int rows, int advance, cudaStream_t st);
 
 }  // namespace smd

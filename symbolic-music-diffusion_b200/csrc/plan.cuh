@@ -228,6 +228,21 @@ struct smd_plan {
   const float* graph_infill_mask = nullptr;
   float* graph_collection = nullptr;
   float* graph_metrics = nullptr;
+  // Langevin chain (smd_langevin_setup / smd_langevin_sample).  It shares the coef / slots / t_ptr / ftab* regions with
+  // the DDPM sampler: each setup invalidates the other (sampler_ready / langevin_ready, the FiLM table, both graphs).
+  // T holds the number of noise levels L while a Langevin schedule is set (the FiLM table has one row per level).
+  bool langevin_ready = false;
+  int lv_kind = 0, lv_steps = 1;   // kind (0 annealed, 1 consistent), steps per level
+  uint32_t lv_key[2] = {0u, 0u};
+  float lv_sigma_last = 0.f;
+  smd::CapturedGraph langevin_graph;
+  int lg_n = -1, lg_rows = 0;
+  const float* lg_params = nullptr;
+  float* lg_x = nullptr;
+  const float* lg_infill_x = nullptr;
+  const float* lg_infill_mask = nullptr;
+  float* lg_collection = nullptr;
+  float* lg_metrics = nullptr;
   cudaStream_t own_stream = nullptr;
   cudaEvent_t own_event = nullptr;
   // training: the FiLM generator (forward and backward) runs on a side stream, concurrently with the trunk

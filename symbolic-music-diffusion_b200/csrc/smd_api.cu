@@ -641,9 +641,11 @@ __global__ void draws_kernel(uint32_t lk0, uint32_t lk1, uint32_t nk0, uint32_t 
 }
 
 // jax.random.uniform (0.2.8): f = bitcast((bits >> 9) | 0x3F800000) - 1; max(minval, f * (maxval - minval) + minval)
-__global__ void threefry_uniform_kernel(uint32_t k0, uint32_t k1, float* out, uint32_t n, float minv, float maxv) {
+// out[j] = element (first + j) of jax.random.uniform(key, (total,), minval, maxval)
+__global__ void threefry_uniform_kernel(uint32_t k0, uint32_t k1, float* out, uint32_t n, uint32_t first, uint32_t total,
+                                        float minv, float maxv) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const uint32_t bits = jax_random_bits(k0, k1, i, n);
+    const uint32_t bits = jax_random_bits(k0, k1, first + i, total);
     const float u01 = __uint_as_float((bits >> 9) | 0x3F800000u) - 1.0f;
     out[i] = fmaxf(minv, __fadd_rn(__fmul_rn(u01, __fsub_rn(maxv, minv)), minv));
   }
@@ -768,6 +770,7 @@ int smd_mdn_plan_create(const smd_config* cfg, int num_components, smd_plan** ou
 void smd_plan_destroy(smd_plan* plan) {
   if (!plan) return;
   plan->sample_graph.drop();
+  plan->langevin_graph.drop();
   plan->train_graph.drop();
   if (plan->evx_join) cudaEventDestroy(plan->evx_join);
   if (plan->ev_gz) cudaEventDestroy(plan->ev_gz);
@@ -1089,19 +1092,23 @@ int smd_sampler_setup(smd_plan* plan, const float* host_betas, int T, const uint
   SMD_CUDA(cudaStreamSynchronize(st));  // host vectors go out of scope
   plan->T = T;
   plan->sampler_ready = true;
+  plan->langevin_ready = false;   // the Langevin chain's tables lived in the same regions
   plan->film_tab_ready = false;
   plan->sample_graph.drop();
+  plan->langevin_graph.drop();
   return SMD_OK;
 }
 
-__global__ void gather_cond_kernel(const float* __restrict__ coef, float* __restrict__ tv, int T) {
+__global__ void gather_cond_kernel(const float* __restrict__ coef, float* __restrict__ tv, int T, int stride,
+                                   int offset) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < T) tv[i] = coef[8 * i + 5];
+  if (i < T) tv[i] = coef[stride * i + offset];
 }
 
-// FiLM scale/shift for every step of the schedule (all samples share t, so this replaces 3K small launches per
-// reverse step by one table lookup): ftab[k][t][:] = DenseFiLM_k(sqrt(alpha_bar_t))   (models/ncsn.py:44-61)
-static int ensure_film_table(smd_plan* plan, const float* params, cudaStream_t st) {
+// FiLM scale/shift for every row of the schedule (all samples share the conditioning value, so this replaces 3K small
+// launches per step by one table lookup): ftab[k][r][:] = DenseFiLM_k(cond_r)   (models/ncsn.py:44-61), with cond_r =
+// coef[stride * r + offset] for the plan->T rows: sqrt(alpha_bar_t) of the DDPM sampler, sigma_l of the Langevin chain
+static int ensure_film_table(smd_plan* plan, const float* params, int stride, int offset, cudaStream_t st) {
   if (plan->cfg.sampler_T <= 0 || plan->T > plan->cfg.sampler_T) return SMD_OK;   // per-step generator instead
   if (plan->film_tab_ready && plan->film_tab_params == params) return SMD_OK;
   const int T = plan->T, Md = plan->cfg.mlp_dims;
@@ -1110,7 +1117,7 @@ static int ensure_film_table(smd_plan* plan, const float* params, cudaStream_t s
   float* e1 = plan->at<float>(plan->reg.ftab_e1);
   float* e2 = plan->at<float>(plan->reg.ftab_e2);
   float* tab = plan->at<float>(plan->reg.ftab);
-  gather_cond_kernel<<<(T + 255) / 256, 256, 0, st>>>(plan->at<float>(plan->reg.coef), tv, T); CNT();
+  gather_cond_kernel<<<(T + 255) / 256, 256, 0, st>>>(plan->at<float>(plan->reg.coef), tv, T, stride, offset); CNT();
   launch_noise_encoding(tv, plan->at<float>(plan->reg.freqs), enc, T, st); CNT();
   for (int k = 0; k < plan->K; ++k) {
     const FilmParams& f = plan->par.block[k].film;
@@ -1178,6 +1185,7 @@ int smd_sampler_set_shard(smd_plan* plan, long long first_row, long long total_r
   plan->shard_first_row = first_row;
   plan->shard_total_rows = total_rows;
   plan->sample_graph.drop();  // kernel args changed
+  plan->langevin_graph.drop();
   return SMD_OK;
 }
 
@@ -1188,7 +1196,7 @@ int smd_ddpm_reverse_step(smd_plan* plan, const float* params, const float* x, i
   if (!plan->sampler_ready) { set_error("smd_sampler_setup has not been called"); return SMD_ERR_STATE; }
   if (t < 0 || t >= plan->T) { set_error("t out of range"); return SMD_ERR_INVALID; }
   if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
-  int rc0 = ensure_film_table(plan, params, static_cast<cudaStream_t>(stream));
+  int rc0 = ensure_film_table(plan, params, 8, 5, static_cast<cudaStream_t>(stream));
   if (rc0) return rc0;
   return reverse_step_impl(plan, params, x, n, t, z, infill_x, infill_mask, infill_z, x_next, eps_hat_or_null,
                            collection, metrics, static_cast<cudaStream_t>(stream));
@@ -1204,7 +1212,7 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int T = plan->T;
   if (metrics) SMD_CUDA(cudaMemsetAsync(metrics, 0, sizeof(float) * 4 * T, st));
-  { int rc0 = ensure_film_table(plan, params, st); if (rc0) return rc0; }
+  { int rc0 = ensure_film_table(plan, params, 8, 5, st); if (rc0) return rc0; }
   if (!use_graph) {
     for (int i = 0; i < steps; ++i) {
       int rc = reverse_step_impl(plan, params, x, n, T - 1 - i, nullptr, infill_x, infill_mask, nullptr, x, nullptr,
@@ -1253,6 +1261,199 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
   return SMD_OK;
 }
 
+// ---- Langevin chain (annealed / consistent Langevin dynamics, utils/ebm_utils.py:89-271) ----------------------------
+
+// Host tables of smd_langevin_setup, float32 in the reference's operation order:
+//   coef[l] = (sigma_l, alpha_l = epsilon (sigma_l / sigma_L)^2, noise_l, 0) with noise_l = sqrt(2 alpha_l) (annealed,
+//   :133-150) or beta sigma_{l+1}, 0 for the last level, beta = sqrt(1 - (1 - epsilon / sigma_L^2)^2) (consistent,
+//   :231-260);  idx[j] = int(linspace(1, L*T, 100)[j]) in float64 like np.linspace (:127-129).
+static int langevin_tables(const float* sig, int L, int T, float epsilon, int kind, float* coef, int* idx) {
+  if (!sig) { set_error("null sigmas"); return SMD_ERR_INVALID; }
+  if (kind != 0 && kind != 1) { set_error("kind must be 0 (annealed) or 1 (consistent)"); return SMD_ERR_INVALID; }
+  if (L < 2 || L > kMaxT) { set_error("the number of noise levels must be in [2, " + std::to_string(kMaxT) + "]"); return SMD_ERR_INVALID; }
+  if (kind == 0 && (T < 1 || static_cast<long long>(L) * T > (1 << 30))) { set_error("steps_per_level out of range"); return SMD_ERR_INVALID; }
+  const float sl = sig[L - 1];
+  const float sl2 = sl * sl;
+  const float r = 1.0f - epsilon / sl2;
+  const float beta = sqrtf(1.0f - r * r);
+  for (int l = 0; l < L; ++l) {
+    const float q = sig[l] / sl;
+    const float alpha = epsilon * (q * q);
+    float* c = coef + static_cast<size_t>(l) * kLangevinCoef;
+    c[0] = sig[l];
+    c[1] = alpha;
+    c[2] = kind == 0 ? sqrtf(2.0f * alpha) : beta * (l < L - 1 ? sig[l + 1] : 0.0f);
+    c[3] = 0.0f;
+  }
+  const long long total = kind == 0 ? static_cast<long long>(L) * T : L;
+  const double step = static_cast<double>(total - 1) / static_cast<double>(kLangevinCollect - 1);
+  for (int j = 0; j < kLangevinCollect; ++j)
+    idx[j] = (j == kLangevinCollect - 1) ? static_cast<int>(total) : static_cast<int>(static_cast<double>(j) * step + 1.0);
+  return SMD_OK;
+}
+
+int smd_langevin_tables(const float* host_sigmas, int L, int steps_per_level, float epsilon, int kind,
+                        int collection_rows, float* host_coef, int* host_slots) {
+  std::vector<float> coef(static_cast<size_t>(std::max(L, 0)) * kLangevinCoef);
+  int idx[kLangevinCollect];
+  const int rc = langevin_tables(host_sigmas, L, steps_per_level, epsilon, kind, coef.data(), idx);
+  if (rc) return rc;
+  if (host_coef) memcpy(host_coef, coef.data(), coef.size() * sizeof(float));
+  if (host_slots) {
+    const long long total = kind == 0 ? static_cast<long long>(L) * steps_per_level : L;
+    for (long long s = 0; s < total; ++s) host_slots[s] = langevin_slot(idx, static_cast<int>(s), collection_rows);
+  }
+  return SMD_OK;
+}
+
+int smd_langevin_setup(smd_plan* plan, const float* host_sigmas, int L, int steps_per_level, float epsilon, int kind,
+                       const uint32_t host_key[2], smd_stream_t stream) {
+  if (!plan || !host_key) { set_error("null argument"); return SMD_ERR_INVALID; }
+  if (reject_mdn(plan, "smd_langevin_setup")) return SMD_ERR_INVALID;
+  std::vector<float> coef(static_cast<size_t>(std::max(L, 0)) * kLangevinCoef);
+  int idx[kLangevinCollect];
+  const int rc = langevin_tables(host_sigmas, L, steps_per_level, epsilon, kind, coef.data(), idx);
+  if (rc) return rc;
+  if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  SMD_CUDA(cudaMemcpyAsync(plan->at<float>(plan->reg.coef), coef.data(), coef.size() * 4, cudaMemcpyHostToDevice, st));
+  SMD_CUDA(cudaMemcpyAsync(plan->at<int>(plan->reg.slots), idx, sizeof(idx), cudaMemcpyHostToDevice, st));
+  SMD_CUDA(cudaStreamSynchronize(st));  // host tables go out of scope
+  plan->T = L;
+  plan->lv_kind = kind;
+  plan->lv_steps = kind == 0 ? steps_per_level : 1;
+  plan->lv_key[0] = host_key[0]; plan->lv_key[1] = host_key[1];
+  plan->lv_sigma_last = host_sigmas[L - 1];
+  plan->langevin_ready = true;
+  plan->sampler_ready = false;   // the DDPM tables lived in the same regions
+  plan->film_tab_ready = false;
+  plan->sample_graph.drop();
+  plan->langevin_graph.drop();
+  return SMD_OK;
+}
+
+// The network call of one chain step: model(x, sigma) into eps_hat with sigma = tvec[0].  row >= 0: FiLM table row
+// `row` (host); row < 0: the row is the chain state's noise level (graph replay).  Without a table (L > sampler_T) the
+// generator runs on tvec itself.
+static int langevin_forward(smd_plan* plan, const float* params, const float* x, int n, int row, cudaStream_t st) {
+  if (plan->film_tab_ready && plan->film_tab_params == params) {
+    plan->film_tab_on = true;
+    plan->film_row = row >= 0 ? row : 0;
+    plan->film_row_dev = row >= 0 ? nullptr : &plan->at<LangevinChainState>(plan->reg.t_ptr)->si;
+  }
+  const int rc = run_forward(plan, params, x, plan->at<float>(plan->reg.tvec), 1, n, plan->at<float>(plan->reg.eps_hat),
+                             st, false);
+  plan->film_tab_on = false;
+  plan->film_row_dev = nullptr;
+  return rc;
+}
+
+static LangevinStepArgs langevin_args(const smd_plan* plan, const float* x, int n) {
+  LangevinStepArgs a;
+  memset(&a, 0, sizeof(a));
+  a.x = x; a.grad = plan->at<float>(plan->reg.eps_hat); a.x_next = const_cast<float*>(x);
+  a.N = n; a.S = plan->cfg.seq_len; a.C = plan->cfg.channels;
+  if (plan->cfg.arch != SMD_ARCH_TRANSFORMER_DDPM) { a.S = plan->cfg.channels; a.C = 1; }   // (N, D) states: axis 1 = D
+  return a;
+}
+
+int smd_langevin_sample(smd_plan* plan, const float* params, float* x, int n, const float* infill_x,
+                        const float* infill_mask, int denoise, float* collection, float* metrics, int use_graph,
+                        smd_stream_t stream) {
+  if (!plan) { set_error("null plan"); return SMD_ERR_INVALID; }
+  if (reject_mdn(plan, "smd_langevin_sample")) return SMD_ERR_INVALID;
+  if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
+  if ((infill_x == nullptr) != (infill_mask == nullptr)) { set_error("infill_x and infill_mask go together"); return SMD_ERR_INVALID; }
+  if (!plan->langevin_ready) { set_error("smd_langevin_setup has not been called"); return SMD_ERR_STATE; }
+  if (plan->lv_kind == 1 && (infill_x || collection)) {
+    set_error("consistent Langevin dynamics has no infilling and no collection");
+    return SMD_ERR_INVALID;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int L = plan->T, T = plan->lv_steps, kind = plan->lv_kind;
+  const int rows = kLangevinCollect + 1 + (denoise ? 1 : 0);
+  float* coef = plan->at<float>(plan->reg.coef);
+  const int* idx = plan->at<int>(plan->reg.slots);
+  float* tvec = plan->at<float>(plan->reg.tvec);
+  LangevinChainState* cst = plan->at<LangevinChainState>(plan->reg.t_ptr);
+  // graph replay: the legacy default stream cannot be captured, so the chain runs on a private stream ordered after st
+  cudaStream_t cs = st;
+  if (use_graph && (st == nullptr || st == cudaStreamLegacy || st == cudaStreamPerThread)) {
+    if (!plan->own_stream) {
+      SMD_CUDA(cudaStreamCreateWithFlags(&plan->own_stream, cudaStreamNonBlocking));
+      SMD_CUDA(cudaEventCreateWithFlags(&plan->own_event, cudaEventDisableTiming));
+    }
+    SMD_CUDA(cudaEventRecord(plan->own_event, st));
+    SMD_CUDA(cudaStreamWaitEvent(plan->own_stream, plan->own_event, 0));
+    cs = plan->own_stream;
+  }
+  if (metrics) SMD_CUDA(cudaMemsetAsync(metrics, 0, sizeof(float) * 4 * L * T, cs));
+  { const int rc0 = ensure_film_table(plan, params, kLangevinCoef, 0, cs); if (rc0) return rc0; }
+  // the chain starts from the setup key at step 0 on every call
+  LangevinChainState init;
+  memset(&init, 0, sizeof(init));
+  init.chain[0] = plan->lv_key[0]; init.chain[1] = plan->lv_key[1];
+  SMD_CUDA(cudaMemcpyAsync(cst, &init, sizeof(init), cudaMemcpyHostToDevice, cs));
+  SMD_CUDA(cudaStreamSynchronize(cs));  // init is a stack variable
+  launch_langevin_advance(cst, coef, collection ? idx : nullptr, tvec, L, T, kind, rows, 0, cs); CNT();
+  // one step: network call -> update (state on the device) -> derive the next step's keys, level, row and sigma
+  auto step = [&](cudaStream_t s) -> int {
+    const int r = langevin_forward(plan, params, x, n, -1, s);
+    if (r) return r;
+    LangevinStepArgs a = langevin_args(plan, x, n);
+    a.infill_x = infill_x; a.infill_mask = infill_mask;
+    a.collection_slot = collection; a.metrics = metrics;
+    a.state = cst; a.coef = coef; a.L = L; a.T = T;
+    if (plan->shard_total_rows > 0) {
+      const long long per = static_cast<long long>(a.S) * a.C;
+      a.rng_first = static_cast<uint32_t>(plan->shard_first_row * per);
+      a.rng_total = static_cast<uint32_t>(plan->shard_total_rows * per);
+    }
+    launch_langevin_step(a, s); CNT();
+    launch_langevin_advance(cst, coef, collection ? idx : nullptr, tvec, L, T, kind, rows, 1, s); CNT();
+    SMD_LAUNCH_CHECK("langevin chain step");
+    return SMD_OK;
+  };
+  const long long total_steps = static_cast<long long>(L) * T;
+  if (!use_graph) {
+    for (long long i = 0; i < total_steps; ++i) {
+      const int rc = step(cs);
+      if (rc) return rc;
+    }
+  } else {
+    const bool same = plan->langevin_graph.exec && plan->lg_n == n && plan->lg_params == params && plan->lg_x == x &&
+                      plan->lg_infill_x == infill_x && plan->lg_infill_mask == infill_mask &&
+                      plan->lg_collection == collection && plan->lg_metrics == metrics && plan->lg_rows == rows;
+    if (!same) {
+      const int rc = plan->langevin_graph.capture(cs, [&] { return step(cs); }, "langevin graph");
+      if (rc) return rc;
+      plan->lg_n = n; plan->lg_params = params; plan->lg_x = x; plan->lg_infill_x = infill_x;
+      plan->lg_infill_mask = infill_mask; plan->lg_collection = collection; plan->lg_metrics = metrics;
+      plan->lg_rows = rows;
+    }
+    for (long long i = 0; i < total_steps; ++i) {
+      const int rc = plan->langevin_graph.launch(cs);
+      if (rc) return rc;
+    }
+  }
+  if (denoise) {
+    // x += sigma_L^2 model(x, sigma_L) (utils/ebm_utils.py:193-196, 265-266); the annealed chain also writes collection[-1]
+    SMD_CUDA(cudaMemcpyAsync(tvec, coef + static_cast<size_t>(L - 1) * kLangevinCoef, 4, cudaMemcpyDeviceToDevice, cs));
+    const int r = langevin_forward(plan, params, x, n, L - 1, cs);
+    if (r) return r;
+    LangevinStepArgs a = langevin_args(plan, x, n);
+    a.alpha = plan->lv_sigma_last * plan->lv_sigma_last;
+    a.collection_slot = collection ? collection + static_cast<size_t>(rows - 1) * n * a.S * a.C : nullptr;
+    launch_langevin_step(a, cs); CNT();
+    SMD_LAUNCH_CHECK("langevin denoise");
+  }
+  if (cs != st) {
+    SMD_CUDA(cudaEventRecord(plan->own_event, cs));
+    SMD_CUDA(cudaStreamWaitEvent(st, plan->own_event, 0));
+  }
+  return SMD_OK;
+}
+
 int smd_threefry_normal_slice(const uint32_t host_key[2], float* out, long long n, long long first, long long total,
                               smd_stream_t stream) {
   if (n < 0 || first < 0 || first + n > total || total > 0xFFFFFFFFll) { set_error("slice out of range"); return SMD_ERR_INVALID; }
@@ -1265,15 +1466,21 @@ int smd_threefry_normal_slice(const uint32_t host_key[2], float* out, long long 
 int smd_threefry_normal(const uint32_t host_key[2], float* out, long long n, smd_stream_t stream) {
   return smd_threefry_normal_slice(host_key, out, n, 0, n, stream);
 }
-int smd_threefry_uniform(const uint32_t host_key[2], float* out, long long n, float minval, float maxval,
-                         smd_stream_t stream) {
-  if (n < 0 || n > 0xFFFFFFFFll) { set_error("n out of range"); return SMD_ERR_INVALID; }
+int smd_threefry_uniform_slice(const uint32_t host_key[2], float* out, long long n, long long first, long long total,
+                               float minval, float maxval, smd_stream_t stream) {
+  if (n < 0 || first < 0 || first + n > total || total > 0xFFFFFFFFll) { set_error("slice out of range"); return SMD_ERR_INVALID; }
   if (n == 0) return SMD_OK;
   threefry_uniform_kernel<<<grid_stride_blocks(n), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      host_key[0], host_key[1], out, static_cast<uint32_t>(n), minval, maxval);
+      host_key[0], host_key[1], out, static_cast<uint32_t>(n), static_cast<uint32_t>(first),
+      static_cast<uint32_t>(total), minval, maxval);
   CNT();
   SMD_LAUNCH_CHECK("threefry_uniform");
   return SMD_OK;
+}
+int smd_threefry_uniform(const uint32_t host_key[2], float* out, long long n, float minval, float maxval,
+                         smd_stream_t stream) {
+  if (n < 0 || n > 0xFFFFFFFFll) { set_error("n out of range"); return SMD_ERR_INVALID; }
+  return smd_threefry_uniform_slice(host_key, out, n, 0, n, minval, maxval, stream);
 }
 int smd_threefry_split(const uint32_t host_key[2], int num, uint32_t* host_out_keys) {
   if (num < 1) { set_error("num must be >= 1"); return SMD_ERR_INVALID; }

@@ -56,16 +56,22 @@ def diffusion_dynamics(rng, model, betas, init, epsilon, T, denoise, infill=Fals
         collection[0] = x
     metrics = torch.zeros((4, len(betas)), dtype=torch.float32, device=x.device)
     eng.sample(x, steps=len(betas), infill_x=ix, infill_mask=im, collection=collection, metrics=metrics, use_graph=True)
-    if shard is not None:
-        # utils/ebm_utils.py:380-384: the metrics are means over the batch -> one weighted (4, T) all-reduce at the end
-        from . import parallel
-        if parallel.world_size() > 1:
-            w = float(n) / float(shard[1])
-            alpha_row = metrics[2].clone()              # alpha_prod is not a batch mean
-            metrics.mul_(w)
-            parallel.all_reduce_sum_(metrics)
-            metrics[2] = alpha_row
+    _reduce_sharded_metrics(metrics, n, shard)
     return x, collection, metrics.unsqueeze(2)
+
+
+def _reduce_sharded_metrics(metrics, n, shard):
+    """The sampler metrics are means over the batch (utils/ebm_utils.py:166-170, 380-384): with shard = (first_row,
+    total_rows) over several ranks, one weighted all-reduce at the end; row 2 (alpha / alpha_prod) is no batch mean."""
+    if shard is None:
+        return
+    from . import parallel
+    if parallel.world_size() > 1:
+        w = float(n) / float(shard[1])
+        alpha_row = metrics[2].clone()
+        metrics.mul_(w)
+        parallel.all_reduce_sum_(metrics)
+        metrics[2] = alpha_row
 
 
 def collate_sampling_metrics(ld_metrics):
@@ -90,13 +96,13 @@ def _collection_slot_fn(total_steps, collection_steps):
 
 
 def annealed_langevin_dynamics(rng, model, sigmas, init, epsilon, T, denoise, infill=False, infill_samples=None,
-                               infill_masks=None):
+                               infill_masks=None, shard=None):
     """utils/ebm_utils.py:89-198 (Song & Ermon): for every noise level T steps x += alpha * score + sqrt(2 alpha) z with
     alpha = epsilon (sigma / sigma_L)^2.  Returns (state, collection (101 + denoise, N, ...), metrics (4, L, T)).
 
-    The network call and the update kernel run on the GPU (smd_forward, smd_langevin_step); the host only walks the
-    (sigma, step) loop and the key schedule `rng, step_rng, infill_rng = split(rng, 3)` of the scan body."""
-    from . import jrandom as random
+    The whole chain runs on the GPU (smd_langevin_sample: CUDA-graph replay of one step, keys from the scan carry
+    `rng, step_rng, infill_rng = split(rng, 3)` derived on the device).  shard = (first_row, total_rows) as in
+    diffusion_dynamics: `init` holds this rank's rows of a global batch."""
     from .nn import _as_device_f32
     x = _as_device_f32(init).clone()
     n = x.shape[0]
@@ -108,61 +114,32 @@ def annealed_langevin_dynamics(rng, model, sigmas, init, epsilon, T, denoise, in
     L = len(sig)
     collection = torch.zeros((101 + int(bool(denoise)),) + tuple(x.shape), dtype=torch.float32, device=x.device)
     collection[0] = x * (1 - im) + ix * im if infill else x
-    slot_of = _collection_slot_fn(L * T, 100)
-    metrics = torch.zeros((L, T, 4), dtype=torch.float32, device=x.device)
-    sigma_dev = torch.empty((1,), dtype=torch.float32, device=x.device)
-    grad = torch.empty_like(x)
-    key = np.asarray(rng, np.uint32)
-    for si in range(L):
-        s = np.float32(sig[si])
-        alpha = np.float32(epsilon) * (s / np.float32(sig[-1])) ** 2              # float32, like the jitted scan
-        sigma_dev.copy_(torch.tensor([float(s)]))
-        for i in range(T):
-            key, step_key, infill_key = random.split(key, 3)
-            eng.forward(x, sigma_dev, out=grad)                                 # model(state, sigma)
-            slot = slot_of(si * T + i + 1)
-            if slot >= collection.shape[0]:
-                slot = -1       # repeated linspace indices (fewer than 100 steps in total): XLA's scatter drops the update
-            eng.langevin_step(x, grad, float(alpha), float(np.sqrt(np.float32(2) * alpha)), step_key=step_key,
-                              infill_x=ix, infill_mask=im, infill_sigma=float(s), infill_key=infill_key, x_next=x,
-                              collection_slot=collection[slot] if slot >= 0 else None, metrics4=metrics[si, i])
-    if denoise:                                                                   # utils/ebm_utils.py:193-196
-        sigma_dev.copy_(torch.tensor([float(sig[-1])]))
-        eng.forward(x, sigma_dev, out=grad)
-        eng.langevin_step(x, grad, float(np.float32(sig[-1]) ** 2), 0.0, x_next=x, collection_slot=collection[-1])
-    return x, collection, metrics.permute(2, 0, 1).contiguous()
+    metrics = torch.zeros((4, L, int(T)), dtype=torch.float32, device=x.device)
+    eng.langevin_setup(sig, int(T), epsilon, "ald", key=(int(rng[0]), int(rng[1])))
+    eng.set_sampler_shard(*(shard if shard is not None else (0, 0)))
+    eng.langevin_sample(x, denoise=bool(denoise), infill_x=ix, infill_mask=im, collection=collection, metrics=metrics)
+    _reduce_sharded_metrics(metrics, n, shard)
+    return x, collection, metrics
 
 
 def consistent_langevin_dynamics(rng, model, sigmas, init, epsilon, T, denoise=True, infill=False, infill_samples=None,
-                                 infill_masks=None):
+                                 infill_masks=None, shard=None):
     """utils/ebm_utils.py:201-271 (Jolicoeur-Martineau et al.): one step per noise level,
     x += alpha * score + beta * sigma_{i+1} * z.  Returns (state, None, metrics (4, L, 1)) -- upstream returns two values
-    although its caller unpacks three (SURVEY section 0); the missing collection is returned as None."""
-    from . import jrandom as random
+    although its caller unpacks three (SURVEY section 0); the missing collection is returned as None.  Runs on the GPU
+    like annealed_langevin_dynamics (keys `rng, step_rng = split(rng)`); shard as there."""
     from .nn import _as_device_f32
     del T
     if infill:
         raise NotImplementedError
     x = _as_device_f32(init).clone()
-    eng = model.engine(x.shape[0])
+    n = x.shape[0]
+    eng = model.engine(n)
     sig = np.asarray(sigmas, np.float32)
     assert len(sig) >= 2
-    L = len(sig)
-    beta = np.sqrt(np.float32(1) - (np.float32(1) - np.float32(epsilon) / sig[-1] ** 2) ** 2).astype(np.float32)
-    metrics = torch.zeros((L, 4), dtype=torch.float32, device=x.device)
-    sigma_dev = torch.empty((1,), dtype=torch.float32, device=x.device)
-    grad = torch.empty_like(x)
-    key = np.asarray(rng, np.uint32)
-    for i in range(L):
-        key, step_key = random.split(key)
-        s = np.float32(sig[i])
-        nxt = np.float32(sig[i + 1]) if i < L - 1 else np.float32(0)
-        alpha = np.float32(epsilon) * (s / np.float32(sig[-1])) ** 2
-        sigma_dev.copy_(torch.tensor([float(s)]))
-        eng.forward(x, sigma_dev, out=grad)
-        eng.langevin_step(x, grad, float(alpha), float(beta * nxt), step_key=step_key, x_next=x, metrics4=metrics[i])
-    if denoise:
-        sigma_dev.copy_(torch.tensor([float(sig[-1])]))
-        eng.forward(x, sigma_dev, out=grad)
-        eng.langevin_step(x, grad, float(np.float32(sig[-1]) ** 2), 0.0, x_next=x)
-    return x, None, metrics.t().contiguous().unsqueeze(2)
+    metrics = torch.zeros((4, len(sig), 1), dtype=torch.float32, device=x.device)
+    eng.langevin_setup(sig, 1, epsilon, "cas", key=(int(rng[0]), int(rng[1])))
+    eng.set_sampler_shard(*(shard if shard is not None else (0, 0)))
+    eng.langevin_sample(x, denoise=bool(denoise), metrics=metrics)
+    _reduce_sharded_metrics(metrics, n, shard)
+    return x, None, metrics

@@ -496,6 +496,36 @@ class Engine:
                                             1 if use_graph else 0, self._stream()))
         return x
 
+    LANGEVIN_KINDS = {"ald": 0, "cas": 1}
+
+    def langevin_setup(self, sigmas: np.ndarray, steps_per_level: int, epsilon: float, kind: str = "ald",
+                       key=(0, 0)) -> None:
+        """Noise levels, step size and chain key of annealed ("ald", utils/ebm_utils.py:89-198) or consistent ("cas",
+        :201-271) Langevin dynamics; replaces a sampler_setup schedule (and vice versa)."""
+        if kind not in self.LANGEVIN_KINDS:
+            raise ValueError(f"unknown Langevin sampler {kind!r} (expected one of {sorted(self.LANGEVIN_KINDS)})")
+        self._ensure_ws()
+        s = np.ascontiguousarray(sigmas, np.float32)
+        k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
+        _lib.check(self.lib.smd_langevin_setup(self._plan, s.ctypes.data_as(C.POINTER(C.c_float)), len(s),
+                                               int(steps_per_level), float(epsilon), self.LANGEVIN_KINDS[kind], k,
+                                               self._stream()))
+
+    def langevin_sample(self, x, denoise: bool = True, infill_x=None, infill_mask=None, collection=None, metrics=None,
+                        use_graph: bool = True):
+        """Runs the whole Langevin chain of langevin_setup in place on x, then the denoising step if ``denoise``.
+        collection (annealed only): (101 + denoise, n, ...) with row 0 left to the caller; metrics: (4, L, T)."""
+        x = _f32c(x, "x")
+        for t, name in ((infill_x, "infill_x"), (infill_mask, "infill_mask"), (collection, "collection"),
+                        (metrics, "metrics")):
+            if t is not None:
+                _f32c(t, name)
+        _lib.check(self.lib.smd_langevin_sample(self._plan, self.params.data_ptr(), x.data_ptr(), x.shape[0],
+                                                _ptr(infill_x), _ptr(infill_mask), 1 if denoise else 0,
+                                                _ptr(collection), _ptr(metrics), 1 if use_graph else 0,
+                                                self._stream()))
+        return x
+
     def launch_count(self) -> int:
         return int(self.lib.smd_launch_count())
 

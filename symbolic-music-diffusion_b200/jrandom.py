@@ -44,11 +44,20 @@ def normal(key, shape, device=None, rows=None) -> torch.Tensor:
     return out
 
 
-def uniform(key, shape, minval: float = 0.0, maxval: float = 1.0, device=None) -> torch.Tensor:
+def uniform(key, shape, minval: float = 0.0, maxval: float = 1.0, device=None, rows=None) -> torch.Tensor:
+    """jax.random.uniform(key, shape, minval=minval, maxval=maxval).  ``rows=(first, count)`` as in ``normal``."""
     lib = _lib.load_library()
-    n = int(np.prod(shape))
-    out = torch.empty(tuple(shape), dtype=torch.float32, device=device or "cuda")
+    shape = tuple(int(s) for s in shape)
+    total = int(np.prod(shape))
     k = (C.c_uint32 * 2)(int(key[0]), int(key[1]))
-    _lib.check(lib.smd_threefry_uniform(k, out.data_ptr(), n, C.c_float(minval), C.c_float(maxval),
-                                        torch.cuda.current_stream().cuda_stream))
+    st = torch.cuda.current_stream().cuda_stream
+    if rows is None:
+        out = torch.empty(shape, dtype=torch.float32, device=device or "cuda")
+        _lib.check(lib.smd_threefry_uniform(k, out.data_ptr(), total, C.c_float(minval), C.c_float(maxval), st))
+        return out
+    first, count = int(rows[0]), int(rows[1])
+    per = total // shape[0]
+    out = torch.empty((count,) + shape[1:], dtype=torch.float32, device=device or "cuda")
+    _lib.check(lib.smd_threefry_uniform_slice(k, out.data_ptr(), count * per, first * per, total, C.c_float(minval),
+                                              C.c_float(maxval), st))
     return out

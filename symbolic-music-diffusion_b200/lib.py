@@ -62,7 +62,14 @@ _SIGNATURES = {
     "smd_threefry_normal_slice": (C.c_int, [C.POINTER(C.c_uint32), _P, C.c_longlong, C.c_longlong, C.c_longlong, _P]),
     "smd_sampler_set_shard": (C.c_int, [_P, C.c_longlong, C.c_longlong]),
     "smd_threefry_uniform": (C.c_int, [C.POINTER(C.c_uint32), _P, C.c_longlong, C.c_float, C.c_float, _P]),
+    "smd_threefry_uniform_slice": (C.c_int, [C.POINTER(C.c_uint32), _P, C.c_longlong, C.c_longlong, C.c_longlong,
+                                             C.c_float, C.c_float, _P]),
     "smd_threefry_split": (C.c_int, [C.POINTER(C.c_uint32), C.c_int, C.POINTER(C.c_uint32)]),
+    "smd_langevin_setup": (C.c_int, [_P, C.POINTER(C.c_float), C.c_int, C.c_int, C.c_float, C.c_int,
+                                     C.POINTER(C.c_uint32), _P]),
+    "smd_langevin_sample": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, C.c_int, _P, _P, C.c_int, _P]),
+    "smd_langevin_tables": (C.c_int, [C.POINTER(C.c_float), C.c_int, C.c_int, C.c_float, C.c_int, C.c_int,
+                                      C.POINTER(C.c_float), C.POINTER(C.c_int)]),
     "smd_gemm_bf16": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                 _P, _P, C.c_int, _P, _P, _P, _P, _P, _P]),
     "smd_debug_forward_save": (C.c_int, [_P, _P, _P, _P, C.c_int, _P, _P]),

@@ -61,20 +61,29 @@ def generate_samples(sample_shape, num_samples, rng_seed=1):
     torch.cuda.synchronize()
     logging.info("Generated samples in %f seconds", time.time() - t0)
     generated = parallel.gather_rows(generated)
-    collection = parallel.gather_rows(collection.transpose(0, 1).contiguous()).transpose(0, 1)
-    return generated.cpu().numpy(), collection.cpu().numpy(), ld_metrics
+    if collection is not None:      # consistent Langevin dynamics keeps no collection
+        collection = parallel.gather_rows(collection.transpose(0, 1).contiguous()).transpose(0, 1).cpu().numpy()
+    return generated.cpu().numpy(), collection, ld_metrics
 
 
 def infill_samples(samples, masks, rng_seed=1):
-    """sample_ncsn.py:189-242: keep the masked (=1) entries of `samples`, regenerate the rest."""
+    """sample_ncsn.py:189-242: keep the masked (=1) entries of `samples`, regenerate the rest with the --sampling
+    chain (ald or ddpm; cas has no infilling, as upstream)."""
     del rng_seed
+    if FLAGS.sampling == "ald":
+        algorithm = ebm_utils.annealed_langevin_dynamics
+    elif FLAGS.sampling == "cas":
+        algorithm = ebm_utils.consistent_langevin_dynamics
+    elif FLAGS.sampling == "ddpm":
+        algorithm = ebm_utils.diffusion_dynamics
+    else:
+        raise ValueError(f"Unknown sampling algorithm: {FLAGS.sampling}")
     rng, optimizer = _restore(FLAGS.model_dir, samples.shape[1:])
     sigmas = ebm_utils.create_noise_schedule(FLAGS.sigma_begin, FLAGS.sigma_end, FLAGS.num_sigmas, FLAGS.schedule_type)
     init_rng, ld_rng = random.split(rng)
     init = random.uniform(init_rng, samples.shape)      # upstream initialises the infill chain with uniform noise
-    generated, collection, ld_metrics = ebm_utils.diffusion_dynamics(ld_rng, optimizer.target, sigmas, init,
-                                                                     FLAGS.ld_epsilon, FLAGS.ld_steps, FLAGS.denoise,
-                                                                     True, samples, masks)
+    generated, collection, ld_metrics = algorithm(ld_rng, optimizer.target, sigmas, init, FLAGS.ld_epsilon,
+                                                  FLAGS.ld_steps, FLAGS.denoise, True, samples, masks)
     return generated.cpu().numpy(), collection.cpu().numpy(), ebm_utils.collate_sampling_metrics(ld_metrics)
 
 
@@ -162,7 +171,8 @@ def main(argv):
             a, normalize=FLAGS.normalize, data_min=eval_ds.min, data_max=eval_ds.max, slice_idx=slice_idx,
             dim_weights=dim_w, out_channels=int(FLAGS.data_shape[-1]))
         out = os.path.join(FLAGS.model_dir, FLAGS.sampling_dir, "ncsn")
-        _save(inv(collection), os.path.join(out, "collection.pkl"))
+        if collection is not None:
+            _save(inv(collection), os.path.join(out, "collection.pkl"))
         _save(inv(real), os.path.join(out, "real.pkl"))
         _save(inv(generated), os.path.join(out, "generated.pkl"))
     parallel.shutdown()

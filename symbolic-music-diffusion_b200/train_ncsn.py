@@ -251,7 +251,7 @@ def sample(scorenet, sigmas, rng, sample_shape, num_samples=2400, sampling="ald"
     """train_ncsn.py:499-551: initial noise from `rng`, dispatch on the sampler, collate metrics.
 
     shard=(rank, world) (not in the reference): this process generates rows [rank*n/world, (rank+1)*n/world) of the
-    num_samples-sample run -- its slice of the initial normal draw and of every step's noise stream."""
+    num_samples-sample run -- its slice of the initial draw and of every step's noise stream."""
     if sampling == "ddpm":
         algorithm = ebm_utils.diffusion_dynamics
     elif sampling == "ald":
@@ -261,21 +261,18 @@ def sample(scorenet, sigmas, rng, sample_shape, num_samples=2400, sampling="ald"
     else:
         raise ValueError(f"Unknown sampling algorithm: {sampling}")
     init_rng, ld_rng = random.split(rng)
-    if sampling != "ddpm":
-        # train_ncsn.py:541-547: uniform start with zero mean / unit variance; no data-parallel sharding of this family
-        rho = float(np.sqrt(np.float32(12)) / 2)
-        init = random.uniform(init_rng, (num_samples, *sample_shape), -rho, rho)
-        generated, collection, ld_metrics = algorithm(ld_rng, scorenet, sigmas, init, epsilon, steps, denoise, False)
-        return generated, collection, ebm_utils.collate_sampling_metrics(ld_metrics)
-    if shard is None or shard[1] <= 1:
-        init = random.normal(init_rng, (num_samples, *sample_shape))
-        generated, collection, ld_metrics = algorithm(ld_rng, scorenet, sigmas, init, epsilon, steps, denoise, False)
-    else:
+    rows, kw = None, {}
+    if shard is not None and shard[1] > 1:
         local = parallel.shard_size(num_samples)
-        first = shard[0] * local
-        init = random.normal(init_rng, (num_samples, *sample_shape), rows=(first, local))
-        generated, collection, ld_metrics = algorithm(ld_rng, scorenet, sigmas, init, epsilon, steps, denoise, False,
-                                                      shard=(first, num_samples))
+        rows, kw = (shard[0] * local, local), dict(shard=(shard[0] * local, num_samples))
+    shape = (num_samples, *sample_shape)
+    if sampling != "ddpm":
+        # train_ncsn.py:541-547: uniform start with zero mean / unit variance
+        rho = float(np.sqrt(np.float32(12)) / 2)
+        init = random.uniform(init_rng, shape, -rho, rho, rows=rows)
+    else:
+        init = random.normal(init_rng, shape, rows=rows)
+    generated, collection, ld_metrics = algorithm(ld_rng, scorenet, sigmas, init, epsilon, steps, denoise, False, **kw)
     return generated, collection, ebm_utils.collate_sampling_metrics(ld_metrics)
 
 
