@@ -87,6 +87,8 @@ long long smd_arena_floats(const smd_plan* plan);
 int smd_tensor_info(const smd_plan* plan, int index, char* name, int name_cap, long long* offset, int* shape4,
                     int* ndim);
 size_t smd_workspace_bytes(const smd_plan* plan);
+/* Binds a device workspace of at least `smd_workspace_bytes` (1024-byte aligned) and zeroes it.  Rebinding forgets the
+ * objective, DSM, sampler and Langevin setups and the packed weights: call those setups and smd_pack_weights again. */
 int smd_bind_workspace(smd_plan* plan, void* workspace, size_t bytes);
 /* Refresh the bf16 tensor-core operand copies from the fp32 arena (after init / restore / every optimizer step). */
 int smd_pack_weights(smd_plan* plan, const float* params, smd_stream_t stream);

@@ -628,7 +628,6 @@ static int grads_entry(smd_plan* p, const float* params, const float* x0, const 
   if (!p->cfg.training) { set_error("plan was not created with training = 1"); return SMD_ERR_STATE; }
   if (!p->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
   if (batch < 1 || batch > p->cfg.max_batch || global_batch < batch) { set_error("batch out of range"); return SMD_ERR_INVALID; }
-  const bool capturable = st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread;
   auto impl = [&](const float* x0_, const float* ua_, const float* eps_, const float* v_, const float* const* ind_,
                   bool capturing) {
     if (objective == kObjSsm)
@@ -636,27 +635,24 @@ static int grads_entry(smd_plan* p, const float* params, const float* x0, const 
     if (objective == kObjMdn) return mdn_grads_impl(p, params, x0_, ind_, batch, global_batch, grads, loss_sum, st, capturing);
     return grads_impl(p, params, x0_, ua_, eps_, ind_, batch, global_batch, grads, loss_sum, st, capturing, objective);
   };
-  if (!capturable) return impl(x0, used_alpha, eps, v, nullptr, false);
+  if (!capturable(st)) return impl(x0, used_alpha, eps, v, nullptr, false);
   // Graph replay: the pass's ~150 launches on three streams (dX chain, weight-gradient GEMMs, FiLM generator) are
   // captured once into one CUDA graph with the same fork / join structure.  The per-step inputs (x0, used_alpha, eps)
   // reach the kernels through a device pointer table, so new input tensors do not force a re-capture; the events a
   // data-parallel caller waits on (smd_wait_tail_grads) are external event-record nodes of the graph.
-  const bool same = p->train_graph.exec && p->tg_params == params && p->tg_grads == grads && p->tg_loss == loss_sum &&
-                    p->tg_batch == batch && p->tg_global == global_batch && p->tg_objective == objective;
+  const GraphKey key = graph_key(params, grads, loss_sum, batch, global_batch, objective);
   const float** ind = p->at<const float*>(p->train.ind);
-  if (!same) {
-    const bool warm = p->tg_warm && p->tg_params == params && p->tg_batch == batch && p->tg_objective == objective;
+  if (!p->train_graph.replays(key)) {
     p->train_graph.drop();
-    p->tg_params = params; p->tg_grads = grads; p->tg_loss = loss_sum; p->tg_batch = batch; p->tg_global = global_batch;
-    p->tg_objective = objective;
-    if (!warm) {
+    const GraphKey warm = graph_key(params, batch, objective);
+    if (p->train_warm != warm) {
       // first use of this configuration runs eagerly: lazy one-time calls (function attributes, stream / event
       // creation) stay out of the capture
-      p->tg_warm = true;
+      p->train_warm = warm;
       return impl(x0, used_alpha, eps, v, nullptr, false);
     }
-    const int rc = p->train_graph.capture(st, [&] { return impl(nullptr, nullptr, nullptr, nullptr, ind, true); },
-                                          "train graph");
+    const int rc = p->train_graph.capture(
+        st, key, [&] { return impl(nullptr, nullptr, nullptr, nullptr, ind, true); }, "train graph");
     if (rc) return rc;
   }
   // (pageable source: the driver stages these 32 bytes before returning, so the host array may die with this frame)

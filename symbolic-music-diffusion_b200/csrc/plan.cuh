@@ -1,7 +1,9 @@
 // Shared internals of libsmd: the plan object, its parameter and workspace layouts, error helpers and launch-count macros.
 #pragma once
+#include <cstdint>
 #include <cstring>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/smd.h"
@@ -133,20 +135,39 @@ struct TrainState {
 // loss kernels receive.
 enum Objective : int { kObjDdpm = 0, kObjDsm = 1, kObjSsm = 2, kObjMdn = 3 };
 
+// The sampler chain whose tables (coef / keys / slots / t_ptr, the FiLM table) the workspace holds: the DDPM sampler
+// and the Langevin chain share those regions, so at most one of them is set up at a time.
+enum Chain : int { kChainNone = 0, kChainDdpm = 1, kChainLangevin = 2 };
+
+// The legacy default stream cannot be captured into a CUDA graph.
+inline bool capturable(cudaStream_t st) { return st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread; }
+
+// The call arguments (pointers and integers) a graph was captured with.
+using GraphKey = std::vector<uintptr_t>;
+template <typename T>
+inline uintptr_t key_word(T* ptr) { return reinterpret_cast<uintptr_t>(ptr); }
+inline uintptr_t key_word(long long v) { return static_cast<uintptr_t>(v); }
+template <typename... A>
+inline GraphKey graph_key(A... a) { return GraphKey{key_word(a)...}; }
+
 // A launch sequence captured once and replayed as one CUDA graph.  g_launches counts the captured launches once per
 // replay (launch), not at capture.
 struct CapturedGraph {
   cudaGraphExec_t exec = nullptr;
   long long nodes = 0;   // launches recorded by the capture
+  GraphKey key;          // the arguments of the capture
 
+  // a replay is valid only for the arguments the graph was captured with
+  bool replays(const GraphKey& k) const { return exec && key == k; }
   void drop() {
     if (exec) cudaGraphExecDestroy(exec);
     exec = nullptr;
+    key.clear();
   }
-  // Replaces the graph by what body() enqueues on st (a capturable stream); returns body's error code or SMD_ERR_CUDA,
-  // leaving no graph behind on failure.
+  // Replaces the graph by what body() enqueues on st (a capturable stream) for the arguments `k`; returns body's error
+  // code or SMD_ERR_CUDA, leaving no graph behind on failure.
   template <typename Body>
-  int capture(cudaStream_t st, Body&& body, const char* what) {
+  int capture(cudaStream_t st, GraphKey k, Body&& body, const char* what) {
     drop();
     cudaGraph_t graph = nullptr;
     const long long before = g_launches.load();
@@ -159,7 +180,7 @@ struct CapturedGraph {
     if (ce != cudaSuccess) { set_error(std::string(what) + " capture: " + cudaGetErrorString(ce)); return SMD_ERR_CUDA; }
     ce = cudaGraphInstantiate(&exec, graph, 0);
     cudaGraphDestroy(graph);
-    if (ce == cudaSuccess) return SMD_OK;
+    if (ce == cudaSuccess) { key = std::move(k); return SMD_OK; }
     exec = nullptr;
     set_error(std::string(what) + " instantiate: " + cudaGetErrorString(ce));
     return SMD_ERR_CUDA;
@@ -211,38 +232,18 @@ struct smd_plan {
   int T = 0;
   int T_obj = 0;  // schedule length of the training objective
   int L_dsm = 0;  // length of the sigma schedule of the denoising-score-matching objective (smd_dsm_setup)
-  // FiLM table of the sampler: [K][T][2*Md]; when film_tab_on, run_forward skips the generator and the tail reads
-  // row film_row (host) or *film_row_dev (graph replay) of the table
-  bool film_tab_ready = false, film_tab_on = false;
-  int film_row = 0;
-  const int* film_row_dev = nullptr;
+  // FiLM table of the sampler: [K][T][2*Md], built for the parameters film_tab_params (see FilmRows)
+  bool film_tab_ready = false;
   const float* film_tab_params = nullptr;
-  bool sampler_ready = false;
   long long shard_first_row = 0, shard_total_rows = 0;   // smd_sampler_set_shard
-  // graph replay of one smd_ddpm_sample step, and the arguments it was captured with
-  smd::CapturedGraph sample_graph;
-  int graph_n = -1;
-  const float* graph_params = nullptr;
-  float* graph_x = nullptr;
-  const float* graph_infill_x = nullptr;
-  const float* graph_infill_mask = nullptr;
-  float* graph_collection = nullptr;
-  float* graph_metrics = nullptr;
-  // Langevin chain (smd_langevin_setup / smd_langevin_sample).  It shares the coef / slots / t_ptr / ftab* regions with
-  // the DDPM sampler: each setup invalidates the other (sampler_ready / langevin_ready, the FiLM table, both graphs).
-  // T holds the number of noise levels L while a Langevin schedule is set (the FiLM table has one row per level).
-  bool langevin_ready = false;
-  int lv_kind = 0, lv_steps = 1;   // kind (0 annealed, 1 consistent), steps per level
+  // The chain set up (smd_sampler_setup / smd_langevin_setup), and the graph replay of one step of it (smd_ddpm_sample
+  // / smd_langevin_sample).  T holds the number of noise levels L while a Langevin schedule is set (the FiLM table has
+  // one row per level).
+  smd::Chain chain = smd::kChainNone;
+  smd::CapturedGraph chain_graph;
+  int lv_kind = 0, lv_steps = 1;   // Langevin: kind (0 annealed, 1 consistent), steps per level
   uint32_t lv_key[2] = {0u, 0u};
   float lv_sigma_last = 0.f;
-  smd::CapturedGraph langevin_graph;
-  int lg_n = -1, lg_rows = 0;
-  const float* lg_params = nullptr;
-  float* lg_x = nullptr;
-  const float* lg_infill_x = nullptr;
-  const float* lg_infill_mask = nullptr;
-  float* lg_collection = nullptr;
-  float* lg_metrics = nullptr;
   cudaStream_t own_stream = nullptr;
   cudaEvent_t own_event = nullptr;
   // training: the FiLM generator (forward and backward) runs on a side stream, concurrently with the trunk
@@ -252,14 +253,10 @@ struct smd_plan {
   smd::TrainState train;
   cudaEvent_t ev_gz = nullptr;      // gradient arena zeroed (on the weight-gradient stream)
   cudaEvent_t evx_join = nullptr;   // "FiLM generator gradients final", waitable from outside the graph
-  // graph replay of the grads entry points (backward.cu), and the arguments it was captured with
+  // graph replay of the grads entry points (backward.cu), and the key (params, batch, objective) of the last call that
+  // ran eagerly: the first call of a configuration runs eagerly, the next one captures
   smd::CapturedGraph train_graph;
-  bool tg_warm = false;
-  const float* tg_params = nullptr;
-  float* tg_grads = nullptr;
-  float* tg_loss = nullptr;
-  int tg_batch = 0, tg_global = 0;
-  smd::Objective tg_objective = smd::kObjDdpm;
+  smd::GraphKey train_warm;
 
   template <typename Tp>
   Tp* at(size_t off) const { return reinterpret_cast<Tp*>(ws + off); }
@@ -273,18 +270,23 @@ inline GemmEpilogue epi() {
   memset(&e, 0, sizeof(e));
   return e;
 }
+// Where the res-blocks' FiLM scale / shift rows come from.  table == nullptr: the FiLM generator runs on the
+// conditioning values t.  Otherwise the sampler's FiLM table (reg.ftab, [K][T][2*Md]): row `row`, or *row_dev when
+// row_dev is set (graph replay).
+struct FilmRows { const float* table = nullptr; int row = 0; const int* row_dev = nullptr; };
 // raw_out: DenseNCSN only -- leave out the final division by sigma (the training path differentiates through it itself)
 // save: training forward -- keep the unfused kernels and write the save-only outputs the backward pass reads
 // tangent: DenseNCSN only -- also push the tangent already cast into reg.xbt through the network (Jacobian-vector
 // product, raw output tangent into reg.yt); it reads the primal row statistics of each LayerNorm
 int run_forward(smd_plan* p, const float* params, const float* x, const float* t, int t_broadcast, int batch,
-                float* y, cudaStream_t st, bool save, bool raw_out = false, bool tangent = false);
+                float* y, cudaStream_t st, bool save, bool raw_out = false, bool tangent = false, FilmRows film = {});
 int train_bind(smd_plan* p);
 int ensure_side_stream(smd_plan* p);
 // Every forward GEMM goes through here (bf16x3 passes, and the per-tile row statistics of wide LayerNorm `ln_slot`).
 cudaError_t gemm(smd_plan* p, const GemmOp& op, int M, GemmEpilogue e, cudaStream_t st, int ln_slot = -1);
 // The residual tail from u[0] (row statistics in stats[0]) through out_ln and the output GEMM into y, M rows.
-int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, float* y, cudaStream_t st, bool tangent);
+int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, float* y, cudaStream_t st, bool tangent,
+             FilmRows film = {});
 // host threefry block function and jax.random.split (out: num x 2 words)
 void h_threefry(uint32_t k0, uint32_t k1, uint32_t& x0, uint32_t& x1);
 void h_split(const uint32_t key[2], int num, uint32_t* out);

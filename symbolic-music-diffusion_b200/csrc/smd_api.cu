@@ -332,25 +332,36 @@ static LnStats ln_stats(smd_plan* p, int ln_slot) {
   return n > 0 ? LnStats{p->at<float>(p->reg.stats_part), n, totals} : LnStats{nullptr, 0, totals};
 }
 
-// FiLM generator for all K blocks: t (R values) -> ss[k][R][2*Md]   (models/ncsn.py:47-61)
-static int run_film(smd_plan* p, const float* params, const float* t, int R, cudaStream_t st, bool save) {
+// Per-block buffers of the FiLM generator: d1 output (after swish), its pre-activation (or null), d2 output, and the
+// block's scale | shift rows.
+struct FilmBuffers { float* e1; float* e1pre; float* e2; float* ss; };
+
+// FiLM generator for all K blocks (models/ncsn.py:47-61): t (R values) -> noise encoding into enc -> per block k,
+// d1 + swish -> d2 -> scale | shift rows, into the buffers bufs(k) returns.
+template <typename BlockBuffers>
+static int film_generator(smd_plan* p, const float* params, const float* t, int R, float* enc, BlockBuffers bufs,
+                          cudaStream_t st, const char* what) {
   const int Md = p->cfg.mlp_dims;
-  const WorkspaceLayout& w = p->reg;
-  float* enc = p->at<float>(w.enc);
-  float* ss = p->at<float>(w.ss);
-  launch_noise_encoding(t, p->at<float>(w.freqs), enc, R, st); CNT();
+  launch_noise_encoding(t, p->at<float>(p->reg.freqs), enc, R, st); CNT();
   for (int k = 0; k < p->K; ++k) {
     const FilmParams& f = p->par.block[k].film;
-    float* e1 = p->at<float>(w.e1[k]);
-    float* e2 = p->at<float>(w.e2[k]);
-    float* e1pre = save ? p->at<float>(w.e1pre[k]) : nullptr;
-    launch_small_linear(enc, params + f.d1.kernel, params + f.d1.bias, e1, R, kFilmEmb, kFilmHid, 2, st, e1pre); CNT();
-    launch_small_linear(e1, params + f.d2.kernel, params + f.d2.bias, e2, R, kFilmHid, kFilmHid, 0, st); CNT();
-    launch_small_linear(e2, params + f.ss.kernel, params + f.ss.bias,
-                        ss + static_cast<size_t>(k) * p->cfg.max_batch * 2 * Md, R, kFilmHid, 2 * Md, 0, st); CNT();
+    const FilmBuffers b = bufs(k);
+    launch_small_linear(enc, params + f.d1.kernel, params + f.d1.bias, b.e1, R, kFilmEmb, kFilmHid, 2, st, b.e1pre); CNT();
+    launch_small_linear(b.e1, params + f.d2.kernel, params + f.d2.bias, b.e2, R, kFilmHid, kFilmHid, 0, st); CNT();
+    launch_small_linear(b.e2, params + f.ss.kernel, params + f.ss.bias, b.ss, R, kFilmHid, 2 * Md, 0, st); CNT();
   }
-  SMD_LAUNCH_CHECK("film");
+  SMD_LAUNCH_CHECK(what);
   return SMD_OK;
+}
+
+// The generator on the forward pass's conditioning values: ss[k][R][2*Md] (and, training, the pre-activations e1pre)
+static int run_film(smd_plan* p, const float* params, const float* t, int R, cudaStream_t st, bool save) {
+  const WorkspaceLayout& w = p->reg;
+  const size_t ss_stride = static_cast<size_t>(p->cfg.max_batch) * 2 * p->cfg.mlp_dims;
+  return film_generator(p, params, t, R, p->at<float>(w.enc), [&](int k) {
+    return FilmBuffers{p->at<float>(w.e1[k]), save ? p->at<float>(w.e1pre[k]) : nullptr, p->at<float>(w.e2[k]),
+                       p->at<float>(w.ss) + k * ss_stride};
+  }, st, "film");
 }
 
 int ensure_side_stream(smd_plan* p) {
@@ -373,7 +384,8 @@ int ensure_side_stream(smd_plan* p) {
 // The FiLM'd residual tail shared by both architectures (models/ncsn.py:173-178, models/shared.py:61-75).
 // On entry u (fp32 [M][Md]) and stats[0] hold the block input and its row statistics.
 // tangent: run the tangent pass next to it (ut[0] and the primal statistics are ready; see run_forward).
-int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, float* y, cudaStream_t st, bool tangent) {
+int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, float* y, cudaStream_t st, bool tangent,
+             FilmRows film) {
   const int Md = p->cfg.mlp_dims, C = p->cfg.channels;
   const WorkspaceLayout& w = p->reg;
   float* stats = p->at<float>(w.stats);
@@ -384,9 +396,9 @@ int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, fl
     const BlockParams& bp = p->par.block[k];
     const float* scale = p->mdn() ? nullptr : ss + static_cast<size_t>(k) * p->cfg.max_batch * 2 * Md;
     const int* frow_dev = nullptr;
-    if (p->film_tab_on) {
-      scale = p->at<float>(w.ftab) + static_cast<size_t>(k) * p->T * 2 * Md;
-      if (p->film_row_dev) frow_dev = p->film_row_dev; else scale += static_cast<size_t>(p->film_row) * 2 * Md;
+    if (film.table) {
+      scale = film.table + static_cast<size_t>(k) * p->T * 2 * Md;
+      if (film.row_dev) frow_dev = film.row_dev; else scale += static_cast<size_t>(film.row) * 2 * Md;
     }
     const float* shift = scale ? scale + Md : nullptr;
     float* u_in = p->at<float>(w.u[k]);
@@ -459,7 +471,7 @@ int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, fl
 }
 
 int run_forward(smd_plan* p, const float* params, const float* x, const float* t, int t_broadcast, int batch,
-                float* y, cudaStream_t st, bool save, bool raw_out, bool tangent) {
+                float* y, cudaStream_t st, bool save, bool raw_out, bool tangent, FilmRows film) {
   const smd_config& c = p->cfg;
   if (!p->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
   if (!p->packed) { set_error("smd_pack_weights has not been called"); return SMD_ERR_STATE; }
@@ -472,7 +484,7 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
   SMD_CUDA(cudaMemsetAsync(stats, 0, static_cast<size_t>(2 * p->K + 1) * p->Mp * 2 * 4, st));
   int rc = SMD_OK;
   bool film_on_side = false;
-  if (!p->film_tab_on && !p->mdn()) {
+  if (!film.table && !p->mdn()) {
     if (save) {
       // training: the FiLM generator only feeds the tail, so it runs on a side stream next to the trunk
       rc = ensure_side_stream(p);
@@ -576,7 +588,7 @@ int run_forward(smd_plan* p, const float* params, const float* x, const float* t
   }
   SMD_LAUNCH_CHECK("trunk");
   if (film_on_side) SMD_CUDA(cudaStreamWaitEvent(st, p->ev_film, 0));
-  rc = run_tail(p, params, M, S, t_broadcast, y, st, tangent);
+  rc = run_tail(p, params, M, S, t_broadcast, y, st, tangent, film);
   if (rc) return rc;
   if (c.arch == SMD_ARCH_DENSE_NCSN && !raw_out) {   // models/ncsn.py:97: output = x / sigmas
     launch_scale_rows(y, t, t_broadcast, batch, S * C, st); CNT();
@@ -694,6 +706,41 @@ static int objective_draws(const smd_plan* plan, const uint32_t host_key[2], int
   return SMD_OK;
 }
 
+// State axes and shard counters of a chain step.  The dense networks' (N, D) states use axis 1 = D (the metrics' axis
+// 1, utils/ebm_utils.py:380-384).  sharded: the step draws its slice of the global threefry streams
+// (smd_sampler_set_shard).
+template <typename StepArgs>
+static void chain_geometry(const smd_plan* plan, StepArgs& a, bool sharded) {
+  a.S = plan->cfg.seq_len; a.C = plan->cfg.channels;
+  if (plan->cfg.arch != SMD_ARCH_TRANSFORMER_DDPM) { a.S = plan->cfg.channels; a.C = 1; }
+  if (sharded && plan->shard_total_rows > 0) {
+    const long long per = static_cast<long long>(a.S) * a.C;
+    a.rng_first = static_cast<uint32_t>(plan->shard_first_row * per);
+    a.rng_total = static_cast<uint32_t>(plan->shard_total_rows * per);
+  }
+}
+
+// Graph replay needs a capturable stream: returns st itself, or the plan's own stream ordered after st (join_replay
+// orders st after it again).
+static int replay_stream(smd_plan* plan, cudaStream_t st, cudaStream_t* cs) {
+  *cs = st;
+  if (capturable(st)) return SMD_OK;
+  if (!plan->own_stream) {
+    SMD_CUDA(cudaStreamCreateWithFlags(&plan->own_stream, cudaStreamNonBlocking));
+    SMD_CUDA(cudaEventCreateWithFlags(&plan->own_event, cudaEventDisableTiming));
+  }
+  SMD_CUDA(cudaEventRecord(plan->own_event, st));
+  SMD_CUDA(cudaStreamWaitEvent(plan->own_stream, plan->own_event, 0));
+  *cs = plan->own_stream;
+  return SMD_OK;
+}
+static int join_replay(smd_plan* plan, cudaStream_t st, cudaStream_t cs) {
+  if (cs == st) return SMD_OK;
+  SMD_CUDA(cudaEventRecord(plan->own_event, cs));
+  SMD_CUDA(cudaStreamWaitEvent(st, plan->own_event, 0));
+  return SMD_OK;
+}
+
 }  // namespace smd
 
 // =====================================================================================================
@@ -769,8 +816,7 @@ int smd_mdn_plan_create(const smd_config* cfg, int num_components, smd_plan** ou
 
 void smd_plan_destroy(smd_plan* plan) {
   if (!plan) return;
-  plan->sample_graph.drop();
-  plan->langevin_graph.drop();
+  plan->chain_graph.drop();
   plan->train_graph.drop();
   if (plan->evx_join) cudaEventDestroy(plan->evx_join);
   if (plan->ev_gz) cudaEventDestroy(plan->ev_gz);
@@ -803,15 +849,26 @@ int smd_tensor_info(const smd_plan* plan, int index, char* name, int name_cap, l
 }
 size_t smd_workspace_bytes(const smd_plan* plan) { return plan->ws_bytes; }
 
+// Forgets all plan state that describes workspace contents (a newly bound workspace starts zeroed): the packed
+// weights, the objective / DSM schedules, the sampler chain and the FiLM table, and the graphs whose kernels point
+// into the old workspace.
+static void forget_workspace_contents(smd_plan* plan) {
+  plan->packed = false;
+  plan->T_obj = 0;
+  plan->L_dsm = 0;
+  plan->chain = kChainNone;
+  plan->chain_graph.drop();
+  plan->film_tab_ready = false;
+  plan->train_graph.drop();
+  plan->train_warm.clear();
+}
+
 int smd_bind_workspace(smd_plan* plan, void* workspace, size_t bytes) {
   if (!workspace || bytes < plan->ws_bytes) { set_error("workspace too small"); return SMD_ERR_INVALID; }
   if (reinterpret_cast<uintptr_t>(workspace) % 1024 != 0) { set_error("workspace must be 1024-byte aligned"); return SMD_ERR_INVALID; }
   plan->ws = static_cast<uint8_t*>(workspace);
+  forget_workspace_contents(plan);
   SMD_CUDA(cudaMemset(workspace, 0, plan->ws_bytes));  // padded rows / columns of every operand start finite
-  plan->packed = false;
-  plan->sampler_ready = false;
-  plan->train_graph.drop();
-  plan->tg_warm = false;
   int rc = build_ops(plan);
   if (rc) return rc;
   float f[64];
@@ -997,8 +1054,8 @@ int smd_langevin_step(smd_plan* plan, const float* x, const float* grad, int n, 
   a.alpha = alpha; a.noise_coef = noise_coef; a.infill_sigma = infill_sigma;
   a.infill_x = infill_x; a.infill_mask = infill_mask; a.infill_z = infill_z;
   a.x_next = x_next; a.collection_slot = collection_slot; a.metrics = metrics4;
-  a.N = n; a.S = plan->cfg.seq_len; a.C = plan->cfg.channels;
-  if (plan->cfg.arch != SMD_ARCH_TRANSFORMER_DDPM) { a.S = plan->cfg.channels; a.C = 1; }   // (N, D) states: axis 1 = D
+  a.N = n;
+  chain_geometry(plan, a, /*sharded=*/false);
   launch_langevin_step(a, static_cast<cudaStream_t>(stream)); CNT();
   SMD_LAUNCH_CHECK("langevin_step");
   return SMD_OK;
@@ -1091,11 +1148,9 @@ int smd_sampler_setup(smd_plan* plan, const float* host_betas, int T, const uint
   SMD_CUDA(cudaMemcpyAsync(plan->at<int>(plan->reg.slots), slots.data(), slots.size() * 4, cudaMemcpyHostToDevice, st));
   SMD_CUDA(cudaStreamSynchronize(st));  // host vectors go out of scope
   plan->T = T;
-  plan->sampler_ready = true;
-  plan->langevin_ready = false;   // the Langevin chain's tables lived in the same regions
+  plan->chain = kChainDdpm;
   plan->film_tab_ready = false;
-  plan->sample_graph.drop();
-  plan->langevin_graph.drop();
+  plan->chain_graph.drop();
   return SMD_OK;
 }
 
@@ -1111,25 +1166,26 @@ __global__ void gather_cond_kernel(const float* __restrict__ coef, float* __rest
 static int ensure_film_table(smd_plan* plan, const float* params, int stride, int offset, cudaStream_t st) {
   if (plan->cfg.sampler_T <= 0 || plan->T > plan->cfg.sampler_T) return SMD_OK;   // per-step generator instead
   if (plan->film_tab_ready && plan->film_tab_params == params) return SMD_OK;
-  const int T = plan->T, Md = plan->cfg.mlp_dims;
-  float* tv = plan->at<float>(plan->reg.ftab_t);
-  float* enc = plan->at<float>(plan->reg.ftab_enc);
-  float* e1 = plan->at<float>(plan->reg.ftab_e1);
-  float* e2 = plan->at<float>(plan->reg.ftab_e2);
-  float* tab = plan->at<float>(plan->reg.ftab);
-  gather_cond_kernel<<<(T + 255) / 256, 256, 0, st>>>(plan->at<float>(plan->reg.coef), tv, T, stride, offset); CNT();
-  launch_noise_encoding(tv, plan->at<float>(plan->reg.freqs), enc, T, st); CNT();
-  for (int k = 0; k < plan->K; ++k) {
-    const FilmParams& f = plan->par.block[k].film;
-    launch_small_linear(enc, params + f.d1.kernel, params + f.d1.bias, e1, T, kFilmEmb, kFilmHid, 2, st); CNT();
-    launch_small_linear(e1, params + f.d2.kernel, params + f.d2.bias, e2, T, kFilmHid, kFilmHid, 0, st); CNT();
-    launch_small_linear(e2, params + f.ss.kernel, params + f.ss.bias,
-                        tab + static_cast<size_t>(k) * T * 2 * Md, T, kFilmHid, 2 * Md, 0, st); CNT();
-  }
-  SMD_LAUNCH_CHECK("film table");
+  const int T = plan->T;
+  const WorkspaceLayout& w = plan->reg;
+  float* tv = plan->at<float>(w.ftab_t);
+  const size_t tab_stride = static_cast<size_t>(T) * 2 * plan->cfg.mlp_dims;
+  gather_cond_kernel<<<(T + 255) / 256, 256, 0, st>>>(plan->at<float>(w.coef), tv, T, stride, offset); CNT();
+  const int rc = film_generator(plan, params, tv, T, plan->at<float>(w.ftab_enc), [&](int k) {
+    return FilmBuffers{plan->at<float>(w.ftab_e1), nullptr, plan->at<float>(w.ftab_e2),
+                       plan->at<float>(w.ftab) + k * tab_stride};
+  }, st, "film table");
+  if (rc) return rc;
   plan->film_tab_ready = true;
   plan->film_tab_params = params;
   return SMD_OK;
+}
+
+// The FiLM table rows of a network call with `params`: row `row`, or *row_dev when row_dev is set; {} (run the
+// generator) when the table was not built for these parameters.
+static FilmRows film_table_rows(const smd_plan* plan, const float* params, int row, const int* row_dev) {
+  if (!plan->film_tab_ready || plan->film_tab_params != params) return FilmRows{};
+  return FilmRows{plan->at<float>(plan->reg.ftab), row, row_dev};
 }
 
 // one reverse step; t < 0 means "read t from the device scalar t_ptr" (graph replay)
@@ -1139,21 +1195,14 @@ static int reverse_step_impl(smd_plan* plan, const float* params, const float* x
   float* tvec = plan->at<float>(plan->reg.tvec);
   int* t_ptr = plan->at<int>(plan->reg.t_ptr);
   const float* coef = plan->at<float>(plan->reg.coef);
-  const bool use_tab = plan->film_tab_ready && plan->film_tab_params == params;
-  if (use_tab) {
-    plan->film_tab_on = true;
-    plan->film_row = (t >= 0) ? t : 0;
-    plan->film_row_dev = (t >= 0) ? nullptr : t_ptr;
-  } else if (t >= 0) {
+  const FilmRows film = film_table_rows(plan, params, t, t >= 0 ? nullptr : t_ptr);
+  if (!film.table) {
     // conditioning value sqrt(alpha_prod_t), shared by every sample (utils/ebm_utils.py:367-369)
-    SMD_CUDA(cudaMemcpyAsync(tvec, coef + 8 * t + 5, 4, cudaMemcpyDeviceToDevice, st));
-  } else {
-    launch_fill_cond(coef, t_ptr, tvec, 1, st); CNT();
+    if (t >= 0) SMD_CUDA(cudaMemcpyAsync(tvec, coef + 8 * t + 5, 4, cudaMemcpyDeviceToDevice, st));
+    else { launch_fill_cond(coef, t_ptr, tvec, 1, st); CNT(); }
   }
   float* eh = eps_hat ? eps_hat : plan->at<float>(plan->reg.eps_hat);
-  int rc = run_forward(plan, params, x, tvec, 1, n, eh, st, false);
-  plan->film_tab_on = false;
-  plan->film_row_dev = nullptr;
+  const int rc = run_forward(plan, params, x, tvec, 1, n, eh, st, false, false, false, film);
   if (rc) return rc;
   ReverseStepArgs a;
   memset(&a, 0, sizeof(a));
@@ -1165,14 +1214,8 @@ static int reverse_step_impl(smd_plan* plan, const float* params, const float* x
   a.t = t;
   a.infill_x = infill_x; a.infill_mask = infill_mask; a.infill_z = infill_z;
   a.x_next = x_next; a.collection = collection; a.metrics = metrics;
-  a.N = n; a.S = plan->cfg.seq_len; a.C = plan->cfg.channels; a.T = plan->T;
-  // 2-D states (N, D) of the dense networks: the metrics' axis 1 (utils/ebm_utils.py:380-384) is D itself
-  if (plan->cfg.arch != SMD_ARCH_TRANSFORMER_DDPM) { a.S = plan->cfg.channels; a.C = 1; }
-  if (plan->shard_total_rows > 0) {
-    const long long per = static_cast<long long>(a.S) * a.C;
-    a.rng_first = static_cast<uint32_t>(plan->shard_first_row * per);
-    a.rng_total = static_cast<uint32_t>(plan->shard_total_rows * per);
-  }
+  a.N = n; a.T = plan->T;
+  chain_geometry(plan, a, /*sharded=*/true);
   launch_reverse_step(a, st); CNT();
   SMD_LAUNCH_CHECK("reverse_step");
   return SMD_OK;
@@ -1184,8 +1227,7 @@ int smd_sampler_set_shard(smd_plan* plan, long long first_row, long long total_r
       total_rows * plan->cfg.seq_len * plan->cfg.channels > 0xFFFFFFFFll) { set_error("bad shard"); return SMD_ERR_INVALID; }
   plan->shard_first_row = first_row;
   plan->shard_total_rows = total_rows;
-  plan->sample_graph.drop();  // kernel args changed
-  plan->langevin_graph.drop();
+  plan->chain_graph.drop();  // kernel args changed
   return SMD_OK;
 }
 
@@ -1193,7 +1235,7 @@ int smd_ddpm_reverse_step(smd_plan* plan, const float* params, const float* x, i
                           const float* infill_x, const float* infill_mask, const float* infill_z, float* x_next,
                           float* eps_hat_or_null, float* collection, float* metrics, smd_stream_t stream) {
   if (reject_mdn(plan, "smd_ddpm_reverse_step")) return SMD_ERR_INVALID;
-  if (!plan->sampler_ready) { set_error("smd_sampler_setup has not been called"); return SMD_ERR_STATE; }
+  if (plan->chain != kChainDdpm) { set_error("smd_sampler_setup has not been called"); return SMD_ERR_STATE; }
   if (t < 0 || t >= plan->T) { set_error("t out of range"); return SMD_ERR_INVALID; }
   if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
   int rc0 = ensure_film_table(plan, params, 8, 5, static_cast<cudaStream_t>(stream));
@@ -1206,7 +1248,7 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
                     const float* infill_mask, float* collection, float* metrics, int use_graph,
                     smd_stream_t stream) {
   if (reject_mdn(plan, "smd_ddpm_sample")) return SMD_ERR_INVALID;
-  if (!plan->sampler_ready) { set_error("smd_sampler_setup has not been called"); return SMD_ERR_STATE; }
+  if (plan->chain != kChainDdpm) { set_error("smd_sampler_setup has not been called"); return SMD_ERR_STATE; }
   if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
   if (steps < 1 || steps > plan->T) { set_error("steps out of range"); return SMD_ERR_INVALID; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1221,44 +1263,27 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
     }
     return SMD_OK;
   }
-  // the legacy default stream cannot be captured: run the replay loop on a private stream ordered after `st`
-  cudaStream_t cs = st;
-  if (st == nullptr || st == cudaStreamLegacy || st == cudaStreamPerThread) {
-    if (!plan->own_stream) {
-      SMD_CUDA(cudaStreamCreateWithFlags(&plan->own_stream, cudaStreamNonBlocking));
-      SMD_CUDA(cudaEventCreateWithFlags(&plan->own_event, cudaEventDisableTiming));
-    }
-    SMD_CUDA(cudaEventRecord(plan->own_event, st));
-    SMD_CUDA(cudaStreamWaitEvent(plan->own_stream, plan->own_event, 0));
-    cs = plan->own_stream;
-  }
+  cudaStream_t cs;
+  { const int rc0 = replay_stream(plan, st, &cs); if (rc0) return rc0; }
   int* t_ptr = plan->at<int>(plan->reg.t_ptr);
   const int t0 = T - 1;
   SMD_CUDA(cudaMemcpyAsync(t_ptr, &t0, sizeof(int), cudaMemcpyHostToDevice, cs));
   SMD_CUDA(cudaStreamSynchronize(cs));  // t0 is a stack variable
-  const bool same = plan->sample_graph.exec && plan->graph_n == n && plan->graph_params == params && plan->graph_x == x &&
-                    plan->graph_infill_x == infill_x && plan->graph_infill_mask == infill_mask &&
-                    plan->graph_collection == collection && plan->graph_metrics == metrics;
-  if (!same) {
-    const int rc = plan->sample_graph.capture(cs, [&] {
+  const GraphKey key = graph_key(n, params, x, infill_x, infill_mask, collection, metrics);
+  if (!plan->chain_graph.replays(key)) {
+    const int rc = plan->chain_graph.capture(cs, key, [&] {
       const int r = reverse_step_impl(plan, params, x, n, -1, nullptr, infill_x, infill_mask, nullptr, x, nullptr,
                                       collection, metrics, cs);
       if (r == SMD_OK) { launch_step_advance(t_ptr, cs); CNT(); }
       return r;
     }, "sampler graph");
     if (rc) return rc;
-    plan->graph_n = n; plan->graph_params = params; plan->graph_x = x; plan->graph_infill_x = infill_x;
-    plan->graph_infill_mask = infill_mask; plan->graph_collection = collection; plan->graph_metrics = metrics;
   }
   for (int i = 0; i < steps; ++i) {
-    const int rc = plan->sample_graph.launch(cs);
+    const int rc = plan->chain_graph.launch(cs);
     if (rc) return rc;
   }
-  if (cs != st) {
-    SMD_CUDA(cudaEventRecord(plan->own_event, cs));
-    SMD_CUDA(cudaStreamWaitEvent(st, plan->own_event, 0));
-  }
-  return SMD_OK;
+  return join_replay(plan, st, cs);
 }
 
 // ---- Langevin chain (annealed / consistent Langevin dynamics, utils/ebm_utils.py:89-271) ----------------------------
@@ -1324,11 +1349,9 @@ int smd_langevin_setup(smd_plan* plan, const float* host_sigmas, int L, int step
   plan->lv_steps = kind == 0 ? steps_per_level : 1;
   plan->lv_key[0] = host_key[0]; plan->lv_key[1] = host_key[1];
   plan->lv_sigma_last = host_sigmas[L - 1];
-  plan->langevin_ready = true;
-  plan->sampler_ready = false;   // the DDPM tables lived in the same regions
+  plan->chain = kChainLangevin;
   plan->film_tab_ready = false;
-  plan->sample_graph.drop();
-  plan->langevin_graph.drop();
+  plan->chain_graph.drop();
   return SMD_OK;
 }
 
@@ -1336,24 +1359,20 @@ int smd_langevin_setup(smd_plan* plan, const float* host_sigmas, int L, int step
 // `row` (host); row < 0: the row is the chain state's noise level (graph replay).  Without a table (L > sampler_T) the
 // generator runs on tvec itself.
 static int langevin_forward(smd_plan* plan, const float* params, const float* x, int n, int row, cudaStream_t st) {
-  if (plan->film_tab_ready && plan->film_tab_params == params) {
-    plan->film_tab_on = true;
-    plan->film_row = row >= 0 ? row : 0;
-    plan->film_row_dev = row >= 0 ? nullptr : &plan->at<LangevinChainState>(plan->reg.t_ptr)->si;
-  }
-  const int rc = run_forward(plan, params, x, plan->at<float>(plan->reg.tvec), 1, n, plan->at<float>(plan->reg.eps_hat),
-                             st, false);
-  plan->film_tab_on = false;
-  plan->film_row_dev = nullptr;
-  return rc;
+  const int* level = &plan->at<LangevinChainState>(plan->reg.t_ptr)->si;
+  const FilmRows film = film_table_rows(plan, params, row, row >= 0 ? nullptr : level);
+  return run_forward(plan, params, x, plan->at<float>(plan->reg.tvec), 1, n, plan->at<float>(plan->reg.eps_hat), st,
+                     false, false, false, film);
 }
 
-static LangevinStepArgs langevin_args(const smd_plan* plan, const float* x, int n) {
+// the in-place update x <- x + alpha eps_hat (+ noise) after a network call; sharded for the chain's steps, not for the
+// final denoising step
+static LangevinStepArgs langevin_args(const smd_plan* plan, const float* x, int n, bool sharded) {
   LangevinStepArgs a;
   memset(&a, 0, sizeof(a));
   a.x = x; a.grad = plan->at<float>(plan->reg.eps_hat); a.x_next = const_cast<float*>(x);
-  a.N = n; a.S = plan->cfg.seq_len; a.C = plan->cfg.channels;
-  if (plan->cfg.arch != SMD_ARCH_TRANSFORMER_DDPM) { a.S = plan->cfg.channels; a.C = 1; }   // (N, D) states: axis 1 = D
+  a.N = n;
+  chain_geometry(plan, a, sharded);
   return a;
 }
 
@@ -1364,7 +1383,7 @@ int smd_langevin_sample(smd_plan* plan, const float* params, float* x, int n, co
   if (reject_mdn(plan, "smd_langevin_sample")) return SMD_ERR_INVALID;
   if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
   if ((infill_x == nullptr) != (infill_mask == nullptr)) { set_error("infill_x and infill_mask go together"); return SMD_ERR_INVALID; }
-  if (!plan->langevin_ready) { set_error("smd_langevin_setup has not been called"); return SMD_ERR_STATE; }
+  if (plan->chain != kChainLangevin) { set_error("smd_langevin_setup has not been called"); return SMD_ERR_STATE; }
   if (plan->lv_kind == 1 && (infill_x || collection)) {
     set_error("consistent Langevin dynamics has no infilling and no collection");
     return SMD_ERR_INVALID;
@@ -1376,17 +1395,8 @@ int smd_langevin_sample(smd_plan* plan, const float* params, float* x, int n, co
   const int* idx = plan->at<int>(plan->reg.slots);
   float* tvec = plan->at<float>(plan->reg.tvec);
   LangevinChainState* cst = plan->at<LangevinChainState>(plan->reg.t_ptr);
-  // graph replay: the legacy default stream cannot be captured, so the chain runs on a private stream ordered after st
   cudaStream_t cs = st;
-  if (use_graph && (st == nullptr || st == cudaStreamLegacy || st == cudaStreamPerThread)) {
-    if (!plan->own_stream) {
-      SMD_CUDA(cudaStreamCreateWithFlags(&plan->own_stream, cudaStreamNonBlocking));
-      SMD_CUDA(cudaEventCreateWithFlags(&plan->own_event, cudaEventDisableTiming));
-    }
-    SMD_CUDA(cudaEventRecord(plan->own_event, st));
-    SMD_CUDA(cudaStreamWaitEvent(plan->own_stream, plan->own_event, 0));
-    cs = plan->own_stream;
-  }
+  if (use_graph) { const int rc0 = replay_stream(plan, st, &cs); if (rc0) return rc0; }
   if (metrics) SMD_CUDA(cudaMemsetAsync(metrics, 0, sizeof(float) * 4 * L * T, cs));
   { const int rc0 = ensure_film_table(plan, params, kLangevinCoef, 0, cs); if (rc0) return rc0; }
   // the chain starts from the setup key at step 0 on every call
@@ -1400,15 +1410,10 @@ int smd_langevin_sample(smd_plan* plan, const float* params, float* x, int n, co
   auto step = [&](cudaStream_t s) -> int {
     const int r = langevin_forward(plan, params, x, n, -1, s);
     if (r) return r;
-    LangevinStepArgs a = langevin_args(plan, x, n);
+    LangevinStepArgs a = langevin_args(plan, x, n, /*sharded=*/true);
     a.infill_x = infill_x; a.infill_mask = infill_mask;
     a.collection_slot = collection; a.metrics = metrics;
     a.state = cst; a.coef = coef; a.L = L; a.T = T;
-    if (plan->shard_total_rows > 0) {
-      const long long per = static_cast<long long>(a.S) * a.C;
-      a.rng_first = static_cast<uint32_t>(plan->shard_first_row * per);
-      a.rng_total = static_cast<uint32_t>(plan->shard_total_rows * per);
-    }
     launch_langevin_step(a, s); CNT();
     launch_langevin_advance(cst, coef, collection ? idx : nullptr, tvec, L, T, kind, rows, 1, s); CNT();
     SMD_LAUNCH_CHECK("langevin chain step");
@@ -1421,18 +1426,13 @@ int smd_langevin_sample(smd_plan* plan, const float* params, float* x, int n, co
       if (rc) return rc;
     }
   } else {
-    const bool same = plan->langevin_graph.exec && plan->lg_n == n && plan->lg_params == params && plan->lg_x == x &&
-                      plan->lg_infill_x == infill_x && plan->lg_infill_mask == infill_mask &&
-                      plan->lg_collection == collection && plan->lg_metrics == metrics && plan->lg_rows == rows;
-    if (!same) {
-      const int rc = plan->langevin_graph.capture(cs, [&] { return step(cs); }, "langevin graph");
+    const GraphKey key = graph_key(n, params, x, infill_x, infill_mask, collection, metrics, rows);
+    if (!plan->chain_graph.replays(key)) {
+      const int rc = plan->chain_graph.capture(cs, key, [&] { return step(cs); }, "langevin graph");
       if (rc) return rc;
-      plan->lg_n = n; plan->lg_params = params; plan->lg_x = x; plan->lg_infill_x = infill_x;
-      plan->lg_infill_mask = infill_mask; plan->lg_collection = collection; plan->lg_metrics = metrics;
-      plan->lg_rows = rows;
     }
     for (long long i = 0; i < total_steps; ++i) {
-      const int rc = plan->langevin_graph.launch(cs);
+      const int rc = plan->chain_graph.launch(cs);
       if (rc) return rc;
     }
   }
@@ -1441,17 +1441,13 @@ int smd_langevin_sample(smd_plan* plan, const float* params, float* x, int n, co
     SMD_CUDA(cudaMemcpyAsync(tvec, coef + static_cast<size_t>(L - 1) * kLangevinCoef, 4, cudaMemcpyDeviceToDevice, cs));
     const int r = langevin_forward(plan, params, x, n, L - 1, cs);
     if (r) return r;
-    LangevinStepArgs a = langevin_args(plan, x, n);
+    LangevinStepArgs a = langevin_args(plan, x, n, /*sharded=*/false);
     a.alpha = plan->lv_sigma_last * plan->lv_sigma_last;
     a.collection_slot = collection ? collection + static_cast<size_t>(rows - 1) * n * a.S * a.C : nullptr;
     launch_langevin_step(a, cs); CNT();
     SMD_LAUNCH_CHECK("langevin denoise");
   }
-  if (cs != st) {
-    SMD_CUDA(cudaEventRecord(plan->own_event, cs));
-    SMD_CUDA(cudaStreamWaitEvent(st, plan->own_event, 0));
-  }
-  return SMD_OK;
+  return join_replay(plan, st, cs);
 }
 
 int smd_threefry_normal_slice(const uint32_t host_key[2], float* out, long long n, long long first, long long total,
