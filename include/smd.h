@@ -15,6 +15,7 @@
  *                                                            utils/ebm_utils.py:89-271 (nested lax.scan, L*T steps)
  *   smd_threefry_*         <- jax.random.{split,normal,...}  (jax 0.2.8, call sites utils/losses.py:271-294,
  *                                                            utils/ebm_utils.py:329,342,360)
+ *   smd_latent_stats       <- frechet_distance / mmd_rbf / mmd_polynomial   utils/metrics.py:24-77 (sample_ncsn.py:69-186)
  *
  * Conventions: every pointer is a DEVICE pointer owned by the caller (PyTorch) unless named host_*; the library
  * allocates no device memory (the caller binds one workspace); all work is asynchronous on the given CUDA stream;
@@ -290,6 +291,25 @@ int smd_mdn_mixture_sample(const float* pi, const float* mu, const float* log_si
 int smd_mdn_sample(smd_plan* plan, const float* params, const uint32_t host_key[2], int n, long long first_row,
                    long long total_rows, float* out, float* chain_or_null, int* components_or_null,
                    smd_stream_t stream);
+
+/* ---- latent-space evaluation (utils/metrics.py:24-77) ------------------------------------------------------ */
+/* Bytes of device workspace smd_latent_stats needs for x (n, d) and y (m, d); 0 for shapes it rejects. */
+size_t smd_latent_stats_workspace_bytes(int n, int m, int d);
+/* No plan needed.  x (n, d), y (m, d): fp32 row-major device arrays (one flattened example per row).  stats: device,
+ * 9 doubles:
+ *   [0] |mean x - mean y|^2   [1] tr cov(x)   [2] tr cov(y)          (ddof = 1, as np.cov)
+ *   [3..5] mean of exp(-rbf_gamma |a-b|^2) over (x,x), (y,y), (x,y) pairs (squared distances clamped at 0)
+ *   [6..8] mean of (poly_gamma <a,b> + poly_coef0)^poly_degree over the same three pair sets
+ * cross (n, m) device fp32 or NULL: (x - mean x)(y - mean y)^T.  The Frechet distance is
+ * stats[0] + stats[1] + stats[2] - 2 |cross|_* / sqrt((n-1)(m-1)) (|.|_*: nuclear norm, the sum of singular values).
+ * Everything comes from one Gram product of the centred, stacked sets on the tensor cores (bf16 hi/lo operand split,
+ * fp32 accumulation) and fp64 kernel sums in a fixed order: repeated calls give bitwise-equal stats.
+ * workspace: device, 256-byte aligned, at least smd_latent_stats_workspace_bytes(n, m, d) bytes.  SMD_ERR_INVALID for a
+ * null x / y / workspace / stats, n or m < 2, d < 1, poly_degree < 1, n + m > 16384 or a workspace that is too small
+ * or misaligned. */
+int smd_latent_stats(const float* x, int n, const float* y, int m, int d, float rbf_gamma, int poly_degree,
+                     float poly_gamma, float poly_coef0, void* workspace, size_t workspace_bytes, double* stats,
+                     float* cross, smd_stream_t stream);
 
 /* ---- jax.random (threefry2x32) on device ------------------------------------------------------------------ */
 int smd_threefry_normal(const uint32_t host_key[2], float* out, long long n, smd_stream_t stream);

@@ -83,6 +83,9 @@ _SIGNATURES = {
     "smd_mdn_mixture_sample": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_longlong,
                                          C.c_longlong, _P, _P, _P]),
     "smd_mdn_sample": (C.c_int, [_P, _P, C.POINTER(C.c_uint32), C.c_int, C.c_longlong, C.c_longlong, _P, _P, _P, _P]),
+    "smd_latent_stats_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "smd_latent_stats": (C.c_int, [_P, C.c_int, _P, C.c_int, C.c_int, C.c_float, C.c_int, C.c_float, C.c_float, _P,
+                                   C.c_size_t, _P, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -6,28 +6,33 @@ Restores the newest checkpoint of --model_dir into a freshly created model (samp
 it samples from optimizer.target, never from the EMA parameters), runs the full reverse chain on the GPU and
 writes ncsn/{real,generated,collection}.pkl under --sampling_dir (sample_ncsn.py:453-471).  With torchrun the
 sample_size is sharded across ranks (replicated parameters, no per-step exchange) and gathered at the end.
+--compute_metrics then scores the samples against the real examples on the GPU (ncsn/metrics.json).
 """
 from __future__ import annotations
 
+import json
 import os
 import pickle
 import time
+import warnings
 
 import numpy as np
 import torch
 from absl import app, flags, logging
 
-from smd_b200 import checkpoints, ebm_utils, input_pipeline, jrandom as random, parallel, train_utils
+from smd_b200 import checkpoints, ebm_utils, input_pipeline, jrandom as random, metrics, parallel, train_utils
 from smd_b200 import train_ncsn  # noqa: F401  (defines the shared training flags)
 
 FLAGS = flags.FLAGS
 flags.DEFINE_integer("sample_seed", 1, "PRNG seed of the sampler.")
 flags.DEFINE_string("sampling_dir", "samples", "Output directory (relative to --model_dir).")
 flags.DEFINE_integer("sample_size", 1000, "Number of samples to draw.")
-flags.DEFINE_bool("compute_metrics", False, "Compute evaluation metrics (out of scope: needs note_seq).")
+flags.DEFINE_bool("compute_metrics", False, "Frechet distance and RBF / polynomial MMD against the real examples of 20 "
+                  "points of the sampling collection and of a random and a real baseline, written to "
+                  "ncsn/metrics.json.")
 flags.DEFINE_bool("compute_final_only", False, "Metrics on the final samples only.")
 flags.DEFINE_bool("flush", True, "Write pickles.")
-flags.DEFINE_bool("animate", False, "Write sampling animations (out of scope).")
+flags.DEFINE_bool("animate", False, "Write sampling animations (not supported: raises ValueError).")
 flags.DEFINE_bool("infill", False, "Infill the middle 16 latents of real examples (sample_ncsn.py:408-427).")
 flags.DEFINE_bool("interpolate", False, "Interpolate between real examples in the diffusion latent space.")
 
@@ -128,11 +133,54 @@ def _save(obj, path):
     logging.info("Saved to %s", path)
 
 
+def evaluation_points(collection, final_only=False):
+    """sample_ncsn.py:96-101: 20 points spread over the sampling collection, or its last point only."""
+    points = collection[np.linspace(0, len(collection) - 1, 20).astype(np.uint32)]
+    return [points[-1]] if final_only else list(points)
+
+
+def evaluate(real, collection, seed, final_only=False, metric_fn=metrics.latent_metrics):
+    """sample_ncsn.py:69-186 with the metrics utils/metrics.py defines (Frechet distance, RBF and polynomial MMD;
+    upstream's precision/recall, realism and NDB calls name functions it never defines).  real (N, ...) and
+    collection (steps, N, ...) are the normalised data.  Returns {model: {evaluation index: {metric: value}}} for
+    model "ncsn" (the collection points), "random" (standard normals shaped like one point; seeded here, unseeded
+    upstream) and "real" (real against itself)."""
+    if collection.shape[1:] != real.shape:
+        raise ValueError(f"collection points {collection.shape[1:]} do not match the real examples {real.shape}")
+    logging.info("Generated sample range: [%f, %f]", collection[-1].min(), collection[-1].max())
+    logging.info("Test sample range: [%f, %f]", real.min(), real.max())
+    if collection[-1].min() < -1 or collection[-1].max() > 1 or real.min() < -1 or real.max() > 1:
+        warnings.warn("Normalize test samples and generated samples to [-1, 1] range.")
+    random_points = [np.random.default_rng(seed).standard_normal(collection[0].shape).astype(np.float32)]
+    results = {}
+    for model, points in [("ncsn", evaluation_points(collection, final_only)), ("random", random_points),
+                          ("real", [real])]:
+        results[model] = {str(i): metric_fn(real, p) for i, p in enumerate(points)}
+    return results
+
+
+def save_metrics(results, out_dir):
+    path = os.path.join(out_dir, "metrics.json")
+    os.makedirs(out_dir, exist_ok=True)
+    with open(path, "w") as f:
+        json.dump(results, f, indent=1, sort_keys=True)
+    logging.info("Saved to %s", path)
+    return path
+
+
+def check_flags():
+    if FLAGS.animate:
+        raise ValueError("--animate writes matplotlib animations, which are out of scope")
+    if FLAGS.compute_metrics and FLAGS.interpolate:
+        # upstream's evaluate asserts collection.shape[1:] == real.shape, which the (9, steps, N, ...) collection of
+        # the interpolation never meets
+        raise ValueError("--compute_metrics does not apply to --interpolate")
+
+
 def main(argv):
     del argv
+    check_flags()
     parallel.init_from_env()
-    if FLAGS.compute_metrics or FLAGS.animate:
-        raise ValueError("--compute_metrics / --animate depend on note_seq / matplotlib code that is out of scope")
     _, eval_ds = input_pipeline.get_dataset(
         dataset=FLAGS.dataset, data_shape=FLAGS.data_shape, problem=FLAGS.problem, batch_size=FLAGS.batch_size,
         normalize=FLAGS.normalize, pca_ckpt=FLAGS.pca_ckpt, slice_ckpt=FLAGS.slice_ckpt,
@@ -175,6 +223,14 @@ def main(argv):
             _save(inv(collection), os.path.join(out, "collection.pkl"))
         _save(inv(real), os.path.join(out, "real.pkl"))
         _save(inv(generated), os.path.join(out, "generated.pkl"))
+    if FLAGS.compute_metrics and parallel.rank() == 0:     # sample_ncsn.py:474-477, on the normalised data
+        if collection is None:                             # consistent Langevin dynamics: the final samples only
+            results = evaluate(real, generated[None], FLAGS.sample_seed, True)
+        else:
+            results = evaluate(real, collection, FLAGS.sample_seed, FLAGS.compute_final_only)
+        ncsn = results["ncsn"]
+        train_utils.log_metrics(ncsn[str(len(ncsn) - 1)], 1, 1)
+        save_metrics(results, os.path.join(FLAGS.model_dir, FLAGS.sampling_dir, "ncsn"))
     parallel.shutdown()
 
 
