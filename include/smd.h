@@ -16,6 +16,8 @@
  *   smd_threefry_*         <- jax.random.{split,normal,...}  (jax 0.2.8, call sites utils/losses.py:271-294,
  *                                                            utils/ebm_utils.py:329,342,360)
  *   smd_latent_stats       <- frechet_distance / mmd_rbf / mmd_polynomial   utils/metrics.py:24-77 (sample_ncsn.py:69-186)
+ *   smd_latent_coverage    <- precision_recall_distribution, precision_recall, realism_scores, ndb_score
+ *                                                            (sample_ncsn.py:132-159; not defined by the reference)
  *
  * Conventions: every pointer is a DEVICE pointer owned by the caller (PyTorch) unless named host_*; the library
  * allocates no device memory (the caller binds one workspace); all work is asynchronous on the given CUDA stream;
@@ -310,6 +312,44 @@ size_t smd_latent_stats_workspace_bytes(int n, int m, int d);
 int smd_latent_stats(const float* x, int n, const float* y, int m, int d, float rbf_gamma, int poly_degree,
                      float poly_gamma, float poly_coef0, void* workspace, size_t workspace_bytes, double* stats,
                      float* cross, smd_stream_t stream);
+
+/* Coverage metrics of the same two sets, from the same Gram product (see smd_latent_coverage). */
+typedef struct {
+  int neighbors;      /* k of the k-NN radii (improved precision / recall, realism), [1, 32] */
+  int prd_clusters;   /* k-means clusters of x and y together per PRD run, [1, 64] and <= n + m */
+  int prd_runs;       /* independent PRD fits (the histograms are averaged over them by the caller) */
+  int ndb_bins;       /* k-means bins of x for NDB, [1, 64] and <= n */
+  int restarts;       /* k-means++ restarts per fit; the one with the lowest inertia is kept */
+  int max_iter;       /* Lloyd iterations per restart at most */
+} smd_coverage_config;   /* metrics.py uses 3, 20, 10, 50, 10, 300 */
+
+/* Bytes of device workspace smd_latent_coverage needs; 0 for a configuration or shapes it rejects. */
+size_t smd_latent_coverage_workspace_bytes(int n, int m, int d, const smd_coverage_config* cfg);
+/* No plan needed.  x (n, d), y (m, d) as for smd_latent_stats; cfg is a host pointer.  With D(a, b) the squared
+ * distance of raw rows, rebuilt in fp64 from the fp32 Gram product as smd_latent_stats does (mean-difference terms for
+ * x-y pairs, clamped at 0), and r_a the k-th smallest D(a, b) over the other rows b of a's set (k = neighbors; self
+ * excluded by index, duplicate rows count):
+ *   counts   device int[2]: [0] y rows b with D(a, b) <= r_a for some x row a; [1] the same with x and y swapped
+ *   realism  device double[m]: max over x rows a of sqrt(r'_a) / (sqrt(D(a, b)) + 1e-5), where r'_a = r_a, or 0 if
+ *            r_a exceeds the median of the x radii (np.percentile(r, 50))
+ *   prd_hist device int[prd_runs][2][prd_clusters]: x and y counts per cluster of a k-means fit of x and y together
+ *   ndb_hist device int[2][ndb_bins]: x and y counts per bin of a k-means fit of x; each y row joins its nearest bin
+ *   iterations device int[2] or NULL: the most Lloyd iterations any restart of the PRD fits / the NDB fit ran
+ * k-means works on distances only: dist(p, C) = S(p, C) / |C| - W_C / (2 |C|^2) with S(p, C) = sum_{b in C} D(p, b) and
+ * W_C = sum_{p in C} S(p, C), the exact squared distance to the mean of C.  A restart seeds by k-means++ from its
+ * uniforms u_0..u_{K-1}: seed 0 is point floor(u_0 N), seed j the smallest index whose prefix sum (point order) of the
+ * min D to the seeds so far exceeds u_j times the total (floor(u_j N) if the total is 0), and every point joins its
+ * nearest seed.  Lloyd iterations reassign every point to argmin_C dist(p, C) (lowest index on ties; empty clusters
+ * stay empty) until no label changes or max_iter.  Each fit keeps the restart of lowest inertia sum_C W_C / (2 |C|)
+ * (lowest restart on ties).  uniforms: device doubles in [0, 1), (prd_runs * prd_clusters + ndb_bins) * restarts of
+ * them: PRD run r, restart s at [(r * restarts + s) * prd_clusters], then NDB restart s at
+ * [prd_runs * restarts * prd_clusters + s * ndb_bins].  Reductions run in a fixed order: repeated calls are bitwise
+ * equal, whatever the workspace held.  SMD_ERR_INVALID for a null argument (iterations aside), n or m < neighbors + 1,
+ * a configuration field out of its range above, restarts, prd_runs or max_iter < 1, prd_runs * restarts > 65535,
+ * n + m > 16384, or a workspace that is too small or not 256-byte aligned. */
+int smd_latent_coverage(const float* x, int n, const float* y, int m, int d, const smd_coverage_config* cfg,
+                        const double* uniforms, void* workspace, size_t workspace_bytes, int* counts, double* realism,
+                        int* prd_hist, int* ndb_hist, int* iterations, smd_stream_t stream);
 
 /* ---- jax.random (threefry2x32) on device ------------------------------------------------------------------ */
 int smd_threefry_normal(const uint32_t host_key[2], float* out, long long n, smd_stream_t stream);

@@ -11,7 +11,8 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libsmd.so")
-SOURCES = ["smd_api.cu", "kernels.cu", "train.cu", "backward.cu", "mdn.cu", "latent_stats.cu"]
+SOURCES = ["smd_api.cu", "kernels.cu", "train.cu", "backward.cu", "mdn.cu", "latent_stats.cu",
+           "latent_coverage.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xptxas", "-v",

@@ -13,23 +13,15 @@
 #include <climits>
 #include <cmath>
 
-#include "plan.cuh"
+#include "latent_gram.cuh"
 
 namespace smd {
 
-static constexpr int kLatentMaxRows = 16384;   // n + m: the fp32 Gram of the stacked sets is (n + m + 2)^2 floats
 static constexpr int kLatentRowsPad = kBM;     // Gram rows / columns padded to the GEMM's 128-row tile
 static constexpr int kMeanCols = 32, kMeanSlices = 32;
 
-struct LatentLayout {
-  int R, Rp, Kp;                  // stacked rows n + m + 2, padded rows, padded K
-  size_t z, z_lo, g, mean, diag, part, delta2, total;
-};
-
-static size_t align256(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
-
-static LatentLayout latent_layout(int n, int m, int d) {
-  LatentLayout L;
+GramLayout gram_layout(int n, int m, int d) {
+  GramLayout L;
   L.R = n + m + 2;
   L.Rp = (L.R + kLatentRowsPad - 1) / kLatentRowsPad * kLatentRowsPad;
   L.Kp = static_cast<int>((static_cast<long long>(d) + 63) / 64 * 64);
@@ -40,27 +32,23 @@ static LatentLayout latent_layout(int n, int m, int d) {
   L.g = off; off = align256(off + static_cast<size_t>(L.Rp) * L.Rp * sizeof(float));
   L.mean = off; off = align256(off + 2 * static_cast<size_t>(d) * sizeof(double));
   L.diag = off; off = align256(off + static_cast<size_t>(n + m) * sizeof(double));
-  L.part = off; off = align256(off + static_cast<size_t>(n + m) * 4 * sizeof(double));
   L.delta2 = off; off = align256(off + sizeof(double));
   L.total = off;
   return L;
 }
 
-__device__ __forceinline__ double warp_sum_f64(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-// fixed-order block sum (every thread gets the result); red holds one double per warp
-__device__ __forceinline__ double block_sum_f64(double v, double* red) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  v = warp_sum_f64(v);
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  double r = 0.0;
-  for (int w = 0; w < nw; ++w) r += red[w];
-  return r;
+// smd_latent_stats' workspace: the Gram region, then the per-row kernel-sum partials
+struct LatentLayout {
+  GramLayout gram;
+  size_t part, total;
+};
+
+static LatentLayout latent_layout(int n, int m, int d) {
+  LatentLayout L;
+  L.gram = gram_layout(n, m, d);
+  L.part = L.gram.total;
+  L.total = align256(L.part + static_cast<size_t>(n + m) * 4 * sizeof(double));
+  return L;
 }
 
 // column means of x (blockIdx.y = 0) and y (1) in fp64: 32 columns per block, 32 row slices summed in order
@@ -217,6 +205,43 @@ latent_finish_kernel(const double* __restrict__ part, const double* __restrict__
   }
 }
 
+int latent_gram(const float* x, int n, const float* y, int m, int d, const GramLayout& L, uint8_t* ws,
+                cudaStream_t st) {
+  auto hi = reinterpret_cast<__nv_bfloat16*>(ws + L.z);
+  auto lo = reinterpret_cast<__nv_bfloat16*>(ws + L.z_lo);
+  float* G = reinterpret_cast<float*>(ws + L.g);
+  double* mean = reinterpret_cast<double*>(ws + L.mean);
+  double* diag = reinterpret_cast<double*>(ws + L.diag);
+  double* delta2 = reinterpret_cast<double*>(ws + L.delta2);
+
+  latent_mean_kernel<<<dim3((d + kMeanCols - 1) / kMeanCols, 2), kMeanCols * kMeanSlices, 0, st>>>(x, n, y, m, d, mean);
+  CNT();
+  const size_t quads = static_cast<size_t>(L.Rp) * (L.Kp / 4);
+  const int split_blocks = static_cast<int>(std::min<size_t>((quads + 255) / 256, static_cast<size_t>(device_sm_count()) * 8));
+  latent_split_kernel<<<split_blocks, 256, 0, st>>>(x, n, y, m, d, mean, L.Rp, L.Kp, hi, lo);
+  CNT();
+  SMD_LAUNCH_CHECK("latent_split");
+
+  // G = Z Z^T in the strict (bf16x3) composition: G = lo hi^T; G += hi lo^T; G = hi hi^T + G
+  GemmOp op;
+  if (!make_gemm_op(&op, hi, static_cast<uint64_t>(L.Rp), hi, static_cast<uint64_t>(L.Rp), L.Rp, L.Kp, kBNMax, 0, 0,
+                    0, 0, L.z_lo - L.z))
+    return SMD_ERR_CUDA;
+  GemmOp o1 = op; o1.tmA = op.tmA_lo;
+  GemmEpilogue e = epi();
+  e.out_f32 = G; e.ld_f32 = L.Rp;
+  SMD_CUDA(launch_gemm(o1, L.Rp, e, st));
+  GemmOp o2 = op; o2.tmB = op.tmB_lo;
+  e.residual = G; e.ld_res = L.Rp;
+  SMD_CUDA(launch_gemm(o2, L.Rp, e, st));
+  SMD_CUDA(launch_gemm(op, L.Rp, e, st));
+
+  latent_diag_kernel<<<1, 1024, 0, st>>>(G, L.Rp, n + m, mean, d, diag, delta2);
+  CNT();
+  SMD_LAUNCH_CHECK("latent_gram");
+  return SMD_OK;
+}
+
 }  // namespace smd
 
 using namespace smd;
@@ -247,39 +272,13 @@ int smd_latent_stats(const float* x, int n, const float* y, int m, int d, float 
   if (reinterpret_cast<uintptr_t>(workspace) & 255u) { set_error("workspace must be 256-byte aligned"); return SMD_ERR_INVALID; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* ws = static_cast<uint8_t*>(workspace);
-  auto hi = reinterpret_cast<__nv_bfloat16*>(ws + L.z);
-  auto lo = reinterpret_cast<__nv_bfloat16*>(ws + L.z_lo);
-  float* G = reinterpret_cast<float*>(ws + L.g);
-  double* mean = reinterpret_cast<double*>(ws + L.mean);
-  double* diag = reinterpret_cast<double*>(ws + L.diag);
+  const GramLayout& Lg = L.gram;
+  if (const int rc = latent_gram(x, n, y, m, d, Lg, ws, st)) return rc;
+  float* G = reinterpret_cast<float*>(ws + Lg.g);
+  double* diag = reinterpret_cast<double*>(ws + Lg.diag);
+  double* delta2 = reinterpret_cast<double*>(ws + Lg.delta2);
   double* part = reinterpret_cast<double*>(ws + L.part);
-  double* delta2 = reinterpret_cast<double*>(ws + L.delta2);
-
-  latent_mean_kernel<<<dim3((d + kMeanCols - 1) / kMeanCols, 2), kMeanCols * kMeanSlices, 0, st>>>(x, n, y, m, d, mean);
-  CNT();
-  const size_t quads = static_cast<size_t>(L.Rp) * (L.Kp / 4);
-  const int split_blocks = static_cast<int>(std::min<size_t>((quads + 255) / 256, static_cast<size_t>(device_sm_count()) * 8));
-  latent_split_kernel<<<split_blocks, 256, 0, st>>>(x, n, y, m, d, mean, L.Rp, L.Kp, hi, lo);
-  CNT();
-  SMD_LAUNCH_CHECK("latent_split");
-
-  // G = Z Z^T in the strict (bf16x3) composition: G = lo hi^T; G += hi lo^T; G = hi hi^T + G
-  GemmOp op;
-  if (!make_gemm_op(&op, hi, static_cast<uint64_t>(L.Rp), hi, static_cast<uint64_t>(L.Rp), L.Rp, L.Kp, kBNMax, 0, 0,
-                    0, 0, L.z_lo - L.z))
-    return SMD_ERR_CUDA;
-  GemmOp o1 = op; o1.tmA = op.tmA_lo;
-  GemmEpilogue e = epi();
-  e.out_f32 = G; e.ld_f32 = L.Rp;
-  SMD_CUDA(launch_gemm(o1, L.Rp, e, st));
-  GemmOp o2 = op; o2.tmB = op.tmB_lo;
-  e.residual = G; e.ld_res = L.Rp;
-  SMD_CUDA(launch_gemm(o2, L.Rp, e, st));
-  SMD_CUDA(launch_gemm(op, L.Rp, e, st));
-
-  latent_diag_kernel<<<1, 1024, 0, st>>>(G, L.Rp, n + m, mean, d, diag, delta2);
-  CNT();
-  latent_kernel_sums_kernel<<<n + m, 256, 0, st>>>(G, L.Rp, n, m, diag, delta2, rbf_gamma, poly_degree, poly_gamma,
+  latent_kernel_sums_kernel<<<n + m, 256, 0, st>>>(G, Lg.Rp, n, m, diag, delta2, rbf_gamma, poly_degree, poly_gamma,
                                                     poly_coef0, part);
   CNT();
   latent_finish_kernel<<<1, 1024, 0, st>>>(part, diag, delta2, n, m, stats);
@@ -287,7 +286,7 @@ int smd_latent_stats(const float* x, int n, const float* y, int m, int d, float 
   SMD_LAUNCH_CHECK("latent_stats");
   if (cross)
     SMD_CUDA(cudaMemcpy2DAsync(cross, static_cast<size_t>(m) * sizeof(float), G + n,
-                               static_cast<size_t>(L.Rp) * sizeof(float), static_cast<size_t>(m) * sizeof(float), n,
+                               static_cast<size_t>(Lg.Rp) * sizeof(float), static_cast<size_t>(m) * sizeof(float), n,
                                cudaMemcpyDeviceToDevice, st));
   return SMD_OK;
 }

@@ -20,6 +20,11 @@ class SmdConfig(C.Structure):
                 ("training", C.c_int), ("sampler_T", C.c_int), ("precision", C.c_int)]
 
 
+class SmdCoverageConfig(C.Structure):
+    _fields_ = [("neighbors", C.c_int), ("prd_clusters", C.c_int), ("prd_runs", C.c_int), ("ndb_bins", C.c_int),
+                ("restarts", C.c_int), ("max_iter", C.c_int)]
+
+
 _P = C.c_void_p
 _SIGNATURES = {
     "smd_last_error": (C.c_char_p, []),
@@ -86,6 +91,9 @@ _SIGNATURES = {
     "smd_latent_stats_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "smd_latent_stats": (C.c_int, [_P, C.c_int, _P, C.c_int, C.c_int, C.c_float, C.c_int, C.c_float, C.c_float, _P,
                                    C.c_size_t, _P, _P, _P]),
+    "smd_latent_coverage_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.POINTER(SmdCoverageConfig)]),
+    "smd_latent_coverage": (C.c_int, [_P, C.c_int, _P, C.c_int, C.c_int, C.POINTER(SmdCoverageConfig), _P, _P,
+                                      C.c_size_t, _P, _P, _P, _P, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -6,7 +6,8 @@ Restores the newest checkpoint of --model_dir into a freshly created model (samp
 it samples from optimizer.target, never from the EMA parameters), runs the full reverse chain on the GPU and
 writes ncsn/{real,generated,collection}.pkl under --sampling_dir (sample_ncsn.py:453-471).  With torchrun the
 sample_size is sharded across ranks (replicated parameters, no per-step exchange) and gathered at the end.
---compute_metrics then scores the samples against the real examples on the GPU (ncsn/metrics.json).
+--compute_metrics then scores the samples against the real examples on the GPU (ncsn/metrics.json); with
+--full_metrics also by the coverage metrics (PRD, improved precision / recall, realism, NDB).
 """
 from __future__ import annotations
 
@@ -31,6 +32,9 @@ flags.DEFINE_bool("compute_metrics", False, "Frechet distance and RBF / polynomi
                   "points of the sampling collection and of a random and a real baseline, written to "
                   "ncsn/metrics.json.")
 flags.DEFINE_bool("compute_final_only", False, "Metrics on the final samples only.")
+flags.DEFINE_bool("full_metrics", False, "With --compute_metrics, also PRD precision / recall / F1, improved precision / "
+                  "recall / F1, realism and NDB (sample_ncsn.py:132-159 of the reference, which never defines them; "
+                  "see metrics.py), k-means seeded from --sample_seed.  Not a reference flag.")
 flags.DEFINE_bool("flush", True, "Write pickles.")
 flags.DEFINE_bool("animate", False, "Write sampling animations (not supported: raises ValueError).")
 flags.DEFINE_bool("infill", False, "Infill the middle 16 latents of real examples (sample_ncsn.py:408-427).")
@@ -141,7 +145,8 @@ def evaluation_points(collection, final_only=False):
 
 def evaluate(real, collection, seed, final_only=False, metric_fn=metrics.latent_metrics):
     """sample_ncsn.py:69-186 with the metrics utils/metrics.py defines (Frechet distance, RBF and polynomial MMD;
-    upstream's precision/recall, realism and NDB calls name functions it never defines).  real (N, ...) and
+    upstream's precision/recall, realism and NDB calls name functions it never defines; metric_fn=full_metrics adds
+    the published metrics of those names).  real (N, ...) and
     collection (steps, N, ...) are the normalised data.  Returns {model: {evaluation index: {metric: value}}} for
     model "ncsn" (the collection points), "random" (standard normals shaped like one point; seeded here, unseeded
     upstream) and "real" (real against itself)."""
@@ -175,6 +180,13 @@ def check_flags():
         # upstream's evaluate asserts collection.shape[1:] == real.shape, which the (9, steps, N, ...) collection of
         # the interpolation never meets
         raise ValueError("--compute_metrics does not apply to --interpolate")
+    if FLAGS.full_metrics and not FLAGS.compute_metrics:
+        raise ValueError("--full_metrics needs --compute_metrics")
+
+
+def full_metrics(real, fake):
+    """The eleven values sample_ncsn.py:132-170 logs: the three distance metrics and the eight coverage metrics."""
+    return {**metrics.latent_metrics(real, fake), **metrics.coverage_metrics(real, fake, seed=FLAGS.sample_seed)}
 
 
 def main(argv):
@@ -224,10 +236,11 @@ def main(argv):
         _save(inv(real), os.path.join(out, "real.pkl"))
         _save(inv(generated), os.path.join(out, "generated.pkl"))
     if FLAGS.compute_metrics and parallel.rank() == 0:     # sample_ncsn.py:474-477, on the normalised data
+        metric_fn = full_metrics if FLAGS.full_metrics else metrics.latent_metrics
         if collection is None:                             # consistent Langevin dynamics: the final samples only
-            results = evaluate(real, generated[None], FLAGS.sample_seed, True)
+            results = evaluate(real, generated[None], FLAGS.sample_seed, True, metric_fn)
         else:
-            results = evaluate(real, collection, FLAGS.sample_seed, FLAGS.compute_final_only)
+            results = evaluate(real, collection, FLAGS.sample_seed, FLAGS.compute_final_only, metric_fn)
         ncsn = results["ncsn"]
         train_utils.log_metrics(ncsn[str(len(ncsn) - 1)], 1, 1)
         save_metrics(results, os.path.join(FLAGS.model_dir, FLAGS.sampling_dir, "ncsn"))
