@@ -115,9 +115,12 @@ inline uint32_t epi_needs(const GemmEpilogue& e) {
   if (e.out_scale != 0.0f && e.out_scale != 1.0f) f |= F_SCALE;
   return f;
 }
+// The fast epilogue kinds store every column of every n-tile: N must be a whole number of tiles.  (An N that is a
+// multiple of 32 but not of BN -- the TransformerMDN head, 2 KCp + Kcp = 960 columns at 10 components -- would write
+// the last tile's columns [N, BN-rounded N) into the next row of an output whose row pitch is N.)
 inline bool epi_clean(const GemmOp& op, const GemmEpilogue& e) {
   auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-  return (op.N % 32 == 0) && (op.BN % 32 == 0) && (!e.residual || ((e.ld_res & 3) == 0 && a16(e.residual))) &&
+  return (op.N % 32 == 0) && (op.BN % 32 == 0) && (op.N % op.BN == 0) && (!e.residual || ((e.ld_res & 3) == 0 && a16(e.residual))) &&
          (!e.out_f32 || ((e.ld_f32 & 3) == 0 && a16(e.out_f32))) &&
          ((!e.out_bf16 && !e.out_bf16_pre) || (e.ld_bf16 & 7) == 0) && (!e.out_bf16 || a16(e.out_bf16)) &&
          (!e.out_bf16_pre || a16(e.out_bf16_pre)) && (!e.gelu_grad_of || ((e.ld_gg & 7) == 0 && a16(e.gelu_grad_of))) &&

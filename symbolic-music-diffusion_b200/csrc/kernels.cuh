@@ -24,7 +24,10 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 // swish(v) = v * sigmoid(v) with sigmoid(v) = 0.5 + 0.5 * tanh(v / 2): one MUFU.TANH instead of exp + IEEE divide
-// (abs error of tanh.approx ~5e-4; every consumer rounds the result to bf16 or feeds a bf16 GEMM operand)
+// (tanh.approx: relative error ~2^-11, so |swishf(v) - swish(v)| <= |v| 2^-12.  Measured on H100 against fp64, every
+// bf16 output stays within half a bf16 spacing plus 2^-16 rms(v).  For v < -3 the result is small and 0.5 + 0.5 tanh
+// cancels: about 10 % of the bf16 outputs there are more than one spacing from the exact swish.  The only consumers
+// are bf16 GEMM operands, where those absolute errors of ~1e-4 are below the operand rounding of the larger inputs.)
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
