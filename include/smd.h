@@ -207,7 +207,8 @@ int smd_sampler_set_shard(smd_plan* plan, long long first_row, long long total_r
 /* One reverse step at index t (T-1 .. 0) on state x (n,S,C), in place allowed (x_next == x).
  * z / infill_z: supplied N(0,1) tensors or NULL -> in-kernel threefry with the tables of smd_sampler_setup.
  * metrics: device (4, T) fp32 or NULL (column T-1-t accumulated: grad_norm, step_norm, alpha_prod, noise_norm).
- * collection: device (41, n, S, C) or NULL. */
+ * collection: device (41, n, S, C) or NULL; rows at linspace(1, T, 40), a step whose summed slot passes row 40
+ * (T < 40 repeats indices) writes none. */
 int smd_ddpm_reverse_step(smd_plan* plan, const float* params, const float* x, int n, int t, const float* z,
                           const float* infill_x, const float* infill_mask, const float* infill_z, float* x_next,
                           float* eps_hat_or_null, float* collection, float* metrics, smd_stream_t stream);

@@ -1141,7 +1141,9 @@ int smd_sampler_setup(smd_plan* plan, const float* host_betas, int T, const uint
     const int image_idx = T - t + 1;
     int sum = 0; bool any = false;
     for (int j = 0; j < 40; ++j) if (idx_tab[j] == image_idx) { sum += j; any = true; }
-    if (any) slots[t] = sum + 1;
+    // below T = 40 linspace repeats indices and the summed slot can pass the 41 collection rows (184 at T = 8); XLA's
+    // scatter drops such an update, so the step writes no row
+    if (any && sum + 1 < 41) slots[t] = sum + 1;
   }
   SMD_CUDA(cudaMemcpyAsync(plan->at<float>(plan->reg.coef), coef.data(), coef.size() * 4, cudaMemcpyHostToDevice, st));
   SMD_CUDA(cudaMemcpyAsync(plan->at<uint32_t>(plan->reg.keys), keys.data(), keys.size() * 4, cudaMemcpyHostToDevice, st));

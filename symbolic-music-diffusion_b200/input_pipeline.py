@@ -286,6 +286,21 @@ class Dataset:
         for b in self.batches_untransformed_norm():
             yield normalize_dataset(b, self.min, self.max).astype(np.float32) if self._norm else b.astype(np.float32)
 
+    def take(self, n: int) -> np.ndarray:
+        """The first n examples (fewer if the split is smaller) of the next pass, as iteration yields them.  The pass
+        is not used up: the next iteration sees the same order, so reading examples does not change what a later
+        evaluation reads."""
+        epoch, rows, count = self._epoch, [], 0
+        try:
+            for b in self:
+                rows.append(b)
+                count += len(b)
+                if count >= n:
+                    break
+        finally:
+            self._epoch = epoch
+        return np.concatenate(rows)[:n] if rows else np.zeros((0,), np.float32)
+
 
 def _tfrecord_examples(pattern: str, shape):
     files = sorted(glob.glob(os.path.expanduser(pattern)))

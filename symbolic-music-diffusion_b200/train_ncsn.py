@@ -5,9 +5,12 @@ Objectives: --loss=ddpm (TransformerDDPM, TransformerDDPM4, DenseDDPM), --loss=d
 with any other architecture raises ValueError).  Other values raise ValueError exactly where the reference would
 dispatch on them.  Data-parallel: launch with torchrun (one process per GPU); the batch is sharded across ranks
 and gradients are summed with one NCCL all-reduce over the flat arena (SURVEY section 8(e)).
+--snapshot_sampling (the default, as in the reference) draws --eval_samples samples from the EMA parameters at every
+snapshot and writes them under --model_dir (snapshot_sampling).
 """
 from __future__ import annotations
 
+import json
 import os
 import time
 
@@ -15,7 +18,8 @@ import numpy as np
 import torch
 from absl import app, flags, logging
 
-from smd_b200 import checkpoints, ebm_utils, input_pipeline, jrandom as random, ncsn, nn, optim, parallel, train_utils
+from smd_b200 import (checkpoints, ebm_utils, input_pipeline, jrandom as random, metrics, ncsn, nn, optim, parallel,
+                      train_utils)
 from smd_b200.losses import denoising_score_matching_loss, diffusion_loss, sliced_score_matching_loss
 
 FLAGS = flags.FLAGS
@@ -175,6 +179,107 @@ def train_step(objective, batch, optimizer, sigmas, rng, learning_rate, ema=None
     return optimizer, metrics
 
 
+def _summary_writer(path):
+    """A tensorboard SummaryWriter logging to `path`, or None when tensorboard cannot be imported (it is optional)."""
+    try:
+        from torch.utils.tensorboard import SummaryWriter
+        return SummaryWriter(path)
+    except Exception:
+        return None
+
+
+LD_METRICS = ("slope", "step", "alpha", "noise")
+
+
+def log_langevin_dynamics(ld_metrics, step, output_dir):
+    """train_ncsn.py:166-184: the per-step statistics of one sampling run, `ld_metrics` as collate_sampling_metrics
+    returns them (num_sigmas lists of T dicts).  Logged to a SummaryWriter under output_dir/sampling_epoch{step} when
+    tensorboard is available, and always written there as ld_metrics.npz: one (num_sigmas, T) float32 array per
+    statistic (slope, step, alpha, noise)."""
+    out = os.path.join(output_dir, f"sampling_epoch{step}")
+    os.makedirs(out, exist_ok=True)
+    arrays = {k: np.asarray([[m[k] for m in level] for level in ld_metrics], np.float32) for k in LD_METRICS}
+    np.savez(os.path.join(out, "ld_metrics.npz"), **arrays)
+    writer = _summary_writer(out)
+    if writer is not None:
+        for i, sigma_metrics in enumerate(ld_metrics):
+            for j, metric in enumerate(sigma_metrics):
+                train_utils.log_metrics(metric, j, len(sigma_metrics), epoch=i, summary_writer=writer, verbose=False)
+        writer.close()
+    return out
+
+
+def log_samples(step, init, real, fake, output_dir, flush=True):
+    """train_ncsn.py:137-163 without the image tiles and scatter plots (out of scope): with `flush`, each set is
+    pickled to output_dir/samples/{init,real,fake}/{step}.pkl."""
+    if flush:
+        for category, samples in (("init", init), ("real", real), ("fake", fake)):
+            input_pipeline.save(samples, os.path.join(output_dir, f"samples/{category}/{step}.pkl"))
+
+
+LATENT_STATS_MAX_ROWS = 16384      # n + m cap of smd_latent_stats (include/smd.h)
+
+
+def snapshot_sampling(optimizer, ema, sigmas, rng, input_shape, train_batches, valid_batches, global_step,
+                      sampling_step, output_dir, writer=None):
+    """train_ncsn.py:405-486: draws --eval_samples samples from the EMA parameters (the trained ones with --noema),
+    logs the Langevin statistics, and writes the initial, real and generated sets.  Returns the advanced `rng`.
+
+    The samples come from the spec's inference engine, which packs its bf16 operands from the EMA arena on the device
+    whenever the arena's version has moved; the training engine is not used.  Every rank draws its rows of the
+    sample (shard=(rank, world), like sample_ncsn.generate_samples), the rows are gathered, and rank 0 alone does the
+    host work.  Deviations from the reference:
+      - `real` is the first --eval_samples examples of the next pass over `valid_batches`.  Upstream takes them after
+        a tf.data shuffle(8 * batch_size) of the unbatched split, which cannot be restated.  A smaller split gives
+        fewer real rows than init and fake (logged as a warning); upstream's log_samples asserts equal shapes.
+      - The pickles are written for every problem (upstream: vae only); the image tiles, scatter plots and score
+        fields are not drawn.
+      - The final samples are scored against `real` on the normalised data with metrics.latent_metrics, logged and
+        appended with global_step to output_dir/samples/metrics.jsonl.  Scoring is skipped with a warning when
+        2 * --eval_samples exceeds the 16384 rows smd_latent_stats takes."""
+    scorenet = optimizer.target.replace(params=ema.params if FLAGS.ema else optimizer.target.arena)
+    # upstream splits off sample_rng but hands `rng` itself to sample() (train_ncsn.py:407-411); reproduced here, so
+    # the sampling key is the training key's next state
+    rng, sample_rng = random.split(rng)
+    del sample_rng
+    world, rank = parallel.world_size(), parallel.rank()
+    generated, collection, ld_metrics = sample(scorenet, sigmas, rng, input_shape, num_samples=FLAGS.eval_samples,
+                                               sampling=FLAGS.sampling, epsilon=FLAGS.ld_epsilon, steps=FLAGS.ld_steps,
+                                               denoise=FLAGS.denoise, shard=(rank, world))
+    generated = parallel.gather_rows(generated)
+    init = None if collection is None else parallel.gather_rows(collection[0].contiguous())
+    if rank != 0:
+        return rng
+    if init is None:
+        # consistent Langevin dynamics keeps no collection: regenerate the initial draw from sample()'s init_rng
+        init = initial_draw(random.split(rng)[0], (FLAGS.eval_samples, *input_shape), FLAGS.sampling)
+    generated, init = generated.cpu().numpy(), init.cpu().numpy()
+    real = valid_batches.take(FLAGS.eval_samples)
+    if len(real) < FLAGS.eval_samples:
+        logging.warning("the validation split holds %d examples: the real set is smaller than --eval_samples=%d",
+                        len(real), FLAGS.eval_samples)
+    if output_dir:
+        log_langevin_dynamics(ld_metrics, sampling_step, output_dir)
+        load = lambda p: input_pipeline.load(os.path.expanduser(p)) if p else None  # noqa: E731
+        pca, slice_idx, dim_w = load(FLAGS.pca_ckpt), load(FLAGS.slice_ckpt), load(FLAGS.dim_weights_ckpt)
+
+        def inv(a, ds):
+            return input_pipeline.inverse_data_transform(a, FLAGS.normalize, pca, ds.min, ds.max, slice_idx, dim_w,
+                                                         out_channels=int(FLAGS.data_shape[-1]))
+        log_samples(global_step, inv(init, train_batches), inv(real, valid_batches), inv(generated, train_batches),
+                    output_dir, flush=True)
+    if 2 * FLAGS.eval_samples > LATENT_STATS_MAX_ROWS:
+        logging.warning("snapshot metrics skipped: 2 * --eval_samples=%d exceeds the %d rows the GPU metrics take",
+                        FLAGS.eval_samples, LATENT_STATS_MAX_ROWS)
+        return rng
+    scores = metrics.latent_metrics(real, generated)
+    train_utils.log_metrics(scores, global_step, train_batches.examples * FLAGS.epochs, summary_writer=writer)
+    if output_dir:
+        with open(os.path.join(output_dir, "samples", "metrics.jsonl"), "a") as f:
+            f.write(json.dumps({"global_step": int(global_step), **scores}) + "\n")
+    return rng
+
+
 def train(train_batches, valid_batches, sigmas, output_dir=None, verbose=True):
     """train_ncsn.py:291-496 (the MNIST / toy plotting branches are out of scope)."""
     objective = _objective()
@@ -193,16 +298,7 @@ def train(train_batches, valid_batches, sigmas, output_dir=None, verbose=True):
     writer = None
     if output_dir and parallel.rank() == 0:
         os.makedirs(output_dir, exist_ok=True)
-        try:
-            from torch.utils.tensorboard import SummaryWriter
-            writer = SummaryWriter(os.path.join(output_dir, "train"))
-        except Exception:  # tensorboard is optional
-            writer = None
-    if FLAGS.snapshot_sampling:
-        # train_ncsn.py:405-486: in-training sampling writes matplotlib / note_seq artefacts (out of scope); every
-        # ddpm-*.cfg passes --nosnapshot_sampling.  Say so instead of silently ignoring the flag.
-        logging.warning("--snapshot_sampling is not implemented on this path (plots / MIDI are out of scope); "
-                        "--eval_samples=%d ignored", FLAGS.eval_samples)
+        writer = _summary_writer(os.path.join(output_dir, "train"))
     examples = train_batches.examples            # batches per epoch (utils/data_utils.py:63-90)
 
     class _LocalRows:                            # rows [rank*B/W, (rank+1)*B/W) of every global batch
@@ -237,6 +333,9 @@ def train(train_batches, valid_batches, sigmas, output_dir=None, verbose=True):
                 if FLAGS.early_stopping and early_stop.should_stop:
                     logging.info("EARLY STOP: Ended training after %s epochs.", epoch + 1)
                     return optimizer
+                if FLAGS.snapshot_sampling:                                 # train_ncsn.py:405-486
+                    rng = snapshot_sampling(optimizer, ema, sigmas, rng, input_shape, train_batches, valid_batches,
+                                            global_step, sampling_step, output_dir, writer)
             if FLAGS.max_steps is not None and global_step >= FLAGS.max_steps:             # train_ncsn.py:492-494
                 if writer is not None:
                     writer.flush()
@@ -265,15 +364,18 @@ def sample(scorenet, sigmas, rng, sample_shape, num_samples=2400, sampling="ald"
     if shard is not None and shard[1] > 1:
         local = parallel.shard_size(num_samples)
         rows, kw = (shard[0] * local, local), dict(shard=(shard[0] * local, num_samples))
-    shape = (num_samples, *sample_shape)
-    if sampling != "ddpm":
-        # train_ncsn.py:541-547: uniform start with zero mean / unit variance
-        rho = float(np.sqrt(np.float32(12)) / 2)
-        init = random.uniform(init_rng, shape, -rho, rho, rows=rows)
-    else:
-        init = random.normal(init_rng, shape, rows=rows)
+    init = initial_draw(init_rng, (num_samples, *sample_shape), sampling, rows=rows)
     generated, collection, ld_metrics = algorithm(ld_rng, scorenet, sigmas, init, epsilon, steps, denoise, False, **kw)
     return generated, collection, ebm_utils.collate_sampling_metrics(ld_metrics)
+
+
+def initial_draw(init_rng, shape, sampling, rows=None):
+    """The start of sample()'s chain (train_ncsn.py:541-549): N(0, 1) for ddpm, otherwise uniform with zero mean and
+    unit variance.  rows=(first, count): only those rows of the draw."""
+    if sampling != "ddpm":
+        rho = float(np.sqrt(np.float32(12)) / 2)
+        return random.uniform(init_rng, shape, -rho, rho, rows=rows)
+    return random.normal(init_rng, shape, rows=rows)
 
 
 def main(argv):
