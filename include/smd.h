@@ -218,6 +218,33 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
                     const float* infill_mask, float* collection, float* metrics, int use_graph,
                     smd_stream_t stream);
 
+/* ---- DDIM chain (Song et al. 2021) over a strided subset of the DDPM schedule; not in the reference ------------ */
+/* host_betas: HOST, T floats (alpha_bar_t = cumprod(1 - betas)[t] in float32, as smd_sampler_setup).  host_steps:
+ * HOST, K strictly increasing indices tau_0 < ... < tau_{K-1} in [0, T).  The chain runs i = K-1 .. 0 with
+ * a = alpha_bar(tau_i), a' = alpha_bar(tau_{i-1}) (1 at i = 0):
+ *   eps = model(x, sqrt(a)),  x0 = clip(sqrt(1/a) x - sqrt(1-a) sqrt(1/a) eps, -1, 1),  eps' = (x - sqrt(a) x0) / sqrt(1-a),
+ *   sig = eta sqrt((1-a')/(1-a)) sqrt(1 - a/a'),  x <- sqrt(a') x0 + sqrt(max(1-a'-sig^2, 0)) eps' + sig z.
+ * The step keys follow diffusion_dynamics' scan carry over K steps (smd_sampler_setup with T = K), as do the collection
+ * rows.  tau = 0..T-1 with eta = 1 is diffusion_dynamics itself; eta = 0 is deterministic given x.  The tables share
+ * the sampler's workspace regions: smd_sampler_setup, smd_langevin_setup and smd_ddim_setup each invalidate the other
+ * two (SMD_ERR_STATE).  SMD_ERR_INVALID for a TransformerMDN plan, T < 1 or T > 8192, K < 1 or K > T, indices not
+ * strictly increasing or out of range, eta < 0 or not finite, or alpha_bar outside (0, 1) at a selected index. */
+int smd_ddim_setup(smd_plan* plan, const float* host_betas, int T, const int* host_steps, int K, float eta,
+                   const uint32_t host_key[2], smd_stream_t stream);
+/* The whole K-step chain on x (n, S, C) or (n, D) in place.  infill_x / infill_mask or NULL: after each step the
+ * masked entries become sqrt(a) x_fix + sqrt(1-a) z_infill (x_fix at t = tau_i = 0).  collection: (41, n, ...) or
+ * NULL, row 0 the caller's.  metrics: (4, K) or NULL (column K-1-i: grad_norm, step_norm, alpha_bar, noise_norm).
+ * One FiLM table row per selected level; use_graph != 0 replays one captured step K times.  smd_sampler_set_shard
+ * slices the noise as for smd_ddpm_sample.  SMD_ERR_INVALID for n > max_batch. */
+int smd_ddim_sample(smd_plan* plan, const float* params, float* x, int n, const float* infill_x,
+                    const float* infill_mask, float* collection, float* metrics, int use_graph, smd_stream_t stream);
+/* Host only: the tables smd_ddim_setup uploads.  host_coef (K x 8: sqrt(1/a), sqrt(1-a) sqrt(1/a), sqrt(a'),
+ * sqrt(max(1-a'-sig^2, 0)), sig, sqrt(a), sqrt(1-a), a), host_keys (K x 4: noise key, infill key of step i) and
+ * host_slots (K: collection row of step i or -1); each may be NULL (host_key only when host_keys is).  Same
+ * rejections as smd_ddim_setup. */
+int smd_ddim_tables(const float* host_betas, int T, const int* host_steps, int K, float eta,
+                    const uint32_t host_key[2], float* host_coef, uint32_t* host_keys, int* host_slots);
+
 /* ---- Langevin chains (annealed / consistent Langevin dynamics of the NCSN family) ------------------------------ */
 /* kind 0 = annealed (utils/ebm_utils.py:89-198), 1 = consistent (:201-271).  host_sigmas: HOST, L floats (L >= 2).
  * steps_per_level: T of the annealed chain (ignored by the consistent one).  host_key: the `rng` the sampler receives.

@@ -888,6 +888,82 @@ void launch_reverse_step(const ReverseStepArgs& a, cudaStream_t st) {
   const int NC = a.N * a.C;
   reverse_step_kernel<<<(4 * NC + 255) / 256, 256, 0, st>>>(a);
 }
+
+// ---------------------------------------------------------------------------------------------------
+// DDIM step after the network call (Song et al. 2021, eq. 12, with the reference's clipped x0 estimate): the
+// reverse_step_kernel layout -- four lanes per (sample, channel) column, a quarter of its S positions each
+// ---------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+ddim_step_kernel(const DdimStepArgs a) {
+  pdl_trigger();
+  pdl_wait();
+  const int si = *a.i_ptr;
+  const float* cf = a.coef + 8 * si;
+  const float sqrt_recip = cf[0], sqrt_m1 = cf[1], c_x0 = cf[2], c_dir = cf[3], sig = cf[4], sqrt_a = cf[5],
+              sqrt_1m = cf[6], abar = cf[7];
+  const uint32_t k0 = a.key_tab[4 * si], k1 = a.key_tab[4 * si + 1], ik0 = a.key_tab[4 * si + 2],
+                 ik1 = a.key_tab[4 * si + 3];
+  const bool t_pos = si > 0 || a.tau0 > 0;     // t = tau_i > 0
+  const int NC = a.N * a.C;
+  const uint32_t total = static_cast<uint32_t>(a.N) * a.S * a.C;
+  const uint32_t rtotal = a.rng_total ? a.rng_total : total, rfirst = a.rng_total ? a.rng_first : 0u;
+  const int slot = a.collection ? a.slot_tab[si] : -1;
+  float m_eps = 0.f, m_step = 0.f, m_noise = 0.f;
+  constexpr int kSG = 4;
+  const int gi = blockIdx.x * blockDim.x + threadIdx.x;
+  const int i = gi / kSG, sg = gi % kSG;
+  float e2 = 0.f, st2 = 0.f, nz2 = 0.f;
+  if (i < NC) {
+    const int n = i / a.C, c = i % a.C;
+    const int per = (a.S + kSG - 1) / kSG;
+    const int s_end = min(a.S, (sg + 1) * per);
+    for (int s = sg * per; s < s_end; ++s) {
+      const uint32_t idx = (static_cast<uint32_t>(n) * a.S + s) * a.C + c;
+      const float x = a.x[idx];
+      const float eh = a.eps_hat[idx];
+      float x0 = __fsub_rn(__fmul_rn(sqrt_recip, x), __fmul_rn(sqrt_m1, eh));
+      x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
+      const float dir = __fdiv_rn(__fsub_rn(x, __fmul_rn(sqrt_a, x0)), sqrt_1m);
+      // sig = 0 (eta = 0, or the last step) draws nothing: the deterministic chain needs no noise stream
+      const float noise = sig != 0.f ? sig * jax_normal_from_bits(jax_random_bits(k0, k1, rfirst + idx, rtotal)) : 0.f;
+      float nx = __fadd_rn(__fadd_rn(__fmul_rn(c_x0, x0), __fmul_rn(c_dir, dir)), noise);
+      if (a.infill_mask) {
+        const float mk = a.infill_mask[idx];
+        const float ix = a.infill_x[idx];
+        float y = ix;
+        if (t_pos) y = sqrt_a * ix + sqrt_1m * jax_normal_from_bits(jax_random_bits(ik0, ik1, rfirst + idx, rtotal));
+        nx = nx * (1.0f - mk) + y * mk;
+      }
+      const float stp = x - nx;
+      e2 += eh * eh; st2 += stp * stp; nz2 += noise * noise;
+      a.x_next[idx] = nx;
+      if (slot >= 0) a.collection[static_cast<size_t>(slot) * total + idx] = nx;
+    }
+  }
+  e2 += __shfl_xor_sync(0xffffffffu, e2, 1); st2 += __shfl_xor_sync(0xffffffffu, st2, 1); nz2 += __shfl_xor_sync(0xffffffffu, nz2, 1);
+  e2 += __shfl_xor_sync(0xffffffffu, e2, 2); st2 += __shfl_xor_sync(0xffffffffu, st2, 2); nz2 += __shfl_xor_sync(0xffffffffu, nz2, 2);
+  if (i < NC && sg == 0) { m_eps = sqrtf(e2 + 1e-10f); m_step = sqrtf(st2 + 1e-10f); m_noise = sqrtf(nz2 + 1e-10f); }
+  if (a.metrics) {
+    __shared__ float red[3][8];
+    m_eps = warp_sum(m_eps); m_step = warp_sum(m_step); m_noise = warp_sum(m_noise);
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+    if (l == 0) { red[0][w] = m_eps; red[1][w] = m_step; red[2][w] = m_noise; }
+    __syncthreads();
+    const int col = a.K - 1 - si;
+    if (threadIdx.x < 3) {
+      float v = 0.f;
+      for (int j = 0; j < (blockDim.x >> 5); ++j) v += red[threadIdx.x][j];
+      const int row = (threadIdx.x == 0) ? 0 : (threadIdx.x == 1 ? 1 : 3);
+      atomicAdd(a.metrics + row * a.K + col, v / static_cast<float>(NC));
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 3) a.metrics[2 * a.K + col] = abar;
+  }
+}
+void launch_ddim_step(const DdimStepArgs& a, cudaStream_t st) {
+  const int NC = a.N * a.C;
+  ddim_step_kernel<<<(4 * NC + 255) / 256, 256, 0, st>>>(a);
+}
+
 __global__ void step_advance_kernel(int* t_ptr) { *t_ptr -= 1; }
 void launch_step_advance(int* t_ptr, cudaStream_t st) { step_advance_kernel<<<1, 1, 0, st>>>(t_ptr); }
 __global__ void fill_cond_kernel(const float* coef, const int* t_ptr, float* cond, int n) {

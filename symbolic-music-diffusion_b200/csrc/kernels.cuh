@@ -219,6 +219,29 @@ struct ReverseStepArgs {
 };
 // One body of the reverse-diffusion scan after the network call (utils/ebm_utils.py:332-394)
 void launch_reverse_step(const ReverseStepArgs& a, cudaStream_t st);
+// DDIM step over a strided subset tau_0 < ... < tau_{K-1} of the schedule (smd_ddim_setup), indexed by the step i:
+// a = alpha_bar(tau_i), a' = alpha_bar(tau_{i-1}) (1 at i = 0), sig = eta sqrt((1-a')/(1-a)) sqrt(1 - a/a').
+struct DdimStepArgs {
+  const float* x;          // state (N, S, C)
+  const float* eps_hat;    // model output eps = model(x, sqrt(a))
+  const uint32_t* key_tab; // device table [K][4] = (noise k0,k1, infill k0,k1) indexed by step i
+  const float* coef;       // device table [K][8]: sqrt(1/a), sqrt(1-a) sqrt(1/a), sqrt(a'), sqrt(max(1-a'-sig^2, 0)),
+                           //                     sig, sqrt(a), sqrt(1-a), a
+  const int* slot_tab;     // device table [K]: collection slot or -1
+  const int* i_ptr;        // device scalar: current step i (graph-replayable)
+  const float* infill_x;   // or null
+  const float* infill_mask;
+  float* x_next;
+  float* collection;       // (41, N, S, C) or null
+  float* metrics;          // device [4][K] accumulators (grad_norm, step_norm, alpha_bar, noise_norm); column K-1-i
+  int N, S, C, K;
+  int tau0;                // tau_0: the step i = 0 is at t = 0 (infill template x_fix itself) when tau_0 == 0
+  uint32_t rng_first, rng_total;   // sharded sampling as ReverseStepArgs
+};
+// x0 = clip(sqrt(1/a) x - sqrt(1-a) sqrt(1/a) eps, -1, 1);  eps' = (x - sqrt(a) x0) / sqrt(1-a);
+// x <- sqrt(a') x0 + sqrt(max(1-a'-sig^2, 0)) eps' + sig z, then the infill blend at t = tau_i, the metrics and the
+// collection row
+void launch_ddim_step(const DdimStepArgs& a, cudaStream_t st);
 // *t_ptr -= 1 ; cond[0..n) = coef[t].sqrt_ap   (device-side step bookkeeping for graph replay)
 void launch_step_advance(int* t_ptr, cudaStream_t st);
 void launch_fill_cond(const float* coef, const int* t_ptr, float* cond, int n, cudaStream_t st);

@@ -135,9 +135,9 @@ struct TrainState {
 // loss kernels receive.
 enum Objective : int { kObjDdpm = 0, kObjDsm = 1, kObjSsm = 2, kObjMdn = 3 };
 
-// The sampler chain whose tables (coef / keys / slots / t_ptr, the FiLM table) the workspace holds: the DDPM sampler
-// and the Langevin chain share those regions, so at most one of them is set up at a time.
-enum Chain : int { kChainNone = 0, kChainDdpm = 1, kChainLangevin = 2 };
+// The sampler chain whose tables (coef / keys / slots / t_ptr, the FiLM table) the workspace holds: the DDPM sampler,
+// the Langevin chain and the DDIM chain share those regions, so at most one of them is set up at a time.
+enum Chain : int { kChainNone = 0, kChainDdpm = 1, kChainLangevin = 2, kChainDdim = 3 };
 
 // The legacy default stream cannot be captured into a CUDA graph.
 inline bool capturable(cudaStream_t st) { return st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread; }
@@ -241,6 +241,7 @@ struct smd_plan {
   // one row per level).
   smd::Chain chain = smd::kChainNone;
   smd::CapturedGraph chain_graph;
+  int ddim_tau0 = 0;               // DDIM: the first selected index tau_0 (plan->T holds the number of steps K)
   int lv_kind = 0, lv_steps = 1;   // Langevin: kind (0 annealed, 1 consistent), steps per level
   uint32_t lv_key[2] = {0u, 0u};
   float lv_sigma_last = 0.f;

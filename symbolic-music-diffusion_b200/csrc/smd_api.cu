@@ -1090,6 +1090,38 @@ int smd_ddpm_draws(smd_plan* plan, const uint32_t host_key[2], int batch, float*
   return smd_ddpm_draws_sharded(plan, host_key, batch, 0, batch, 1, used_alpha, eps, labels_or_null, stream);
 }
 
+// Keys of a reverse scan of T steps (t = T-1 .. 0): rng,key = split(rng); rng,infill = split(rng); rng,noise =
+// split(rng) per step; keys[4t .. 4t+3] = (noise, infill)
+static void scan_keys(const uint32_t host_key[2], int T, uint32_t* keys) {
+  uint32_t rng[2] = {host_key[0], host_key[1]};
+  for (int t = T - 1; t >= 0; --t) {
+    uint32_t o[4];
+    h_split(rng, 2, o); rng[0] = o[0]; rng[1] = o[1];
+    h_split(rng, 2, o); rng[0] = o[0]; rng[1] = o[1];
+    keys[4 * t + 2] = o[2]; keys[4 * t + 3] = o[3];
+    h_split(rng, 2, o); rng[0] = o[0]; rng[1] = o[1];
+    keys[4 * t + 0] = o[2]; keys[4 * t + 1] = o[3];
+  }
+}
+
+// Collection slots of a reverse scan of T steps (utils/ebm_utils.py:320-325, 387-394): collection_idx =
+// linspace(1, T, 40).astype(int32); the step at t writes row sum(j : idx[j] == T - t + 1) + 1, or none (slots[t] = -1)
+static void collection_slots(int T, int* slots) {
+  int idx_tab[40];
+  for (int j = 0; j < 40; ++j) {
+    const float v = (40 > 1) ? (1.0f + static_cast<float>(j) * (static_cast<float>(T - 1) / 39.0f)) : 1.0f;
+    idx_tab[j] = (j == 39) ? T : static_cast<int>(v);
+  }
+  for (int t = 0; t < T; ++t) {
+    const int image_idx = T - t + 1;
+    int sum = 0; bool any = false;
+    for (int j = 0; j < 40; ++j) if (idx_tab[j] == image_idx) { sum += j; any = true; }
+    // below T = 40 linspace repeats indices and the summed slot can pass the 41 collection rows (184 at T = 8); XLA's
+    // scatter drops such an update, so the step writes no row
+    slots[t] = (any && sum + 1 < 41) ? sum + 1 : -1;
+  }
+}
+
 int smd_sampler_setup(smd_plan* plan, const float* host_betas, int T, const uint32_t host_key[2],
                       smd_stream_t stream) {
   if (reject_mdn(plan, "smd_sampler_setup")) return SMD_ERR_INVALID;
@@ -1119,32 +1151,10 @@ int smd_sampler_setup(smd_plan* plan, const float* host_betas, int T, const uint
     c[0] = sqrt_recip; c[1] = sqrt_m1; c[2] = mu1; c[3] = mu2; c[4] = sigma;
     c[5] = sqrtf(ap[i]); c[6] = sqrtf(1.0f - ap[i]); c[7] = ap[i];
   }
-  // keys: per scan step (t = T-1 .. 0): rng,key = split(rng); rng,infill = split(rng); rng,noise = split(rng)
   std::vector<uint32_t> keys(static_cast<size_t>(T) * 4);
-  uint32_t rng[2] = {host_key[0], host_key[1]};
-  for (int t = T - 1; t >= 0; --t) {
-    uint32_t o[4];
-    h_split(rng, 2, o); rng[0] = o[0]; rng[1] = o[1];
-    h_split(rng, 2, o); rng[0] = o[0]; rng[1] = o[1];
-    keys[4 * t + 2] = o[2]; keys[4 * t + 3] = o[3];
-    h_split(rng, 2, o); rng[0] = o[0]; rng[1] = o[1];
-    keys[4 * t + 0] = o[2]; keys[4 * t + 1] = o[3];
-  }
-  // collection slots (utils/ebm_utils.py:320-325, 387-394): collection_idx = linspace(1, T, 40).astype(int32)
+  scan_keys(host_key, T, keys.data());
   std::vector<int> slots(T, -1);
-  int idx_tab[40];
-  for (int j = 0; j < 40; ++j) {
-    const float v = (40 > 1) ? (1.0f + static_cast<float>(j) * (static_cast<float>(T - 1) / 39.0f)) : 1.0f;
-    idx_tab[j] = (j == 39) ? T : static_cast<int>(v);
-  }
-  for (int t = 0; t < T; ++t) {
-    const int image_idx = T - t + 1;
-    int sum = 0; bool any = false;
-    for (int j = 0; j < 40; ++j) if (idx_tab[j] == image_idx) { sum += j; any = true; }
-    // below T = 40 linspace repeats indices and the summed slot can pass the 41 collection rows (184 at T = 8); XLA's
-    // scatter drops such an update, so the step writes no row
-    if (any && sum + 1 < 41) slots[t] = sum + 1;
-  }
+  collection_slots(T, slots.data());
   SMD_CUDA(cudaMemcpyAsync(plan->at<float>(plan->reg.coef), coef.data(), coef.size() * 4, cudaMemcpyHostToDevice, st));
   SMD_CUDA(cudaMemcpyAsync(plan->at<uint32_t>(plan->reg.keys), keys.data(), keys.size() * 4, cudaMemcpyHostToDevice, st));
   SMD_CUDA(cudaMemcpyAsync(plan->at<int>(plan->reg.slots), slots.data(), slots.size() * 4, cudaMemcpyHostToDevice, st));
@@ -1282,6 +1292,146 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
     if (rc) return rc;
   }
   for (int i = 0; i < steps; ++i) {
+    const int rc = plan->chain_graph.launch(cs);
+    if (rc) return rc;
+  }
+  return join_replay(plan, st, cs);
+}
+
+// ---- DDIM chain (Song et al. 2021) over a strided subset of the DDPM schedule -----------------------------------------
+
+// Host tables of smd_ddim_setup for the K selected indices tau_i (alpha_bar in float32 as smd_sampler_setup, the
+// coefficients in float64 from it, rounded to float32):
+//   coef[i] = (sqrt(1/a), sqrt(1-a) sqrt(1/a), sqrt(a'), sqrt(max(1-a'-sig^2, 0)), sig, sqrt(a), sqrt(1-a), a)
+// with a = alpha_bar(tau_i), a' = alpha_bar(tau_{i-1}) (1 at i = 0), sig = eta sqrt((1-a')/(1-a)) sqrt(1 - a/a').
+static int ddim_tables(const float* betas, int T, const int* steps, int K, float eta, float* coef) {
+  if (!betas || !steps) { set_error("null betas or steps"); return SMD_ERR_INVALID; }
+  if (T < 1 || T > kMaxT) { set_error("T out of range"); return SMD_ERR_INVALID; }
+  if (K < 1 || K > T) { set_error("the number of DDIM steps must be in [1, T]"); return SMD_ERR_INVALID; }
+  if (!std::isfinite(eta) || eta < 0.f) { set_error("eta must be finite and >= 0"); return SMD_ERR_INVALID; }
+  for (int i = 0; i < K; ++i)
+    if (steps[i] < 0 || steps[i] >= T || (i > 0 && steps[i] <= steps[i - 1])) {
+      set_error("the DDIM steps must be strictly increasing indices in [0, T)");
+      return SMD_ERR_INVALID;
+    }
+  std::vector<float> ap(T);
+  float run = 1.0f;
+  for (int t = 0; t < T; ++t) { const float al = 1.0f - betas[t]; run = (t == 0) ? al : run * al; ap[t] = run; }
+  for (int i = 0; i < K; ++i) {
+    if (!(ap[steps[i]] > 0.f && ap[steps[i]] < 1.f)) {
+      set_error("alpha_bar must lie in (0, 1) at every selected step");
+      return SMD_ERR_INVALID;
+    }
+    // float64 from the float32 alpha_bar, rounded once: near t = 0, 1 - a' - sig^2 cancels (at eta = 1 it is
+    // alpha_t (1-a')^2 / (1-a), far below 1 - a'), which float32 arithmetic would leave good to a few 1e-5 only
+    const double a = ap[steps[i]], ap_prev = i > 0 ? ap[steps[i - 1]] : 1.0;
+    const double sig = static_cast<double>(eta) * sqrt((1.0 - ap_prev) / (1.0 - a)) * sqrt(std::max(1.0 - a / ap_prev, 0.0));
+    const double c64[8] = {sqrt(1.0 / a), sqrt(1.0 - a) * sqrt(1.0 / a), sqrt(ap_prev),
+                           sqrt(std::max(1.0 - ap_prev - sig * sig, 0.0)), sig, sqrt(a), sqrt(1.0 - a), a};
+    for (int j = 0; j < 8; ++j) coef[static_cast<size_t>(i) * 8 + j] = static_cast<float>(c64[j]);
+  }
+  return SMD_OK;
+}
+
+int smd_ddim_tables(const float* host_betas, int T, const int* host_steps, int K, float eta,
+                    const uint32_t host_key[2], float* host_coef, uint32_t* host_keys, int* host_slots) {
+  std::vector<float> coef(static_cast<size_t>(std::max(K, 0)) * 8);
+  const int rc = ddim_tables(host_betas, T, host_steps, K, eta, coef.data());
+  if (rc) return rc;
+  if (host_keys && !host_key) { set_error("host_keys needs host_key"); return SMD_ERR_INVALID; }
+  if (host_coef) memcpy(host_coef, coef.data(), coef.size() * sizeof(float));
+  if (host_keys) scan_keys(host_key, K, host_keys);
+  if (host_slots) collection_slots(K, host_slots);
+  return SMD_OK;
+}
+
+int smd_ddim_setup(smd_plan* plan, const float* host_betas, int T, const int* host_steps, int K, float eta,
+                   const uint32_t host_key[2], smd_stream_t stream) {
+  if (!plan || !host_key) { set_error("null argument"); return SMD_ERR_INVALID; }
+  if (reject_mdn(plan, "smd_ddim_setup")) return SMD_ERR_INVALID;
+  std::vector<float> coef(static_cast<size_t>(std::max(K, 0)) * 8);
+  const int rc = ddim_tables(host_betas, T, host_steps, K, eta, coef.data());
+  if (rc) return rc;
+  if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
+  // K <= T <= kMaxT rows: the tables fit the coef / keys / slots regions of the DDPM sampler
+  std::vector<uint32_t> keys(static_cast<size_t>(K) * 4);
+  scan_keys(host_key, K, keys.data());
+  std::vector<int> slots(K);
+  collection_slots(K, slots.data());
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  SMD_CUDA(cudaMemcpyAsync(plan->at<float>(plan->reg.coef), coef.data(), coef.size() * 4, cudaMemcpyHostToDevice, st));
+  SMD_CUDA(cudaMemcpyAsync(plan->at<uint32_t>(plan->reg.keys), keys.data(), keys.size() * 4, cudaMemcpyHostToDevice, st));
+  SMD_CUDA(cudaMemcpyAsync(plan->at<int>(plan->reg.slots), slots.data(), slots.size() * 4, cudaMemcpyHostToDevice, st));
+  SMD_CUDA(cudaStreamSynchronize(st));  // host tables go out of scope
+  plan->T = K;
+  plan->ddim_tau0 = host_steps[0];
+  plan->chain = kChainDdim;
+  plan->film_tab_ready = false;
+  plan->chain_graph.drop();
+  return SMD_OK;
+}
+
+// One DDIM step at the device step counter i = *t_ptr: network call on sqrt(a) (FiLM table row i, or the generator on
+// coef[i].sqrt(a)), the fused update, then i -= 1.  The eager loop and the captured graph run this same sequence.
+static int ddim_step(smd_plan* plan, const float* params, float* x, int n, const float* infill_x,
+                     const float* infill_mask, float* collection, float* metrics, cudaStream_t st) {
+  float* tvec = plan->at<float>(plan->reg.tvec);
+  int* t_ptr = plan->at<int>(plan->reg.t_ptr);
+  const float* coef = plan->at<float>(plan->reg.coef);
+  const FilmRows film = film_table_rows(plan, params, -1, t_ptr);
+  if (!film.table) { launch_fill_cond(coef, t_ptr, tvec, 1, st); CNT(); }
+  float* eh = plan->at<float>(plan->reg.eps_hat);
+  const int rc = run_forward(plan, params, x, tvec, 1, n, eh, st, false, false, false, film);
+  if (rc) return rc;
+  DdimStepArgs a;
+  memset(&a, 0, sizeof(a));
+  a.x = x; a.eps_hat = eh;
+  a.key_tab = plan->at<uint32_t>(plan->reg.keys);
+  a.coef = coef;
+  a.slot_tab = plan->at<int>(plan->reg.slots);
+  a.i_ptr = t_ptr;
+  a.infill_x = infill_x; a.infill_mask = infill_mask;
+  a.x_next = x; a.collection = collection; a.metrics = metrics;
+  a.N = n; a.K = plan->T; a.tau0 = plan->ddim_tau0;
+  chain_geometry(plan, a, /*sharded=*/true);
+  launch_ddim_step(a, st); CNT();
+  launch_step_advance(t_ptr, st); CNT();
+  SMD_LAUNCH_CHECK("ddim_step");
+  return SMD_OK;
+}
+
+int smd_ddim_sample(smd_plan* plan, const float* params, float* x, int n, const float* infill_x,
+                    const float* infill_mask, float* collection, float* metrics, int use_graph, smd_stream_t stream) {
+  if (!plan) { set_error("null plan"); return SMD_ERR_INVALID; }
+  if (reject_mdn(plan, "smd_ddim_sample")) return SMD_ERR_INVALID;
+  if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
+  if ((infill_x == nullptr) != (infill_mask == nullptr)) { set_error("infill_x and infill_mask go together"); return SMD_ERR_INVALID; }
+  if (plan->chain != kChainDdim) { set_error("smd_ddim_setup has not been called"); return SMD_ERR_STATE; }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int K = plan->T;
+  cudaStream_t cs = st;
+  if (use_graph) { const int rc0 = replay_stream(plan, st, &cs); if (rc0) return rc0; }
+  if (metrics) SMD_CUDA(cudaMemsetAsync(metrics, 0, sizeof(float) * 4 * K, cs));
+  { const int rc0 = ensure_film_table(plan, params, 8, 5, cs); if (rc0) return rc0; }
+  int* t_ptr = plan->at<int>(plan->reg.t_ptr);
+  const int i0 = K - 1;
+  SMD_CUDA(cudaMemcpyAsync(t_ptr, &i0, sizeof(int), cudaMemcpyHostToDevice, cs));
+  SMD_CUDA(cudaStreamSynchronize(cs));  // i0 is a stack variable
+  if (!use_graph) {
+    for (int i = 0; i < K; ++i) {
+      const int rc = ddim_step(plan, params, x, n, infill_x, infill_mask, collection, metrics, cs);
+      if (rc) return rc;
+    }
+    return SMD_OK;
+  }
+  const GraphKey key = graph_key(n, params, x, infill_x, infill_mask, collection, metrics);
+  if (!plan->chain_graph.replays(key)) {
+    const int rc = plan->chain_graph.capture(cs, key, [&] {
+      return ddim_step(plan, params, x, n, infill_x, infill_mask, collection, metrics, cs);
+    }, "ddim graph");
+    if (rc) return rc;
+  }
+  for (int i = 0; i < K; ++i) {
     const int rc = plan->chain_graph.launch(cs);
     if (rc) return rc;
   }

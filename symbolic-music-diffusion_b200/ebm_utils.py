@@ -60,6 +60,62 @@ def diffusion_dynamics(rng, model, betas, init, epsilon, T, denoise, infill=Fals
     return x, collection, metrics.unsqueeze(2)
 
 
+DDIM_SCHEDULES = ("uniform", "quadratic")
+
+
+def ddim_schedule(T, K, schedule="uniform"):
+    """The K indices tau_0 < ... < tau_{K-1} of a T-step schedule that the DDIM chain visits (int32):
+    uniform tau_i = round(i (T-1) / (K-1)), quadratic tau_i = round((T-1) (i / (K-1))^2), both [T-1] for K = 1 (round
+    half to even, in float64).  ValueError for K outside [1, T], an unknown schedule, or quadratic indices that are not
+    strictly increasing (too many steps for T)."""
+    T, K = int(T), int(K)
+    if schedule not in DDIM_SCHEDULES:
+        raise ValueError(f"unknown DDIM schedule {schedule!r} (expected one of {list(DDIM_SCHEDULES)})")
+    if K < 1 or K > T:
+        raise ValueError(f"the number of DDIM steps must be in [1, T = {T}], got {K}")
+    if K == 1:
+        return np.asarray([T - 1], np.int32)
+    i = np.arange(K, dtype=np.float64)
+    if schedule == "uniform":
+        tau = np.rint(i * (T - 1) / (K - 1))
+    else:
+        tau = np.rint((T - 1) * (i / (K - 1)) ** 2)
+    tau = tau.astype(np.int32)
+    if np.any(np.diff(tau) <= 0):
+        raise ValueError(f"the {schedule} schedule of {K} steps over T = {T} repeats indices")
+    return tau
+
+
+def ddim_dynamics(rng, model, betas, init, epsilon, T, denoise, infill=False, infill_samples=None, infill_masks=None,
+                  shard=None, steps=50, eta=0.0, schedule="uniform"):
+    """DDIM (Song et al. 2021) over `steps` levels of the DDPM schedule `betas` picked by `schedule` (ddim_schedule),
+    with the clipped x0 estimate of diffusion_dynamics and noise scale eta (0: deterministic given `init`, 1 with all
+    T levels: diffusion_dynamics itself).  Not in the reference.  Returns (state, collection (41, N, *shape),
+    ld_metrics (4, steps, 1)); keys, collection rows, infill and shard as diffusion_dynamics with T replaced by the
+    number of steps.  epsilon / T / denoise are null, as there."""
+    from .nn import _as_device_f32
+    del epsilon, T, denoise
+    x = _as_device_f32(init).clone()
+    n = x.shape[0]
+    eng = model.engine(n)
+    betas = np.asarray(betas, np.float32)
+    tau = ddim_schedule(len(betas), steps, schedule)
+    eng.ddim_setup(betas, tau, eta, key=(int(rng[0]), int(rng[1])))
+    eng.set_sampler_shard(*(shard if shard is not None else (0, 0)))
+    ix = im = None
+    collection = torch.zeros((41,) + tuple(x.shape), dtype=torch.float32, device=x.device)
+    if infill:
+        ix = _as_device_f32(infill_samples)
+        im = _as_device_f32(infill_masks)
+        collection[0] = x * (1 - im) + ix * im
+    else:
+        collection[0] = x
+    metrics = torch.zeros((4, len(tau)), dtype=torch.float32, device=x.device)
+    eng.ddim_sample(x, infill_x=ix, infill_mask=im, collection=collection, metrics=metrics, use_graph=True)
+    _reduce_sharded_metrics(metrics, n, shard)
+    return x, collection, metrics.unsqueeze(2)
+
+
 def _reduce_sharded_metrics(metrics, n, shard):
     """The sampler metrics are means over the batch (utils/ebm_utils.py:166-170, 380-384): with shard = (first_row,
     total_rows) over several ranks, one weighted all-reduce at the end; row 2 (alpha / alpha_prod) is no batch mean."""

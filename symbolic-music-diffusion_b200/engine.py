@@ -496,6 +496,30 @@ class Engine:
                                             1 if use_graph else 0, self._stream()))
         return x
 
+    def ddim_setup(self, betas: np.ndarray, steps, eta: float = 0.0, key=(0, 0)) -> None:
+        """DDIM over the strictly increasing indices `steps` of the schedule `betas` (include/smd.h smd_ddim_setup);
+        replaces a sampler_setup or langevin_setup schedule (and vice versa)."""
+        self._ensure_ws()
+        b = np.ascontiguousarray(betas, np.float32)
+        s = np.ascontiguousarray(steps, np.int32)
+        k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
+        _lib.check(self.lib.smd_ddim_setup(self._plan, b.ctypes.data_as(C.POINTER(C.c_float)), len(b),
+                                           s.ctypes.data_as(C.POINTER(C.c_int)), len(s), float(eta), k,
+                                           self._stream()))
+
+    def ddim_sample(self, x, infill_x=None, infill_mask=None, collection=None, metrics=None, use_graph: bool = True):
+        """Runs the whole DDIM chain of ddim_setup in place on x.  collection: (41, n, ...) with row 0 left to the
+        caller; metrics: (4, K)."""
+        x = _f32c(x, "x")
+        for t, name in ((infill_x, "infill_x"), (infill_mask, "infill_mask"), (collection, "collection"),
+                        (metrics, "metrics")):
+            if t is not None:
+                _f32c(t, name)
+        _lib.check(self.lib.smd_ddim_sample(self._plan, self.params.data_ptr(), x.data_ptr(), x.shape[0],
+                                            _ptr(infill_x), _ptr(infill_mask), _ptr(collection), _ptr(metrics),
+                                            1 if use_graph else 0, self._stream()))
+        return x
+
     LANGEVIN_KINDS = {"ald": 0, "cas": 1}
 
     def langevin_setup(self, sigmas: np.ndarray, steps_per_level: int, epsilon: float, kind: str = "ald",

@@ -70,6 +70,12 @@ _SIGNATURES = {
     "smd_threefry_uniform_slice": (C.c_int, [C.POINTER(C.c_uint32), _P, C.c_longlong, C.c_longlong, C.c_longlong,
                                              C.c_float, C.c_float, _P]),
     "smd_threefry_split": (C.c_int, [C.POINTER(C.c_uint32), C.c_int, C.POINTER(C.c_uint32)]),
+    "smd_ddim_setup": (C.c_int, [_P, C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_int), C.c_int, C.c_float,
+                                 C.POINTER(C.c_uint32), _P]),
+    "smd_ddim_sample": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, C.c_int, _P]),
+    "smd_ddim_tables": (C.c_int, [C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_int), C.c_int, C.c_float,
+                                  C.POINTER(C.c_uint32), C.POINTER(C.c_float), C.POINTER(C.c_uint32),
+                                  C.POINTER(C.c_int)]),
     "smd_langevin_setup": (C.c_int, [_P, C.POINTER(C.c_float), C.c_int, C.c_int, C.c_float, C.c_int,
                                      C.POINTER(C.c_uint32), _P]),
     "smd_langevin_sample": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, C.c_int, _P, _P, C.c_int, _P]),

@@ -77,7 +77,7 @@ def generate_samples(sample_shape, num_samples, rng_seed=1):
 
 def infill_samples(samples, masks, rng_seed=1):
     """sample_ncsn.py:189-242: keep the masked (=1) entries of `samples`, regenerate the rest with the --sampling
-    chain (ald or ddpm; cas has no infilling, as upstream)."""
+    chain (ald, ddpm or ddim; cas has no infilling, as upstream)."""
     del rng_seed
     if FLAGS.sampling == "ald":
         algorithm = ebm_utils.annealed_langevin_dynamics
@@ -85,6 +85,8 @@ def infill_samples(samples, masks, rng_seed=1):
         algorithm = ebm_utils.consistent_langevin_dynamics
     elif FLAGS.sampling == "ddpm":
         algorithm = ebm_utils.diffusion_dynamics
+    elif FLAGS.sampling == "ddim":
+        algorithm = train_ncsn.ddim_algorithm()
     else:
         raise ValueError(f"Unknown sampling algorithm: {FLAGS.sampling}")
     rng, optimizer = _restore(FLAGS.model_dir, samples.shape[1:])

@@ -10,6 +10,7 @@ snapshot and writes them under --model_dir (snapshot_sampling).
 """
 from __future__ import annotations
 
+import functools
 import json
 import os
 import time
@@ -50,7 +51,8 @@ flags.DEFINE_enum("schedule_type", "geometric", ["geometric", "linear", "fibonac
 flags.DEFINE_integer("num_sigmas", 15, "Length of the noise schedule.")
 flags.DEFINE_integer("ld_steps", 100, "Langevin steps per noise level (null for ddpm).")
 flags.DEFINE_float("ld_epsilon", 2e-6, "Langevin step size (null for ddpm).")
-flags.DEFINE_enum("sampling", "ald", ["ald", "cas", "ddpm"], "Sampling algorithm.")
+flags.DEFINE_enum("sampling", "ald", ["ald", "cas", "ddpm", "ddim"],
+                  "Sampling algorithm (ddim is an addition of this implementation, see --ddim_steps).")
 flags.DEFINE_bool("ema", True, "Track an exponential moving average of the parameters.")
 flags.DEFINE_float("mu", 0.999, "EMA momentum.")
 flags.DEFINE_bool("denoise", True, "Expected-denoised-sample step (null for ddpm).")
@@ -74,6 +76,9 @@ flags.DEFINE_bool("verbose", True, "Verbose logging.")
 # --- additions of this implementation (not in the reference) ------------------------------------------------
 flags.DEFINE_bool("synthetic", False, "Use synthetic N(0,1) latents of --data_shape instead of reading --dataset.")
 flags.DEFINE_integer("synthetic_examples", 4096, "Examples per split with --synthetic.")
+flags.DEFINE_integer("ddim_steps", 50, "--sampling=ddim: noise levels of the DDPM schedule the chain visits.")
+flags.DEFINE_float("ddim_eta", 0.0, "--sampling=ddim: noise scale (0: deterministic; 1 with all levels: ddpm).")
+flags.DEFINE_enum("ddim_schedule", "uniform", ["uniform", "quadratic"], "--sampling=ddim: spacing of the levels.")
 
 
 def model_kwargs():
@@ -353,6 +358,8 @@ def sample(scorenet, sigmas, rng, sample_shape, num_samples=2400, sampling="ald"
     num_samples-sample run -- its slice of the initial draw and of every step's noise stream."""
     if sampling == "ddpm":
         algorithm = ebm_utils.diffusion_dynamics
+    elif sampling == "ddim":
+        algorithm = ddim_algorithm()
     elif sampling == "ald":
         algorithm = ebm_utils.annealed_langevin_dynamics
     elif sampling == "cas":
@@ -369,10 +376,17 @@ def sample(scorenet, sigmas, rng, sample_shape, num_samples=2400, sampling="ald"
     return generated, collection, ebm_utils.collate_sampling_metrics(ld_metrics)
 
 
+def ddim_algorithm():
+    """ebm_utils.ddim_dynamics with --ddim_steps, --ddim_eta and --ddim_schedule bound: the signature of the other
+    samplers."""
+    return functools.partial(ebm_utils.ddim_dynamics, steps=FLAGS.ddim_steps, eta=FLAGS.ddim_eta,
+                             schedule=FLAGS.ddim_schedule)
+
+
 def initial_draw(init_rng, shape, sampling, rows=None):
-    """The start of sample()'s chain (train_ncsn.py:541-549): N(0, 1) for ddpm, otherwise uniform with zero mean and
-    unit variance.  rows=(first, count): only those rows of the draw."""
-    if sampling != "ddpm":
+    """The start of sample()'s chain (train_ncsn.py:541-549): N(0, 1) for ddpm and ddim, otherwise uniform with zero
+    mean and unit variance.  rows=(first, count): only those rows of the draw."""
+    if sampling not in ("ddpm", "ddim"):
         rho = float(np.sqrt(np.float32(12)) / 2)
         return random.uniform(init_rng, shape, -rho, rho, rows=rows)
     return random.normal(init_rng, shape, rows=rows)
