@@ -103,6 +103,46 @@ def ln_film_swish_bwd(g: Tensor, x: Tensor, gamma: Tensor, beta: Tensor, scale: 
     return dx, dgamma, dbeta, (dz * y).sum(dim=1), dz.sum(dim=1)
 
 
+def ssm_ln_film_swish_bwd(g: Tensor, gt: Tensor, x: Tensor, xt: Tensor, gamma: Tensor, beta: Tensor,
+                          scale: Tensor | None = None, shift: Tensor | None = None, stats: Tensor | None = None,
+                          act: str | None = "swish"):
+    """Sliced score matching's reverse pass through out = act(scale * LayerNorm(x) + shift) AND its tangent
+    out' = J_out(x) x': the gradient of <g, out> + <g', out'> with respect to x, x', gamma, beta, scale and shift.
+
+    Conventions as ln_film_swish_bwd: x, xt, g, gt are (B, S, N) with one FiLM pair (B, N) per example; scale=None is a
+    plain LayerNorm; act is "swish" or None; mean and variance take the values of the (sum, sumsq) stats.  Derived by
+    float64 autograd, not from the kernel's closed form: out' is the JVP of out (double-vjp), and the statistics carry
+    the stats' values while differentiating as functions of x.  Returns dx, dxt, dgamma, dbeta, dscale, dshift (the
+    last two (B, N), or None without FiLM)."""
+    n = x.shape[-1]
+    st = row_stats(x) if stats is None else stats
+    m_dev = (st[..., 0] / n).unsqueeze(-1)
+    v_dev = st[..., 1].unsqueeze(-1) / n - m_dev * m_dev
+    film = scale is not None
+    with torch.enable_grad():
+        leaves = [t.detach().clone().requires_grad_(True) for t in (x, xt, gamma, beta)]
+        if film:
+            leaves += [t.detach().clone().requires_grad_(True) for t in (scale, shift)]
+        xl, xtl, gl, bl = leaves[:4]
+        m_live = xl.mean(dim=-1, keepdim=True)
+        v_live = (xl * xl).mean(dim=-1, keepdim=True) - m_live * m_live
+        mean = m_live + (m_dev - m_live).detach()
+        var = v_live + (v_dev - v_live).detach()
+        z = (xl - mean) * torch.rsqrt(var + LN_EPS) * gl + bl
+        if film:
+            z = leaves[4][:, None, :] * z + leaves[5][:, None, :]
+        out = z * torch.sigmoid(z) if act == "swish" else z
+        w = torch.zeros_like(out, requires_grad=True)
+        vjp, = torch.autograd.grad(out, xl, w, create_graph=True)
+        out_t, = torch.autograd.grad(vjp, w, xtl, create_graph=True)
+        obj = (g * out).sum() + (gt * out_t).sum()
+        grads = torch.autograd.grad(obj, leaves, allow_unused=True)
+    grads = [torch.zeros_like(leaf) if d is None else d.detach() for d, leaf in zip(grads, leaves)]
+    dx, dxt, dgamma, dbeta = grads[:4]
+    dgamma, dbeta = dgamma.reshape(n), dbeta.reshape(n)
+    return (dx, dxt, dgamma, dbeta) + (tuple(grads[4:]) if film else (None, None))
+
+
 # ----------------------------------------------------------------------------------------------------------------
 # multi-head attention core (q scaled by 1 / sqrt(depth) before the dot product)
 # ----------------------------------------------------------------------------------------------------------------

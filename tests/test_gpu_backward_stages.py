@@ -147,17 +147,17 @@ class PlanView:
 
 def check_stages(eng, batch, rep, eps=None, objective="ddpm", global_batch=None):
     """The stage rules after one gradient call of `batch` examples on `eng`.  objective: "ddpm" / "dsm" (eps given: the
-    loss seed is checked), "mdn" (TransformerMDN: every rule below the head adjoint) or "ssm" (GEMM-type rules only)."""
+    loss seed is checked) or "mdn" (TransformerMDN: every rule below the head adjoint).  Sliced score matching has a
+    file of its own (test_gpu_ssm_backward_stages.py)."""
     torch.cuda.synchronize()
     v = PlanView(eng)
     cfg = eng.cfg
     dense = cfg.arch in ("DenseDDPM", "DenseNCSN")
-    mdn, ssm = objective == "mdn", objective == "ssm"
+    mdn = objective == "mdn"
     S, Cc, Md, H = eng.seq_len, cfg.channels, cfg.mlp_dims, cfg.num_heads
     Lt = 0 if dense else cfg.num_layers
     K = cfg.num_layers if dense else cfg.num_mlp_layers
     M, Bmax = batch * S, eng.max_batch
-    Mk, Bk = _ceil(M, 64), _ceil(batch, 64)
     gb = global_batch or batch
     if mdn:
         kc = cfg.mdn_components
@@ -168,12 +168,6 @@ def check_stages(eng, batch, rep, eps=None, objective="ddpm", global_batch=None)
         Hp = _ceil(Cc, 64)
         heads = [("out.", 0, Cc)]
     stats_all = v.f32("stats", 2 * K + 1, _ceil(Bmax * S, 256), 2)[:, :M]
-
-    def dw(x, g, *tangent):
-        ref = R.dense_bwd_w(x, g)
-        for xt, gt in zip(tangent[::2], tangent[1::2]):
-            ref = ref + R.dense_bwd_w(xt, gt)       # sliced score matching: primal product + tangent product
-        return ref
 
     # ------------------------------------------------------------------ loss seed
     dz = v.b16("t.dpred16", M, Hp)
@@ -187,16 +181,13 @@ def check_stages(eng, batch, rep, eps=None, objective="ddpm", global_batch=None)
         rep.rel("loss seed per-example loss", v.f32("t.loss", batch), loss, B_SEED)
         rep.rel("loss seed loss_sum", eng.loss_sum.to(F64), loss.sum().reshape(1), B_SEED)
         rep.grad(v, "out.bias", R.dense_bwd_b(dpred32), B_SEED, "colsum out.bias")
-    elif ssm:
-        rep.grad(v, "out.bias", R.dense_bwd_b(v.f32("t.dpred32", M, Cc)), B_SEED, "colsum out.bias")
     if not mdn and Hp > Cc:
         rep.zero("dpred16 pad columns", v.raw("t.dpred16", (M, Hp), torch.bfloat16)[:, Cc:])
 
     # ------------------------------------------------------------------ output projection / MDN head
     act_out = v.b16("t.act_out", M, Md)
     for pre, off, cols in heads:
-        tang = (v.b16(f"t.actt{2 * K}", M, Md), v.b16("t.dpredt16", M, Hp)[:, :Cc]) if ssm else ()
-        rep.grad(v, pre + "kernel", dw(act_out, dz[:, off:off + cols], *tang), B_DW, f"dW {pre}kernel")
+        rep.grad(v, pre + "kernel", R.dense_bwd_w(act_out, dz[:, off:off + cols]), B_DW, f"dW {pre}kernel")
         if mdn:
             rep.grad(v, pre + "bias", R.dense_bwd_b(dz[:, off:off + cols]), B_SEED, f"colsum {pre}bias")
 
@@ -220,68 +211,45 @@ def check_stages(eng, batch, rep, eps=None, objective="ddpm", global_batch=None)
         rep.grad(v, bias_name, R.dense_bwd_b(dx), b_bias or b_sums, f"{rule} dbias -> {bias_name}")
         return dx, dss
 
-    if not ssm:
-        # -------------------------------------------------------------- final LayerNorm
-        for k in range(K + 1):
-            rep.rel(f"stats of t.u{k}", stats_all[2 * k], R.row_stats(v.f32(f"t.u{k}", M, Md)), B_SEED)
-        g = R.bf16_round(R.dense_bwd_x(dz, v.b16("w.out_pad", Md, Hp)))
-        du, _ = wide_ln("out_ln", g, v.f32(f"t.u{K}", M, Md), stats_all[2 * K], "out_ln.", None, None, f"t.du16_{K}",
-                        f"k{K - 1}.res.b.bias", B_LNWIDE)   # (a short reduction: the re-rounded dX output agrees)
+    # ------------------------------------------------------------------ final LayerNorm
+    for k in range(K + 1):
+        rep.rel(f"stats of t.u{k}", stats_all[2 * k], R.row_stats(v.f32(f"t.u{k}", M, Md)), B_SEED)
+    g = R.bf16_round(R.dense_bwd_x(dz, v.b16("w.out_pad", Md, Hp)))
+    du, _ = wide_ln("out_ln", g, v.f32(f"t.u{K}", M, Md), stats_all[2 * K], "out_ln.", None, None, f"t.du16_{K}",
+                    f"k{K - 1}.res.b.bias", B_LNWIDE)   # (a short reduction: the re-rounded dX output agrees)
 
     # ------------------------------------------------------------------ FiLM'd residual blocks
     for k in range(K - 1, -1, -1):
         pre = f"k{k}.res."
         du16_next, dr16t = v.b16(f"t.du16_{k + 1}", M, Md), v.b16(f"t.dr16t_{k}", M, Md)
-        tb = (v.b16(f"t.actt{2 * k + 1}", M, Md), v.b16(f"t.dut16_{k + 1}", M, Md)) if ssm else ()
-        ta = (v.b16(f"t.actt{2 * k}", M, Md), v.b16(f"t.drt16_{k}", M, Md)) if ssm else ()
-        rep.grad(v, pre + "b.kernel", dw(v.b16(f"t.actb{k}", M, Md), du16_next, *tb), B_DW, f"dWb[{k}]")
-        rep.grad(v, pre + "a.kernel", dw(v.b16(f"t.acta{k}", M, Md), dr16t, *ta), B_DW, f"dWa[{k}]")
-        if not ssm:
-            # TransformerMDN has no FiLM generator: its blocks read the identity pair kept in block 0
-            film_k = 0 if mdn else k
-            g = R.bf16_round(R.dense_bwd_x(du16_next, v.w16(pre + "b.kernel")))
-            _, dss_b = wide_ln(f"ln_b[{k}]", g, v.b16(f"t.r1_{k}", M, Md), stats_all[2 * k + 1], pre + "ln_b.", film_k,
-                               None, f"t.dr16t_{k}", pre + "a.bias", b_wide_sums(M), far=FAR_LN_B,
-                               not_nearest=NOT_NEAREST_LN_B)
-            g = R.bf16_round(R.dense_bwd_x(dr16t, v.w16(pre + "a.kernel")))
-            b_sums = b_bias = b_wide_sums(M)
-            if k == 0:   # the last dX output of the call is still in t.g16: this launch's incoming gradient is known
-                g16 = v.b16("t.g16", M, Md)
-                rep.bf16("dXa[0] -> t.g16", g16, R.dense_bwd_x(dr16t, v.w16(pre + "a.kernel")))
-                g, b_sums, b_bias = g16, B_LN128, B_LNWIDE   # (dbias also sums the residual adjoint the test carries)
-            prev_bias = f"k{k - 1}.res.b.bias" if k > 0 else ("post.bias" if Lt else "in.bias")
-            du, dss_a = wide_ln(f"ln_a[{k}]", g, v.f32(f"t.u{k}", M, Md), stats_all[2 * k], pre + "ln_a.", film_k, du,
-                                f"t.du16_{k}", prev_bias, b_sums, b_bias)
+        rep.grad(v, pre + "b.kernel", R.dense_bwd_w(v.b16(f"t.actb{k}", M, Md), du16_next), B_DW, f"dWb[{k}]")
+        rep.grad(v, pre + "a.kernel", R.dense_bwd_w(v.b16(f"t.acta{k}", M, Md), dr16t), B_DW, f"dWa[{k}]")
+        # TransformerMDN has no FiLM generator: its blocks read the identity pair kept in block 0
+        film_k = 0 if mdn else k
+        g = R.bf16_round(R.dense_bwd_x(du16_next, v.w16(pre + "b.kernel")))
+        _, dss_b = wide_ln(f"ln_b[{k}]", g, v.b16(f"t.r1_{k}", M, Md), stats_all[2 * k + 1], pre + "ln_b.", film_k,
+                           None, f"t.dr16t_{k}", pre + "a.bias", b_wide_sums(M), far=FAR_LN_B,
+                           not_nearest=NOT_NEAREST_LN_B)
+        g = R.bf16_round(R.dense_bwd_x(dr16t, v.w16(pre + "a.kernel")))
+        b_sums = b_bias = b_wide_sums(M)
+        if k == 0:   # the last dX output of the call is still in t.g16: this launch's incoming gradient is known
+            g16 = v.b16("t.g16", M, Md)
+            rep.bf16("dXa[0] -> t.g16", g16, R.dense_bwd_x(dr16t, v.w16(pre + "a.kernel")))
+            g, b_sums, b_bias = g16, B_LN128, B_LNWIDE   # (dbias also sums the residual adjoint the test carries)
+        prev_bias = f"k{k - 1}.res.b.bias" if k > 0 else ("post.bias" if Lt else "in.bias")
+        du, dss_a = wide_ln(f"ln_a[{k}]", g, v.f32(f"t.u{k}", M, Md), stats_all[2 * k], pre + "ln_a.", film_k, du,
+                            f"t.du16_{k}", prev_bias, b_sums, b_bias)
         if mdn:
             continue
         dss = v.f32("t.dss", K, Bmax, 2 * Md)[k, :batch]
-        if not ssm:
-            rep.rel(f"FiLM pair adjoint dss[{k}]", dss, dss_a + dss_b, b_wide_sums(S) / 4)
-        # ---------------------------------------------------------- FiLM generator of block k
-        fp = f"k{k}.film."
-        dss16, e2_16 = R.bf16_round(dss), R.bf16_round(v.f32(f"t.e2_{k}", batch, 512))
-        f = R.film_generator_bwd(dss16, v.f32("enc", batch, 128), v.f32(f"t.e1pre{k}", batch, 512),
-                                 v.f32(f"t.e1_{k}", batch, 512), e2_16, v.w16(fp + "ss.kernel"),
-                                 v.param(fp + "d2.kernel"))
-        rep.grad(v, fp + "ss.bias", R.dense_bwd_b(dss), B_SEED, f"colsum film.ss.bias[{k}]")
-        rep.grad(v, fp + "ss.kernel", f["ss.kernel"], B_DW, f"dWss[{k}]")
-        for name in ("d2.bias", "d2.kernel", "d1.bias", "d1.kernel"):
-            rep.grad(v, fp + name, f[name], B_DW, f"film generator {name}[{k}]")
-        if k == 0:   # the generator's scratch buffers hold the block that ran last
-            rep.rel("film generator dss16 = bf16(dss)", v.b16("t.dss16", batch, 2 * Md), dss16, B_EXACT)
-            rep.rel("film generator e2_16 = bf16(e2)", v.b16("t.e2_16", batch, 512), e2_16, B_EXACT)
-            rep.rel("film generator dXss -> t.de2", v.f32("t.de2", batch, 512), f["de2"], B_DW)
-            rep.rel("film generator dX d2 -> t.de", v.f32("t.de", batch, 512), f["de1"], B_DW)
-            if Bk != batch:
-                rep.zero("tail rows of t.dss16", v.raw("t.dss16", (Bk, 2 * Md), torch.bfloat16)[batch:])
-                rep.zero("tail rows of t.e2_16", v.raw("t.e2_16", (Bk, 512), torch.bfloat16)[batch:])
+        rep.rel(f"FiLM pair adjoint dss[{k}]", dss, dss_a + dss_b, b_wide_sums(S) / 4)
+        film_generator_rules(v, rep, k, batch, dss)
 
     du16_0 = v.b16("t.du16_0", M, Md)
     if dense:
         # ---------------------------------------------------------- input projection of the dense models
         Cp = _ceil(Cc, 64)
-        tang = (v.b16("xbt", M, Cp)[:, :Cc], v.b16("t.dut16_0", M, Md)) if ssm else ()
-        rep.grad(v, "in.kernel", dw(v.b16("xb", M, Cp)[:, :Cc], du16_0, *tang), B_DW, "dWin")
+        rep.grad(v, "in.kernel", R.dense_bwd_w(v.b16("xb", M, Cp)[:, :Cc], du16_0), B_DW, "dWin")
     else:
         # ---------------------------------------------------------- post dense + post LayerNorm
         def ln128(rule, g, h_name, pre, dres, dx16_name, bias_name):
@@ -295,7 +263,7 @@ def check_stages(eng, batch, rep, eps=None, objective="ddpm", global_batch=None)
             rep.grad(v, bias_name, R.dense_bwd_b(dx), B_LN128, f"{rule} dbias -> {bias_name}")
             return dx
 
-        rep.grad(v, "post.kernel", dw(v.b16("t.a_post", M, 128), du16_0), B_DW, "dWpost")
+        rep.grad(v, "post.kernel", R.dense_bwd_w(v.b16("t.a_post", M, 128), du16_0), B_DW, "dWpost")
         dh = ln128("post_ln", R.dense_bwd_x(du16_0, v.w16("post.kernel")), f"t.h{2 * Lt}", "post_ln.", None,
                    f"t.dh16a{Lt - 1}", f"l{Lt - 1}.ffn2.bias")
         for l in range(Lt - 1, -1, -1):
@@ -305,14 +273,14 @@ def check_stages(eng, batch, rep, eps=None, objective="ddpm", global_batch=None)
             ref = R.dense_bwd_x(dh16a, v.w16(pre + "ffn2.kernel")) * R.gelu_tanh_grad(v.b16(f"t.hpre{l}", M, Md))
             dr16 = v.b16(f"t.dr16_{l}", M, Md)
             rep.bf16(f"dX2[{l}] x gelu'(hpre) -> t.dr16_{l}", dr16, ref)
-            rep.grad(v, pre + "ffn2.kernel", dw(v.b16(f"t.hid{l}", M, Md), dh16a), B_DW, f"dW2[{l}]")
+            rep.grad(v, pre + "ffn2.kernel", R.dense_bwd_w(v.b16(f"t.hid{l}", M, Md), dh16a), B_DW, f"dW2[{l}]")
             rep.grad(v, pre + "ffn1.bias", R.dense_bwd_b(dr16), B_SEED, f"colsum ffn1.bias[{l}]")
-            rep.grad(v, pre + "ffn1.kernel", dw(v.b16(f"t.a2_{l}", M, 128), dr16), B_DW, f"dW1[{l}]")
+            rep.grad(v, pre + "ffn1.kernel", R.dense_bwd_w(v.b16(f"t.a2_{l}", M, 128), dr16), B_DW, f"dW1[{l}]")
             dh = ln128(f"ln2[{l}]", R.dense_bwd_x(dr16, v.w16(pre + "ffn1.kernel")), f"t.h{2 * l + 1}", pre + "ln2.",
                        dh, f"t.dh16b{l}", pre + "attn.out.bias")
             # attention
             dh16b = v.b16(f"t.dh16b{l}", M, 128)
-            rep.grad(v, pre + "attn.out.kernel", dw(v.b16(f"t.o{l}", M, 128), dh16b), B_DW, f"dWo[{l}]")
+            rep.grad(v, pre + "attn.out.kernel", R.dense_bwd_w(v.b16(f"t.o{l}", M, 128), dh16b), B_DW, f"dWo[{l}]")
             probs = v.f32(f"t.probs{l}", batch, H, S, S)
             if mdn:
                 rep.zero(f"probs[{l}] above the diagonal", probs * torch.ones_like(probs[0, 0]).triu(1))
@@ -327,36 +295,63 @@ def check_stages(eng, batch, rep, eps=None, objective="ddpm", global_batch=None)
                 rep.bf16(f"attention bwd[{l}] -> t.dqkv16_{l}", dqkv16, dqkv)
             rep.grad(v, pre + "attn.qkv.bias", R.dense_bwd_b(dqkv), B_TF32_SUM if tf32 else B_SEED,
                      f"attention bwd[{l}] dbias")
-            rep.grad(v, pre + "attn.qkv.kernel", dw(v.b16(f"t.a1_{l}", M, 128), dqkv16), B_DW, f"dWqkv[{l}]")
+            rep.grad(v, pre + "attn.qkv.kernel", R.dense_bwd_w(v.b16(f"t.a1_{l}", M, 128), dqkv16), B_DW, f"dWqkv[{l}]")
             dh = ln128(f"ln1[{l}]", R.dense_bwd_x(dqkv16, v.w16(pre + "attn.qkv.kernel")), f"t.h{2 * l}", pre + "ln1.",
                        dh, f"t.dh16a{l - 1}" if l > 0 else None, f"l{l - 1}.ffn2.bias" if l > 0 else "in.bias")
         dh_dev = v.f32("t.dh", M, 128)
         rep.rel("trunk residual adjoint -> t.dh", dh_dev, dh, B_LN128)
         # ---------------------------------------------------------- embedding
-        rep.grad(v, "in.kernel", dw(v.f32("xt", M, Cc), dh_dev), B_SEED * 2, "embedding bwd")
+        rep.grad(v, "in.kernel", R.dense_bwd_w(v.f32("xt", M, Cc), dh_dev), B_SEED * 2, "embedding bwd")
 
     # ------------------------------------------------------------------ reduction-tail rows of the MN-major operands
-    if Mk != M:
-        fam = [(f"t.du16_{k}", Md) for k in range(K + 1)] + [(f"t.dr16t_{k}", Md) for k in range(K)]
-        fam += [("t.dpred16", Hp)]
-        for l in range(Lt):
-            fam += [(f"t.dh16a{l}", 128), (f"t.dh16b{l}", 128), (f"t.dr16_{l}", Md), (f"t.dqkv16_{l}", 384)]
-        if ssm:
-            fam += [(f"t.dut16_{k}", Md) for k in range(K + 1)] + [(f"t.drt16_{k}", Md) for k in range(K)]
-            fam += [("t.dpredt16", Hp)]
-        bad = [n for n, cols in fam if bool((v.raw(n, (Mk, cols), torch.bfloat16)[M:] != 0).any())]
-        print(f"[parity] {rep.case} rows [{M}, {Mk}) of {len(fam)} gradient operands: nonzero in {bad}")
-        rep.rules += 1
-        if bad:
-            rep.failed.append(("reduction-tail rows not zero", bad, []))
+    fam = [(f"t.du16_{k}", Md) for k in range(K + 1)] + [(f"t.dr16t_{k}", Md) for k in range(K)]
+    fam += [("t.dpred16", Hp)]
+    for l in range(Lt):
+        fam += [(f"t.dh16a{l}", 128), (f"t.dh16b{l}", 128), (f"t.dr16_{l}", Md), (f"t.dqkv16_{l}", 384)]
+    reduction_tail_rules(v, rep, M, fam)
     return rep
 
 
-def assert_complete(eng, rep, but=()):
+def film_generator_rules(v, rep, k, batch, dss):
+    """The FiLM generator backward of block k (ten launches on the side stream) from the device's pair adjoint dss."""
+    Md = v.eng.cfg.mlp_dims
+    Bk = _ceil(batch, 64)
+    fp = f"k{k}.film."
+    dss16, e2_16 = R.bf16_round(dss), R.bf16_round(v.f32(f"t.e2_{k}", batch, 512))
+    f = R.film_generator_bwd(dss16, v.f32("enc", batch, 128), v.f32(f"t.e1pre{k}", batch, 512),
+                             v.f32(f"t.e1_{k}", batch, 512), e2_16, v.w16(fp + "ss.kernel"),
+                             v.param(fp + "d2.kernel"))
+    rep.grad(v, fp + "ss.bias", R.dense_bwd_b(dss), B_SEED, f"colsum film.ss.bias[{k}]")
+    rep.grad(v, fp + "ss.kernel", f["ss.kernel"], B_DW, f"dWss[{k}]")
+    for name in ("d2.bias", "d2.kernel", "d1.bias", "d1.kernel"):
+        rep.grad(v, fp + name, f[name], B_DW, f"film generator {name}[{k}]")
+    if k == 0:   # the generator's scratch buffers hold the block that ran last
+        rep.rel("film generator dss16 = bf16(dss)", v.b16("t.dss16", batch, 2 * Md), dss16, B_EXACT)
+        rep.rel("film generator e2_16 = bf16(e2)", v.b16("t.e2_16", batch, 512), e2_16, B_EXACT)
+        rep.rel("film generator dXss -> t.de2", v.f32("t.de2", batch, 512), f["de2"], B_DW)
+        rep.rel("film generator dX d2 -> t.de", v.f32("t.de", batch, 512), f["de1"], B_DW)
+        if Bk != batch:
+            rep.zero("tail rows of t.dss16", v.raw("t.dss16", (Bk, 2 * Md), torch.bfloat16)[batch:])
+            rep.zero("tail rows of t.e2_16", v.raw("t.e2_16", (Bk, 512), torch.bfloat16)[batch:])
+
+
+def reduction_tail_rules(v, rep, M, fam):
+    """Rows [M, Mk) of the MN-major gradient operands fam = [(name, columns)] are zero (bwd_begin)."""
+    Mk = _ceil(M, 64)
+    if Mk == M:
+        return
+    bad = [n for n, cols in fam if bool((v.raw(n, (Mk, cols), torch.bfloat16)[M:] != 0).any())]
+    print(f"[parity] {rep.case} rows [{M}, {Mk}) of {len(fam)} gradient operands: nonzero in {bad}")
+    rep.rules += 1
+    if bad:
+        rep.failed.append(("reduction-tail rows not zero", bad, []))
+
+
+def assert_complete(eng, rep):
     """Every tensor of the parameter arena got its gradient checked by some rule."""
     names = [name for name, _, _ in eng.layout]
     assert len(names) == eng.lib.smd_num_tensors(eng._plan)
-    missing = [n for n in names if n not in rep.covered and not n.endswith(tuple(but))]
+    missing = [n for n in names if n not in rep.covered]
     print(f"[parity] {rep.case} parameter tensors: {len(names)}, not covered by a rule: {missing}")
     assert not missing, missing
 
@@ -534,15 +529,15 @@ def test_denoising_score_matching_seed_and_output_projection(lib):
 
 
 def test_sliced_score_matching_weight_gradients_sum_primal_and_tangent_products(lib):
-    """SSM accumulates the tangent product onto the primal product in place (the GEMM's residual is its own output)."""
+    """SSM accumulates the tangent product onto the primal product in place (the GEMM's residual is its own output).
+    DenseNCSN C 64, two blocks, nine examples: every rule of test_gpu_ssm_backward_stages.py (which holds the other
+    SSM shapes), the second-order LayerNorm backward included, and no parameter tensor left out."""
+    from tests import test_gpu_forward_stages as FW
+    from tests import test_gpu_ssm_backward_stages as SSM
     batch = 9
     eng, inputs = _ncsn(batch)
-    eng.compute_ssm_grads(*inputs)
-    rep = check_stages(eng, batch, Report("ssm"), objective="ssm")
-    # the LayerNorm parameters and the biases fed by the second-order LayerNorm backward are outside the GEMM-type rules
-    assert_complete(eng, rep, but=("ln_a.scale", "ln_a.bias", "ln_b.scale", "ln_b.bias", "out_ln.scale", "out_ln.bias",
-                                   "res.a.bias", "res.b.bias", "in.bias"))
-    rep.finish()
+    _, n = FW._counted(eng, lambda: eng.compute_ssm_grads(*inputs))
+    SSM.check_ssm_call(eng, FW.Report("ssm"), inputs, batch, batch, n)
 
 
 def test_transformer_mdn_trunk_and_head(lib):
