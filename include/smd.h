@@ -226,8 +226,8 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
  *   sig = eta sqrt((1-a')/(1-a)) sqrt(1 - a/a'),  x <- sqrt(a') x0 + sqrt(max(1-a'-sig^2, 0)) eps' + sig z.
  * The step keys follow diffusion_dynamics' scan carry over K steps (smd_sampler_setup with T = K), as do the collection
  * rows.  tau = 0..T-1 with eta = 1 is diffusion_dynamics itself; eta = 0 is deterministic given x.  The tables share
- * the sampler's workspace regions: smd_sampler_setup, smd_langevin_setup and smd_ddim_setup each invalidate the other
- * two (SMD_ERR_STATE).  SMD_ERR_INVALID for a TransformerMDN plan, T < 1 or T > 8192, K < 1 or K > T, indices not
+ * the sampler's workspace regions: smd_sampler_setup, smd_langevin_setup, smd_ddim_setup and smd_ddim_encode_setup
+ * each invalidate the other three (SMD_ERR_STATE).  SMD_ERR_INVALID for a TransformerMDN plan, T < 1 or T > 8192, K < 1 or K > T, indices not
  * strictly increasing or out of range, eta < 0 or not finite, or alpha_bar outside (0, 1) at a selected index. */
 int smd_ddim_setup(smd_plan* plan, const float* host_betas, int T, const int* host_steps, int K, float eta,
                    const uint32_t host_key[2], smd_stream_t stream);
@@ -244,6 +244,26 @@ int smd_ddim_sample(smd_plan* plan, const float* params, float* x, int n, const 
  * rejections as smd_ddim_setup. */
 int smd_ddim_tables(const float* host_betas, int T, const int* host_steps, int K, float eta,
                     const uint32_t host_key[2], float* host_coef, uint32_t* host_keys, int* host_slots);
+
+/* ---- DDIM encoder (Song et al. 2021, sections 4.3 and 5.4): the eta = 0 DDIM chain from data towards noise -------- */
+/* host_betas / host_steps as smd_ddim_setup.  The levels are a_{-1} = 1 (the data) and a_i = alpha_bar(tau_i); step
+ * i = 0 .. K-1 goes from a = a_{i-1} to a' = a_i:
+ *   eps = model(x, sqrt(a)),  x0 = sqrt(1/a) x - sqrt(1-a) sqrt(1/a) eps  (not clipped),  x <- sqrt(a') x0 + sqrt(1-a') eps.
+ * At i = 0, x0 = x exactly.  This mirrors smd_ddim_sample at eta = 0 over the same levels: smd_ddim_sample on the code
+ * returns the data up to discretisation error.  The table shares the sampler's workspace regions: smd_sampler_setup,
+ * smd_langevin_setup, smd_ddim_setup and smd_ddim_encode_setup each invalidate the other three (SMD_ERR_STATE).
+ * SMD_ERR_INVALID for a TransformerMDN plan and for the arguments smd_ddim_setup rejects (there is no eta). */
+int smd_ddim_encode_setup(smd_plan* plan, const float* host_betas, int T, const int* host_steps, int K,
+                          smd_stream_t stream);
+/* The whole K-step encoder on x (n, S, C) or (n, D) in place: x holds the code x_T afterwards.  One FiLM table row per
+ * level; use_graph != 0 replays one captured step K times.  Deterministic: no noise, so smd_sampler_set_shard does not
+ * apply.  SMD_ERR_STATE without smd_ddim_encode_setup; SMD_ERR_INVALID for n outside [1, max_batch] or a TransformerMDN
+ * plan. */
+int smd_ddim_encode(smd_plan* plan, const float* params, float* x, int n, int use_graph, smd_stream_t stream);
+/* Host only: the table smd_ddim_encode_setup uploads, host_coef (K x 8) with row i = step i: sqrt(1/a),
+ * sqrt(1-a) sqrt(1/a), sqrt(a'), sqrt(1-a'), sqrt(a) (the conditioning value), 0, 0, 0.  Computed in float64 from the
+ * float32 alpha_bar and rounded once.  host_coef may be NULL.  Same rejections as smd_ddim_encode_setup. */
+int smd_ddim_encode_tables(const float* host_betas, int T, const int* host_steps, int K, float* host_coef);
 
 /* ---- Langevin chains (annealed / consistent Langevin dynamics of the NCSN family) ------------------------------ */
 /* kind 0 = annealed (utils/ebm_utils.py:89-198), 1 = consistent (:201-271).  host_sigmas: HOST, L floats (L >= 2).

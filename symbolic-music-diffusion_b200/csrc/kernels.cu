@@ -964,16 +964,49 @@ void launch_ddim_step(const DdimStepArgs& a, cudaStream_t st) {
   ddim_step_kernel<<<(4 * NC + 255) / 256, 256, 0, st>>>(a);
 }
 
+// ---------------------------------------------------------------------------------------------------
+// DDIM encoder step (Song et al. 2021, sections 4.3 and 5.4): the eta = 0 update from data towards noise, with the x0
+// estimate unclipped so that the decoder can invert it.  The ddim_step_kernel layout: four lanes per (sample, channel)
+// column, a quarter of its S positions each
+// ---------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+ddim_encode_step_kernel(const DdimEncodeStepArgs a) {
+  pdl_trigger();
+  pdl_wait();
+  const float* cf = a.coef + 8 * (*a.r_ptr);
+  const float sqrt_recip = cf[0], sqrt_m1 = cf[1], c_x0 = cf[2], c_eps = cf[3];
+  const int NC = a.N * a.C;
+  constexpr int kSG = 4;
+  const int gi = blockIdx.x * blockDim.x + threadIdx.x;
+  const int i = gi / kSG, sg = gi % kSG;
+  if (i >= NC) return;
+  const int n = i / a.C, c = i % a.C;
+  const int per = (a.S + kSG - 1) / kSG;
+  const int s_end = min(a.S, (sg + 1) * per);
+  for (int s = sg * per; s < s_end; ++s) {
+    const size_t idx = (static_cast<size_t>(n) * a.S + s) * a.C + c;
+    const float x = a.x[idx];
+    const float eh = a.eps_hat[idx];
+    // at the first step (a = 1) the coefficients are 1 and 0, so x0 = x exactly
+    const float x0 = __fsub_rn(__fmul_rn(sqrt_recip, x), __fmul_rn(sqrt_m1, eh));
+    a.x_next[idx] = __fadd_rn(__fmul_rn(c_x0, x0), __fmul_rn(c_eps, eh));
+  }
+}
+void launch_ddim_encode_step(const DdimEncodeStepArgs& a, cudaStream_t st) {
+  const int NC = a.N * a.C;
+  ddim_encode_step_kernel<<<(4 * NC + 255) / 256, 256, 0, st>>>(a);
+}
+
 __global__ void step_advance_kernel(int* t_ptr) { *t_ptr -= 1; }
 void launch_step_advance(int* t_ptr, cudaStream_t st) { step_advance_kernel<<<1, 1, 0, st>>>(t_ptr); }
-__global__ void fill_cond_kernel(const float* coef, const int* t_ptr, float* cond, int n) {
+__global__ void fill_cond_kernel(const float* coef, int offset, const int* t_ptr, float* cond, int n) {
   pdl_trigger();
   pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) cond[i] = coef[8 * (*t_ptr) + 5];
+  if (i < n) cond[i] = coef[8 * (*t_ptr) + offset];
 }
-void launch_fill_cond(const float* coef, const int* t_ptr, float* cond, int n, cudaStream_t st) {
-  fill_cond_kernel<<<(n + 255) / 256, 256, 0, st>>>(coef, t_ptr, cond, n);
+void launch_fill_cond(const float* coef, int offset, const int* t_ptr, float* cond, int n, cudaStream_t st) {
+  fill_cond_kernel<<<(n + 255) / 256, 256, 0, st>>>(coef, offset, t_ptr, cond, n);
 }
 
 // ---------------------------------------------------------------------------------------------------

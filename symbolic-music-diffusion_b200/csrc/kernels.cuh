@@ -242,9 +242,24 @@ struct DdimStepArgs {
 // x <- sqrt(a') x0 + sqrt(max(1-a'-sig^2, 0)) eps' + sig z, then the infill blend at t = tau_i, the metrics and the
 // collection row
 void launch_ddim_step(const DdimStepArgs& a, cudaStream_t st);
-// *t_ptr -= 1 ; cond[0..n) = coef[t].sqrt_ap   (device-side step bookkeeping for graph replay)
+// DDIM encoder step (smd_ddim_encode_setup), the eta = 0 DDIM step run from data towards noise: step i goes from
+// a = a_{i-1} (1 at i = 0) to a' = a_i = alpha_bar(tau_i).  The table is stored last step first: row r = K-1-i, so the
+// counter that step_advance decrements from K-1 visits i = 0 .. K-1.
+struct DdimEncodeStepArgs {
+  const float* x;          // state (N, S, C)
+  const float* eps_hat;    // model output eps = model(x, sqrt(a))
+  const float* coef;       // device table [K][8], row K-1-i: sqrt(1/a), sqrt(1-a) sqrt(1/a), sqrt(a'), sqrt(1-a'),
+                           //                                 sqrt(a), 0, 0, 0
+  const int* r_ptr;        // device scalar: current row K-1-i (graph-replayable)
+  float* x_next;
+  int N, S, C;
+};
+// x0 = sqrt(1/a) x - sqrt(1-a) sqrt(1/a) eps (not clipped);  x <- sqrt(a') x0 + sqrt(1-a') eps
+void launch_ddim_encode_step(const DdimEncodeStepArgs& a, cudaStream_t st);
+// *t_ptr -= 1 ; cond[0..n) = coef[8 t + offset], the conditioning column of the chain's table (device-side step
+// bookkeeping for graph replay)
 void launch_step_advance(int* t_ptr, cudaStream_t st);
-void launch_fill_cond(const float* coef, const int* t_ptr, float* cond, int n, cudaStream_t st);
+void launch_fill_cond(const float* coef, int offset, const int* t_ptr, float* cond, int n, cudaStream_t st);
 
 // loss[b] = mean_{s,c} (eps - pred)^2 ; dpred = -2 (eps - pred) * gscale                (utils/losses.py:304-308)
 void launch_ddpm_loss(const float* eps, const float* pred, float* loss_per_example, float* dpred_or_null,

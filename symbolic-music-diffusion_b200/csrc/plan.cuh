@@ -136,8 +136,9 @@ struct TrainState {
 enum Objective : int { kObjDdpm = 0, kObjDsm = 1, kObjSsm = 2, kObjMdn = 3 };
 
 // The sampler chain whose tables (coef / keys / slots / t_ptr, the FiLM table) the workspace holds: the DDPM sampler,
-// the Langevin chain and the DDIM chain share those regions, so at most one of them is set up at a time.
-enum Chain : int { kChainNone = 0, kChainDdpm = 1, kChainLangevin = 2, kChainDdim = 3 };
+// the Langevin chain, the DDIM chain and the DDIM encoder share those regions, so at most one of them is set up at a
+// time.
+enum Chain : int { kChainNone = 0, kChainDdpm = 1, kChainLangevin = 2, kChainDdim = 3, kChainDdimEncode = 4 };
 
 // The legacy default stream cannot be captured into a CUDA graph.
 inline bool capturable(cudaStream_t st) { return st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread; }

@@ -1211,7 +1211,7 @@ static int reverse_step_impl(smd_plan* plan, const float* params, const float* x
   if (!film.table) {
     // conditioning value sqrt(alpha_prod_t), shared by every sample (utils/ebm_utils.py:367-369)
     if (t >= 0) SMD_CUDA(cudaMemcpyAsync(tvec, coef + 8 * t + 5, 4, cudaMemcpyDeviceToDevice, st));
-    else { launch_fill_cond(coef, t_ptr, tvec, 1, st); CNT(); }
+    else { launch_fill_cond(coef, 5, t_ptr, tvec, 1, st); CNT(); }
   }
   float* eh = eps_hat ? eps_hat : plan->at<float>(plan->reg.eps_hat);
   const int rc = run_forward(plan, params, x, tvec, 1, n, eh, st, false, false, false, film);
@@ -1300,11 +1300,9 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
 
 // ---- DDIM chain (Song et al. 2021) over a strided subset of the DDPM schedule -----------------------------------------
 
-// Host tables of smd_ddim_setup for the K selected indices tau_i (alpha_bar in float32 as smd_sampler_setup, the
-// coefficients in float64 from it, rounded to float32):
-//   coef[i] = (sqrt(1/a), sqrt(1-a) sqrt(1/a), sqrt(a'), sqrt(max(1-a'-sig^2, 0)), sig, sqrt(a), sqrt(1-a), a)
-// with a = alpha_bar(tau_i), a' = alpha_bar(tau_{i-1}) (1 at i = 0), sig = eta sqrt((1-a')/(1-a)) sqrt(1 - a/a').
-static int ddim_tables(const float* betas, int T, const int* steps, int K, float eta, float* coef) {
+// The float32 alpha_bar (smd_sampler_setup's cumulative product) at the K selected indices tau_i, after the argument
+// checks the DDIM chain and the DDIM encoder share (the encoder passes eta = 0).
+static int ddim_levels(const float* betas, int T, const int* steps, int K, float eta, std::vector<float>& levels) {
   if (!betas || !steps) { set_error("null betas or steps"); return SMD_ERR_INVALID; }
   if (T < 1 || T > kMaxT) { set_error("T out of range"); return SMD_ERR_INVALID; }
   if (K < 1 || K > T) { set_error("the number of DDIM steps must be in [1, T]"); return SMD_ERR_INVALID; }
@@ -1317,14 +1315,29 @@ static int ddim_tables(const float* betas, int T, const int* steps, int K, float
   std::vector<float> ap(T);
   float run = 1.0f;
   for (int t = 0; t < T; ++t) { const float al = 1.0f - betas[t]; run = (t == 0) ? al : run * al; ap[t] = run; }
+  levels.resize(K);
   for (int i = 0; i < K; ++i) {
     if (!(ap[steps[i]] > 0.f && ap[steps[i]] < 1.f)) {
       set_error("alpha_bar must lie in (0, 1) at every selected step");
       return SMD_ERR_INVALID;
     }
+    levels[i] = ap[steps[i]];
+  }
+  return SMD_OK;
+}
+
+// Host tables of smd_ddim_setup for the K selected indices tau_i (alpha_bar in float32 as smd_sampler_setup, the
+// coefficients in float64 from it, rounded to float32):
+//   coef[i] = (sqrt(1/a), sqrt(1-a) sqrt(1/a), sqrt(a'), sqrt(max(1-a'-sig^2, 0)), sig, sqrt(a), sqrt(1-a), a)
+// with a = alpha_bar(tau_i), a' = alpha_bar(tau_{i-1}) (1 at i = 0), sig = eta sqrt((1-a')/(1-a)) sqrt(1 - a/a').
+static int ddim_tables(const float* betas, int T, const int* steps, int K, float eta, float* coef) {
+  std::vector<float> ap;
+  const int rc = ddim_levels(betas, T, steps, K, eta, ap);
+  if (rc) return rc;
+  for (int i = 0; i < K; ++i) {
     // float64 from the float32 alpha_bar, rounded once: near t = 0, 1 - a' - sig^2 cancels (at eta = 1 it is
     // alpha_t (1-a')^2 / (1-a), far below 1 - a'), which float32 arithmetic would leave good to a few 1e-5 only
-    const double a = ap[steps[i]], ap_prev = i > 0 ? ap[steps[i - 1]] : 1.0;
+    const double a = ap[i], ap_prev = i > 0 ? ap[i - 1] : 1.0;
     const double sig = static_cast<double>(eta) * sqrt((1.0 - ap_prev) / (1.0 - a)) * sqrt(std::max(1.0 - a / ap_prev, 0.0));
     const double c64[8] = {sqrt(1.0 / a), sqrt(1.0 - a) * sqrt(1.0 / a), sqrt(ap_prev),
                            sqrt(std::max(1.0 - ap_prev - sig * sig, 0.0)), sig, sqrt(a), sqrt(1.0 - a), a};
@@ -1379,7 +1392,7 @@ static int ddim_step(smd_plan* plan, const float* params, float* x, int n, const
   int* t_ptr = plan->at<int>(plan->reg.t_ptr);
   const float* coef = plan->at<float>(plan->reg.coef);
   const FilmRows film = film_table_rows(plan, params, -1, t_ptr);
-  if (!film.table) { launch_fill_cond(coef, t_ptr, tvec, 1, st); CNT(); }
+  if (!film.table) { launch_fill_cond(coef, 5, t_ptr, tvec, 1, st); CNT(); }
   float* eh = plan->at<float>(plan->reg.eps_hat);
   const int rc = run_forward(plan, params, x, tvec, 1, n, eh, st, false, false, false, film);
   if (rc) return rc;
@@ -1429,6 +1442,114 @@ int smd_ddim_sample(smd_plan* plan, const float* params, float* x, int n, const 
     const int rc = plan->chain_graph.capture(cs, key, [&] {
       return ddim_step(plan, params, x, n, infill_x, infill_mask, collection, metrics, cs);
     }, "ddim graph");
+    if (rc) return rc;
+  }
+  for (int i = 0; i < K; ++i) {
+    const int rc = plan->chain_graph.launch(cs);
+    if (rc) return rc;
+  }
+  return join_replay(plan, st, cs);
+}
+
+// ---- DDIM encoder (Song et al. 2021, sections 4.3 and 5.4): the eta = 0 chain run from data towards noise -------------
+
+// Host table of smd_ddim_encode_setup, one row per step i = 0 .. K-1 (alpha_bar in float32 as smd_ddim_setup, the
+// coefficients in float64 from it, rounded to float32):
+//   coef[i] = (sqrt(1/a), sqrt(1-a) sqrt(1/a), sqrt(a'), sqrt(1-a'), sqrt(a), 0, 0, 0)
+// with a = alpha_bar(tau_{i-1}) (1 at i = 0: the data) and a' = alpha_bar(tau_i).
+static int ddim_encode_tables(const float* betas, int T, const int* steps, int K, float* coef) {
+  std::vector<float> ap;
+  const int rc = ddim_levels(betas, T, steps, K, 0.f, ap);
+  if (rc) return rc;
+  for (int i = 0; i < K; ++i) {
+    const double a = i > 0 ? ap[i - 1] : 1.0, a_next = ap[i];
+    const double c64[8] = {sqrt(1.0 / a), sqrt(1.0 - a) * sqrt(1.0 / a), sqrt(a_next), sqrt(1.0 - a_next), sqrt(a),
+                           0.0, 0.0, 0.0};
+    for (int j = 0; j < 8; ++j) coef[static_cast<size_t>(i) * 8 + j] = static_cast<float>(c64[j]);
+  }
+  return SMD_OK;
+}
+
+int smd_ddim_encode_tables(const float* host_betas, int T, const int* host_steps, int K, float* host_coef) {
+  std::vector<float> coef(static_cast<size_t>(std::max(K, 0)) * 8);
+  const int rc = ddim_encode_tables(host_betas, T, host_steps, K, coef.data());
+  if (rc) return rc;
+  if (host_coef) memcpy(host_coef, coef.data(), coef.size() * sizeof(float));
+  return SMD_OK;
+}
+
+int smd_ddim_encode_setup(smd_plan* plan, const float* host_betas, int T, const int* host_steps, int K,
+                          smd_stream_t stream) {
+  if (!plan) { set_error("null plan"); return SMD_ERR_INVALID; }
+  if (reject_mdn(plan, "smd_ddim_encode_setup")) return SMD_ERR_INVALID;
+  std::vector<float> coef(static_cast<size_t>(std::max(K, 0)) * 8);
+  const int rc = ddim_encode_tables(host_betas, T, host_steps, K, coef.data());
+  if (rc) return rc;
+  if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
+  // the step counter counts down (launch_step_advance) from K-1, so the device table holds step i in row K-1-i; the
+  // FiLM table follows the same rows.  K <= T <= kMaxT rows fit the sampler's coef region.
+  std::vector<float> rows(coef.size());
+  for (int i = 0; i < K; ++i)
+    memcpy(&rows[static_cast<size_t>(K - 1 - i) * 8], &coef[static_cast<size_t>(i) * 8], 8 * sizeof(float));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  SMD_CUDA(cudaMemcpyAsync(plan->at<float>(plan->reg.coef), rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, st));
+  SMD_CUDA(cudaStreamSynchronize(st));  // the host table goes out of scope
+  plan->T = K;
+  plan->chain = kChainDdimEncode;
+  plan->film_tab_ready = false;
+  plan->chain_graph.drop();
+  return SMD_OK;
+}
+
+// One encoder step at the device row r = *t_ptr = K-1-i: network call on sqrt(a) (FiLM table row r, or the generator on
+// coef[r].sqrt(a)), the update, then r -= 1.  The eager loop and the captured graph run this same sequence.
+static int ddim_encode_step(smd_plan* plan, const float* params, float* x, int n, cudaStream_t st) {
+  float* tvec = plan->at<float>(plan->reg.tvec);
+  int* t_ptr = plan->at<int>(plan->reg.t_ptr);
+  const float* coef = plan->at<float>(plan->reg.coef);
+  const FilmRows film = film_table_rows(plan, params, -1, t_ptr);
+  if (!film.table) { launch_fill_cond(coef, 4, t_ptr, tvec, 1, st); CNT(); }
+  float* eh = plan->at<float>(plan->reg.eps_hat);
+  const int rc = run_forward(plan, params, x, tvec, 1, n, eh, st, false, false, false, film);
+  if (rc) return rc;
+  DdimEncodeStepArgs a;
+  memset(&a, 0, sizeof(a));
+  a.x = x; a.eps_hat = eh; a.coef = coef; a.r_ptr = t_ptr; a.x_next = x;
+  a.N = n;
+  // the state axes of chain_geometry: (N, D) states of the dense networks use S = D, C = 1
+  a.S = plan->cfg.seq_len; a.C = plan->cfg.channels;
+  if (plan->cfg.arch != SMD_ARCH_TRANSFORMER_DDPM) { a.S = plan->cfg.channels; a.C = 1; }
+  launch_ddim_encode_step(a, st); CNT();
+  launch_step_advance(t_ptr, st); CNT();
+  SMD_LAUNCH_CHECK("ddim_encode_step");
+  return SMD_OK;
+}
+
+int smd_ddim_encode(smd_plan* plan, const float* params, float* x, int n, int use_graph, smd_stream_t stream) {
+  if (!plan) { set_error("null plan"); return SMD_ERR_INVALID; }
+  if (reject_mdn(plan, "smd_ddim_encode")) return SMD_ERR_INVALID;
+  if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
+  if (plan->chain != kChainDdimEncode) { set_error("smd_ddim_encode_setup has not been called"); return SMD_ERR_STATE; }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int K = plan->T;
+  cudaStream_t cs = st;
+  if (use_graph) { const int rc0 = replay_stream(plan, st, &cs); if (rc0) return rc0; }
+  { const int rc0 = ensure_film_table(plan, params, 8, 4, cs); if (rc0) return rc0; }
+  int* t_ptr = plan->at<int>(plan->reg.t_ptr);
+  const int r0 = K - 1;
+  SMD_CUDA(cudaMemcpyAsync(t_ptr, &r0, sizeof(int), cudaMemcpyHostToDevice, cs));
+  SMD_CUDA(cudaStreamSynchronize(cs));  // r0 is a stack variable
+  if (!use_graph) {
+    for (int i = 0; i < K; ++i) {
+      const int rc = ddim_encode_step(plan, params, x, n, cs);
+      if (rc) return rc;
+    }
+    return SMD_OK;
+  }
+  const GraphKey key = graph_key(n, params, x);
+  if (!plan->chain_graph.replays(key)) {
+    const int rc = plan->chain_graph.capture(cs, key, [&] { return ddim_encode_step(plan, params, x, n, cs); },
+                                             "ddim encode graph");
     if (rc) return rc;
   }
   for (int i = 0; i < K; ++i) {

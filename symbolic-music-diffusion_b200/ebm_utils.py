@@ -116,6 +116,46 @@ def ddim_dynamics(rng, model, betas, init, epsilon, T, denoise, infill=False, in
     return x, collection, metrics.unsqueeze(2)
 
 
+def ddim_encode(model, betas, x0, steps=50, schedule="uniform"):
+    """The deterministic DDIM encoder (Song et al. 2021, sections 4.3 and 5.4): the eta = 0 DDIM chain run from the
+    data x0 towards noise over the `steps` levels of `betas` that `schedule` picks (ddim_schedule), with the x0
+    estimate unclipped.  Returns the codes x_T (float32, on the device); ddim_dynamics at eta = 0 over the same levels
+    decodes them back to x0 up to discretisation error.  Not in the reference."""
+    from .nn import _as_device_f32
+    x = _as_device_f32(x0).clone()
+    eng = model.engine(x.shape[0])
+    betas = np.asarray(betas, np.float32)
+    eng.ddim_encode_setup(betas, ddim_schedule(len(betas), steps, schedule))
+    eng.ddim_encode(x, use_graph=True)
+    return x
+
+
+def slerp(z0, z1, alpha):
+    """Spherical interpolation between the rows of z0 and z1 (each example flattened), in float64: sin((1-alpha)
+    theta) / sin(theta) z0 + sin(alpha theta) / sin(theta) z1 with theta the angle between the two rows.  Exactly z0
+    at alpha = 0 and z1 at alpha = 1; linear interpolation for rows whose angle is below 1e-6.  A linear mix of two
+    near-Gaussian codes shrinks towards the origin (to about 0.7 of their norm at the midpoint), off the shell the
+    decoder expects (Song et al. 2021, appendix D.5).  Returns a float64 tensor shaped like z0, on z0's device."""
+    a = torch.as_tensor(z0).to(torch.float64)
+    b = torch.as_tensor(z1).to(device=a.device, dtype=torch.float64)
+    if a.shape != b.shape:
+        raise ValueError(f"slerp needs equally shaped endpoints, got {tuple(a.shape)} and {tuple(b.shape)}")
+    alpha = float(alpha)
+    if alpha == 0.0:
+        return a.clone()
+    if alpha == 1.0:
+        return b.clone()
+    fa, fb = a.reshape(a.shape[0], -1), b.reshape(b.shape[0], -1)
+    norms = fa.norm(dim=1) * fb.norm(dim=1)
+    cos = torch.where(norms > 0, (fa * fb).sum(dim=1) / torch.where(norms > 0, norms, 1.0), 1.0)
+    theta = torch.arccos(cos.clamp(-1.0, 1.0))
+    linear = theta < 1e-6
+    sin = torch.where(linear, 1.0, torch.sin(theta))
+    w0 = torch.where(linear, 1.0 - alpha, torch.sin((1.0 - alpha) * theta) / sin)
+    w1 = torch.where(linear, alpha, torch.sin(alpha * theta) / sin)
+    return (w0[:, None] * fa + w1[:, None] * fb).reshape(a.shape)
+
+
 def _reduce_sharded_metrics(metrics, n, shard):
     """The sampler metrics are means over the batch (utils/ebm_utils.py:166-170, 380-384): with shard = (first_row,
     total_rows) over several ranks, one weighted all-reduce at the end; row 2 (alpha / alpha_prod) is no batch mean."""

@@ -520,6 +520,23 @@ class Engine:
                                             1 if use_graph else 0, self._stream()))
         return x
 
+    def ddim_encode_setup(self, betas: np.ndarray, steps) -> None:
+        """The deterministic DDIM encoder over the strictly increasing indices `steps` of the schedule `betas`
+        (include/smd.h smd_ddim_encode_setup); replaces a sampler_setup, langevin_setup or ddim_setup schedule (and
+        vice versa)."""
+        self._ensure_ws()
+        b = np.ascontiguousarray(betas, np.float32)
+        s = np.ascontiguousarray(steps, np.int32)
+        _lib.check(self.lib.smd_ddim_encode_setup(self._plan, b.ctypes.data_as(C.POINTER(C.c_float)), len(b),
+                                                  s.ctypes.data_as(C.POINTER(C.c_int)), len(s), self._stream()))
+
+    def ddim_encode(self, x, use_graph: bool = True):
+        """Runs the whole encoder of ddim_encode_setup in place on x: data in, codes x_T out."""
+        x = _f32c(x, "x")
+        _lib.check(self.lib.smd_ddim_encode(self._plan, self.params.data_ptr(), x.data_ptr(), x.shape[0],
+                                            1 if use_graph else 0, self._stream()))
+        return x
+
     LANGEVIN_KINDS = {"ald": 0, "cas": 1}
 
     def langevin_setup(self, sigmas: np.ndarray, steps_per_level: int, epsilon: float, kind: str = "ald",

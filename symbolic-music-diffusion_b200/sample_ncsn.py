@@ -4,8 +4,10 @@
 
 Restores the newest checkpoint of --model_dir into a freshly created model (sample_ncsn.py:331-342; like upstream
 it samples from optimizer.target, never from the EMA parameters), runs the full reverse chain on the GPU and
-writes ncsn/{real,generated,collection}.pkl under --sampling_dir (sample_ncsn.py:453-471).  With torchrun the
-sample_size is sharded across ranks (replicated parameters, no per-step exchange) and gathered at the end.
+writes ncsn/{real,generated,collection}.pkl under --sampling_dir (sample_ncsn.py:453-471).  --interpolate with
+--interpolate_encoder=ddim encodes with the deterministic DDIM encoder instead and also writes
+ncsn/reconstruction.json.  With torchrun the sample_size is sharded across ranks (replicated parameters, no per-step
+exchange) and gathered at the end.
 --compute_metrics then scores the samples against the real examples on the GPU (ncsn/metrics.json); with
 --full_metrics also by the coverage metrics (PRD, improved precision / recall, realism, NDB).
 """
@@ -39,6 +41,11 @@ flags.DEFINE_bool("flush", True, "Write pickles.")
 flags.DEFINE_bool("animate", False, "Write sampling animations (not supported: raises ValueError).")
 flags.DEFINE_bool("infill", False, "Infill the middle 16 latents of real examples (sample_ncsn.py:408-427).")
 flags.DEFINE_bool("interpolate", False, "Interpolate between real examples in the diffusion latent space.")
+flags.DEFINE_enum("interpolate_encoder", "stochastic", ["stochastic", "ddim"],
+                  "--interpolate: stochastic is the reference's q(x_T | x_0) encoder with linear interpolation and the "
+                  "ddpm decoder; ddim (needs --sampling=ddim and --ddim_eta=0) encodes with the deterministic DDIM "
+                  "encoder over --ddim_steps / --ddim_schedule, interpolates spherically and decodes with the eta = 0 "
+                  "DDIM chain, and writes ncsn/reconstruction.json.  ddim is not a reference option.")
 
 
 def _restore(model_dir, shape, batch_size=1):
@@ -132,6 +139,48 @@ def diffusion_decoder(z_list, rng_seed=1):
     return gen, collects, metrics
 
 
+def ddim_interpolate(starts, rng_seed=1):
+    """--interpolate_encoder=ddim (not in the reference): the deterministic DDIM encoder (Song et al. 2021, sections 4.3
+    and 5.4) maps each start to its code; the goals' codes are the starts' codes rolled by one row, as the goals are
+    the rolled starts and the encoder is deterministic.  Each of the 9 spherical interpolants (ebm_utils.slerp) is
+    decoded by the eta = 0 DDIM chain over the same levels.  Under torchrun every rank encodes and decodes its own
+    rows; the rows are gathered.  Returns generated (9, N, ...) and collection (9, 41, N, ...), normalised."""
+    rng = random.PRNGKey(rng_seed)        # the decoder draws nothing at eta = 0: the key only fills the key table
+    betas = ebm_utils.create_noise_schedule(FLAGS.sigma_begin, FLAGS.sigma_end, FLAGS.num_sigmas, FLAGS.schedule_type)
+    _, optimizer = _restore(FLAGS.model_dir, starts.shape[1:])
+    world, rank = parallel.world_size(), parallel.rank()
+    local = parallel.shard_size(len(starts))
+    rows = slice(rank * local, (rank + 1) * local)
+    t0 = time.time()
+    codes = ebm_utils.ddim_encode(optimizer.target, betas, starts[rows], steps=FLAGS.ddim_steps,
+                                  schedule=FLAGS.ddim_schedule)
+    codes = parallel.gather_rows(codes)
+    goal_codes = torch.roll(codes, shifts=1, dims=0)
+    kw = dict(shard=(rank * local, len(starts))) if world > 1 else {}
+    gen, colls = [], []
+    for i, alpha in enumerate(np.linspace(0.0, 1.0, 9)):
+        z = ebm_utils.slerp(codes, goal_codes, float(alpha)).to(torch.float32)[rows].contiguous()
+        x, collection, _ = ebm_utils.ddim_dynamics(rng, optimizer.target, betas, z, None, None, None, False,
+                                                   steps=FLAGS.ddim_steps, eta=0.0, schedule=FLAGS.ddim_schedule, **kw)
+        gen.append(parallel.gather_rows(x).cpu().numpy())
+        colls.append(parallel.gather_rows(collection.transpose(0, 1).contiguous()).transpose(0, 1).cpu().numpy())
+        logging.info("Generated samples %i out of %i", i, 9)
+    torch.cuda.synchronize()
+    logging.info("Encoded and decoded the interpolants in %f seconds", time.time() - t0)
+    return np.stack(gen), np.stack(colls)
+
+
+def reconstruction_errors(generated, starts, goals):
+    """How far the alpha = 0 and alpha = 1 interpolants lie from the examples they encode, in normalised units: the mean
+    squared and the largest absolute error of decode(encode(x)) against x."""
+    out = {}
+    for name, got, want in (("start", generated[0], starts), ("goal", generated[-1], goals)):
+        d = np.asarray(got, np.float64) - np.asarray(want, np.float64)
+        out[f"{name}_mse"] = float(np.mean(d * d))
+        out[f"{name}_max_abs"] = float(np.max(np.abs(d)))
+    return out
+
+
 def _save(obj, path):
     os.makedirs(os.path.dirname(path), exist_ok=True)
     with open(path, "wb") as f:
@@ -184,6 +233,14 @@ def check_flags():
         raise ValueError("--compute_metrics does not apply to --interpolate")
     if FLAGS.full_metrics and not FLAGS.compute_metrics:
         raise ValueError("--full_metrics needs --compute_metrics")
+    if FLAGS.interpolate_encoder == "ddim":
+        if not FLAGS.interpolate:
+            raise ValueError("--interpolate_encoder=ddim needs --interpolate")
+        if FLAGS.sampling != "ddim":
+            raise ValueError("--interpolate_encoder=ddim needs --sampling=ddim")
+        if FLAGS.ddim_eta != 0.0:
+            raise ValueError("--interpolate_encoder=ddim needs --ddim_eta=0: the encoder inverts the deterministic "
+                             "chain only")
 
 
 def full_metrics(real, fake):
@@ -216,6 +273,18 @@ def main(argv):
         masks[:, :8, :] = 1
         masks[:, -8:, :] = 1                               # first and last 8 are held fixed
         generated, collection, _ = infill_samples(samples, masks, FLAGS.sample_seed)
+    elif FLAGS.interpolate and FLAGS.interpolate_encoder == "ddim":
+        starts = real
+        goals = np.roll(starts, shift=1, axis=0)
+        generated, collection = ddim_interpolate(starts, FLAGS.sample_seed)
+        recon = reconstruction_errors(generated, starts, goals)
+        logging.info("Reconstruction (normalised units): %s", json.dumps(recon, sort_keys=True))
+        if parallel.rank() == 0:
+            out = os.path.join(FLAGS.model_dir, FLAGS.sampling_dir, "ncsn")
+            os.makedirs(out, exist_ok=True)
+            with open(os.path.join(out, "reconstruction.json"), "w") as f:
+                json.dump(dict(recon, ddim_steps=FLAGS.ddim_steps, ddim_schedule=FLAGS.ddim_schedule), f, indent=1,
+                          sort_keys=True)
     elif FLAGS.interpolate:                                # sample_ncsn.py:429-438
         starts = real
         goals = np.roll(starts, shift=1, axis=0)
