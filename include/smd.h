@@ -270,7 +270,8 @@ int smd_ddim_encode_tables(const float* host_betas, int T, const int* host_steps
  * steps_per_level: T of the annealed chain (ignored by the consistent one).  host_key: the `rng` the sampler receives.
  * Builds the per-level table (sigma, alpha = epsilon (sigma / sigma_L)^2, noise coefficient sqrt(2 alpha) or
  * beta sigma_{l+1}) and the collection indices linspace(1, L*T, 100) in the workspace.  It shares those regions with
- * smd_sampler_setup: each of the two invalidates the other (the other sampler then returns SMD_ERR_STATE).
+ * the other chains: smd_sampler_setup, smd_langevin_setup, smd_ddim_setup and smd_ddim_encode_setup each invalidate
+ * the other three (SMD_ERR_STATE).
  * SMD_ERR_INVALID for a TransformerMDN plan, L < 2 or L > 8192, an unknown kind or (annealed) T < 1. */
 int smd_langevin_setup(smd_plan* plan, const float* host_sigmas, int L, int steps_per_level, float epsilon, int kind,
                        const uint32_t host_key[2], smd_stream_t stream);

@@ -811,26 +811,40 @@ void launch_cast_bf16(const float* src, __nv_bfloat16* dst, size_t n, cudaStream
 }
 
 // ---------------------------------------------------------------------------------------------------
-// reverse-diffusion step after the network call (utils/ebm_utils.py:332-394)
-// thread = (sample n, channel c); loops over the S positions so the axis=1 norms reduce in registers
+// Chain step bodies after the network call
 // ---------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-reverse_step_kernel(const ReverseStepArgs a) {
-  pdl_trigger();
-  pdl_wait();
-  const int t = a.t_ptr ? *a.t_ptr : a.t;
-  const float* cf = a.coef + 8 * t;
-  const float sqrt_recip = cf[0], sqrt_m1 = cf[1], mu1 = cf[2], mu2 = cf[3], sigma = cf[4], sqrt_ap = cf[5],
-              sqrt_1m = cf[6], alpha_prod = cf[7];
-  uint32_t k0 = a.key0, k1 = a.key1, ik0 = 0, ik1 = 0;
-  if (a.key_tab) { k0 = a.key_tab[4 * t]; k1 = a.key_tab[4 * t + 1]; ik0 = a.key_tab[4 * t + 2]; ik1 = a.key_tab[4 * t + 3]; }
+// Block reduction of a chain step's per-column norms (m[0..2]: eps / grad, step, noise; 0 on lanes without a column)
+// into the batch means over NC columns: metrics rows 0, 1 and 3 (`stride` floats apart) accumulate them, block 0
+// writes `scalar` into row 2.  Every thread of the block calls it.
+__device__ __forceinline__ void step_metrics(float* met, size_t stride, float (&m)[3], float scalar, int NC) {
+  __shared__ float red[3][8];
+  m[0] = warp_sum(m[0]); m[1] = warp_sum(m[1]); m[2] = warp_sum(m[2]);
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  if (l == 0) { red[0][w] = m[0]; red[1][w] = m[1]; red[2][w] = m[2]; }
+  __syncthreads();
+  if (threadIdx.x < 3) {
+    float v = 0.f;
+    for (int j = 0; j < (blockDim.x >> 5); ++j) v += red[threadIdx.x][j];
+    const int row = (threadIdx.x == 0) ? 0 : (threadIdx.x == 1 ? 1 : 3);
+    atomicAdd(met + row * stride, v / static_cast<float>(NC));
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 3) met[2 * stride] = scalar;
+}
+
+// The reverse_step_kernel / ddim_step_kernel body: four adjacent lanes share one (sample, channel) column and take a
+// quarter of its S positions each -- 4x the threads and a quarter of the serial threefry chain per thread.  Per
+// element: z (when draw_noise: the supplied z, or threefry(k0, k1)), nx = update(x, eps_hat, z, noise), the infill
+// blend with y = infill_x, or sqrt_ap infill_x + sqrt_1m iz when draw_infill (iz: the supplied infill_z, or
+// threefry(ik0, ik1)), the state and the collection row `slot` (< 0: none).  m receives the column norms
+// sqrt(sum eps_hat^2 + 1e-10), of x - nx and of noise on the first lane of the column (two shuffles), 0 elsewhere.
+template <typename Args, typename Update>
+__device__ __forceinline__ void column_step(const Args& a, const float* z_in, const float* infill_z, uint32_t k0,
+                                            uint32_t k1, uint32_t ik0, uint32_t ik1, bool draw_noise,
+                                            bool draw_infill, float sqrt_ap, float sqrt_1m, int slot, Update update,
+                                            float (&m)[3]) {
   const int NC = a.N * a.C;
   const uint32_t total = static_cast<uint32_t>(a.N) * a.S * a.C;
   const uint32_t rtotal = a.rng_total ? a.rng_total : total, rfirst = a.rng_total ? a.rng_first : 0u;
-  const int slot = (a.slot_tab && a.collection) ? a.slot_tab[t] : -1;
-  float m_eps = 0.f, m_step = 0.f, m_noise = 0.f;
-  // four adjacent lanes share one (sample, channel) column and take a quarter of its S positions each: 4x the
-  // threads and a quarter of the serial threefry chain per thread (the axis-1 norms are folded with two shuffles)
   constexpr int kSG = 4;
   const int gi = blockIdx.x * blockDim.x + threadIdx.x;
   const int i = gi / kSG, sg = gi % kSG;
@@ -844,17 +858,15 @@ reverse_step_kernel(const ReverseStepArgs a) {
       const float x = a.x[idx];
       const float eh = a.eps_hat[idx];
       float z = 0.f;
-      if (t > 0) z = a.z ? a.z[idx] : jax_normal_from_bits(jax_random_bits(k0, k1, rfirst + idx, rtotal));
-      const float noise = z * sigma;
-      float recon = __fsub_rn(__fmul_rn(sqrt_recip, x), __fmul_rn(sqrt_m1, eh));
-      recon = fminf(fmaxf(recon, -1.0f), 1.0f);
-      float nx = __fadd_rn(__fadd_rn(__fmul_rn(mu1, recon), __fmul_rn(mu2, x)), noise);
+      if (draw_noise) z = z_in ? z_in[idx] : jax_normal_from_bits(jax_random_bits(k0, k1, rfirst + idx, rtotal));
+      float noise;
+      float nx = update(x, eh, z, noise);
       if (a.infill_mask) {
         const float mk = a.infill_mask[idx];
         const float ix = a.infill_x[idx];
         float y = ix;
-        if (t > 0) {
-          const float iz = a.infill_z ? a.infill_z[idx] : jax_normal_from_bits(jax_random_bits(ik0, ik1, rfirst + idx, rtotal));
+        if (draw_infill) {
+          const float iz = infill_z ? infill_z[idx] : jax_normal_from_bits(jax_random_bits(ik0, ik1, rfirst + idx, rtotal));
           y = sqrt_ap * ix + sqrt_1m * iz;
         }
         nx = nx * (1.0f - mk) + y * mk;
@@ -867,32 +879,37 @@ reverse_step_kernel(const ReverseStepArgs a) {
   }
   e2 += __shfl_xor_sync(0xffffffffu, e2, 1); st2 += __shfl_xor_sync(0xffffffffu, st2, 1); nz2 += __shfl_xor_sync(0xffffffffu, nz2, 1);
   e2 += __shfl_xor_sync(0xffffffffu, e2, 2); st2 += __shfl_xor_sync(0xffffffffu, st2, 2); nz2 += __shfl_xor_sync(0xffffffffu, nz2, 2);
-  if (i < NC && sg == 0) { m_eps = sqrtf(e2 + 1e-10f); m_step = sqrtf(st2 + 1e-10f); m_noise = sqrtf(nz2 + 1e-10f); }
-  if (a.metrics) {
-    __shared__ float red[3][8];
-    m_eps = warp_sum(m_eps); m_step = warp_sum(m_step); m_noise = warp_sum(m_noise);
-    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-    if (l == 0) { red[0][w] = m_eps; red[1][w] = m_step; red[2][w] = m_noise; }
-    __syncthreads();
-    if (threadIdx.x < 3) {
-      float v = 0.f;
-      for (int j = 0; j < (blockDim.x >> 5); ++j) v += red[threadIdx.x][j];
-      const int si = a.T - 1 - t;
-      const int row = (threadIdx.x == 0) ? 0 : (threadIdx.x == 1 ? 1 : 3);
-      atomicAdd(a.metrics + row * a.T + si, v / static_cast<float>(NC));
-    }
-    if (blockIdx.x == 0 && threadIdx.x == 3) a.metrics[2 * a.T + (a.T - 1 - t)] = alpha_prod;
-  }
+  m[0] = m[1] = m[2] = 0.f;
+  if (i < NC && sg == 0) { m[0] = sqrtf(e2 + 1e-10f); m[1] = sqrtf(st2 + 1e-10f); m[2] = sqrtf(nz2 + 1e-10f); }
+}
+
+// reverse-diffusion step (utils/ebm_utils.py:332-394)
+__global__ void __launch_bounds__(256)
+reverse_step_kernel(const ReverseStepArgs a) {
+  pdl_trigger();
+  pdl_wait();
+  const int t = a.t_ptr ? *a.t_ptr : a.t;
+  const float* cf = a.coef + 8 * t;
+  const float sqrt_recip = cf[0], sqrt_m1 = cf[1], mu1 = cf[2], mu2 = cf[3], sigma = cf[4];
+  uint32_t k0 = a.key0, k1 = a.key1, ik0 = 0, ik1 = 0;
+  if (a.key_tab) { k0 = a.key_tab[4 * t]; k1 = a.key_tab[4 * t + 1]; ik0 = a.key_tab[4 * t + 2]; ik1 = a.key_tab[4 * t + 3]; }
+  const int slot = (a.slot_tab && a.collection) ? a.slot_tab[t] : -1;
+  float m[3];
+  column_step(a, a.z, a.infill_z, k0, k1, ik0, ik1, t > 0, t > 0, cf[5], cf[6], slot,
+              [&](float x, float eh, float z, float& noise) {
+                noise = z * sigma;
+                float recon = __fsub_rn(__fmul_rn(sqrt_recip, x), __fmul_rn(sqrt_m1, eh));
+                recon = fminf(fmaxf(recon, -1.0f), 1.0f);
+                return __fadd_rn(__fadd_rn(__fmul_rn(mu1, recon), __fmul_rn(mu2, x)), noise);
+              }, m);
+  if (a.metrics) step_metrics(a.metrics + (a.T - 1 - t), a.T, m, cf[7], a.N * a.C);
 }
 void launch_reverse_step(const ReverseStepArgs& a, cudaStream_t st) {
   const int NC = a.N * a.C;
   reverse_step_kernel<<<(4 * NC + 255) / 256, 256, 0, st>>>(a);
 }
 
-// ---------------------------------------------------------------------------------------------------
-// DDIM step after the network call (Song et al. 2021, eq. 12, with the reference's clipped x0 estimate): the
-// reverse_step_kernel layout -- four lanes per (sample, channel) column, a quarter of its S positions each
-// ---------------------------------------------------------------------------------------------------
+// DDIM step (Song et al. 2021, eq. 12, with the reference's clipped x0 estimate)
 __global__ void __launch_bounds__(256)
 ddim_step_kernel(const DdimStepArgs a) {
   pdl_trigger();
@@ -900,64 +917,22 @@ ddim_step_kernel(const DdimStepArgs a) {
   const int si = *a.i_ptr;
   const float* cf = a.coef + 8 * si;
   const float sqrt_recip = cf[0], sqrt_m1 = cf[1], c_x0 = cf[2], c_dir = cf[3], sig = cf[4], sqrt_a = cf[5],
-              sqrt_1m = cf[6], abar = cf[7];
+              sqrt_1m = cf[6];
   const uint32_t k0 = a.key_tab[4 * si], k1 = a.key_tab[4 * si + 1], ik0 = a.key_tab[4 * si + 2],
                  ik1 = a.key_tab[4 * si + 3];
   const bool t_pos = si > 0 || a.tau0 > 0;     // t = tau_i > 0
-  const int NC = a.N * a.C;
-  const uint32_t total = static_cast<uint32_t>(a.N) * a.S * a.C;
-  const uint32_t rtotal = a.rng_total ? a.rng_total : total, rfirst = a.rng_total ? a.rng_first : 0u;
   const int slot = a.collection ? a.slot_tab[si] : -1;
-  float m_eps = 0.f, m_step = 0.f, m_noise = 0.f;
-  constexpr int kSG = 4;
-  const int gi = blockIdx.x * blockDim.x + threadIdx.x;
-  const int i = gi / kSG, sg = gi % kSG;
-  float e2 = 0.f, st2 = 0.f, nz2 = 0.f;
-  if (i < NC) {
-    const int n = i / a.C, c = i % a.C;
-    const int per = (a.S + kSG - 1) / kSG;
-    const int s_end = min(a.S, (sg + 1) * per);
-    for (int s = sg * per; s < s_end; ++s) {
-      const uint32_t idx = (static_cast<uint32_t>(n) * a.S + s) * a.C + c;
-      const float x = a.x[idx];
-      const float eh = a.eps_hat[idx];
-      float x0 = __fsub_rn(__fmul_rn(sqrt_recip, x), __fmul_rn(sqrt_m1, eh));
-      x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
-      const float dir = __fdiv_rn(__fsub_rn(x, __fmul_rn(sqrt_a, x0)), sqrt_1m);
-      // sig = 0 (eta = 0, or the last step) draws nothing: the deterministic chain needs no noise stream
-      const float noise = sig != 0.f ? sig * jax_normal_from_bits(jax_random_bits(k0, k1, rfirst + idx, rtotal)) : 0.f;
-      float nx = __fadd_rn(__fadd_rn(__fmul_rn(c_x0, x0), __fmul_rn(c_dir, dir)), noise);
-      if (a.infill_mask) {
-        const float mk = a.infill_mask[idx];
-        const float ix = a.infill_x[idx];
-        float y = ix;
-        if (t_pos) y = sqrt_a * ix + sqrt_1m * jax_normal_from_bits(jax_random_bits(ik0, ik1, rfirst + idx, rtotal));
-        nx = nx * (1.0f - mk) + y * mk;
-      }
-      const float stp = x - nx;
-      e2 += eh * eh; st2 += stp * stp; nz2 += noise * noise;
-      a.x_next[idx] = nx;
-      if (slot >= 0) a.collection[static_cast<size_t>(slot) * total + idx] = nx;
-    }
-  }
-  e2 += __shfl_xor_sync(0xffffffffu, e2, 1); st2 += __shfl_xor_sync(0xffffffffu, st2, 1); nz2 += __shfl_xor_sync(0xffffffffu, nz2, 1);
-  e2 += __shfl_xor_sync(0xffffffffu, e2, 2); st2 += __shfl_xor_sync(0xffffffffu, st2, 2); nz2 += __shfl_xor_sync(0xffffffffu, nz2, 2);
-  if (i < NC && sg == 0) { m_eps = sqrtf(e2 + 1e-10f); m_step = sqrtf(st2 + 1e-10f); m_noise = sqrtf(nz2 + 1e-10f); }
-  if (a.metrics) {
-    __shared__ float red[3][8];
-    m_eps = warp_sum(m_eps); m_step = warp_sum(m_step); m_noise = warp_sum(m_noise);
-    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-    if (l == 0) { red[0][w] = m_eps; red[1][w] = m_step; red[2][w] = m_noise; }
-    __syncthreads();
-    const int col = a.K - 1 - si;
-    if (threadIdx.x < 3) {
-      float v = 0.f;
-      for (int j = 0; j < (blockDim.x >> 5); ++j) v += red[threadIdx.x][j];
-      const int row = (threadIdx.x == 0) ? 0 : (threadIdx.x == 1 ? 1 : 3);
-      atomicAdd(a.metrics + row * a.K + col, v / static_cast<float>(NC));
-    }
-    if (blockIdx.x == 0 && threadIdx.x == 3) a.metrics[2 * a.K + col] = abar;
-  }
+  float m[3];
+  // sig = 0 (eta = 0, or the last step) draws nothing: the deterministic chain needs no noise stream
+  column_step(a, nullptr, nullptr, k0, k1, ik0, ik1, sig != 0.f, t_pos, sqrt_a, sqrt_1m, slot,
+              [&](float x, float eh, float z, float& noise) {
+                float x0 = __fsub_rn(__fmul_rn(sqrt_recip, x), __fmul_rn(sqrt_m1, eh));
+                x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
+                const float dir = __fdiv_rn(__fsub_rn(x, __fmul_rn(sqrt_a, x0)), sqrt_1m);
+                noise = sig != 0.f ? sig * z : 0.f;
+                return __fadd_rn(__fadd_rn(__fmul_rn(c_x0, x0), __fmul_rn(c_dir, dir)), noise);
+              }, m);
+  if (a.metrics) step_metrics(a.metrics + (a.K - 1 - si), a.K, m, cf[7], a.N * a.C);
 }
 void launch_ddim_step(const DdimStepArgs& a, cudaStream_t st) {
   const int NC = a.N * a.C;
@@ -1224,7 +1199,7 @@ __global__ void __launch_bounds__(256) langevin_step_kernel(const LangevinStepAr
     coll = (coll && cs->slot >= 0) ? coll + static_cast<size_t>(cs->slot) * total : nullptr;
     if (met) { met += static_cast<size_t>(cs->si) * a.T + cs->i; mstride = static_cast<size_t>(a.L) * a.T; }
   }
-  float m_g = 0.f, m_s = 0.f, m_n = 0.f;
+  float m[3] = {0.f, 0.f, 0.f};   // grad_norm, step_norm, noise_norm (metrics rows 0, 1, 3; row 2: alpha)
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < NC) {
     const int n = i / a.C, c = i % a.C;
@@ -1246,22 +1221,9 @@ __global__ void __launch_bounds__(256) langevin_step_kernel(const LangevinStepAr
       a.x_next[idx] = nx;
       if (coll) coll[idx] = nx;
     }
-    m_g = sqrtf(g2 + 1e-10f); m_s = sqrtf(s2 + 1e-10f); m_n = sqrtf(n2 + 1e-10f);
+    m[0] = sqrtf(g2 + 1e-10f); m[1] = sqrtf(s2 + 1e-10f); m[2] = sqrtf(n2 + 1e-10f);
   }
-  if (met) {
-    __shared__ float red[3][8];
-    m_g = warp_sum(m_g); m_s = warp_sum(m_s); m_n = warp_sum(m_n);
-    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-    if (l == 0) { red[0][w] = m_g; red[1][w] = m_s; red[2][w] = m_n; }
-    __syncthreads();
-    if (threadIdx.x < 3) {
-      float v = 0.f;
-      for (int j = 0; j < (blockDim.x >> 5); ++j) v += red[threadIdx.x][j];
-      const int rowi = (threadIdx.x == 0) ? 0 : (threadIdx.x == 1 ? 1 : 3);   // grad_norm, step_norm, (alpha), noise_norm
-      atomicAdd(met + rowi * mstride, v / static_cast<float>(NC));
-    }
-    if (blockIdx.x == 0 && threadIdx.x == 3) met[2 * mstride] = alpha;
-  }
+  if (met) step_metrics(met, mstride, m, alpha, NC);
 }
 void launch_langevin_step(const LangevinStepArgs& a, cudaStream_t st) {
   const int NC = a.N * a.C;

@@ -139,6 +139,16 @@ enum Objective : int { kObjDdpm = 0, kObjDsm = 1, kObjSsm = 2, kObjMdn = 3 };
 // the Langevin chain, the DDIM chain and the DDIM encoder share those regions, so at most one of them is set up at a
 // time.
 enum Chain : int { kChainNone = 0, kChainDdpm = 1, kChainLangevin = 2, kChainDdim = 3, kChainDdimEncode = 4 };
+// The chain set up in the workspace and the per-chain values its calls read back.
+struct ChainSetup {
+  Chain kind = kChainNone;
+  int rows = 0;                 // rows of the coef and FiLM tables: T (DDPM), K (DDIM, encoder), L (Langevin)
+  int steps = 1;                // Langevin: steps per level (1 for the consistent chain and for the other chains)
+  int tau0 = 0;                 // DDIM: the first selected index tau_0
+  int lv_kind = 0;              // Langevin: 0 annealed, 1 consistent
+  uint32_t key[2] = {0u, 0u};   // Langevin: the chain key
+  float sigma_last = 0.f;       // Langevin: sigma_L
+};
 
 // The legacy default stream cannot be captured into a CUDA graph.
 inline bool capturable(cudaStream_t st) { return st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread; }
@@ -230,22 +240,16 @@ struct smd_plan {
   std::vector<GemmOp> op_ta, op_tb;   // DenseNCSN tangent pass: same weights, tangent activations, no bias
   GemmOp op_tin, op_tout;
   // sampler
-  int T = 0;
   int T_obj = 0;  // schedule length of the training objective
   int L_dsm = 0;  // length of the sigma schedule of the denoising-score-matching objective (smd_dsm_setup)
   // FiLM table of the sampler: [K][T][2*Md], built for the parameters film_tab_params (see FilmRows)
   bool film_tab_ready = false;
   const float* film_tab_params = nullptr;
   long long shard_first_row = 0, shard_total_rows = 0;   // smd_sampler_set_shard
-  // The chain set up (smd_sampler_setup / smd_langevin_setup), and the graph replay of one step of it (smd_ddpm_sample
-  // / smd_langevin_sample).  T holds the number of noise levels L while a Langevin schedule is set (the FiLM table has
-  // one row per level).
-  smd::Chain chain = smd::kChainNone;
+  // The chain set up (smd_sampler_setup, smd_ddim_setup, smd_ddim_encode_setup or smd_langevin_setup), and the graph
+  // replay of one step of it (smd_ddpm_sample, smd_ddim_sample, smd_ddim_encode or smd_langevin_sample).
+  smd::ChainSetup chain;
   smd::CapturedGraph chain_graph;
-  int ddim_tau0 = 0;               // DDIM: the first selected index tau_0 (plan->T holds the number of steps K)
-  int lv_kind = 0, lv_steps = 1;   // Langevin: kind (0 annealed, 1 consistent), steps per level
-  uint32_t lv_key[2] = {0u, 0u};
-  float lv_sigma_last = 0.f;
   cudaStream_t own_stream = nullptr;
   cudaEvent_t own_event = nullptr;
   // training: the FiLM generator (forward and backward) runs on a side stream, concurrently with the trunk

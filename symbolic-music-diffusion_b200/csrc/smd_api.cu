@@ -397,7 +397,7 @@ int run_tail(smd_plan* p, const float* params, int M, int S, int t_broadcast, fl
     const float* scale = p->mdn() ? nullptr : ss + static_cast<size_t>(k) * p->cfg.max_batch * 2 * Md;
     const int* frow_dev = nullptr;
     if (film.table) {
-      scale = film.table + static_cast<size_t>(k) * p->T * 2 * Md;
+      scale = film.table + static_cast<size_t>(k) * p->chain.rows * 2 * Md;
       if (film.row_dev) frow_dev = film.row_dev; else scale += static_cast<size_t>(film.row) * 2 * Md;
     }
     const float* shift = scale ? scale + Md : nullptr;
@@ -706,13 +706,18 @@ static int objective_draws(const smd_plan* plan, const uint32_t host_key[2], int
   return SMD_OK;
 }
 
-// State axes and shard counters of a chain step.  The dense networks' (N, D) states use axis 1 = D (the metrics' axis
-// 1, utils/ebm_utils.py:380-384).  sharded: the step draws its slice of the global threefry streams
+// State axes of a chain step.  The dense networks' (N, D) states use axis 1 = D (the metrics' axis 1,
+// utils/ebm_utils.py:380-384).
+template <typename StepArgs>
+static void state_axes(const smd_plan* plan, StepArgs& a) {
+  a.S = plan->cfg.seq_len; a.C = plan->cfg.channels;
+  if (plan->cfg.arch != SMD_ARCH_TRANSFORMER_DDPM) { a.S = plan->cfg.channels; a.C = 1; }
+}
+// State axes and shard counters of a chain step.  sharded: the step draws its slice of the global threefry streams
 // (smd_sampler_set_shard).
 template <typename StepArgs>
 static void chain_geometry(const smd_plan* plan, StepArgs& a, bool sharded) {
-  a.S = plan->cfg.seq_len; a.C = plan->cfg.channels;
-  if (plan->cfg.arch != SMD_ARCH_TRANSFORMER_DDPM) { a.S = plan->cfg.channels; a.C = 1; }
+  state_axes(plan, a);
   if (sharded && plan->shard_total_rows > 0) {
     const long long per = static_cast<long long>(a.S) * a.C;
     a.rng_first = static_cast<uint32_t>(plan->shard_first_row * per);
@@ -739,6 +744,91 @@ static int join_replay(smd_plan* plan, cudaStream_t st, cudaStream_t cs) {
   SMD_CUDA(cudaEventRecord(plan->own_event, cs));
   SMD_CUDA(cudaStreamWaitEvent(st, plan->own_event, 0));
   return SMD_OK;
+}
+
+// Installs a chain in the workspace: uploads its coef table (rows x width floats) and, when given, its keys table
+// (rows x 4) and slots table (nslots ints), then forgets the FiLM table and the step graph of the chain before.
+static int install_chain(smd_plan* plan, Chain kind, int rows, const float* coef, int width, const uint32_t* keys,
+                         const int* slots, int nslots, cudaStream_t st) {
+  const size_t n = static_cast<size_t>(rows);
+  SMD_CUDA(cudaMemcpyAsync(plan->at<float>(plan->reg.coef), coef, n * width * 4, cudaMemcpyHostToDevice, st));
+  if (keys) SMD_CUDA(cudaMemcpyAsync(plan->at<uint32_t>(plan->reg.keys), keys, n * 16, cudaMemcpyHostToDevice, st));
+  if (slots) SMD_CUDA(cudaMemcpyAsync(plan->at<int>(plan->reg.slots), slots, nslots * 4, cudaMemcpyHostToDevice, st));
+  SMD_CUDA(cudaStreamSynchronize(st));  // the host tables go out of scope
+  plan->chain = ChainSetup{};
+  plan->chain.kind = kind;
+  plan->chain.rows = rows;
+  plan->film_tab_ready = false;
+  plan->chain_graph.drop();
+  return SMD_OK;
+}
+
+__global__ void gather_cond_kernel(const float* __restrict__ coef, float* __restrict__ tv, int T, int stride,
+                                   int offset) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < T) tv[i] = coef[stride * i + offset];
+}
+
+// FiLM scale/shift for every row of the schedule (all samples share the conditioning value, so this replaces 3K small
+// launches per step by one table lookup): ftab[k][r][:] = DenseFiLM_k(cond_r)   (models/ncsn.py:44-61), with cond_r =
+// coef[stride * r + offset] for the chain's rows: sqrt(alpha_bar) of the DDPM and DDIM chains and of the encoder,
+// sigma_l of the Langevin chain
+static int ensure_film_table(smd_plan* plan, const float* params, int stride, int offset, cudaStream_t st) {
+  if (plan->cfg.sampler_T <= 0 || plan->chain.rows > plan->cfg.sampler_T) return SMD_OK;   // per-step generator instead
+  if (plan->film_tab_ready && plan->film_tab_params == params) return SMD_OK;
+  const int T = plan->chain.rows;
+  const WorkspaceLayout& w = plan->reg;
+  float* tv = plan->at<float>(w.ftab_t);
+  const size_t tab_stride = static_cast<size_t>(T) * 2 * plan->cfg.mlp_dims;
+  gather_cond_kernel<<<(T + 255) / 256, 256, 0, st>>>(plan->at<float>(w.coef), tv, T, stride, offset); CNT();
+  const int rc = film_generator(plan, params, tv, T, plan->at<float>(w.ftab_enc), [&](int k) {
+    return FilmBuffers{plan->at<float>(w.ftab_e1), nullptr, plan->at<float>(w.ftab_e2),
+                       plan->at<float>(w.ftab) + k * tab_stride};
+  }, st, "film table");
+  if (rc) return rc;
+  plan->film_tab_ready = true;
+  plan->film_tab_params = params;
+  return SMD_OK;
+}
+
+// Sets the device step counter (t_ptr) that the DDPM and DDIM chains and the encoder read and step_advance decrements.
+static int set_step_counter(smd_plan* plan, int first, cudaStream_t st) {
+  SMD_CUDA(cudaMemcpyAsync(plan->at<int>(plan->reg.t_ptr), &first, sizeof(int), cudaMemcpyHostToDevice, st));
+  SMD_CUDA(cudaStreamSynchronize(st));  // `first` is a stack variable
+  return SMD_OK;
+}
+
+// One call of the chain set up: on the replay stream cs (st itself when eager), zero metrics (4 x rows x steps-per-row
+// floats) when given, build the FiLM table on coef column `cond_col` (rows of cond_stride floats), run prologue(cs),
+// then either `steps` x eager_step(cs), or step(cs) captured once under `key` and replayed `steps` times, then
+// epilogue(cs), and order st after cs.
+template <typename Prologue, typename Step, typename EagerStep, typename Epilogue>
+static int run_chain(smd_plan* plan, const float* params, cudaStream_t st, int use_graph, float* metrics,
+                     int cond_stride, int cond_col, long long steps, const GraphKey& key, const char* what,
+                     Prologue&& prologue, Step&& step, EagerStep&& eager_step, Epilogue&& epilogue) {
+  cudaStream_t cs = st;
+  if (use_graph) { const int rc = replay_stream(plan, st, &cs); if (rc) return rc; }
+  if (metrics)
+    SMD_CUDA(cudaMemsetAsync(metrics, 0, sizeof(float) * 4 * plan->chain.rows * plan->chain.steps, cs));
+  { const int rc = ensure_film_table(plan, params, cond_stride, cond_col, cs); if (rc) return rc; }
+  { const int rc = prologue(cs); if (rc) return rc; }
+  if (!use_graph) {
+    for (long long i = 0; i < steps; ++i) {
+      const int rc = eager_step(cs);
+      if (rc) return rc;
+    }
+  } else {
+    if (!plan->chain_graph.replays(key)) {
+      const int rc = plan->chain_graph.capture(cs, key, [&] { return step(cs); }, what);
+      if (rc) return rc;
+    }
+    for (long long i = 0; i < steps; ++i) {
+      const int rc = plan->chain_graph.launch(cs);
+      if (rc) return rc;
+    }
+  }
+  { const int rc = epilogue(cs); if (rc) return rc; }
+  return join_replay(plan, st, cs);
 }
 
 }  // namespace smd
@@ -856,7 +946,7 @@ static void forget_workspace_contents(smd_plan* plan) {
   plan->packed = false;
   plan->T_obj = 0;
   plan->L_dsm = 0;
-  plan->chain = kChainNone;
+  plan->chain = ChainSetup{};
   plan->chain_graph.drop();
   plan->film_tab_ready = false;
   plan->train_graph.drop();
@@ -1127,7 +1217,6 @@ int smd_sampler_setup(smd_plan* plan, const float* host_betas, int T, const uint
   if (reject_mdn(plan, "smd_sampler_setup")) return SMD_ERR_INVALID;
   if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
   if (T < 1 || T > kMaxT) { set_error("T out of range"); return SMD_ERR_INVALID; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   // utils/ebm_utils.py:315-318, 332-357, 363-364 -- float32, same operation order
   std::vector<float> coef(static_cast<size_t>(T) * 8);
   std::vector<float> ap(T), app(T), al(T);
@@ -1155,42 +1244,8 @@ int smd_sampler_setup(smd_plan* plan, const float* host_betas, int T, const uint
   scan_keys(host_key, T, keys.data());
   std::vector<int> slots(T, -1);
   collection_slots(T, slots.data());
-  SMD_CUDA(cudaMemcpyAsync(plan->at<float>(plan->reg.coef), coef.data(), coef.size() * 4, cudaMemcpyHostToDevice, st));
-  SMD_CUDA(cudaMemcpyAsync(plan->at<uint32_t>(plan->reg.keys), keys.data(), keys.size() * 4, cudaMemcpyHostToDevice, st));
-  SMD_CUDA(cudaMemcpyAsync(plan->at<int>(plan->reg.slots), slots.data(), slots.size() * 4, cudaMemcpyHostToDevice, st));
-  SMD_CUDA(cudaStreamSynchronize(st));  // host vectors go out of scope
-  plan->T = T;
-  plan->chain = kChainDdpm;
-  plan->film_tab_ready = false;
-  plan->chain_graph.drop();
-  return SMD_OK;
-}
-
-__global__ void gather_cond_kernel(const float* __restrict__ coef, float* __restrict__ tv, int T, int stride,
-                                   int offset) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < T) tv[i] = coef[stride * i + offset];
-}
-
-// FiLM scale/shift for every row of the schedule (all samples share the conditioning value, so this replaces 3K small
-// launches per step by one table lookup): ftab[k][r][:] = DenseFiLM_k(cond_r)   (models/ncsn.py:44-61), with cond_r =
-// coef[stride * r + offset] for the plan->T rows: sqrt(alpha_bar_t) of the DDPM sampler, sigma_l of the Langevin chain
-static int ensure_film_table(smd_plan* plan, const float* params, int stride, int offset, cudaStream_t st) {
-  if (plan->cfg.sampler_T <= 0 || plan->T > plan->cfg.sampler_T) return SMD_OK;   // per-step generator instead
-  if (plan->film_tab_ready && plan->film_tab_params == params) return SMD_OK;
-  const int T = plan->T;
-  const WorkspaceLayout& w = plan->reg;
-  float* tv = plan->at<float>(w.ftab_t);
-  const size_t tab_stride = static_cast<size_t>(T) * 2 * plan->cfg.mlp_dims;
-  gather_cond_kernel<<<(T + 255) / 256, 256, 0, st>>>(plan->at<float>(w.coef), tv, T, stride, offset); CNT();
-  const int rc = film_generator(plan, params, tv, T, plan->at<float>(w.ftab_enc), [&](int k) {
-    return FilmBuffers{plan->at<float>(w.ftab_e1), nullptr, plan->at<float>(w.ftab_e2),
-                       plan->at<float>(w.ftab) + k * tab_stride};
-  }, st, "film table");
-  if (rc) return rc;
-  plan->film_tab_ready = true;
-  plan->film_tab_params = params;
-  return SMD_OK;
+  return install_chain(plan, kChainDdpm, T, coef.data(), 8, keys.data(), slots.data(), T,
+                       static_cast<cudaStream_t>(stream));
 }
 
 // The FiLM table rows of a network call with `params`: row `row`, or *row_dev when row_dev is set; {} (run the
@@ -1198,6 +1253,20 @@ static int ensure_film_table(smd_plan* plan, const float* params, int stride, in
 static FilmRows film_table_rows(const smd_plan* plan, const float* params, int row, const int* row_dev) {
   if (!plan->film_tab_ready || plan->film_tab_params != params) return FilmRows{};
   return FilmRows{plan->at<float>(plan->reg.ftab), row, row_dev};
+}
+
+// The checks a call on a set-up chain shares, argument errors first: 1 <= n <= max_batch, infill_x and infill_mask
+// come together, and `kind` is the chain set up.
+static int check_chain_call(const smd_plan* plan, const char* fn, Chain kind, int n, const float* infill_x,
+                            const float* infill_mask) {
+  static const char* const setup_fn[] = {"", "smd_sampler_setup", "smd_langevin_setup", "smd_ddim_setup",
+                                         "smd_ddim_encode_setup"};
+  if (!plan) { set_error("null plan"); return SMD_ERR_INVALID; }
+  if (reject_mdn(plan, fn)) return SMD_ERR_INVALID;
+  if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
+  if ((infill_x == nullptr) != (infill_mask == nullptr)) { set_error("infill_x and infill_mask go together"); return SMD_ERR_INVALID; }
+  if (plan->chain.kind != kind) { set_error(std::string(setup_fn[kind]) + " has not been called"); return SMD_ERR_STATE; }
+  return SMD_OK;
 }
 
 // one reverse step; t < 0 means "read t from the device scalar t_ptr" (graph replay)
@@ -1226,7 +1295,7 @@ static int reverse_step_impl(smd_plan* plan, const float* params, const float* x
   a.t = t;
   a.infill_x = infill_x; a.infill_mask = infill_mask; a.infill_z = infill_z;
   a.x_next = x_next; a.collection = collection; a.metrics = metrics;
-  a.N = n; a.T = plan->T;
+  a.N = n; a.T = plan->chain.rows;
   chain_geometry(plan, a, /*sharded=*/true);
   launch_reverse_step(a, st); CNT();
   SMD_LAUNCH_CHECK("reverse_step");
@@ -1246,56 +1315,40 @@ int smd_sampler_set_shard(smd_plan* plan, long long first_row, long long total_r
 int smd_ddpm_reverse_step(smd_plan* plan, const float* params, const float* x, int n, int t, const float* z,
                           const float* infill_x, const float* infill_mask, const float* infill_z, float* x_next,
                           float* eps_hat_or_null, float* collection, float* metrics, smd_stream_t stream) {
-  if (reject_mdn(plan, "smd_ddpm_reverse_step")) return SMD_ERR_INVALID;
-  if (plan->chain != kChainDdpm) { set_error("smd_sampler_setup has not been called"); return SMD_ERR_STATE; }
-  if (t < 0 || t >= plan->T) { set_error("t out of range"); return SMD_ERR_INVALID; }
-  if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
+  const int rc = check_chain_call(plan, "smd_ddpm_reverse_step", kChainDdpm, n, infill_x, infill_mask);
+  if (rc) return rc;
+  if (t < 0 || t >= plan->chain.rows) { set_error("t out of range"); return SMD_ERR_INVALID; }
   int rc0 = ensure_film_table(plan, params, 8, 5, static_cast<cudaStream_t>(stream));
   if (rc0) return rc0;
   return reverse_step_impl(plan, params, x, n, t, z, infill_x, infill_mask, infill_z, x_next, eps_hat_or_null,
                            collection, metrics, static_cast<cudaStream_t>(stream));
 }
 
+static int no_epilogue(cudaStream_t) { return SMD_OK; }
+
 int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int steps, const float* infill_x,
                     const float* infill_mask, float* collection, float* metrics, int use_graph,
                     smd_stream_t stream) {
-  if (reject_mdn(plan, "smd_ddpm_sample")) return SMD_ERR_INVALID;
-  if (plan->chain != kChainDdpm) { set_error("smd_sampler_setup has not been called"); return SMD_ERR_STATE; }
-  if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
-  if (steps < 1 || steps > plan->T) { set_error("steps out of range"); return SMD_ERR_INVALID; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int T = plan->T;
-  if (metrics) SMD_CUDA(cudaMemsetAsync(metrics, 0, sizeof(float) * 4 * T, st));
-  { int rc0 = ensure_film_table(plan, params, 8, 5, st); if (rc0) return rc0; }
-  if (!use_graph) {
-    for (int i = 0; i < steps; ++i) {
-      int rc = reverse_step_impl(plan, params, x, n, T - 1 - i, nullptr, infill_x, infill_mask, nullptr, x, nullptr,
-                                 collection, metrics, st);
-      if (rc) return rc;
-    }
-    return SMD_OK;
-  }
-  cudaStream_t cs;
-  { const int rc0 = replay_stream(plan, st, &cs); if (rc0) return rc0; }
-  int* t_ptr = plan->at<int>(plan->reg.t_ptr);
-  const int t0 = T - 1;
-  SMD_CUDA(cudaMemcpyAsync(t_ptr, &t0, sizeof(int), cudaMemcpyHostToDevice, cs));
-  SMD_CUDA(cudaStreamSynchronize(cs));  // t0 is a stack variable
-  const GraphKey key = graph_key(n, params, x, infill_x, infill_mask, collection, metrics);
-  if (!plan->chain_graph.replays(key)) {
-    const int rc = plan->chain_graph.capture(cs, key, [&] {
-      const int r = reverse_step_impl(plan, params, x, n, -1, nullptr, infill_x, infill_mask, nullptr, x, nullptr,
-                                      collection, metrics, cs);
-      if (r == SMD_OK) { launch_step_advance(t_ptr, cs); CNT(); }
-      return r;
-    }, "sampler graph");
-    if (rc) return rc;
-  }
-  for (int i = 0; i < steps; ++i) {
-    const int rc = plan->chain_graph.launch(cs);
-    if (rc) return rc;
-  }
-  return join_replay(plan, st, cs);
+  const int rc = check_chain_call(plan, "smd_ddpm_sample", kChainDdpm, n, infill_x, infill_mask);
+  if (rc) return rc;
+  const int T = plan->chain.rows;
+  if (steps < 1 || steps > T) { set_error("steps out of range"); return SMD_ERR_INVALID; }
+  // the eager loop steps t = T-1, T-2, ... from the host; the graph reads t from the device counter
+  int t = T;
+  return run_chain(plan, params, static_cast<cudaStream_t>(stream), use_graph, metrics, 8, 5, steps,
+                   graph_key(n, params, x, infill_x, infill_mask, collection, metrics), "sampler graph",
+                   [&](cudaStream_t s) { return use_graph ? set_step_counter(plan, T - 1, s) : SMD_OK; },
+                   [&](cudaStream_t s) {
+                     const int r = reverse_step_impl(plan, params, x, n, -1, nullptr, infill_x, infill_mask, nullptr,
+                                                     x, nullptr, collection, metrics, s);
+                     if (r == SMD_OK) { launch_step_advance(plan->at<int>(plan->reg.t_ptr), s); CNT(); }
+                     return r;
+                   },
+                   [&](cudaStream_t s) {
+                     return reverse_step_impl(plan, params, x, n, --t, nullptr, infill_x, infill_mask, nullptr, x,
+                                              nullptr, collection, metrics, s);
+                   },
+                   no_epilogue);
 }
 
 // ---- DDIM chain (Song et al. 2021) over a strided subset of the DDPM schedule -----------------------------------------
@@ -1362,25 +1415,18 @@ int smd_ddim_setup(smd_plan* plan, const float* host_betas, int T, const int* ho
                    const uint32_t host_key[2], smd_stream_t stream) {
   if (!plan || !host_key) { set_error("null argument"); return SMD_ERR_INVALID; }
   if (reject_mdn(plan, "smd_ddim_setup")) return SMD_ERR_INVALID;
-  std::vector<float> coef(static_cast<size_t>(std::max(K, 0)) * 8);
-  const int rc = ddim_tables(host_betas, T, host_steps, K, eta, coef.data());
+  const size_t rows = static_cast<size_t>(std::max(K, 0));
+  std::vector<float> coef(rows * 8);
+  std::vector<uint32_t> keys(rows * 4);
+  std::vector<int> slots(rows);
+  const int rc = smd_ddim_tables(host_betas, T, host_steps, K, eta, host_key, coef.data(), keys.data(), slots.data());
   if (rc) return rc;
   if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
   // K <= T <= kMaxT rows: the tables fit the coef / keys / slots regions of the DDPM sampler
-  std::vector<uint32_t> keys(static_cast<size_t>(K) * 4);
-  scan_keys(host_key, K, keys.data());
-  std::vector<int> slots(K);
-  collection_slots(K, slots.data());
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  SMD_CUDA(cudaMemcpyAsync(plan->at<float>(plan->reg.coef), coef.data(), coef.size() * 4, cudaMemcpyHostToDevice, st));
-  SMD_CUDA(cudaMemcpyAsync(plan->at<uint32_t>(plan->reg.keys), keys.data(), keys.size() * 4, cudaMemcpyHostToDevice, st));
-  SMD_CUDA(cudaMemcpyAsync(plan->at<int>(plan->reg.slots), slots.data(), slots.size() * 4, cudaMemcpyHostToDevice, st));
-  SMD_CUDA(cudaStreamSynchronize(st));  // host tables go out of scope
-  plan->T = K;
-  plan->ddim_tau0 = host_steps[0];
-  plan->chain = kChainDdim;
-  plan->film_tab_ready = false;
-  plan->chain_graph.drop();
+  const int rc2 = install_chain(plan, kChainDdim, K, coef.data(), 8, keys.data(), slots.data(), K,
+                                static_cast<cudaStream_t>(stream));
+  if (rc2) return rc2;
+  plan->chain.tau0 = host_steps[0];
   return SMD_OK;
 }
 
@@ -1405,7 +1451,7 @@ static int ddim_step(smd_plan* plan, const float* params, float* x, int n, const
   a.i_ptr = t_ptr;
   a.infill_x = infill_x; a.infill_mask = infill_mask;
   a.x_next = x; a.collection = collection; a.metrics = metrics;
-  a.N = n; a.K = plan->T; a.tau0 = plan->ddim_tau0;
+  a.N = n; a.K = plan->chain.rows; a.tau0 = plan->chain.tau0;
   chain_geometry(plan, a, /*sharded=*/true);
   launch_ddim_step(a, st); CNT();
   launch_step_advance(t_ptr, st); CNT();
@@ -1415,40 +1461,15 @@ static int ddim_step(smd_plan* plan, const float* params, float* x, int n, const
 
 int smd_ddim_sample(smd_plan* plan, const float* params, float* x, int n, const float* infill_x,
                     const float* infill_mask, float* collection, float* metrics, int use_graph, smd_stream_t stream) {
-  if (!plan) { set_error("null plan"); return SMD_ERR_INVALID; }
-  if (reject_mdn(plan, "smd_ddim_sample")) return SMD_ERR_INVALID;
-  if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
-  if ((infill_x == nullptr) != (infill_mask == nullptr)) { set_error("infill_x and infill_mask go together"); return SMD_ERR_INVALID; }
-  if (plan->chain != kChainDdim) { set_error("smd_ddim_setup has not been called"); return SMD_ERR_STATE; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int K = plan->T;
-  cudaStream_t cs = st;
-  if (use_graph) { const int rc0 = replay_stream(plan, st, &cs); if (rc0) return rc0; }
-  if (metrics) SMD_CUDA(cudaMemsetAsync(metrics, 0, sizeof(float) * 4 * K, cs));
-  { const int rc0 = ensure_film_table(plan, params, 8, 5, cs); if (rc0) return rc0; }
-  int* t_ptr = plan->at<int>(plan->reg.t_ptr);
-  const int i0 = K - 1;
-  SMD_CUDA(cudaMemcpyAsync(t_ptr, &i0, sizeof(int), cudaMemcpyHostToDevice, cs));
-  SMD_CUDA(cudaStreamSynchronize(cs));  // i0 is a stack variable
-  if (!use_graph) {
-    for (int i = 0; i < K; ++i) {
-      const int rc = ddim_step(plan, params, x, n, infill_x, infill_mask, collection, metrics, cs);
-      if (rc) return rc;
-    }
-    return SMD_OK;
-  }
-  const GraphKey key = graph_key(n, params, x, infill_x, infill_mask, collection, metrics);
-  if (!plan->chain_graph.replays(key)) {
-    const int rc = plan->chain_graph.capture(cs, key, [&] {
-      return ddim_step(plan, params, x, n, infill_x, infill_mask, collection, metrics, cs);
-    }, "ddim graph");
-    if (rc) return rc;
-  }
-  for (int i = 0; i < K; ++i) {
-    const int rc = plan->chain_graph.launch(cs);
-    if (rc) return rc;
-  }
-  return join_replay(plan, st, cs);
+  const int rc = check_chain_call(plan, "smd_ddim_sample", kChainDdim, n, infill_x, infill_mask);
+  if (rc) return rc;
+  const int K = plan->chain.rows;
+  auto step = [&](cudaStream_t s) {
+    return ddim_step(plan, params, x, n, infill_x, infill_mask, collection, metrics, s);
+  };
+  return run_chain(plan, params, static_cast<cudaStream_t>(stream), use_graph, metrics, 8, 5, K,
+                   graph_key(n, params, x, infill_x, infill_mask, collection, metrics), "ddim graph",
+                   [&](cudaStream_t s) { return set_step_counter(plan, K - 1, s); }, step, step, no_epilogue);
 }
 
 // ---- DDIM encoder (Song et al. 2021, sections 4.3 and 5.4): the eta = 0 chain run from data towards noise -------------
@@ -1491,14 +1512,8 @@ int smd_ddim_encode_setup(smd_plan* plan, const float* host_betas, int T, const 
   std::vector<float> rows(coef.size());
   for (int i = 0; i < K; ++i)
     memcpy(&rows[static_cast<size_t>(K - 1 - i) * 8], &coef[static_cast<size_t>(i) * 8], 8 * sizeof(float));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  SMD_CUDA(cudaMemcpyAsync(plan->at<float>(plan->reg.coef), rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, st));
-  SMD_CUDA(cudaStreamSynchronize(st));  // the host table goes out of scope
-  plan->T = K;
-  plan->chain = kChainDdimEncode;
-  plan->film_tab_ready = false;
-  plan->chain_graph.drop();
-  return SMD_OK;
+  return install_chain(plan, kChainDdimEncode, K, rows.data(), 8, nullptr, nullptr, 0,
+                       static_cast<cudaStream_t>(stream));
 }
 
 // One encoder step at the device row r = *t_ptr = K-1-i: network call on sqrt(a) (FiLM table row r, or the generator on
@@ -1516,9 +1531,7 @@ static int ddim_encode_step(smd_plan* plan, const float* params, float* x, int n
   memset(&a, 0, sizeof(a));
   a.x = x; a.eps_hat = eh; a.coef = coef; a.r_ptr = t_ptr; a.x_next = x;
   a.N = n;
-  // the state axes of chain_geometry: (N, D) states of the dense networks use S = D, C = 1
-  a.S = plan->cfg.seq_len; a.C = plan->cfg.channels;
-  if (plan->cfg.arch != SMD_ARCH_TRANSFORMER_DDPM) { a.S = plan->cfg.channels; a.C = 1; }
+  state_axes(plan, a);
   launch_ddim_encode_step(a, st); CNT();
   launch_step_advance(t_ptr, st); CNT();
   SMD_LAUNCH_CHECK("ddim_encode_step");
@@ -1526,37 +1539,13 @@ static int ddim_encode_step(smd_plan* plan, const float* params, float* x, int n
 }
 
 int smd_ddim_encode(smd_plan* plan, const float* params, float* x, int n, int use_graph, smd_stream_t stream) {
-  if (!plan) { set_error("null plan"); return SMD_ERR_INVALID; }
-  if (reject_mdn(plan, "smd_ddim_encode")) return SMD_ERR_INVALID;
-  if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
-  if (plan->chain != kChainDdimEncode) { set_error("smd_ddim_encode_setup has not been called"); return SMD_ERR_STATE; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int K = plan->T;
-  cudaStream_t cs = st;
-  if (use_graph) { const int rc0 = replay_stream(plan, st, &cs); if (rc0) return rc0; }
-  { const int rc0 = ensure_film_table(plan, params, 8, 4, cs); if (rc0) return rc0; }
-  int* t_ptr = plan->at<int>(plan->reg.t_ptr);
-  const int r0 = K - 1;
-  SMD_CUDA(cudaMemcpyAsync(t_ptr, &r0, sizeof(int), cudaMemcpyHostToDevice, cs));
-  SMD_CUDA(cudaStreamSynchronize(cs));  // r0 is a stack variable
-  if (!use_graph) {
-    for (int i = 0; i < K; ++i) {
-      const int rc = ddim_encode_step(plan, params, x, n, cs);
-      if (rc) return rc;
-    }
-    return SMD_OK;
-  }
-  const GraphKey key = graph_key(n, params, x);
-  if (!plan->chain_graph.replays(key)) {
-    const int rc = plan->chain_graph.capture(cs, key, [&] { return ddim_encode_step(plan, params, x, n, cs); },
-                                             "ddim encode graph");
-    if (rc) return rc;
-  }
-  for (int i = 0; i < K; ++i) {
-    const int rc = plan->chain_graph.launch(cs);
-    if (rc) return rc;
-  }
-  return join_replay(plan, st, cs);
+  const int rc = check_chain_call(plan, "smd_ddim_encode", kChainDdimEncode, n, nullptr, nullptr);
+  if (rc) return rc;
+  const int K = plan->chain.rows;
+  auto step = [&](cudaStream_t s) { return ddim_encode_step(plan, params, x, n, s); };
+  return run_chain(plan, params, static_cast<cudaStream_t>(stream), use_graph, nullptr, 8, 4, K,
+                   graph_key(n, params, x), "ddim encode graph",
+                   [&](cudaStream_t s) { return set_step_counter(plan, K - 1, s); }, step, step, no_epilogue);
 }
 
 // ---- Langevin chain (annealed / consistent Langevin dynamics, utils/ebm_utils.py:89-271) ----------------------------
@@ -1613,18 +1602,14 @@ int smd_langevin_setup(smd_plan* plan, const float* host_sigmas, int L, int step
   const int rc = langevin_tables(host_sigmas, L, steps_per_level, epsilon, kind, coef.data(), idx);
   if (rc) return rc;
   if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  SMD_CUDA(cudaMemcpyAsync(plan->at<float>(plan->reg.coef), coef.data(), coef.size() * 4, cudaMemcpyHostToDevice, st));
-  SMD_CUDA(cudaMemcpyAsync(plan->at<int>(plan->reg.slots), idx, sizeof(idx), cudaMemcpyHostToDevice, st));
-  SMD_CUDA(cudaStreamSynchronize(st));  // host tables go out of scope
-  plan->T = L;
-  plan->lv_kind = kind;
-  plan->lv_steps = kind == 0 ? steps_per_level : 1;
-  plan->lv_key[0] = host_key[0]; plan->lv_key[1] = host_key[1];
-  plan->lv_sigma_last = host_sigmas[L - 1];
-  plan->chain = kChainLangevin;
-  plan->film_tab_ready = false;
-  plan->chain_graph.drop();
+  const int rc2 = install_chain(plan, kChainLangevin, L, coef.data(), kLangevinCoef, nullptr, idx, kLangevinCollect,
+                                static_cast<cudaStream_t>(stream));
+  if (rc2) return rc2;
+  ChainSetup& c = plan->chain;
+  c.lv_kind = kind;
+  c.steps = kind == 0 ? steps_per_level : 1;
+  c.key[0] = host_key[0]; c.key[1] = host_key[1];
+  c.sigma_last = host_sigmas[L - 1];
   return SMD_OK;
 }
 
@@ -1652,33 +1637,28 @@ static LangevinStepArgs langevin_args(const smd_plan* plan, const float* x, int 
 int smd_langevin_sample(smd_plan* plan, const float* params, float* x, int n, const float* infill_x,
                         const float* infill_mask, int denoise, float* collection, float* metrics, int use_graph,
                         smd_stream_t stream) {
-  if (!plan) { set_error("null plan"); return SMD_ERR_INVALID; }
-  if (reject_mdn(plan, "smd_langevin_sample")) return SMD_ERR_INVALID;
-  if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
-  if ((infill_x == nullptr) != (infill_mask == nullptr)) { set_error("infill_x and infill_mask go together"); return SMD_ERR_INVALID; }
-  if (plan->chain != kChainLangevin) { set_error("smd_langevin_setup has not been called"); return SMD_ERR_STATE; }
-  if (plan->lv_kind == 1 && (infill_x || collection)) {
+  const int rc = check_chain_call(plan, "smd_langevin_sample", kChainLangevin, n, infill_x, infill_mask);
+  if (rc) return rc;
+  if (plan->chain.lv_kind == 1 && (infill_x || collection)) {
     set_error("consistent Langevin dynamics has no infilling and no collection");
     return SMD_ERR_INVALID;
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int L = plan->T, T = plan->lv_steps, kind = plan->lv_kind;
+  const int L = plan->chain.rows, T = plan->chain.steps, kind = plan->chain.lv_kind;
   const int rows = kLangevinCollect + 1 + (denoise ? 1 : 0);
   float* coef = plan->at<float>(plan->reg.coef);
   const int* idx = plan->at<int>(plan->reg.slots);
   float* tvec = plan->at<float>(plan->reg.tvec);
   LangevinChainState* cst = plan->at<LangevinChainState>(plan->reg.t_ptr);
-  cudaStream_t cs = st;
-  if (use_graph) { const int rc0 = replay_stream(plan, st, &cs); if (rc0) return rc0; }
-  if (metrics) SMD_CUDA(cudaMemsetAsync(metrics, 0, sizeof(float) * 4 * L * T, cs));
-  { const int rc0 = ensure_film_table(plan, params, kLangevinCoef, 0, cs); if (rc0) return rc0; }
   // the chain starts from the setup key at step 0 on every call
-  LangevinChainState init;
-  memset(&init, 0, sizeof(init));
-  init.chain[0] = plan->lv_key[0]; init.chain[1] = plan->lv_key[1];
-  SMD_CUDA(cudaMemcpyAsync(cst, &init, sizeof(init), cudaMemcpyHostToDevice, cs));
-  SMD_CUDA(cudaStreamSynchronize(cs));  // init is a stack variable
-  launch_langevin_advance(cst, coef, collection ? idx : nullptr, tvec, L, T, kind, rows, 0, cs); CNT();
+  auto prologue = [&](cudaStream_t s) -> int {
+    LangevinChainState init;
+    memset(&init, 0, sizeof(init));
+    init.chain[0] = plan->chain.key[0]; init.chain[1] = plan->chain.key[1];
+    SMD_CUDA(cudaMemcpyAsync(cst, &init, sizeof(init), cudaMemcpyHostToDevice, s));
+    SMD_CUDA(cudaStreamSynchronize(s));  // init is a stack variable
+    launch_langevin_advance(cst, coef, collection ? idx : nullptr, tvec, L, T, kind, rows, 0, s); CNT();
+    return SMD_OK;
+  };
   // one step: network call -> update (state on the device) -> derive the next step's keys, level, row and sigma
   auto step = [&](cudaStream_t s) -> int {
     const int r = langevin_forward(plan, params, x, n, -1, s);
@@ -1692,35 +1672,23 @@ int smd_langevin_sample(smd_plan* plan, const float* params, float* x, int n, co
     SMD_LAUNCH_CHECK("langevin chain step");
     return SMD_OK;
   };
-  const long long total_steps = static_cast<long long>(L) * T;
-  if (!use_graph) {
-    for (long long i = 0; i < total_steps; ++i) {
-      const int rc = step(cs);
-      if (rc) return rc;
-    }
-  } else {
-    const GraphKey key = graph_key(n, params, x, infill_x, infill_mask, collection, metrics, rows);
-    if (!plan->chain_graph.replays(key)) {
-      const int rc = plan->chain_graph.capture(cs, key, [&] { return step(cs); }, "langevin graph");
-      if (rc) return rc;
-    }
-    for (long long i = 0; i < total_steps; ++i) {
-      const int rc = plan->chain_graph.launch(cs);
-      if (rc) return rc;
-    }
-  }
-  if (denoise) {
-    // x += sigma_L^2 model(x, sigma_L) (utils/ebm_utils.py:193-196, 265-266); the annealed chain also writes collection[-1]
-    SMD_CUDA(cudaMemcpyAsync(tvec, coef + static_cast<size_t>(L - 1) * kLangevinCoef, 4, cudaMemcpyDeviceToDevice, cs));
-    const int r = langevin_forward(plan, params, x, n, L - 1, cs);
+  // x += sigma_L^2 model(x, sigma_L) (utils/ebm_utils.py:193-196, 265-266); the annealed chain also writes collection[-1]
+  auto denoise_step = [&](cudaStream_t s) -> int {
+    if (!denoise) return SMD_OK;
+    SMD_CUDA(cudaMemcpyAsync(tvec, coef + static_cast<size_t>(L - 1) * kLangevinCoef, 4, cudaMemcpyDeviceToDevice, s));
+    const int r = langevin_forward(plan, params, x, n, L - 1, s);
     if (r) return r;
     LangevinStepArgs a = langevin_args(plan, x, n, /*sharded=*/false);
-    a.alpha = plan->lv_sigma_last * plan->lv_sigma_last;
+    a.alpha = plan->chain.sigma_last * plan->chain.sigma_last;
     a.collection_slot = collection ? collection + static_cast<size_t>(rows - 1) * n * a.S * a.C : nullptr;
-    launch_langevin_step(a, cs); CNT();
+    launch_langevin_step(a, s); CNT();
     SMD_LAUNCH_CHECK("langevin denoise");
-  }
-  return join_replay(plan, st, cs);
+    return SMD_OK;
+  };
+  return run_chain(plan, params, static_cast<cudaStream_t>(stream), use_graph, metrics, kLangevinCoef, 0,
+                   static_cast<long long>(L) * T,
+                   graph_key(n, params, x, infill_x, infill_mask, collection, metrics, rows), "langevin graph",
+                   prologue, step, step, denoise_step);
 }
 
 int smd_threefry_normal_slice(const uint32_t host_key[2], float* out, long long n, long long first, long long total,

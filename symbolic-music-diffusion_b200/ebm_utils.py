@@ -34,30 +34,41 @@ def diffusion_dynamics(rng, model, betas, init, epsilon, T, denoise, infill=Fals
 
     epsilon / T / denoise are null parameters upstream too.  The whole chain runs on the GPU (CUDA-graph replay of
     one reverse step); the noise of every step comes from `rng` with the reference's three splits per step."""
-    from .nn import _as_device_f32
     del epsilon, T, denoise
+    betas = np.asarray(betas, np.float32)
+
+    def run(eng, x, ix, im, collection, metrics):
+        eng.sampler_setup(betas, key=(int(rng[0]), int(rng[1])))
+        eng.sample(x, steps=len(betas), infill_x=ix, infill_mask=im, collection=collection, metrics=metrics,
+                   use_graph=True)
+    x, collection, metrics = _device_chain(model, init, shard, (4, len(betas)), 41, infill, infill_samples,
+                                           infill_masks, run)
+    return x, collection, metrics.unsqueeze(2)
+
+
+def _device_chain(model, init, shard, metrics_shape, collection_rows, infill, infill_samples, infill_masks, run):
+    """What the sampler chains on the GPU share: x = a device copy of `init`, the engine for its batch with the shard
+    (first_row, total_rows) set (`init` holds this rank's rows of a global batch; the per-step noise is the same slice
+    of the global threefry stream), a collection of `collection_rows` rows (0: none) whose row 0 is the start, zeroed
+    metrics; run(eng, x, infill_x, infill_mask, collection, metrics) sets up and runs the chain, then the batch-mean
+    metrics are reduced over ranks.  Returns (x, collection, metrics)."""
+    from .nn import _as_device_f32
     x = _as_device_f32(init).clone()
     n = x.shape[0]
     eng = model.engine(n)
-    betas = np.asarray(betas, np.float32)
-    eng.sampler_setup(betas, key=(int(rng[0]), int(rng[1])))
-    # shard = (first_row, total_rows): `init` holds this rank's rows of a global batch; the per-step noise is the same
-    # slice of the global threefry stream and the batch-mean metrics are reduced over ranks below
     eng.set_sampler_shard(*(shard if shard is not None else (0, 0)))
-    ix = im = None
-    collection = torch.zeros((41,) + tuple(x.shape), dtype=torch.float32, device=x.device)
-    if infill:
-        ix = _as_device_f32(infill_samples)
-        im = _as_device_f32(infill_masks)
+    ix = _as_device_f32(infill_samples) if infill else None
+    im = _as_device_f32(infill_masks) if infill else None
+    collection = None
+    if collection_rows:
+        collection = torch.zeros((collection_rows,) + tuple(x.shape), dtype=torch.float32, device=x.device)
         # utils/ebm_utils.py:321-323,398: the merged start only goes to collection[0]; the scan itself starts from the
         # raw `init` (the first step's blend overwrites the masked entries anyway)
-        collection[0] = x * (1 - im) + ix * im
-    else:
-        collection[0] = x
-    metrics = torch.zeros((4, len(betas)), dtype=torch.float32, device=x.device)
-    eng.sample(x, steps=len(betas), infill_x=ix, infill_mask=im, collection=collection, metrics=metrics, use_graph=True)
+        collection[0] = x * (1 - im) + ix * im if infill else x
+    metrics = torch.zeros(metrics_shape, dtype=torch.float32, device=x.device)
+    run(eng, x, ix, im, collection, metrics)
     _reduce_sharded_metrics(metrics, n, shard)
-    return x, collection, metrics.unsqueeze(2)
+    return x, collection, metrics
 
 
 DDIM_SCHEDULES = ("uniform", "quadratic")
@@ -93,26 +104,15 @@ def ddim_dynamics(rng, model, betas, init, epsilon, T, denoise, infill=False, in
     T levels: diffusion_dynamics itself).  Not in the reference.  Returns (state, collection (41, N, *shape),
     ld_metrics (4, steps, 1)); keys, collection rows, infill and shard as diffusion_dynamics with T replaced by the
     number of steps.  epsilon / T / denoise are null, as there."""
-    from .nn import _as_device_f32
     del epsilon, T, denoise
-    x = _as_device_f32(init).clone()
-    n = x.shape[0]
-    eng = model.engine(n)
     betas = np.asarray(betas, np.float32)
     tau = ddim_schedule(len(betas), steps, schedule)
-    eng.ddim_setup(betas, tau, eta, key=(int(rng[0]), int(rng[1])))
-    eng.set_sampler_shard(*(shard if shard is not None else (0, 0)))
-    ix = im = None
-    collection = torch.zeros((41,) + tuple(x.shape), dtype=torch.float32, device=x.device)
-    if infill:
-        ix = _as_device_f32(infill_samples)
-        im = _as_device_f32(infill_masks)
-        collection[0] = x * (1 - im) + ix * im
-    else:
-        collection[0] = x
-    metrics = torch.zeros((4, len(tau)), dtype=torch.float32, device=x.device)
-    eng.ddim_sample(x, infill_x=ix, infill_mask=im, collection=collection, metrics=metrics, use_graph=True)
-    _reduce_sharded_metrics(metrics, n, shard)
+
+    def run(eng, x, ix, im, collection, metrics):
+        eng.ddim_setup(betas, tau, eta, key=(int(rng[0]), int(rng[1])))
+        eng.ddim_sample(x, infill_x=ix, infill_mask=im, collection=collection, metrics=metrics, use_graph=True)
+    x, collection, metrics = _device_chain(model, init, shard, (4, len(tau)), 41, infill, infill_samples,
+                                           infill_masks, run)
     return x, collection, metrics.unsqueeze(2)
 
 
@@ -199,23 +199,15 @@ def annealed_langevin_dynamics(rng, model, sigmas, init, epsilon, T, denoise, in
     The whole chain runs on the GPU (smd_langevin_sample: CUDA-graph replay of one step, keys from the scan carry
     `rng, step_rng, infill_rng = split(rng, 3)` derived on the device).  shard = (first_row, total_rows) as in
     diffusion_dynamics: `init` holds this rank's rows of a global batch."""
-    from .nn import _as_device_f32
-    x = _as_device_f32(init).clone()
-    n = x.shape[0]
-    eng = model.engine(n)
     sig = np.asarray(sigmas, np.float32)
     assert len(sig) >= 2
-    ix = _as_device_f32(infill_samples) if infill else None
-    im = _as_device_f32(infill_masks) if infill else None
-    L = len(sig)
-    collection = torch.zeros((101 + int(bool(denoise)),) + tuple(x.shape), dtype=torch.float32, device=x.device)
-    collection[0] = x * (1 - im) + ix * im if infill else x
-    metrics = torch.zeros((4, L, int(T)), dtype=torch.float32, device=x.device)
-    eng.langevin_setup(sig, int(T), epsilon, "ald", key=(int(rng[0]), int(rng[1])))
-    eng.set_sampler_shard(*(shard if shard is not None else (0, 0)))
-    eng.langevin_sample(x, denoise=bool(denoise), infill_x=ix, infill_mask=im, collection=collection, metrics=metrics)
-    _reduce_sharded_metrics(metrics, n, shard)
-    return x, collection, metrics
+
+    def run(eng, x, ix, im, collection, metrics):
+        eng.langevin_setup(sig, int(T), epsilon, "ald", key=(int(rng[0]), int(rng[1])))
+        eng.langevin_sample(x, denoise=bool(denoise), infill_x=ix, infill_mask=im, collection=collection,
+                            metrics=metrics)
+    return _device_chain(model, init, shard, (4, len(sig), int(T)), 101 + int(bool(denoise)), infill, infill_samples,
+                         infill_masks, run)
 
 
 def consistent_langevin_dynamics(rng, model, sigmas, init, epsilon, T, denoise=True, infill=False, infill_samples=None,
@@ -224,18 +216,13 @@ def consistent_langevin_dynamics(rng, model, sigmas, init, epsilon, T, denoise=T
     x += alpha * score + beta * sigma_{i+1} * z.  Returns (state, None, metrics (4, L, 1)) -- upstream returns two values
     although its caller unpacks three (SURVEY section 0); the missing collection is returned as None.  Runs on the GPU
     like annealed_langevin_dynamics (keys `rng, step_rng = split(rng)`); shard as there."""
-    from .nn import _as_device_f32
     del T
     if infill:
         raise NotImplementedError
-    x = _as_device_f32(init).clone()
-    n = x.shape[0]
-    eng = model.engine(n)
     sig = np.asarray(sigmas, np.float32)
     assert len(sig) >= 2
-    metrics = torch.zeros((4, len(sig), 1), dtype=torch.float32, device=x.device)
-    eng.langevin_setup(sig, 1, epsilon, "cas", key=(int(rng[0]), int(rng[1])))
-    eng.set_sampler_shard(*(shard if shard is not None else (0, 0)))
-    eng.langevin_sample(x, denoise=bool(denoise), metrics=metrics)
-    _reduce_sharded_metrics(metrics, n, shard)
-    return x, None, metrics
+
+    def run(eng, x, ix, im, collection, metrics):
+        eng.langevin_setup(sig, 1, epsilon, "cas", key=(int(rng[0]), int(rng[1])))
+        eng.langevin_sample(x, denoise=bool(denoise), metrics=metrics)
+    return _device_chain(model, init, shard, (4, len(sig), 1), 0, False, None, None, run)

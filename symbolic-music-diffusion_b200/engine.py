@@ -55,6 +55,18 @@ def _f32c(t: torch.Tensor, name: str) -> torch.Tensor:
     return t
 
 
+def _f32c_optional(**tensors) -> None:
+    """_f32c on each of the keyword tensors that is not None."""
+    for name, t in tensors.items():
+        if t is not None:
+            _f32c(t, name)
+
+
+def _key(key):
+    """A jax PRNG key (two integers) as the uint32[2] the C ABI takes; None stays None."""
+    return None if key is None else (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
+
+
 class Engine:
     def __init__(self, cfg: ModelConfig, max_batch: int, cta_group: int = 2, training: bool = False,
                  device: Optional[str] = None, sampler_T: Optional[int] = None, precision: Optional[str] = None):
@@ -243,7 +255,7 @@ class Engine:
         out = [torch.empty((batch,), dtype=torch.float32, device=dev)]
         out += [torch.empty(shape, dtype=torch.float32, device=dev) for _ in range(2 if rademacher else 1)]
         labels = torch.empty((batch,), dtype=torch.int32, device=dev) if want_labels else None
-        k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
+        k = _key(key)
         _lib.check(fn(self._plan, k, int(global_batch or batch), int(first_row), batch, 1 if continuous_noise else 0,
                       *[t.data_ptr() for t in out], _ptr(labels), self._stream()))
         return tuple(out) + (labels,) if want_labels else tuple(out)
@@ -309,10 +321,10 @@ class Engine:
                       collection_slot=None, metrics4=None):
         x = _f32c(x, "x"); grad = _f32c(grad, "grad")
         x_next = torch.empty_like(x) if x_next is None else x_next
-        mk = lambda k: None if k is None else (C.c_uint32 * 2)(int(k[0]) & 0xFFFFFFFF, int(k[1]) & 0xFFFFFFFF)
         _lib.check(self.lib.smd_langevin_step(self._plan, x.data_ptr(), grad.data_ptr(), x.shape[0], float(alpha),
-                                              float(noise_coef), mk(step_key), _ptr(z), _ptr(infill_x), _ptr(infill_mask),
-                                              float(infill_sigma), mk(infill_key), _ptr(infill_z), x_next.data_ptr(),
+                                              float(noise_coef), _key(step_key), _ptr(z), _ptr(infill_x),
+                                              _ptr(infill_mask),
+                                              float(infill_sigma), _key(infill_key), _ptr(infill_z), x_next.data_ptr(),
                                               _ptr(collection_slot), _ptr(metrics4), self._stream()))
         return x_next
 
@@ -355,7 +367,7 @@ class Engine:
         out = torch.empty((n, S, Cc), dtype=torch.float32, device=dev)
         ch = torch.empty_like(out) if chain else None
         comp = torch.empty((n, S), dtype=torch.int32, device=dev) if components else None
-        k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
+        k = _key(key)
         _lib.check(self.lib.smd_mdn_sample(self._plan, self.params.data_ptr(), k, int(n), int(first_row),
                                            int(total_rows), out.data_ptr(), _ptr(ch), _ptr(comp), self._stream()))
         res = (out,) + ((ch,) if chain else ()) + ((comp,) if components else ())
@@ -374,7 +386,7 @@ class Engine:
         rows = pi.numel() // kc
         out = torch.empty(tuple(pi.shape[:-1]) + (Cc,), dtype=torch.float32, device=pi.device)
         comp = torch.empty(tuple(pi.shape[:-1]), dtype=torch.int32, device=pi.device) if components else None
-        k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
+        k = _key(key)
         _lib.check(self.lib.smd_mdn_mixture_sample(pi.data_ptr(), mu.data_ptr(), log_sigma.data_ptr(), rows, Cc, kc, k,
                                                    int(first_row), int(total_rows), out.data_ptr(), _ptr(comp),
                                                    self._stream()))
@@ -466,7 +478,7 @@ class Engine:
     def sampler_setup(self, betas: np.ndarray, key=(0, 0)) -> None:
         self._ensure_ws()
         b = np.ascontiguousarray(betas, np.float32)
-        k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
+        k = _key(key)
         _lib.check(self.lib.smd_sampler_setup(self._plan, b.ctypes.data_as(C.POINTER(C.c_float)), len(b), k,
                                               self._stream()))
         self._sampler_T = len(b)
@@ -490,6 +502,7 @@ class Engine:
                metrics=None, use_graph: bool = True):
         """Runs `steps` reverse steps in place on x (n, S, C)."""
         x = _f32c(x, "x")
+        _f32c_optional(infill_x=infill_x, infill_mask=infill_mask, collection=collection, metrics=metrics)
         steps = self._sampler_T if steps is None else int(steps)
         _lib.check(self.lib.smd_ddpm_sample(self._plan, self.params.data_ptr(), x.data_ptr(), x.shape[0], steps,
                                             _ptr(infill_x), _ptr(infill_mask), _ptr(collection), _ptr(metrics),
@@ -502,7 +515,7 @@ class Engine:
         self._ensure_ws()
         b = np.ascontiguousarray(betas, np.float32)
         s = np.ascontiguousarray(steps, np.int32)
-        k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
+        k = _key(key)
         _lib.check(self.lib.smd_ddim_setup(self._plan, b.ctypes.data_as(C.POINTER(C.c_float)), len(b),
                                            s.ctypes.data_as(C.POINTER(C.c_int)), len(s), float(eta), k,
                                            self._stream()))
@@ -511,10 +524,7 @@ class Engine:
         """Runs the whole DDIM chain of ddim_setup in place on x.  collection: (41, n, ...) with row 0 left to the
         caller; metrics: (4, K)."""
         x = _f32c(x, "x")
-        for t, name in ((infill_x, "infill_x"), (infill_mask, "infill_mask"), (collection, "collection"),
-                        (metrics, "metrics")):
-            if t is not None:
-                _f32c(t, name)
+        _f32c_optional(infill_x=infill_x, infill_mask=infill_mask, collection=collection, metrics=metrics)
         _lib.check(self.lib.smd_ddim_sample(self._plan, self.params.data_ptr(), x.data_ptr(), x.shape[0],
                                             _ptr(infill_x), _ptr(infill_mask), _ptr(collection), _ptr(metrics),
                                             1 if use_graph else 0, self._stream()))
@@ -547,7 +557,7 @@ class Engine:
             raise ValueError(f"unknown Langevin sampler {kind!r} (expected one of {sorted(self.LANGEVIN_KINDS)})")
         self._ensure_ws()
         s = np.ascontiguousarray(sigmas, np.float32)
-        k = (C.c_uint32 * 2)(int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF)
+        k = _key(key)
         _lib.check(self.lib.smd_langevin_setup(self._plan, s.ctypes.data_as(C.POINTER(C.c_float)), len(s),
                                                int(steps_per_level), float(epsilon), self.LANGEVIN_KINDS[kind], k,
                                                self._stream()))
@@ -557,10 +567,7 @@ class Engine:
         """Runs the whole Langevin chain of langevin_setup in place on x, then the denoising step if ``denoise``.
         collection (annealed only): (101 + denoise, n, ...) with row 0 left to the caller; metrics: (4, L, T)."""
         x = _f32c(x, "x")
-        for t, name in ((infill_x, "infill_x"), (infill_mask, "infill_mask"), (collection, "collection"),
-                        (metrics, "metrics")):
-            if t is not None:
-                _f32c(t, name)
+        _f32c_optional(infill_x=infill_x, infill_mask=infill_mask, collection=collection, metrics=metrics)
         _lib.check(self.lib.smd_langevin_sample(self._plan, self.params.data_ptr(), x.data_ptr(), x.shape[0],
                                                 _ptr(infill_x), _ptr(infill_mask), 1 if denoise else 0,
                                                 _ptr(collection), _ptr(metrics), 1 if use_graph else 0,

@@ -259,6 +259,12 @@ def test_setups_invalidate_each_other(lib):
     with pytest.raises(L.SmdError, match="smd_ddim_setup"):
         eng.ddim_sample(x.clone())
     eng.langevin_sample(x.clone())
+    eng.sampler_setup(BETAS, key=(0, 1))
+    for half in (dict(infill_x=x), dict(infill_mask=torch.ones_like(x))):
+        with pytest.raises(ValueError, match="infill_x and infill_mask go together"):
+            eng.sample(x.clone(), steps=3, **half)
+        with pytest.raises(ValueError, match="infill_x and infill_mask go together"):
+            eng.reverse_step(x.clone(), 2, **half)
     eng.ddim_setup(BETAS, steps, 0.0)
     with pytest.raises(ValueError, match="n out of range"):
         eng.ddim_sample(torch.zeros((16,) + shape, device="cuda"))
