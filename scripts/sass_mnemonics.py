@@ -10,7 +10,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "symbolic-music-diffusion_b200", "libsmd.so")
-KEYS = ["HGMMA", "HGMMA.64x256x16", "UTMALDG", "UTMASTG", "SYNCS", "HMMA", "MUFU.TANH", "LDGSTS", "UBLKCP", "ACQBULK", "RED", "ATOM",
+KEYS = ["HGMMA", "HGMMA.64x256x16", "HGMMA.64x32x16", "UTMALDG", "UTMASTG", "SYNCS", "HMMA", "MUFU.TANH", "LDGSTS", "UBLKCP", "ACQBULK", "RED", "ATOM",
         "USETMAXREG", "STL", "LDL"]
 
 

@@ -50,7 +50,9 @@ inline bool make_tmap_bf16(CUtensorMap* out, const void* base, uint64_t rows, ui
 struct GemmOp {
   CUtensorMap tmA, tmB;
   CUtensorMap tmA_lo, tmB_lo;   // strict-precision mode: the lo halves of both operands (has_lo)
+  CUtensorMap tmX;              // swapped-operand layout (has_swap): A with 32-row boxes (B: tmB)
   bool has_lo = false;
+  bool has_swap = false;
   int N = 0, K = 0, BN = 0, a_mn = 0, b_mn = 0, k_splits = 1;
 };
 
@@ -85,6 +87,13 @@ inline bool make_gemm_op(GemmOp* op, const void* A, uint64_t a_rows, const void*
   if (!ok) return false;
   if (!b_mn) ok = make_tmap_bf16(&op->tmB, B, b_rows_total, static_cast<uint64_t>(K), static_cast<uint32_t>(BN < kBNMax ? BN : kBNMax));
   else ok = make_tmap_bf16(&op->tmB, B, k_rows_b ? k_rows_b : static_cast<uint64_t>(K), b_rows_total, 64, b_pitch);
+  // 128 output columns with K-major token rows: the swapped-operand layout (gemm_bf16_wgmma_swap_kernel) serves the
+  // launches gemm_kind gives it.  Not in strict-precision mode, whose three-pass launches swap tmA / tmB for the lo
+  // halves.
+  if (ok && N == kBNMax && BN == kBNMax && !a_mn && !lo_bytes) {
+    ok = make_tmap_bf16(&op->tmX, A, a_rows, static_cast<uint64_t>(K), GemmSmemSwap::kTok);
+    op->has_swap = ok;
+  }
   return ok;
 }
 
@@ -171,6 +180,7 @@ struct GemmKind {
   uint32_t flags;
   int ew;
   bool wide = false;   // 128 x 256 tiles (GemmSmemWide); ew is then unused
+  bool swap = false;   // swapped operands, 32-token tiles (GemmSmemSwap); ew is then unused
 };
 // the 128-wide tiles a launch of an op built with BN = kBNWide runs when gemm_kind does not give it the wide layout
 inline GemmOp narrow_op(const GemmOp& op) {
@@ -196,6 +206,13 @@ inline GemmKind gemm_kind(const GemmOp& op, int M, const GemmEpilogue& ep) {
   }
   if (ep.lo_delta != 0) return {kEpiStrict, 8};   // strict-precision mode (bf16x3)
   const uint32_t need = epi_needs(ep);
+  // N = 128 with tokens as M: four times as many CTAs as 128 x 128 tiles, every row still whole in one CTA.  Measured
+  // (scripts/trunk_gemm_bench.py, H100 SXM): the LayerNorm kinds are faster at 4096 and at 32 000 tokens; the fp32
+  // (dX) kinds are as fast or faster while the 128 x 128 tiles fit in one round, and slower once those run several
+  // rounds with the dedicated-epilogue overlap (32 000 tokens, K >= 384).
+  if (op.has_swap && gemm_k_splits(op) == 1 && epi_clean(op, ep) && (need & ~kEpiSwap) == 0 &&
+      ((need & F_LN) || gemm_tiles(op, M) <= device_sm_count()))
+    return {kEpiSwap, 0, false, true};
   if (epi_clean(op, ep)) {
     auto fits = [&](uint32_t kind) { return (need & ~kind) == 0; };
     // short-K GEMMs are epilogue-bound: give them a third epilogue warp per row quadrant
@@ -262,8 +279,37 @@ inline cudaError_t launch_gemm_wide(const GemmOp& op, int M, const GemmEpilogue&
   return launch_persistent(gemm_bf16_wgmma_wide_kernel<kF>, tiles, SM::kThreads, SM::kTotal, st, op.tmA, op.tmB, sh, ep);
 }
 
+// one CTA per 32-token tile; programmatic dependent launch unless SMD_PDL=0
+inline cudaError_t launch_gemm_swap(const GemmOp& op, int M, const GemmEpilogue& ep, cudaStream_t st) {
+  using SM = GemmSmemSwap;
+  static bool attr_set = false;
+  if (!attr_set) {
+    for (auto k : {gemm_bf16_wgmma_swap_kernel<0>, gemm_bf16_wgmma_swap_kernel<1>}) {
+      const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kTotal);
+      if (e != cudaSuccess) return e;
+    }
+    attr_set = true;
+  }
+  GemmShape sh;
+  sh.M = M; sh.N = op.N; sh.K = op.K; sh.BN = op.N; sh.a_mn = 0; sh.b_mn = op.b_mn; sh.k_splits = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(static_cast<unsigned>(M > 0 ? (M + SM::kTok - 1) / SM::kTok : 1));
+  cfg.blockDim = dim3(SM::kThreads);
+  cfg.dynamicSmemBytes = SM::kTotal;
+  cfg.stream = st;
+  cudaLaunchAttribute attrs[1];
+  attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attrs[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attrs;
+  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return cudaLaunchKernelEx(&cfg, op.b_mn ? gemm_bf16_wgmma_swap_kernel<1> : gemm_bf16_wgmma_swap_kernel<0>, op.tmB,
+                            op.tmX, sh, ep);
+}
+
 inline cudaError_t launch_gemm(const GemmOp& wop, int M, const GemmEpilogue& ep, cudaStream_t st) {
   const GemmKind k = gemm_kind(wop, M, ep);
+  if (k.swap) return launch_gemm_swap(wop, M, ep, st);
   if (k.wide) {
     return k.flags == kEpiF32 ? launch_gemm_wide<kEpiF32>(wop, M, ep, st) : launch_gemm_wide<kEpiBf16>(wop, M, ep, st);
   }

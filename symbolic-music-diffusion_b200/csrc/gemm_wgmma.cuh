@@ -1108,4 +1108,201 @@ gemm_bf16_wgmma_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
   __syncthreads();
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Swapped-operand layout for GEMMs with N = 128 output columns and tokens as M (the trunk's out-projection, FFN down
+// and dX GEMMs).  128 x 128 tiles give such a launch only M / 128 CTAs (32 for 4096 tokens on 132 SMs).  Here the
+// weight's 128 output features are the wgmma M dimension (two consumer warpgroups x m64) and 32 tokens are its N
+// dimension (m64n32k16), so the launch runs M / 32 CTAs, two per SM:
+//
+//   D^T[128][32 tokens] = W^T[128][K] * X[32 tokens][K]^T
+//
+// W is the (in, out) weight read MN-major ([K][128], forward) or the plain weight read K-major ([128][K], dX), through
+// the op's B tensor map; X is the K-major activation / adjoint.  Each output element is still one fp32 chain over K in
+// the same k-block order, so the outputs are those of the 128 x 128 layout.  Every CTA reads the whole weight from L2
+// (64 MB per 4096-token launch at K = 2048): sharing it across a 2- or 4-CTA cluster by TMA multicast measured no
+// faster at 2 and slower at 4 (H100 SXM, 700 W).  A CTA owns whole 128-wide output rows, so the full-row LayerNorm
+// stays in the CTA: the accumulators are staged transposed ([token][feature]) in shared memory over the drained
+// operand ring, and eight threads per token row run bias, residual, LayerNorm and the coalesced fp32 / bf16 stores.
+// 288 threads: warps 0-7 are the consumer warpgroups (and the epilogue), warp 8 the TMA producer.
+struct GemmSmemSwap {
+  static constexpr int kTok = 32;                          // tokens per tile (the wgmma N)
+  static constexpr int kABytes = kBNMax * kBK * 2;         // 16 KB weight tile
+  static constexpr int kBBytes = kTok * kBK * 2;           // 4 KB activation tile
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kStages = 5;
+  static constexpr int kBarBytes = 128;
+  static constexpr int kOutPitch = kBNMax + 4;             // floats per staged token row: conflict-free fragment stores
+  static constexpr int kTotal = kStages * kStageBytes + kBarBytes + 1024;
+  static constexpr int kThreads = 288;
+  static_assert(kTok * kOutPitch * 4 <= kStages * kStageBytes, "the staged output tile must fit over the ring");
+  static_assert(2 * kStages * 8 <= kBarBytes, "mbarriers do not fit their region");
+  static_assert(2 * (kTotal + 1024) <= 233472, "two CTAs must fit in one SM's shared memory");
+};
+// the epilogue features of the swapped layout: bias, residual, fp32 out, bf16 out (plain or full-row LayerNorm)
+static constexpr uint32_t kEpiSwap = F_BIAS | F_RES | F_F32 | F_BF16 | F_LN;
+
+template <int kTA>
+__device__ __forceinline__ void swap_mainloop(float (&d)[16], uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                              int nkb, uint32_t wg, uint32_t lane) {
+  using SM = GemmSmemSwap;
+  // per-k16 advance of the weight descriptor: two 8-row atoms MN-major, 32 B inside a K-major row
+  const uint32_t a_kadv = kTA ? 2048u : 32u, a_lbo = kTA ? 8192u : 0u;
+  int stage = 0, prev = -1;
+  uint32_t phase = 0;
+  for (int kb = 0; kb < nkb; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t sA = smem_u32(smem + stage * SM::kStageBytes) + wg * 8192u;   // this warpgroup's 64 features
+    const uint32_t sB = smem_u32(smem + stage * SM::kStageBytes + SM::kABytes);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBK / 16; ++k)
+      wgmma_m64n32k16_bf16<kTA>(d, make_smem_desc_sw128(sA + k * a_kadv, a_lbo, 1024u),
+                                make_smem_desc_sw128(sB + k * 32u, 0u, 1024u), (kb | k) != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();                       // the previous k block's MMAs are done: its slot can be refilled
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    prev = stage;
+    if (++stage == SM::kStages) { stage = 0; phase ^= 1u; }
+  }
+  wgmma_wait<0>();
+  if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+}
+
+// tmW: the weight (the op's tmB: 128-row boxes K-major, 64 x 64 boxes MN-major); tmX: the activation [M][K], 32-row
+// boxes.  kTA: 1 = W is MN-major [K][128].  One token tile per CTA.
+template <int kTA>
+__global__ void __launch_bounds__(GemmSmemSwap::kThreads, 2)
+gemm_bf16_wgmma_swap_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX,
+                            const GemmShape sh, const __grid_constant__ GemmEpilogue ep) {
+  using SM = GemmSmemSwap;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SM::kStages * SM::kStageBytes);   // [kStages]
+  uint64_t* empty_bar = full_bar + SM::kStages;                                              // [kStages]
+  const uint32_t warp = threadIdx.x >> 5;
+  const uint32_t lane = threadIdx.x & 31;
+  const int m0 = static_cast<int>(blockIdx.x) * SM::kTok;
+  const int nkb = sh.K / kBK;
+
+  pdl_trigger();
+  if (warp == 8 && elect_one()) {
+    tma_prefetch_desc(&tmW);
+    tma_prefetch_desc(&tmX);
+  }
+  if (warp == 0 && elect_one()) {
+    for (int i = 0; i < SM::kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);   // one arrival per consumer warp
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (warp == 8) {
+    // ===================== TMA producer =====================
+    if (elect_one()) {
+      int stage = 0; uint32_t phase = 0;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1u);
+        uint8_t* sA = smem + stage * SM::kStageBytes;
+        const int k0 = kb * kBK;
+        mbar_arrive_expect_tx(&full_bar[stage], static_cast<uint32_t>(SM::kStageBytes));
+        if constexpr (kTA)
+          for (int j = 0; j < kBNMax / 64; ++j) tma_load_2d(&tmW, &full_bar[stage], sA + j * 8192, 64 * j, k0);
+        else tma_load_2d(&tmW, &full_bar[stage], sA, k0, 0);
+        tma_load_2d(&tmX, &full_bar[stage], sA + SM::kABytes, k0, m0);
+        if (++stage == SM::kStages) { stage = 0; phase ^= 1u; }
+      }
+    }
+  } else {
+    // ===================== consumer warpgroups: K loop, then the epilogue =====================
+    const uint32_t wg = warp >> 2;
+    float d[16];
+    swap_mainloop<kTA>(d, smem, full_bar, empty_bar, nkb, wg, lane);
+    // Every k block has landed and been read by both warpgroups: nothing writes the ring any more, the staged
+    // output tile [token][feature] may cover it.
+    float* out_tile = reinterpret_cast<float*>(smem);
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    {
+      // fragment: feature 64 wg + 16 (warp & 3) + lane / 4 + 8 h, token 8 j + 2 (lane & 3) + e  ->  d[4 j + 2 h + e]
+      const int f = static_cast<int>(wg * 64u + (warp & 3u) * 16u + (lane >> 2));
+      const int t = 2 * static_cast<int>(lane & 3u);
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) out_tile[(8 * j + t + e) * SM::kOutPitch + f + 8 * h] = d[4 * j + 2 * h + e];
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    // eight threads per token row; thread `sub` owns the 16-byte column chunks sub + 8 q (q < 4), so every global
+    // access instruction of a row's eight threads covers 128 contiguous fp32 bytes (64 bf16 bytes)
+    const int r = static_cast<int>(threadIdx.x >> 3), sub = static_cast<int>(threadIdx.x & 7u);
+    const int row = m0 + r;
+    const bool row_ok = row < sh.M;
+    float v[16];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int c = 4 * (sub + 8 * q);
+      const float4 a = *reinterpret_cast<const float4*>(out_tile + r * SM::kOutPitch + c);
+      v[4 * q] = a.x; v[4 * q + 1] = a.y; v[4 * q + 2] = a.z; v[4 * q + 3] = a.w;
+      if (ep.bias != nullptr) {
+        const float4 b = __ldg(reinterpret_cast<const float4*>(ep.bias + c));
+        add_pair(v[4 * q], v[4 * q + 1], b.x, b.y);
+        add_pair(v[4 * q + 2], v[4 * q + 3], b.z, b.w);
+      }
+      if (ep.residual != nullptr && row_ok) {
+        const float4 b = *reinterpret_cast<const float4*>(ep.residual + static_cast<size_t>(row) * ep.ld_res + c);
+        add_pair(v[4 * q], v[4 * q + 1], b.x, b.y);
+        add_pair(v[4 * q + 2], v[4 * q + 3], b.z, b.w);
+      }
+    }
+    if (ep.out_f32 != nullptr && row_ok) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        *reinterpret_cast<float4*>(ep.out_f32 + static_cast<size_t>(row) * ep.ld_f32 + 4 * (sub + 8 * q)) =
+            make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+    }
+    if (ep.out_bf16 != nullptr) {
+      float w[16];
+      if (ep.ln_gamma != nullptr) {
+        // full-row LayerNorm over the 128 columns the row's eight threads hold (flax: E[x^2] - E[x]^2, eps 1e-6)
+        float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) { s1 += v[i]; s2 = fmaf(v[i], v[i], s2); }
+#pragma unroll
+        for (int o = 1; o < 8; o <<= 1) {
+          s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+          s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+        }
+        const float inv_n = 1.0f / static_cast<float>(kBNMax);
+        const float mean = s1 * inv_n;
+        const float rstd = rsqrtf(s2 * inv_n - mean * mean + 1e-6f);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int c = 4 * (sub + 8 * q);
+          const float4 g = __ldg(reinterpret_cast<const float4*>(ep.ln_gamma + c));
+          const float4 b = __ldg(reinterpret_cast<const float4*>(ep.ln_beta + c));
+          w[4 * q] = (v[4 * q] - mean) * (rstd * g.x) + b.x;
+          w[4 * q + 1] = (v[4 * q + 1] - mean) * (rstd * g.y) + b.y;
+          w[4 * q + 2] = (v[4 * q + 2] - mean) * (rstd * g.z) + b.z;
+          w[4 * q + 3] = (v[4 * q + 3] - mean) * (rstd * g.w) + b.w;
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) w[i] = v[i];
+      }
+      if (row_ok) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+          *reinterpret_cast<uint2*>(ep.out_bf16 + static_cast<size_t>(row) * ep.ld_bf16 + 4 * (sub + 8 * q)) =
+              make_uint2(pack_bf16x2(w[4 * q], w[4 * q + 1]), pack_bf16x2(w[4 * q + 2], w[4 * q + 3]));
+      }
+    }
+  }
+  __syncwarp();
+  __syncthreads();
+}
+
 }  // namespace smd

@@ -140,6 +140,20 @@ __device__ __forceinline__ void wgmma_m64n256k16_bf16(float (&d)[128], uint64_t 
       : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(kTA), "n"(kTB));
 }
 
+// d[64 x 32] (+)= A[64 x 16] * B[16 x 32], B K-major: the m64n128k16 product over 32 columns.  Thread t holds d[i] at
+// the same (row, column) as in the n128 form, with i / 4 running over 4 column octets.
+template <int kTA>
+__device__ __forceinline__ void wgmma_m64n32k16_bf16(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(kTA));
+}
+
 // ---------------------------------------------------------------- per-warpgroup register budget
 // Hands registers back to / takes them from the CTA's pool; executed by all 128 threads of a warpgroup.
 template <int kRegs>
