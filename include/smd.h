@@ -421,6 +421,12 @@ int smd_threefry_split(const uint32_t host_key[2], int num, uint32_t* host_out_k
 int smd_gemm_bf16(const void* A, const void* B, int M, int N, int K, int a_mn, int b_mn, int BN, int cta_group,
                   const float* bias, const float* residual, int act, float* out_f32, void* out_bf16,
                   float* row_stats, const float* ln_gamma, const float* ln_beta, smd_stream_t stream);
+/* The same product with the epilogue pieces smd_gemm_bf16 does not take: out_bf16_pre (bf16 of v before the
+ * activation, pitch N), gelu_grad_of (bf16 [M][N]: v *= gelu'(x)), and per-tile row-statistics partials (stats_part,
+ * with row_stats set; *nslots receives the slots per row, may be NULL).  NULL skips a piece. */
+int smd_gemm_bf16_epi(const void* A, const void* B, int M, int N, int K, int a_mn, int b_mn, const float* bias,
+                      int act, float* out_f32, void* out_bf16, void* out_bf16_pre, const void* gelu_grad_of,
+                      float* row_stats, float* stats_part, int* nslots, smd_stream_t stream);
 /* forward pass that keeps every intermediate in the training save buffers (plan must have training = 1) */
 int smd_debug_forward_save(smd_plan* plan, const float* params, const float* x, const float* t, int batch, float* y,
                            smd_stream_t stream);

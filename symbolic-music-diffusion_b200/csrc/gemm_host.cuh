@@ -8,6 +8,7 @@
 #include <atomic>
 #include <string>
 #include "gemm_wgmma.cuh"
+#include "gemm_expand.cuh"
 #include "fused_wgmma.cuh"
 
 namespace smd {
@@ -181,6 +182,7 @@ struct GemmKind {
   int ew;
   bool wide = false;   // 128 x 256 tiles (GemmSmemWide); ew is then unused
   bool swap = false;   // swapped operands, 32-token tiles (GemmSmemSwap); ew is then unused
+  bool expand = false; // row-resident A, bulk-store epilogue (GemmSmemExpand); ew is then unused
 };
 // the 128-wide tiles a launch of an op built with BN = kBNWide runs when gemm_kind does not give it the wide layout
 inline GemmOp narrow_op(const GemmOp& op) {
@@ -213,6 +215,14 @@ inline GemmKind gemm_kind(const GemmOp& op, int M, const GemmEpilogue& ep) {
   if (op.has_swap && gemm_k_splits(op) == 1 && epi_clean(op, ep) && (need & ~kEpiSwap) == 0 &&
       ((need & F_LN) || gemm_tiles(op, M) <= device_sm_count()))
     return {kEpiSwap, 0, false, true};
+  // K <= 128 and N >= 384 (FFN up, its GELU adjoint, post dense, QKV): the launch is an output stream, which the
+  // row-resident layout writes with bulk stores while the next tile's wgmma runs.
+  if (!op.a_mn && op.K == GemmSmemExpand<kEpiF32>::kKMax && op.BN == kBNMax && op.N % (2 * kBNMax) == 0 && op.N >= 512 &&
+      gemm_k_splits(op) == 1 && epi_clean(op, ep)) {
+    if ((need & F_F32) && (need & ~kEpiF32) == 0) return {kEpiF32, 0, false, false, true};
+    if ((need & F_BF16) && (need & ~(kEpiAct & ~F_STATS)) == 0) return {kEpiAct, 0, false, false, true};
+    if (need == kEpiGG) return {kEpiGG, 0, false, false, true};
+  }
   if (epi_clean(op, ep)) {
     auto fits = [&](uint32_t kind) { return (need & ~kind) == 0; };
     // short-K GEMMs are epilogue-bound: give them a third epilogue warp per row quadrant
@@ -236,6 +246,7 @@ inline GemmKind gemm_kind(const GemmOp& op, int M, const GemmEpilogue& ep) {
 inline int stats_slots_for(const GemmOp& op, int M, const GemmEpilogue& ep) {
   const GemmKind k = gemm_kind(op, M, ep);
   if (k.wide) return (op.N / kBNWide) * GemmSmemWide::kEpiGroups;
+  if (k.expand) return (op.N / kBNMax) * GemmSmemExpand<kEpiF32>::kEpiGroups;
   const GemmOp o = narrow_op(op);
   return ((o.N + o.BN - 1) / o.BN) * epi_groups(k.ew);
 }
@@ -307,9 +318,53 @@ inline cudaError_t launch_gemm_swap(const GemmOp& op, int M, const GemmEpilogue&
                             op.tmX, sh, ep);
 }
 
+// The n-tiles of a row block are split into the most column groups of an even number of tiles that still give every
+// CTA an SM of its own: 32 row blocks x 4 groups of 512 columns for 4096 tokens at N = 2048; one group (all 16
+// n-tiles) once the row blocks alone fill the machine.
+inline int expand_groups(int M, int N) {
+  const int num_m = (M + kBM - 1) / kBM, pairs = N / (2 * kBNMax);
+  for (int g = pairs; g > 1; --g)
+    if (pairs % g == 0 && num_m * g <= device_sm_count()) return g;
+  return 1;
+}
+template <uint32_t kF>
+inline cudaError_t launch_gemm_expand(const GemmOp& op, int M, const GemmEpilogue& ep, cudaStream_t st) {
+  using SM = GemmSmemExpand<kF>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    for (auto k : {gemm_bf16_wgmma_expand_kernel<kF, 0>, gemm_bf16_wgmma_expand_kernel<kF, 1>}) {
+      const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kTotal);
+      if (e != cudaSuccess) return e;
+    }
+    attr_set = true;
+  }
+  GemmShape sh;
+  sh.M = M; sh.N = op.N; sh.K = op.K; sh.BN = kBNMax; sh.a_mn = 0; sh.b_mn = op.b_mn; sh.k_splits = 1;
+  const int groups = expand_groups(M, op.N);
+  const int tpc = op.N / kBNMax / groups;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(static_cast<unsigned>((M > 0 ? (M + kBM - 1) / kBM : 1) * groups));
+  cfg.blockDim = dim3(SM::kThreads);
+  cfg.dynamicSmemBytes = SM::kTotal;
+  cfg.stream = st;
+  cudaLaunchAttribute attrs[1];
+  attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attrs[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attrs;
+  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return cudaLaunchKernelEx(&cfg, op.b_mn ? gemm_bf16_wgmma_expand_kernel<kF, 1> : gemm_bf16_wgmma_expand_kernel<kF, 0>,
+                            op.tmA, op.tmB, sh, tpc, ep);
+}
+
 inline cudaError_t launch_gemm(const GemmOp& wop, int M, const GemmEpilogue& ep, cudaStream_t st) {
   const GemmKind k = gemm_kind(wop, M, ep);
   if (k.swap) return launch_gemm_swap(wop, M, ep, st);
+  if (k.expand) {
+    return k.flags == kEpiF32 ? launch_gemm_expand<kEpiF32>(wop, M, ep, st)
+           : k.flags == kEpiAct ? launch_gemm_expand<kEpiAct>(wop, M, ep, st)
+                                : launch_gemm_expand<kEpiGG>(wop, M, ep, st);
+  }
   if (k.wide) {
     return k.flags == kEpiF32 ? launch_gemm_wide<kEpiF32>(wop, M, ep, st) : launch_gemm_wide<kEpiBf16>(wop, M, ep, st);
   }

@@ -1762,4 +1762,23 @@ int smd_gemm_bf16(const void* A, const void* B, int M, int N, int K, int a_mn, i
   return SMD_OK;
 }
 
+int smd_gemm_bf16_epi(const void* A, const void* B, int M, int N, int K, int a_mn, int b_mn, const float* bias,
+                      int act, float* out_f32, void* out_bf16, void* out_bf16_pre, const void* gelu_grad_of,
+                      float* row_stats, float* stats_part, int* nslots, smd_stream_t stream) {
+  GemmOp op;
+  if (!make_gemm_op(&op, A, static_cast<uint64_t>(M), B, static_cast<uint64_t>(N), N, K, choose_bn(N), a_mn, b_mn))
+    return SMD_ERR_CUDA;
+  GemmEpilogue e = epi();
+  e.bias = bias; e.act = act;
+  e.out_f32 = out_f32; e.ld_f32 = N;
+  e.out_bf16 = static_cast<__nv_bfloat16*>(out_bf16); e.ld_bf16 = N;
+  e.out_bf16_pre = static_cast<__nv_bfloat16*>(out_bf16_pre);
+  e.gelu_grad_of = static_cast<const __nv_bfloat16*>(gelu_grad_of); e.ld_gg = N;
+  e.row_stats = row_stats; e.stats_part = row_stats ? stats_part : nullptr;
+  if (nslots) *nslots = e.stats_part ? stats_slots_for(op, M, e) : 0;
+  SMD_CUDA(launch_gemm(op, M, e, static_cast<cudaStream_t>(stream)));
+  SMD_LAUNCH_CHECK("gemm");
+  return SMD_OK;
+}
+
 }  // extern "C"

@@ -87,6 +87,8 @@ _SIGNATURES = {
                                       C.POINTER(C.c_float), C.POINTER(C.c_int)]),
     "smd_gemm_bf16": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                 _P, _P, C.c_int, _P, _P, _P, _P, _P, _P]),
+    "smd_gemm_bf16_epi": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P,
+                                    _P, _P, _P, _P, _P]),
     "smd_debug_forward_save": (C.c_int, [_P, _P, _P, _P, C.c_int, _P, _P]),
     "smd_debug_buffer": (C.c_int, [_P, C.c_char_p, C.POINTER(_P), C.POINTER(C.c_size_t)]),
     "smd_launch_count": (C.c_longlong, []),
