@@ -42,6 +42,7 @@ Largest errors measured on an H100 80GB HBM3 (SXM, 700 W power limit) over all c
   spacing and 0.25 / 0.75 not the nearest
 """
 import ctypes as C
+import time
 
 import numpy as np
 import pytest
@@ -429,6 +430,8 @@ CASES = {
     "S64_H16_b3": ("TransformerDDPM", dict(num_layers=1, num_heads=16, num_mlp_layers=1, channels=42, seq_len=64), 3, {}),
     "H4_b3": ("TransformerDDPM", dict(num_layers=1, num_heads=4, num_mlp_layers=1, channels=42), 3, {}),     # tf32, dh 32
     "H32_b3": ("TransformerDDPM", dict(num_layers=1, num_heads=32, num_mlp_layers=1, channels=42), 3, {}),   # SIMT, dh 4
+    # head dim 8 at S 32 (the large model): attn_block_kernel<8, 32> and the tf32 training-save attention
+    "H16_b3": ("TransformerDDPM", dict(num_layers=1, num_heads=16, num_mlp_layers=1, channels=42), 3, {}),
     "S128_H16_b2": ("TransformerDDPM", dict(num_layers=1, num_heads=16, num_mlp_layers=1, channels=42, seq_len=128), 2,
                     {}),
     # generic embed, output N 146 of 192, 1024-thread ln_film_act
@@ -502,17 +505,27 @@ def test_sampler_film_table_and_table_rows(lib):
     """A training plan with sampler_T = 1000: the FiLM table (gather + generator on all T conditioning values), one
     eager reverse step reading table row t, and one graph-replayed step reading the row through the device step
     counter (film_row_dev)."""
-    arch, kw, n = "TransformerDDPM", T_KW, 3
-    eng = _engine(arch, kw, n, sampler_T=1000)
+    check_sampler_step(_engine("TransformerDDPM", T_KW, 3, sampler_T=1000), 3, "sampler")
+
+
+def check_sampler_step(eng, n, name, shard=None, inference_plan=False):
+    """The rules of the DDPM sampler on a training plan with sampler_T = 1000, for n samples: the FiLM table, one eager
+    reverse step at t = 500 with supplied noise (every forward launch, the step itself), then one graph-replayed step
+    that must equal an eager step at t = T - 1 bit for bit.  shard: (first_row, total_rows) of set_sampler_shard.
+    inference_plan: an inference plan of max_batch n (the one sample_ncsn and bench.py run) must replay the same step
+    to the same bits as this training plan."""
+    S, Cc = eng.seq_len, eng.cfg.channels
     betas = O.create_noise_schedule(1e-6, 0.01, 1000, "linear")
     eng.sampler_setup(betas, key=(0, 1))
-    x, _ = _inputs(n, (32, 42), seed=24)
-    z = torch.from_numpy(np.random.default_rng(25).standard_normal((n, 32, 42)).astype(np.float32)).cuda()
+    if shard is not None:
+        eng.set_sampler_shard(*shard)
+    x, _ = _inputs(n, (S, Cc), seed=24)
+    z = torch.from_numpy(np.random.default_rng(25).standard_normal((n, S, Cc)).astype(np.float32)).cuda()
     eh = torch.empty_like(x)
     x_next, cnt = _counted(eng, lambda: eng.reverse_step(x, 500, z=z, eps_hat=eh))
-    rep = Report("sampler eager step t=500")
+    rep = Report(f"{name} eager step t=500")
     v = BW.PlanView(eng)
-    K, Md, T = kw["num_mlp_layers"], eng.cfg.mlp_dims, 1000
+    K, Md, T = eng.cfg.num_mlp_layers, eng.cfg.mlp_dims, 1000
     # ---- the table: gather of the conditioning values, then the generator over all T rows
     tv = v.f32("ftab.t", T)
     rep.exact("FiLM table conditioning values ftab.t = coef[:, 5]", tv, v.f32("coef", T, 8)[:, 5])
@@ -533,7 +546,10 @@ def test_sampler_film_table_and_table_rows(lib):
                 e2 @ v.param(fp + "ss.kernel") + v.param(fp + "ss.bias"), B_DW)
         for part in ("d1", "d2", "ss"):
             rep.launch(f"table {part}[{k}]")
+    t0 = time.perf_counter()
     check_forward(eng, rep, x, None, n, save=False, y=eh, table_row=500)
+    print(f"[parity] {name}: float64 restatement of the forward of {n * S} tokens took "
+          f"{time.perf_counter() - t0:.1f} s")
     coef = O.reverse_coefficients(betas)
     ref, _, _ = O.reverse_step(lambda s, c: eh.to(F64), x.to(F64), 500, coef, z.to(F64))
     rep.rel("reverse step -> x_next", x_next, ref, B_SEED)
@@ -543,8 +559,8 @@ def test_sampler_film_table_and_table_rows(lib):
     # ---- graph: the step counter starts at T - 1 and is read on the device
     x2 = x.clone()
     _, cnt = _counted(eng, lambda: eng.sample(x2, steps=1, use_graph=True))
-    rep = Report("sampler replayed step t=999")
-    graph_eh = v.f32("eps_hat", n, 32, 42).clone()
+    rep = Report(f"{name} replayed step t=999")
+    graph_eh = v.f32("eps_hat", n, S, Cc).clone()
     v = check_forward(eng, rep, x, None, n, save=False, y=graph_eh, table_row=T - 1)
     rep.exact("step_advance: device step counter", v.raw("t_ptr", (1,), torch.int32).to(F64),
               torch.tensor([T - 2], dtype=F64, device="cuda"))
@@ -560,6 +576,22 @@ def test_sampler_film_table_and_table_rows(lib):
     rep.launch("reverse_step (threefry noise)")
     rep.expect_launches(cnt)
     rep.finish()
+    if not inference_plan:
+        return
+    # ---- the inference plan of the same model: the rules above read a training plan's buffers; the chains run here
+    from smd_b200 import Engine
+    inf = Engine(eng.cfg, max_batch=n, training=False)
+    inf.set_params(eng.params)
+    inf.sampler_setup(betas, key=(0, 1))
+    if shard is not None:
+        inf.set_sampler_shard(*shard)
+    x3 = x.clone()
+    inf.sample(x3, steps=1, use_graph=True)
+    torch.cuda.synchronize()
+    rep = Report(f"{name} inference plan")
+    rep.exact("replayed step x_next on an inference plan = on the training plan", x3, x2)
+    rep.finish()
+    del inf
 
 
 def test_dense_ncsn_tangent_pass_and_output_scale(lib):
