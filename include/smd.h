@@ -226,8 +226,8 @@ int smd_ddpm_sample(smd_plan* plan, const float* params, float* x, int n, int st
  *   sig = eta sqrt((1-a')/(1-a)) sqrt(1 - a/a'),  x <- sqrt(a') x0 + sqrt(max(1-a'-sig^2, 0)) eps' + sig z.
  * The step keys follow diffusion_dynamics' scan carry over K steps (smd_sampler_setup with T = K), as do the collection
  * rows.  tau = 0..T-1 with eta = 1 is diffusion_dynamics itself; eta = 0 is deterministic given x.  The tables share
- * the sampler's workspace regions: smd_sampler_setup, smd_langevin_setup, smd_ddim_setup and smd_ddim_encode_setup
- * each invalidate the other three (SMD_ERR_STATE).  SMD_ERR_INVALID for a TransformerMDN plan, T < 1 or T > 8192, K < 1 or K > T, indices not
+ * the sampler's workspace regions: smd_sampler_setup, smd_langevin_setup, smd_ddim_setup, smd_ddim_encode_setup and
+ * smd_dpm_setup each invalidate the other four (SMD_ERR_STATE).  SMD_ERR_INVALID for a TransformerMDN plan, T < 1 or T > 8192, K < 1 or K > T, indices not
  * strictly increasing or out of range, eta < 0 or not finite, or alpha_bar outside (0, 1) at a selected index. */
 int smd_ddim_setup(smd_plan* plan, const float* host_betas, int T, const int* host_steps, int K, float eta,
                    const uint32_t host_key[2], smd_stream_t stream);
@@ -251,7 +251,8 @@ int smd_ddim_tables(const float* host_betas, int T, const int* host_steps, int K
  *   eps = model(x, sqrt(a)),  x0 = sqrt(1/a) x - sqrt(1-a) sqrt(1/a) eps  (not clipped),  x <- sqrt(a') x0 + sqrt(1-a') eps.
  * At i = 0, x0 = x exactly.  This mirrors smd_ddim_sample at eta = 0 over the same levels: smd_ddim_sample on the code
  * returns the data up to discretisation error.  The table shares the sampler's workspace regions: smd_sampler_setup,
- * smd_langevin_setup, smd_ddim_setup and smd_ddim_encode_setup each invalidate the other three (SMD_ERR_STATE).
+ * smd_langevin_setup, smd_ddim_setup, smd_ddim_encode_setup and smd_dpm_setup each invalidate the other four
+ * (SMD_ERR_STATE).
  * SMD_ERR_INVALID for a TransformerMDN plan and for the arguments smd_ddim_setup rejects (there is no eta). */
 int smd_ddim_encode_setup(smd_plan* plan, const float* host_betas, int T, const int* host_steps, int K,
                           smd_stream_t stream);
@@ -265,13 +266,43 @@ int smd_ddim_encode(smd_plan* plan, const float* params, float* x, int n, int us
  * float32 alpha_bar and rounded once.  host_coef may be NULL.  Same rejections as smd_ddim_encode_setup. */
 int smd_ddim_encode_tables(const float* host_betas, int T, const int* host_steps, int K, float* host_coef);
 
+/* ---- DPM-Solver++ multistep chain (Lu et al. 2022, Algorithm 2 and its third-order form); not in the reference ---- */
+/* host_betas / host_steps as smd_ddim_setup: the levels are a_i = alpha_bar(tau_i), i = K-1 .. 0, and a_{-1} = 1 (the
+ * data), with alpha = sqrt(a), sigma = sqrt(1-a), lambda = log(alpha / sigma).  Step i goes from level i to level i-1
+ * with h = lambda_{i-1} - lambda_i:
+ *   eps = model(x, sqrt(a_i)),  m0 = clip(sqrt(1/a) x - sqrt(1-a) sqrt(1/a) eps, -1, 1)  (the DDIM chain's estimate),
+ *   x <- c_x x + c_0 m0 + c_1 m1 + c_2 m2,
+ * where m1, m2 are the estimates of steps i+1 and i+2.  The step counted j = K-1-i from the noisiest has the order
+ * min(order, j+1); the last step (i = 0) is first order, x <- m0.  Order 1 is the DDIM eta = 0 step; orders 2 and 3
+ * reuse the history and so still cost one network call per step.  The coefficients are computed in float64 from the
+ * float32 alpha_bar and rounded once.  The step draws no noise; the key and slot tables are the DDIM chain's, so
+ * infill draws what smd_ddim_setup's chain draws.  The tables share the sampler's workspace regions:
+ * smd_sampler_setup, smd_langevin_setup, smd_ddim_setup, smd_ddim_encode_setup and smd_dpm_setup each invalidate the
+ * other four (SMD_ERR_STATE).  SMD_ERR_INVALID for a TransformerMDN plan, an order outside {1, 2, 3} and the
+ * arguments smd_ddim_setup rejects (there is no eta). */
+int smd_dpm_setup(smd_plan* plan, const float* host_betas, int T, const int* host_steps, int K, int order,
+                  const uint32_t host_key[2], smd_stream_t stream);
+/* The whole K-step chain on x (n, S, C) or (n, D) in place.  history: DEVICE, (order - 1) x n x S x C floats of
+ * scratch that the chain owns for the call (its contents on entry are ignored; NULL allowed for order 1).
+ * infill_x / infill_mask, collection, metrics (noise_norm row 0), use_graph and smd_sampler_set_shard as
+ * smd_ddim_sample; each rank keeps the history of its own rows.  SMD_ERR_STATE without smd_dpm_setup;
+ * SMD_ERR_INVALID for n outside [1, max_batch], infill_x without infill_mask or the reverse, or a NULL history with
+ * order > 1. */
+int smd_dpm_sample(smd_plan* plan, const float* params, float* x, int n, float* history, const float* infill_x,
+                   const float* infill_mask, float* collection, float* metrics, int use_graph, smd_stream_t stream);
+/* Host only: the tables smd_dpm_setup uploads.  host_coef (K x 8: sqrt(1/a), sqrt(1-a) sqrt(1/a), c_x, c_0, c_1,
+ * sqrt(a), c_2, a), host_keys (K x 4) and host_slots (K) as smd_ddim_tables; each may be NULL (host_key only when
+ * host_keys is).  Coefficients an order leaves unused are exactly 0.  Same rejections as smd_dpm_setup. */
+int smd_dpm_tables(const float* host_betas, int T, const int* host_steps, int K, int order,
+                   const uint32_t host_key[2], float* host_coef, uint32_t* host_keys, int* host_slots);
+
 /* ---- Langevin chains (annealed / consistent Langevin dynamics of the NCSN family) ------------------------------ */
 /* kind 0 = annealed (utils/ebm_utils.py:89-198), 1 = consistent (:201-271).  host_sigmas: HOST, L floats (L >= 2).
  * steps_per_level: T of the annealed chain (ignored by the consistent one).  host_key: the `rng` the sampler receives.
  * Builds the per-level table (sigma, alpha = epsilon (sigma / sigma_L)^2, noise coefficient sqrt(2 alpha) or
  * beta sigma_{l+1}) and the collection indices linspace(1, L*T, 100) in the workspace.  It shares those regions with
- * the other chains: smd_sampler_setup, smd_langevin_setup, smd_ddim_setup and smd_ddim_encode_setup each invalidate
- * the other three (SMD_ERR_STATE).
+ * the other chains: smd_sampler_setup, smd_langevin_setup, smd_ddim_setup, smd_ddim_encode_setup and smd_dpm_setup
+ * each invalidate the other four (SMD_ERR_STATE).
  * SMD_ERR_INVALID for a TransformerMDN plan, L < 2 or L > 8192, an unknown kind or (annealed) T < 1. */
 int smd_langevin_setup(smd_plan* plan, const float* host_sigmas, int L, int steps_per_level, float epsilon, int kind,
                        const uint32_t host_key[2], smd_stream_t stream);

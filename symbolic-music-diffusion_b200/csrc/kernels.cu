@@ -831,9 +831,11 @@ __device__ __forceinline__ void step_metrics(float* met, size_t stride, float (&
   if (blockIdx.x == 0 && threadIdx.x == 3) met[2 * stride] = scalar;
 }
 
-// The reverse_step_kernel / ddim_step_kernel body: four adjacent lanes share one (sample, channel) column and take a
-// quarter of its S positions each -- 4x the threads and a quarter of the serial threefry chain per thread.  Per
-// element: z (when draw_noise: the supplied z, or threefry(k0, k1)), nx = update(x, eps_hat, z, noise), the infill
+// The reverse_step_kernel / ddim_step_kernel / dpm_step_kernel body: four adjacent lanes share one (sample, channel)
+// column and take a quarter of its S positions each -- 4x the threads and a quarter of the serial threefry chain per
+// thread.  Per element idx: z (when draw_noise: the supplied z, or threefry(k0, k1)), nx = update(x, eps_hat, z, noise,
+// pos) with pos = s * N * C + (n * C + c) the element's position-major index (a permutation of idx under which the
+// lanes of one warp step touch 4 runs of 8 consecutive floats whatever S and C are), the infill
 // blend with y = infill_x, or sqrt_ap infill_x + sqrt_1m iz when draw_infill (iz: the supplied infill_z, or
 // threefry(ik0, ik1)), the state and the collection row `slot` (< 0: none).  m receives the column norms
 // sqrt(sum eps_hat^2 + 1e-10), of x - nx and of noise on the first lane of the column (two shuffles), 0 elsewhere.
@@ -860,7 +862,7 @@ __device__ __forceinline__ void column_step(const Args& a, const float* z_in, co
       float z = 0.f;
       if (draw_noise) z = z_in ? z_in[idx] : jax_normal_from_bits(jax_random_bits(k0, k1, rfirst + idx, rtotal));
       float noise;
-      float nx = update(x, eh, z, noise);
+      float nx = update(x, eh, z, noise, static_cast<uint32_t>(s) * NC + i);
       if (a.infill_mask) {
         const float mk = a.infill_mask[idx];
         const float ix = a.infill_x[idx];
@@ -896,7 +898,7 @@ reverse_step_kernel(const ReverseStepArgs a) {
   const int slot = (a.slot_tab && a.collection) ? a.slot_tab[t] : -1;
   float m[3];
   column_step(a, a.z, a.infill_z, k0, k1, ik0, ik1, t > 0, t > 0, cf[5], cf[6], slot,
-              [&](float x, float eh, float z, float& noise) {
+              [&](float x, float eh, float z, float& noise, uint32_t) {
                 noise = z * sigma;
                 float recon = __fsub_rn(__fmul_rn(sqrt_recip, x), __fmul_rn(sqrt_m1, eh));
                 recon = fminf(fmaxf(recon, -1.0f), 1.0f);
@@ -925,7 +927,7 @@ ddim_step_kernel(const DdimStepArgs a) {
   float m[3];
   // sig = 0 (eta = 0, or the last step) draws nothing: the deterministic chain needs no noise stream
   column_step(a, nullptr, nullptr, k0, k1, ik0, ik1, sig != 0.f, t_pos, sqrt_a, sqrt_1m, slot,
-              [&](float x, float eh, float z, float& noise) {
+              [&](float x, float eh, float z, float& noise, uint32_t) {
                 float x0 = __fsub_rn(__fmul_rn(sqrt_recip, x), __fmul_rn(sqrt_m1, eh));
                 x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
                 const float dir = __fdiv_rn(__fsub_rn(x, __fmul_rn(sqrt_a, x0)), sqrt_1m);
@@ -937,6 +939,44 @@ ddim_step_kernel(const DdimStepArgs a) {
 void launch_ddim_step(const DdimStepArgs& a, cudaStream_t st) {
   const int NC = a.N * a.C;
   ddim_step_kernel<<<(4 * NC + 255) / 256, 256, 0, st>>>(a);
+}
+
+// DPM-Solver++ multistep step (Lu et al. 2022, Algorithm 2 and its third-order form), linear in (x, m0, m1, m2)
+__global__ void __launch_bounds__(256)
+dpm_step_kernel(const DpmStepArgs a) {
+  pdl_trigger();
+  pdl_wait();
+  const int si = *a.i_ptr;
+  const float* cf = a.coef + 8 * si;
+  const float sqrt_recip = cf[0], sqrt_m1 = cf[1], c_x = cf[2], c_0 = cf[3], c_1 = cf[4], sqrt_a = cf[5],
+              c_2 = cf[6];
+  // the infill template's sqrt(1-a): the DDPM chain's float32 value
+  const float sqrt_1m = __fsqrt_rn(__fsub_rn(1.0f, cf[7]));
+  const uint32_t ik0 = a.key_tab[4 * si + 2], ik1 = a.key_tab[4 * si + 3];
+  const bool t_pos = si > 0 || a.tau0 > 0;     // t = tau_i > 0
+  const int slot = a.collection ? a.slot_tab[si] : -1;
+  float* h1 = a.history;
+  float* h2 = a.history + static_cast<size_t>(a.N) * a.S * a.C;
+  float m[3];
+  column_step(a, nullptr, nullptr, 0u, 0u, ik0, ik1, false, t_pos, sqrt_a, sqrt_1m, slot,
+              [&](float x, float eh, float, float& noise, uint32_t pos) {
+                float m0 = __fsub_rn(__fmul_rn(sqrt_recip, x), __fmul_rn(sqrt_m1, eh));
+                m0 = fminf(fmaxf(m0, -1.0f), 1.0f);
+                float nx = __fadd_rn(__fmul_rn(c_x, x), __fmul_rn(c_0, m0));
+                // a zero coefficient leaves its history unread: it is not written yet at the first steps
+                float m1 = 0.f;
+                if (c_1 != 0.f) { m1 = h1[pos]; nx = __fadd_rn(nx, __fmul_rn(c_1, m1)); }
+                if (c_2 != 0.f) nx = __fadd_rn(nx, __fmul_rn(c_2, h2[pos]));
+                if (a.hist_slots > 1 && c_1 != 0.f) h2[pos] = m1;
+                if (a.hist_slots > 0) h1[pos] = m0;
+                noise = 0.f;
+                return nx;
+              }, m);
+  if (a.metrics) step_metrics(a.metrics + (a.K - 1 - si), a.K, m, cf[7], a.N * a.C);
+}
+void launch_dpm_step(const DpmStepArgs& a, cudaStream_t st) {
+  const int NC = a.N * a.C;
+  dpm_step_kernel<<<(4 * NC + 255) / 256, 256, 0, st>>>(a);
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -242,6 +242,31 @@ struct DdimStepArgs {
 // x <- sqrt(a') x0 + sqrt(max(1-a'-sig^2, 0)) eps' + sig z, then the infill blend at t = tau_i, the metrics and the
 // collection row
 void launch_ddim_step(const DdimStepArgs& a, cudaStream_t st);
+// DPM-Solver++ multistep step over the DDIM chain's levels (smd_dpm_setup), indexed by the step i: from level i to
+// level i-1, with m0 the clipped x0 estimate of this step and m1, m2 those of steps i+1 and i+2 (the history).
+struct DpmStepArgs {
+  const float* x;          // state (N, S, C)
+  const float* eps_hat;    // model output eps = model(x, sqrt(a))
+  const uint32_t* key_tab; // device table [K][4] = (noise k0,k1 (unused), infill k0,k1) indexed by step i
+  const float* coef;       // device table [K][8]: sqrt(1/a), sqrt(1-a) sqrt(1/a), c_x, c_0, c_1, sqrt(a), c_2, a
+  const int* slot_tab;     // device table [K]: collection slot or -1
+  const int* i_ptr;        // device scalar: current step i (graph-replayable)
+  const float* infill_x;   // or null
+  const float* infill_mask;
+  float* history;          // hist_slots x (S, N, C): m1, then m2, position-major so that the four lanes of a column
+                           // coalesce (null when hist_slots = 0)
+  float* x_next;
+  float* collection;       // (41, N, S, C) or null
+  float* metrics;          // device [4][K] accumulators (grad_norm, step_norm, alpha_bar, noise_norm); column K-1-i
+  int N, S, C, K;
+  int hist_slots;          // order - 1
+  int tau0;                // tau_0: the step i = 0 is at t = 0 (infill template x_fix itself) when tau_0 == 0
+  uint32_t rng_first, rng_total;   // sharded sampling as ReverseStepArgs
+};
+// m0 = clip(sqrt(1/a) x - sqrt(1-a) sqrt(1/a) eps, -1, 1);  x <- c_x x + c_0 m0 + c_1 m1 + c_2 m2, where a zero c_1 /
+// c_2 leaves m1 / m2 unread; then hist2 <- m1, hist1 <- m0 (as many slots as there are), the infill blend at t = tau_i
+// (sqrt(1-a) in float32 from a), the metrics (noise_norm 0) and the collection row
+void launch_dpm_step(const DpmStepArgs& a, cudaStream_t st);
 // DDIM encoder step (smd_ddim_encode_setup), the eta = 0 DDIM step run from data towards noise: step i goes from
 // a = a_{i-1} (1 at i = 0) to a' = a_i = alpha_bar(tau_i).  The table is stored last step first: row r = K-1-i, so the
 // counter that step_advance decrements from K-1 visits i = 0 .. K-1.

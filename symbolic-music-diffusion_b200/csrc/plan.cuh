@@ -136,15 +136,17 @@ struct TrainState {
 enum Objective : int { kObjDdpm = 0, kObjDsm = 1, kObjSsm = 2, kObjMdn = 3 };
 
 // The sampler chain whose tables (coef / keys / slots / t_ptr, the FiLM table) the workspace holds: the DDPM sampler,
-// the Langevin chain, the DDIM chain and the DDIM encoder share those regions, so at most one of them is set up at a
-// time.
-enum Chain : int { kChainNone = 0, kChainDdpm = 1, kChainLangevin = 2, kChainDdim = 3, kChainDdimEncode = 4 };
+// the Langevin chain, the DDIM chain, the DDIM encoder and the DPM-Solver++ chain share those regions, so at most one of
+// them is set up at a time.
+enum Chain : int { kChainNone = 0, kChainDdpm = 1, kChainLangevin = 2, kChainDdim = 3, kChainDdimEncode = 4,
+                   kChainDpm = 5 };
 // The chain set up in the workspace and the per-chain values its calls read back.
 struct ChainSetup {
   Chain kind = kChainNone;
-  int rows = 0;                 // rows of the coef and FiLM tables: T (DDPM), K (DDIM, encoder), L (Langevin)
+  int rows = 0;                 // rows of the coef and FiLM tables: T (DDPM), K (DDIM, encoder, DPM), L (Langevin)
   int steps = 1;                // Langevin: steps per level (1 for the consistent chain and for the other chains)
-  int tau0 = 0;                 // DDIM: the first selected index tau_0
+  int tau0 = 0;                 // DDIM, DPM: the first selected index tau_0
+  int order = 0;                // DPM: the solver order (1, 2 or 3)
   int lv_kind = 0;              // Langevin: 0 annealed, 1 consistent
   uint32_t key[2] = {0u, 0u};   // Langevin: the chain key
   float sigma_last = 0.f;       // Langevin: sigma_L
@@ -246,8 +248,9 @@ struct smd_plan {
   bool film_tab_ready = false;
   const float* film_tab_params = nullptr;
   long long shard_first_row = 0, shard_total_rows = 0;   // smd_sampler_set_shard
-  // The chain set up (smd_sampler_setup, smd_ddim_setup, smd_ddim_encode_setup or smd_langevin_setup), and the graph
-  // replay of one step of it (smd_ddpm_sample, smd_ddim_sample, smd_ddim_encode or smd_langevin_sample).
+  // The chain set up (smd_sampler_setup, smd_ddim_setup, smd_ddim_encode_setup, smd_dpm_setup or smd_langevin_setup),
+  // and the graph replay of one step of it (smd_ddpm_sample, smd_ddim_sample, smd_ddim_encode, smd_dpm_sample or
+  // smd_langevin_sample).
   smd::ChainSetup chain;
   smd::CapturedGraph chain_graph;
   cudaStream_t own_stream = nullptr;

@@ -1260,7 +1260,7 @@ static FilmRows film_table_rows(const smd_plan* plan, const float* params, int r
 static int check_chain_call(const smd_plan* plan, const char* fn, Chain kind, int n, const float* infill_x,
                             const float* infill_mask) {
   static const char* const setup_fn[] = {"", "smd_sampler_setup", "smd_langevin_setup", "smd_ddim_setup",
-                                         "smd_ddim_encode_setup"};
+                                         "smd_ddim_encode_setup", "smd_dpm_setup"};
   if (!plan) { set_error("null plan"); return SMD_ERR_INVALID; }
   if (reject_mdn(plan, fn)) return SMD_ERR_INVALID;
   if (n < 1 || n > plan->cfg.max_batch) { set_error("n out of range"); return SMD_ERR_INVALID; }
@@ -1545,6 +1545,133 @@ int smd_ddim_encode(smd_plan* plan, const float* params, float* x, int n, int us
   auto step = [&](cudaStream_t s) { return ddim_encode_step(plan, params, x, n, s); };
   return run_chain(plan, params, static_cast<cudaStream_t>(stream), use_graph, nullptr, 8, 4, K,
                    graph_key(n, params, x), "ddim encode graph",
+                   [&](cudaStream_t s) { return set_step_counter(plan, K - 1, s); }, step, step, no_epilogue);
+}
+
+// ---- DPM-Solver++ multistep chain (Lu et al. 2022) over the DDIM chain's levels --------------------------------------
+
+// Host table of smd_dpm_setup for the K selected indices tau_i and the solver order (alpha_bar in float32 as
+// smd_ddim_setup, the coefficients in float64 from it, rounded to float32):
+//   coef[i] = (sqrt(1/a), sqrt(1-a) sqrt(1/a), c_x, c_0, c_1, sqrt(a), c_2, a)
+// with a = alpha_bar(tau_i), so that x' = c_x x + c_0 m0 + c_1 m1 + c_2 m2 is the step from level i to level i-1 of the
+// order min(order, K-i), first order at i = 0 (x' = m0).  Coefficients an order leaves unused are exactly 0.
+static int dpm_tables(const float* betas, int T, const int* steps, int K, int order, float* coef) {
+  if (order < 1 || order > 3) { set_error("the DPM-Solver order must be 1, 2 or 3"); return SMD_ERR_INVALID; }
+  std::vector<float> ap;
+  const int rc = ddim_levels(betas, T, steps, K, 0.f, ap);
+  if (rc) return rc;
+  // lambda = log(alpha / sigma), the half log-SNR of level i (0 <= i < K)
+  auto lam = [&](int i) { const double a = ap[i]; return log(sqrt(a) / sqrt(1.0 - a)); };
+  for (int i = 0; i < K; ++i) {
+    const double a = ap[i];
+    const int ord = i == 0 ? 1 : std::min(order, K - i);
+    double cx = 0.0, c0 = 1.0, c1 = 0.0, c2 = 0.0;      // the last step, into a = 1: x' = m0
+    if (i > 0) {
+      const double at = ap[i - 1], alpha_t = sqrt(at), sigma_t = sqrt(1.0 - at);
+      const double h = lam(i - 1) - lam(i);
+      // phi1 = e^-h - 1 and the phi2, phi3 built on it: expm1 keeps them accurate at small h
+      const double phi1 = expm1(-h), phi2 = phi1 / h + 1.0, phi3 = phi2 / h - 0.5;
+      cx = sigma_t / sqrt(1.0 - a);
+      c0 = -alpha_t * phi1;
+      if (ord == 2) {
+        // D = (1 + 1/(2 r0)) m0 - 1/(2 r0) m1
+        const double r0 = (lam(i) - lam(i + 1)) / h, A = c0;
+        c0 = A * (1.0 + 0.5 / r0);
+        c1 = -A * 0.5 / r0;
+      } else if (ord == 3) {
+        // D1_0 = (m0 - m1)/r0, D1_1 = (m1 - m2)/r1, D1 = D1_0 + r0/(r0+r1) (D1_0 - D1_1), D2 = (D1_0 - D1_1)/(r0+r1);
+        // x' = c_x x - alpha_t phi1 m0 + alpha_t phi2 D1 - alpha_t phi3 D2, gathered per m
+        const double r0 = (lam(i) - lam(i + 1)) / h, r1 = (lam(i + 1) - lam(i + 2)) / h;
+        const double u = 1.0 / r0, v = 1.0 / r1, w = r0 / (r0 + r1), q = 1.0 / (r0 + r1);
+        const double p2 = alpha_t * phi2, p3 = alpha_t * phi3;
+        c0 = -alpha_t * phi1 + p2 * (1.0 + w) * u - p3 * q * u;
+        c1 = -p2 * ((1.0 + w) * u + w * v) + p3 * q * (u + v);
+        c2 = p2 * w * v - p3 * q * v;
+      }
+    }
+    const double c64[8] = {sqrt(1.0 / a), sqrt(1.0 - a) * sqrt(1.0 / a), cx, c0, c1, sqrt(a), c2, a};
+    for (int j = 0; j < 8; ++j) coef[static_cast<size_t>(i) * 8 + j] = static_cast<float>(c64[j]);
+  }
+  return SMD_OK;
+}
+
+int smd_dpm_tables(const float* host_betas, int T, const int* host_steps, int K, int order,
+                   const uint32_t host_key[2], float* host_coef, uint32_t* host_keys, int* host_slots) {
+  std::vector<float> coef(static_cast<size_t>(std::max(K, 0)) * 8);
+  const int rc = dpm_tables(host_betas, T, host_steps, K, order, coef.data());
+  if (rc) return rc;
+  if (host_keys && !host_key) { set_error("host_keys needs host_key"); return SMD_ERR_INVALID; }
+  if (host_coef) memcpy(host_coef, coef.data(), coef.size() * sizeof(float));
+  if (host_keys) scan_keys(host_key, K, host_keys);
+  if (host_slots) collection_slots(K, host_slots);
+  return SMD_OK;
+}
+
+int smd_dpm_setup(smd_plan* plan, const float* host_betas, int T, const int* host_steps, int K, int order,
+                  const uint32_t host_key[2], smd_stream_t stream) {
+  if (!plan || !host_key) { set_error("null argument"); return SMD_ERR_INVALID; }
+  if (reject_mdn(plan, "smd_dpm_setup")) return SMD_ERR_INVALID;
+  const size_t rows = static_cast<size_t>(std::max(K, 0));
+  std::vector<float> coef(rows * 8);
+  std::vector<uint32_t> keys(rows * 4);
+  std::vector<int> slots(rows);
+  const int rc = smd_dpm_tables(host_betas, T, host_steps, K, order, host_key, coef.data(), keys.data(), slots.data());
+  if (rc) return rc;
+  if (!plan->ws) { set_error("workspace not bound"); return SMD_ERR_STATE; }
+  // K <= T <= kMaxT rows of stride 8: the tables fit the coef / keys / slots regions of the DDPM sampler
+  const int rc2 = install_chain(plan, kChainDpm, K, coef.data(), 8, keys.data(), slots.data(), K,
+                                static_cast<cudaStream_t>(stream));
+  if (rc2) return rc2;
+  plan->chain.tau0 = host_steps[0];
+  plan->chain.order = order;
+  return SMD_OK;
+}
+
+// One DPM-Solver++ step at the device step counter i = *t_ptr: network call on sqrt(a) (FiLM table row i, or the
+// generator on coef[i].sqrt(a)), the fused update with the history, then i -= 1.  The eager loop and the captured graph
+// run this same sequence.
+static int dpm_step(smd_plan* plan, const float* params, float* x, int n, float* history, const float* infill_x,
+                    const float* infill_mask, float* collection, float* metrics, cudaStream_t st) {
+  float* tvec = plan->at<float>(plan->reg.tvec);
+  int* t_ptr = plan->at<int>(plan->reg.t_ptr);
+  const float* coef = plan->at<float>(plan->reg.coef);
+  const FilmRows film = film_table_rows(plan, params, -1, t_ptr);
+  if (!film.table) { launch_fill_cond(coef, 5, t_ptr, tvec, 1, st); CNT(); }
+  float* eh = plan->at<float>(plan->reg.eps_hat);
+  const int rc = run_forward(plan, params, x, tvec, 1, n, eh, st, false, false, false, film);
+  if (rc) return rc;
+  DpmStepArgs a;
+  memset(&a, 0, sizeof(a));
+  a.x = x; a.eps_hat = eh;
+  a.key_tab = plan->at<uint32_t>(plan->reg.keys);
+  a.coef = coef;
+  a.slot_tab = plan->at<int>(plan->reg.slots);
+  a.i_ptr = t_ptr;
+  a.infill_x = infill_x; a.infill_mask = infill_mask;
+  a.history = history; a.hist_slots = plan->chain.order - 1;
+  a.x_next = x; a.collection = collection; a.metrics = metrics;
+  a.N = n; a.K = plan->chain.rows; a.tau0 = plan->chain.tau0;
+  chain_geometry(plan, a, /*sharded=*/true);
+  launch_dpm_step(a, st); CNT();
+  launch_step_advance(t_ptr, st); CNT();
+  SMD_LAUNCH_CHECK("dpm_step");
+  return SMD_OK;
+}
+
+int smd_dpm_sample(smd_plan* plan, const float* params, float* x, int n, float* history, const float* infill_x,
+                   const float* infill_mask, float* collection, float* metrics, int use_graph, smd_stream_t stream) {
+  const int rc = check_chain_call(plan, "smd_dpm_sample", kChainDpm, n, infill_x, infill_mask);
+  if (rc) return rc;
+  if (!history && plan->chain.order > 1) {
+    set_error("an order-" + std::to_string(plan->chain.order) + " DPM-Solver chain needs a history buffer");
+    return SMD_ERR_INVALID;
+  }
+  const int K = plan->chain.rows;
+  auto step = [&](cudaStream_t s) {
+    return dpm_step(plan, params, x, n, history, infill_x, infill_mask, collection, metrics, s);
+  };
+  return run_chain(plan, params, static_cast<cudaStream_t>(stream), use_graph, metrics, 8, 5, K,
+                   graph_key(n, params, x, history, infill_x, infill_mask, collection, metrics), "dpm graph",
                    [&](cudaStream_t s) { return set_step_counter(plan, K - 1, s); }, step, step, no_epilogue);
 }
 

@@ -116,6 +116,31 @@ def ddim_dynamics(rng, model, betas, init, epsilon, T, denoise, infill=False, in
     return x, collection, metrics.unsqueeze(2)
 
 
+DPM_ORDERS = (1, 2, 3)
+
+
+def dpm_solver_dynamics(rng, model, betas, init, epsilon, T, denoise, infill=False, infill_samples=None,
+                        infill_masks=None, shard=None, steps=20, order=2, schedule="uniform"):
+    """DPM-Solver++ multistep (Lu et al. 2022) of `order` (1, 2 or 3) over `steps` levels of the DDPM schedule `betas`
+    picked by `schedule` (ddim_schedule): the probability-flow ODE that ddim_dynamics at eta = 0 integrates to first
+    order, to second or third order at the same one network call per step, with the clipped x0 estimate of
+    diffusion_dynamics.  Order 1 is ddim_dynamics at eta = 0.  Deterministic given `init`.  Not in the reference.
+    Returns (state, collection (41, N, *shape), ld_metrics (4, steps, 1)); keys, collection rows, infill and shard as
+    ddim_dynamics.  epsilon / T / denoise are null, as there."""
+    del epsilon, T, denoise
+    if order not in DPM_ORDERS:
+        raise ValueError(f"the DPM-Solver order must be one of {list(DPM_ORDERS)}, got {order!r}")
+    betas = np.asarray(betas, np.float32)
+    tau = ddim_schedule(len(betas), steps, schedule)
+
+    def run(eng, x, ix, im, collection, metrics):
+        eng.dpm_setup(betas, tau, order, key=(int(rng[0]), int(rng[1])))
+        eng.dpm_sample(x, infill_x=ix, infill_mask=im, collection=collection, metrics=metrics, use_graph=True)
+    x, collection, metrics = _device_chain(model, init, shard, (4, len(tau)), 41, infill, infill_samples,
+                                           infill_masks, run)
+    return x, collection, metrics.unsqueeze(2)
+
+
 def ddim_encode(model, betas, x0, steps=50, schedule="uniform"):
     """The deterministic DDIM encoder (Song et al. 2021, sections 4.3 and 5.4): the eta = 0 DDIM chain run from the
     data x0 towards noise over the `steps` levels of `betas` that `schedule` picks (ddim_schedule), with the x0

@@ -111,6 +111,8 @@ class Engine:
         self._ws: Optional[torch.Tensor] = None
         self.params: Optional[torch.Tensor] = None
         self._sampler_T = 0
+        self._dpm_order = 1                        # dpm_setup's order, and the history dpm_sample keeps for it
+        self._dpm_hist: Optional[torch.Tensor] = None
 
     def __del__(self):
         try:
@@ -545,6 +547,40 @@ class Engine:
         x = _f32c(x, "x")
         _lib.check(self.lib.smd_ddim_encode(self._plan, self.params.data_ptr(), x.data_ptr(), x.shape[0],
                                             1 if use_graph else 0, self._stream()))
+        return x
+
+    def dpm_setup(self, betas: np.ndarray, steps, order: int = 2, key=(0, 0)) -> None:
+        """DPM-Solver++ multistep of `order` (1, 2 or 3) over the strictly increasing indices `steps` of the schedule
+        `betas` (include/smd.h smd_dpm_setup); replaces a sampler_setup, langevin_setup, ddim_setup or
+        ddim_encode_setup schedule (and vice versa)."""
+        self._ensure_ws()
+        b = np.ascontiguousarray(betas, np.float32)
+        s = np.ascontiguousarray(steps, np.int32)
+        k = _key(key)
+        _lib.check(self.lib.smd_dpm_setup(self._plan, b.ctypes.data_as(C.POINTER(C.c_float)), len(b),
+                                          s.ctypes.data_as(C.POINTER(C.c_int)), len(s), int(order), k,
+                                          self._stream()))
+        self._dpm_order = int(order)
+
+    def _dpm_history(self, x):
+        """The (order - 1, n, ...) scratch of the data estimates the DPM-Solver chain reuses, kept while x's shape and
+        device stay the same (so a replayed graph keeps its buffer); None for order 1."""
+        if self._dpm_order < 2:
+            return None
+        shape = (self._dpm_order - 1,) + tuple(x.shape)
+        h = self._dpm_hist
+        if h is None or tuple(h.shape) != shape or h.device != x.device:
+            h = self._dpm_hist = torch.empty(shape, dtype=torch.float32, device=x.device)
+        return h
+
+    def dpm_sample(self, x, infill_x=None, infill_mask=None, collection=None, metrics=None, use_graph: bool = True):
+        """Runs the whole DPM-Solver++ chain of dpm_setup in place on x.  collection: (41, n, ...) with row 0 left to
+        the caller; metrics: (4, K)."""
+        x = _f32c(x, "x")
+        _f32c_optional(infill_x=infill_x, infill_mask=infill_mask, collection=collection, metrics=metrics)
+        _lib.check(self.lib.smd_dpm_sample(self._plan, self.params.data_ptr(), x.data_ptr(), x.shape[0],
+                                           _ptr(self._dpm_history(x)), _ptr(infill_x), _ptr(infill_mask),
+                                           _ptr(collection), _ptr(metrics), 1 if use_graph else 0, self._stream()))
         return x
 
     LANGEVIN_KINDS = {"ald": 0, "cas": 1}

@@ -80,6 +80,12 @@ _SIGNATURES = {
     "smd_ddim_encode": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P]),
     "smd_ddim_encode_tables": (C.c_int, [C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_int), C.c_int,
                                          C.POINTER(C.c_float)]),
+    "smd_dpm_setup": (C.c_int, [_P, C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int,
+                                C.POINTER(C.c_uint32), _P]),
+    "smd_dpm_sample": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, _P, C.c_int, _P]),
+    "smd_dpm_tables": (C.c_int, [C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int,
+                                 C.POINTER(C.c_uint32), C.POINTER(C.c_float), C.POINTER(C.c_uint32),
+                                 C.POINTER(C.c_int)]),
     "smd_langevin_setup": (C.c_int, [_P, C.POINTER(C.c_float), C.c_int, C.c_int, C.c_float, C.c_int,
                                      C.POINTER(C.c_uint32), _P]),
     "smd_langevin_sample": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, C.c_int, _P, _P, C.c_int, _P]),

@@ -84,7 +84,7 @@ def generate_samples(sample_shape, num_samples, rng_seed=1):
 
 def infill_samples(samples, masks, rng_seed=1):
     """sample_ncsn.py:189-242: keep the masked (=1) entries of `samples`, regenerate the rest with the --sampling
-    chain (ald, ddpm or ddim; cas has no infilling, as upstream)."""
+    chain (ald, ddpm, ddim or dpm; cas has no infilling, as upstream)."""
     del rng_seed
     if FLAGS.sampling == "ald":
         algorithm = ebm_utils.annealed_langevin_dynamics
@@ -94,6 +94,8 @@ def infill_samples(samples, masks, rng_seed=1):
         algorithm = ebm_utils.diffusion_dynamics
     elif FLAGS.sampling == "ddim":
         algorithm = train_ncsn.ddim_algorithm()
+    elif FLAGS.sampling == "dpm":
+        algorithm = train_ncsn.dpm_algorithm()
     else:
         raise ValueError(f"Unknown sampling algorithm: {FLAGS.sampling}")
     rng, optimizer = _restore(FLAGS.model_dir, samples.shape[1:])
@@ -233,6 +235,9 @@ def check_flags():
         raise ValueError("--compute_metrics does not apply to --interpolate")
     if FLAGS.full_metrics and not FLAGS.compute_metrics:
         raise ValueError("--full_metrics needs --compute_metrics")
+    if FLAGS.interpolate and FLAGS.sampling == "dpm":
+        raise ValueError("--interpolate does not take --sampling=dpm: its encoders and decoders are the ddpm and ddim "
+                         "chains")
     if FLAGS.interpolate_encoder == "ddim":
         if not FLAGS.interpolate:
             raise ValueError("--interpolate_encoder=ddim needs --interpolate")

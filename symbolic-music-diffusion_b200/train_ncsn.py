@@ -51,8 +51,9 @@ flags.DEFINE_enum("schedule_type", "geometric", ["geometric", "linear", "fibonac
 flags.DEFINE_integer("num_sigmas", 15, "Length of the noise schedule.")
 flags.DEFINE_integer("ld_steps", 100, "Langevin steps per noise level (null for ddpm).")
 flags.DEFINE_float("ld_epsilon", 2e-6, "Langevin step size (null for ddpm).")
-flags.DEFINE_enum("sampling", "ald", ["ald", "cas", "ddpm", "ddim"],
-                  "Sampling algorithm (ddim is an addition of this implementation, see --ddim_steps).")
+flags.DEFINE_enum("sampling", "ald", ["ald", "cas", "ddpm", "ddim", "dpm"],
+                  "Sampling algorithm (ddim and dpm are additions of this implementation, see --ddim_steps and "
+                  "--dpm_steps).")
 flags.DEFINE_bool("ema", True, "Track an exponential moving average of the parameters.")
 flags.DEFINE_float("mu", 0.999, "EMA momentum.")
 flags.DEFINE_bool("denoise", True, "Expected-denoised-sample step (null for ddpm).")
@@ -79,6 +80,11 @@ flags.DEFINE_integer("synthetic_examples", 4096, "Examples per split with --synt
 flags.DEFINE_integer("ddim_steps", 50, "--sampling=ddim: noise levels of the DDPM schedule the chain visits.")
 flags.DEFINE_float("ddim_eta", 0.0, "--sampling=ddim: noise scale (0: deterministic; 1 with all levels: ddpm).")
 flags.DEFINE_enum("ddim_schedule", "uniform", ["uniform", "quadratic"], "--sampling=ddim: spacing of the levels.")
+flags.DEFINE_integer("dpm_steps", 20, "--sampling=dpm: noise levels of the DDPM schedule the DPM-Solver++ chain "
+                     "visits.")
+flags.DEFINE_integer("dpm_order", 2, "--sampling=dpm: solver order (1: the DDIM eta = 0 step).", lower_bound=1,
+                     upper_bound=3)
+flags.DEFINE_enum("dpm_schedule", "uniform", ["uniform", "quadratic"], "--sampling=dpm: spacing of the levels.")
 
 
 def model_kwargs():
@@ -360,6 +366,8 @@ def sample(scorenet, sigmas, rng, sample_shape, num_samples=2400, sampling="ald"
         algorithm = ebm_utils.diffusion_dynamics
     elif sampling == "ddim":
         algorithm = ddim_algorithm()
+    elif sampling == "dpm":
+        algorithm = dpm_algorithm()
     elif sampling == "ald":
         algorithm = ebm_utils.annealed_langevin_dynamics
     elif sampling == "cas":
@@ -383,10 +391,17 @@ def ddim_algorithm():
                              schedule=FLAGS.ddim_schedule)
 
 
+def dpm_algorithm():
+    """ebm_utils.dpm_solver_dynamics with --dpm_steps, --dpm_order and --dpm_schedule bound: the signature of the other
+    samplers."""
+    return functools.partial(ebm_utils.dpm_solver_dynamics, steps=FLAGS.dpm_steps, order=FLAGS.dpm_order,
+                             schedule=FLAGS.dpm_schedule)
+
+
 def initial_draw(init_rng, shape, sampling, rows=None):
-    """The start of sample()'s chain (train_ncsn.py:541-549): N(0, 1) for ddpm and ddim, otherwise uniform with zero
-    mean and unit variance.  rows=(first, count): only those rows of the draw."""
-    if sampling not in ("ddpm", "ddim"):
+    """The start of sample()'s chain (train_ncsn.py:541-549): N(0, 1) for ddpm, ddim and dpm, otherwise uniform with
+    zero mean and unit variance.  rows=(first, count): only those rows of the draw."""
+    if sampling not in ("ddpm", "ddim", "dpm"):
         rho = float(np.sqrt(np.float32(12)) / 2)
         return random.uniform(init_rng, shape, -rho, rho, rows=rows)
     return random.normal(init_rng, shape, rows=rows)
