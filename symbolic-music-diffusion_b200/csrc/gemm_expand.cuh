@@ -5,20 +5,37 @@
 // At K <= 128 the K loop is two k blocks; such a launch is an output stream (64 KB of bf16 / fp32 per 128 x 128 tile
 // against 32 KB of operands).  Here a CTA owns one 128-row block and a run of n-tiles: it loads its A rows once with
 // TMA and keeps them, the 128 x K weight tiles stream from L2 through a two-stage ring, and each tile's outputs leave
-// through 1-D bulk stores (cp.async.bulk, one per output row) from a shared-memory staging buffer, so no warp waits on
-// its global stores.
+// through 1-D bulk stores (cp.async.bulk, one per output row) from shared-memory staging, so no warp waits on its
+// global stores.
 //
 // 384 threads: warp 0 is the producer, warpgroups 1 and 2 own 64 rows of every tile each.  A consumer warpgroup keeps
 // two accumulator sets: it issues tile j + 1's wgmma before it runs tile j's epilogue from the accumulator fragments.
+// The epilogue goes out in 64-column half-tiles through a ring of three staging slots per warpgroup, each holding the
+// half-tile of every output: while a warpgroup stages half-tile q, the bulk stores of q - 1 and q - 2 are still in
+// flight, and only those of q - 3 (the slot's previous contents) must have read their source.  A single full-tile
+// buffer would make each tile's staging wait for the previous tile's stores, and two of them do not fit next to the
+// resident A rows and the weight ring.
 //
 // Every output is bit-identical to the 128 x 128 layouts': the same m64n128k16 sequence over K (same k-step order),
-// then the same per-element epilogue arithmetic (bias add, act_apply, gelu_tanh_grad_f, bf16 rounding).  The row
-// statistics go to the per-tile slots that stats_slots_for reports, three column groups per n-tile (group g sums the
-// 32-column chunks g and g + 3 with chunk_stats, in that order), so the totals ln_film_act forms are unchanged too.
+// then the same per-element epilogue arithmetic (bias add, act_apply's operations, gelu_tanh_grad_f, bf16 rounding).
+// The row statistics go to the per-tile slots that stats_slots_for reports, three column groups per n-tile (group g
+// sums the 32-column chunks g and g + 3 with chunk_stats, in that order, read back from the tile's two staged halves),
+// so the totals ln_film_act forms are unchanged too.
 #pragma once
 #include "gemm_wgmma.cuh"
 
 namespace smd {
+
+// act_apply with the activation selected instead of branched on: the same operations, so the same bits.  ep.act is
+// uniform, but a branch around every element's tanh keeps ptxas from overlapping one element's MUFU latency with the
+// next element's arithmetic, which made the FFN-up staging latency-bound.
+__device__ __forceinline__ float act_apply_select(float v, int act) {
+  const float c = 0.7978845608028654f;
+  const float h = 0.5f * v;
+  const float u = act == ACT_GELU_TANH ? v * fmaf(v * v, 0.044715f * c, c) : h;
+  const float y = fmaf(h, tanh_fast(u), h);
+  return act == ACT_GELU_TANH || act == ACT_SWISH ? y : v;
+}
 
 template <uint32_t kF>
 struct GemmSmemExpand {
@@ -27,18 +44,26 @@ struct GemmSmemExpand {
   static constexpr int kABytes = kBM * kKMax * 2;             // 32 KB: the CTA's A rows, two 64-wide k blocks
   static constexpr int kBBytes = kBNMax * kKMax * 2;          // 32 KB: one weight tile
   static constexpr int kStages = 2;
-  static constexpr int kHPitch = kBNMax * 2 + 16;             // bytes per staged bf16 row (padded: conflict-free)
-  static constexpr int kFPitch = kBNMax * 4 + 16;             // bytes per staged fp32 row
+  static constexpr int kHPitch = kBNMax * 2 + 16;             // bytes per gelu_grad_of row (padded: conflict-free)
   static constexpr int kHBytes = kGG ? kBM * kHPitch : 0;     // the tile of gelu_grad_of, per stage
-  // per consumer warpgroup (64 rows): fp32 out, or bf16 out (+ the bf16 pre-activation for kEpiAct)
-  static constexpr int kOutBytes = (kF == kEpiF32) ? 64 * kFPitch : (kF == kEpiAct ? 2 : 1) * 64 * kHPitch;
+  // Staging ring, per consumer warpgroup: kSlots slots of one 64-row x 64-column half-tile of every output (fp32 out,
+  // or bf16 out + the bf16 pre-activation for kEpiAct, or bf16 out), rows padded by 16 bytes (conflict-free), then
+  // the half-tile's 64 bias values (kEpiAct, kEpiF32).
+  static constexpr int kHalf = kBNMax / 2;
+  static constexpr int kOuts = kF == kEpiAct ? 2 : 1;
+  static constexpr int kSPitch = kHalf * (kF == kEpiF32 ? 4 : 2) + 16;
+  static constexpr int kBiasOff = kOuts * 64 * kSPitch;
+  static constexpr int kSlotBytes = kBiasOff + (kGG ? 0 : kHalf * 4);   // 18 688 (kEpiAct), 17 664 (kEpiF32), 9 216
+  static constexpr int kSlots = 3;
   static constexpr int kBarBytes = 128;
-  static constexpr int kTotal = 1024 + kABytes + kStages * (kBBytes + kHBytes) + 2 * kOutBytes + kBarBytes;
+  // 211 584 (kEpiAct), 205 440 (kEpiF32), 224 384 (kEpiGG) bytes
+  static constexpr int kTotal = 1024 + kABytes + kStages * (kBBytes + kHBytes) + 2 * kSlots * kSlotBytes + kBarBytes;
   static constexpr int kThreads = 384;
   static constexpr int kEpiGroups = 3;                        // statistics slots per (row, n-tile)
   static constexpr int kProdRegs = 40, kMmaRegs = 232;
   static_assert(kProdRegs + 2 * kMmaRegs <= 3 * 170, "register budgets exceed the CTA's file");
   static_assert(kTotal <= GemmSmem<8>::kMaxSmem, "shared memory");
+  static_assert(kSPitch % 16 == 0 && kSlotBytes % 16 == 0, "bulk-store sources must be 16-byte aligned");
   static_assert((1 + 2 * kStages + (kGG ? 2 * kStages : 0)) * 8 <= kBarBytes, "mbarriers do not fit their region");
 };
 
@@ -58,8 +83,8 @@ gemm_bf16_wgmma_expand_kernel(const __grid_constant__ CUtensorMap tmA, const __g
   uint8_t* sA = smem;
   uint8_t* sB = sA + SM::kABytes;                                   // [kStages][kBBytes]
   uint8_t* sH = sB + SM::kStages * SM::kBBytes;                     // [kStages][kHBytes]
-  uint8_t* sOut = sH + SM::kStages * SM::kHBytes;                   // [2 warpgroups][kOutBytes]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sOut + 2 * SM::kOutBytes);
+  uint8_t* sOut = sH + SM::kStages * SM::kHBytes;                   // [2 warpgroups][kSlots][kSlotBytes]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sOut + 2 * SM::kSlots * SM::kSlotBytes);
   uint64_t* a_full = bars;
   uint64_t* b_full = bars + 1;                                      // [kStages]
   uint64_t* b_empty = b_full + SM::kStages;                         // [kStages]
@@ -139,12 +164,18 @@ gemm_bf16_wgmma_expand_kernel(const __grid_constant__ CUtensorMap tmA, const __g
   const uint32_t wg = (warp - 4u) >> 2;
   const uint32_t tid = threadIdx.x - 128u - wg * 128u;              // thread index inside the warpgroup
   auto wg_bar = [wg] { asm volatile("bar.sync %0, 128;" ::"r"(1u + wg) : "memory"); };
-  uint8_t* out = sOut + wg * SM::kOutBytes;
+  uint8_t* ring = sOut + wg * (SM::kSlots * SM::kSlotBytes);
   // this thread's fragment: rows r_frag + 8 h of the warpgroup's 64, columns 8 j + c_frag + {0, 1} -> d[4 j + 2 h + e]
   const int r_frag = static_cast<int>(((warp - 4u) & 3u) * 16u + (lane >> 2));
   const int c_frag = 2 * static_cast<int>(lane & 3u);
   const int row0 = m0 + static_cast<int>(wg) * 64;                  // first row of this warpgroup
-  const bool issuer = tid < 64 && row0 + static_cast<int>(tid) < sh.M;   // stores row `tid` of each output
+  // the half-tile's bulk stores, one per row and output, spread over all four warps: thread tid stores output
+  // st_part of row st_row (kEpiAct), or row st_row from the even threads (one output)
+  const int st_row = SM::kOuts == 2 ? static_cast<int>(tid & 63u) : static_cast<int>(tid >> 1);
+  const int st_part = SM::kOuts == 2 ? static_cast<int>(tid >> 6) : static_cast<int>(tid & 1u);
+  bool storer = row0 + st_row < sh.M;                               // rows >= M are never stored
+  if constexpr (kF == kEpiAct) storer = storer && (st_part == 0 || ep.out_bf16_pre != nullptr);
+  else storer = storer && st_part == 0;
 
   auto issue = [&](float (&d)[64], int i) {
     const int s = i % SM::kStages;
@@ -169,95 +200,124 @@ gemm_bf16_wgmma_expand_kernel(const __grid_constant__ CUtensorMap tmA, const __g
     if (lane == 0) mbar_arrive(&b_empty[i % SM::kStages]);
   };
 
+  // Tile i leaves as half-tiles q = 2 i + h, staged in ring slot q % kSlots.  Every thread commits one bulk group per
+  // half-tile (empty if it stores nothing), so waiting until kSlots - 1 groups remain means half-tile q - kSlots, the
+  // slot's previous contents, has been read out.
+  // The bias of half-tile q + 1 is read from global memory while half-tile q is staged: thread tid < 64 holds its
+  // column tid and puts it into the slot before the slot's first barrier, so the staging reads it from shared memory.
+  float bias_next = 0.f;
+  auto load_bias = [&](int q) {
+    if constexpr (!kGG) {
+      if (ep.bias != nullptr && tid < 64u && q < 2 * tpc)
+        bias_next = __ldg(ep.bias + (nt0 + q / 2) * kBNMax + SM::kHalf * (q % 2) + static_cast<int>(tid));
+    }
+  };
+  load_bias(0);
   auto epilogue = [&](const float (&d)[64], int i) {
     const int n0 = (nt0 + i) * kBNMax;
     const int s = i % SM::kStages;
     if constexpr (kGG) mbar_wait(&h_full[s], static_cast<uint32_t>(i / SM::kStages) & 1u);
-    // the previous tile's bulk stores have read the staging buffer
-    if (issuer) bulk_wait_read();
-    wg_bar();
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int col = 8 * j + c_frag;
-      float2 bj = make_float2(0.f, 0.f);
-      if constexpr (kF != kEpiGG) {
-        if (ep.bias != nullptr) bj = __ldg(reinterpret_cast<const float2*>(ep.bias + n0 + col));
+    for (int h = 0; h < 2; ++h) {
+      uint8_t* slot = ring + ((2 * i + h) % SM::kSlots) * SM::kSlotBytes;
+      const float* sbias = reinterpret_cast<const float*>(slot + SM::kBiasOff);
+      if constexpr (!kGG) {
+        // the slot's bias was last read while half-tile q - kSlots was staged, before this thread's later barriers
+        if (ep.bias != nullptr && tid < 64u) reinterpret_cast<float*>(slot + SM::kBiasOff)[tid] = bias_next;
+        load_bias(2 * i + h + 1);
       }
+      bulk_wait_read<SM::kSlots - 1>();
+      wg_bar();
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = r_frag + 8 * h;
-        float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
-        if constexpr (kF == kEpiF32) {
-          if (ep.bias != nullptr) add_pair(v0, v1, bj.x, bj.y);
-          *reinterpret_cast<float2*>(out + r * SM::kFPitch + col * 4) = make_float2(v0, v1);
-        } else if constexpr (kF == kEpiAct) {
-          if (ep.bias != nullptr) add_pair(v0, v1, bj.x, bj.y);
-          *reinterpret_cast<uint32_t*>(out + r * SM::kHPitch + col * 2) =
-              pack_bf16x2(act_apply(v0, ep.act), act_apply(v1, ep.act));
-          *reinterpret_cast<uint32_t*>(out + (64 + r) * SM::kHPitch + col * 2) = pack_bf16x2(v0, v1);
-        } else {
-          const uint8_t* hrow = sH + s * SM::kHBytes + (static_cast<int>(wg) * 64 + r) * SM::kHPitch;
-          const float2 g = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(hrow + col * 2));
-          v0 *= gelu_tanh_grad_f(g.x);
-          v1 *= gelu_tanh_grad_f(g.y);
-          *reinterpret_cast<uint32_t*>(out + r * SM::kHPitch + col * 2) = pack_bf16x2(v0, v1);
+      for (int jh = 0; jh < 8; ++jh) {
+        const int j = 8 * h + jh;               // column octet of the tile
+        const int col = 8 * jh + c_frag;        // column inside the half-tile
+        float2 bj = make_float2(0.f, 0.f);
+        if constexpr (kF != kEpiGG) {
+          if (ep.bias != nullptr) bj = *reinterpret_cast<const float2*>(sbias + col);
+        }
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int r = r_frag + 8 * e;
+          float v0 = d[4 * j + 2 * e], v1 = d[4 * j + 2 * e + 1];
+          if constexpr (kF == kEpiF32) {
+            if (ep.bias != nullptr) add_pair(v0, v1, bj.x, bj.y);
+            *reinterpret_cast<float2*>(slot + r * SM::kSPitch + col * 4) = make_float2(v0, v1);
+          } else if constexpr (kF == kEpiAct) {
+            if (ep.bias != nullptr) add_pair(v0, v1, bj.x, bj.y);
+            *reinterpret_cast<uint32_t*>(slot + r * SM::kSPitch + col * 2) =
+                pack_bf16x2(act_apply_select(v0, ep.act), act_apply_select(v1, ep.act));
+            *reinterpret_cast<uint32_t*>(slot + (64 + r) * SM::kSPitch + col * 2) = pack_bf16x2(v0, v1);
+          } else {
+            const uint8_t* hrow = sH + s * SM::kHBytes + (static_cast<int>(wg) * 64 + r) * SM::kHPitch;
+            const float2 g =
+                __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(hrow + (SM::kHalf * h + col) * 2));
+            v0 *= gelu_tanh_grad_f(g.x);
+            v1 *= gelu_tanh_grad_f(g.y);
+            *reinterpret_cast<uint32_t*>(slot + r * SM::kSPitch + col * 2) = pack_bf16x2(v0, v1);
+          }
         }
       }
+      if constexpr (kGG) {
+        if (h == 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&h_empty[s]);
+        }
+      }
+      fence_proxy_async_smem();   // the staged half-tile is read by the bulk-copy (async) proxy
+      wg_bar();
+      if (storer) {
+        const size_t row = static_cast<size_t>(row0 + st_row);
+        const int c0 = n0 + SM::kHalf * h;
+        if constexpr (kF == kEpiF32) {
+          bulk_store_1d(ep.out_f32 + row * ep.ld_f32 + c0, slot + st_row * SM::kSPitch, SM::kHalf * 4);
+        } else {
+          __nv_bfloat16* dst = st_part == 0 ? ep.out_bf16 : ep.out_bf16_pre;
+          bulk_store_1d(dst + row * ep.ld_bf16 + c0, slot + (64 * st_part + st_row) * SM::kSPitch, SM::kHalf * 2);
+        }
+      }
+      bulk_commit();
     }
-    if constexpr (kGG) {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&h_empty[s]);
-    }
-    fence_proxy_async_smem();   // the staged tile is read by the bulk-copy (async) proxy
-    wg_bar();
     if constexpr (kF == kEpiF32) {
       if (ep.row_stats != nullptr) {
-        // two threads per row: part 0 sums column group 0 (chunks 0 and 3), part 1 groups 1 and 2
+        // From the tile's two staged halves, once the accumulators are dead (their slots are next written by
+        // half-tiles 2 i + 3 and 2 i + 4, after barriers this thread has not reached yet).  Two threads per row: part 0
+        // sums chunk 0, then chunk 3 (column group 0); part 1 sums chunk 1 (group 1), then chunk 2 (group 2).
         const int r = static_cast<int>(tid & 63u), part = static_cast<int>(tid >> 6);
         const int row = row0 + r;
         if (row < sh.M) {
-          const float* srow = reinterpret_cast<const float*>(out + r * SM::kFPitch);
-          const int nslots = (sh.N / kBNMax) * SM::kEpiGroups;
-#pragma unroll
-          for (int gi = 0; gi < 2; ++gi) {
-            const int g = part == 0 ? 0 : gi + 1;
-            if (part == 0 && gi == 1) break;
-            float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-            for (int ci = 0; ci < 2; ++ci) {
-              const int c = g + 3 * ci;
-              if (c >= 4) break;
-              float v[32];
-#pragma unroll
-              for (int q = 0; q < 8; ++q) {
-                const float4 t = reinterpret_cast<const float4*>(srow + 32 * c)[q];
-                v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
-              }
-              chunk_stats(v, s1, s2);
-            }
+          const size_t slot0 =
+              static_cast<size_t>(row) * ((sh.N / kBNMax) * SM::kEpiGroups) + (nt0 + i) * SM::kEpiGroups;
+          auto put = [&](int g, float s1, float s2) {
             if (ep.stats_part != nullptr) {
-              reinterpret_cast<float2*>(ep.stats_part)[static_cast<size_t>(row) * nslots + (nt0 + i) * SM::kEpiGroups + g] =
-                  make_float2(s1, s2);
+              reinterpret_cast<float2*>(ep.stats_part)[slot0 + g] = make_float2(s1, s2);
             } else {
               atomicAdd(ep.row_stats + 2 * static_cast<size_t>(row), s1);
               atomicAdd(ep.row_stats + 2 * static_cast<size_t>(row) + 1, s2);
             }
+          };
+          auto add_chunk = [&](int q, int half_chunk, float& s1, float& s2) {   // half-tile q, its chunk 0 or 1
+            const float4* src = reinterpret_cast<const float4*>(ring + (q % SM::kSlots) * SM::kSlotBytes +
+                                                                r * SM::kSPitch + half_chunk * 128);
+            float v[32];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+              const float4 t = src[k];
+              v[4 * k] = t.x; v[4 * k + 1] = t.y; v[4 * k + 2] = t.z; v[4 * k + 3] = t.w;
+            }
+            chunk_stats(v, s1, s2);
+          };
+          float s1 = 0.f, s2 = 0.f;
+          add_chunk(2 * i, part, s1, s2);
+          if (part == 1) {
+            put(1, s1, s2);
+            s1 = 0.f;
+            s2 = 0.f;
           }
+          add_chunk(2 * i + 1, 1 - part, s1, s2);
+          put(part == 0 ? 0 : 2, s1, s2);
         }
       }
-    }
-    if (issuer) {
-      const size_t row = static_cast<size_t>(row0) + tid;
-      if constexpr (kF == kEpiF32) {
-        bulk_store_1d(ep.out_f32 + row * ep.ld_f32 + n0, out + tid * SM::kFPitch, kBNMax * 4);
-      } else {
-        bulk_store_1d(ep.out_bf16 + row * ep.ld_bf16 + n0, out + tid * SM::kHPitch, kBNMax * 2);
-        if constexpr (kF == kEpiAct) {
-          if (ep.out_bf16_pre != nullptr)
-            bulk_store_1d(ep.out_bf16_pre + row * ep.ld_bf16 + n0, out + (64 + tid) * SM::kHPitch, kBNMax * 2);
-        }
-      }
-      bulk_commit();
     }
   };
 
@@ -270,8 +330,8 @@ gemm_bf16_wgmma_expand_kernel(const __grid_constant__ CUtensorMap tmA, const __g
   }
   issue(db, tpc - 1); wgmma_wait<1>(); release_b(tpc - 2); epilogue(da, tpc - 2);
   wgmma_wait<0>(); release_b(tpc - 1); epilogue(db, tpc - 1);
-  // the outputs are written before the CTA (and its staging buffer) goes away
-  if (issuer) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+  // the outputs are written before the CTA (and its staging ring) goes away
+  asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
 }  // namespace smd

@@ -104,8 +104,12 @@ __device__ __forceinline__ void bulk_store_1d(void* dst, const void* smem_src, u
                ::"l"(reinterpret_cast<uint64_t>(dst)), "r"(smem_u32(smem_src)), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// this thread's bulk stores have finished reading their shared-memory sources (the buffer may be rewritten)
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// all but this thread's kPending most recent bulk groups have finished reading their shared-memory sources (those
+// buffers may be rewritten)
+template <int kPending>
+__device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(kPending) : "memory");
+}
 // ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
